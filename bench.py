@@ -10,7 +10,7 @@ V=K=16384, 8x8x4 codes) + the ImageNet RQ-VAE decoder, random-init weights, synt
 only exchange is one all_gather of the finished [B,8,8,4] int64 code maps before the decoder (north star).
 `--model` selects the other BASELINE configs (2: ffhq355m, 4: cc3m654m / cc3m654m_16, 5: t2i3900m / t2i3900m_16).
 
-Arithmetic: the fast tier -- fp16 weights / activations / KV on tcgen05 with fp32 accumulation, the reference's own GPU
+Arithmetic: the fast tier -- fp16 weights / activations / KV on wgmma with fp32 accumulation, the reference's own GPU
 sampling class (fp16 autocast, main_sampling_fid.py:216); `--dtype bf16` selects bf16, `--precision exact` the fp32 tier.
 
 Prints ONE JSON line (rank 0).  `value`: images/sec with inputs resident in HBM; `e2e`: same through the public API with
@@ -19,6 +19,8 @@ pinned HOST inputs (labels + empty code map) copied H2D and the finished pixels 
 the fast tier's teacher-forced / free-running statistics against the reference-generated trajectories of this model
 (tests/golden/ar.pt) measured in this run; `strong`: the fixed-total-batch point (global batch 64 split over N GPUs).
 `--impl reference` times the CPU oracle port of the reference's own PyTorch path on the host cores (rank 0 only).
+`--dump-outputs DIR` writes what the last timed step returned (codes, pixels) as DIR/<name>.npy; with the same arguments the inputs
+are identical from run to run, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -28,6 +30,8 @@ import sys
 import threading
 import time
 
+import numpy as np
+
 ROOT = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.join(ROOT, "rq-vae-transformer_b200")
 for p in (ROOT, PKG):
@@ -36,9 +40,6 @@ for p in (ROOT, PKG):
 
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
-
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture (profiles/), or None
-TRAFFIC_NCU = {"gemm_tc_fc2": 19736320}   # profiles/ncu_ar_chain_r2_raw.csv, fc2 launch: 19.74 MB read + 0 B written (partials stay in L2)
 
 MODELS = {
     # name: (E, heads, n_body, n_head_layers, V, block, vocab_cond, cond_len, vae attn_res, vae ch_mult, top_p, default B, text)
@@ -92,7 +93,7 @@ def build_models(name, device, precision, tiny_vae=False):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)"""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -132,10 +133,10 @@ def ar_bytes_per_position(name, B, wbytes):
 
 
 def gemm_kernel_roofline(ar, B, hbm_peak, peak_src):
-    """The step's dominant kernel (ncu launch list, profiles/): gemm_tc_kernel<64,8> at the split-K shapes.  Timed live: a
+    """The step's dominant kernel: gemm_tc_kernel<64,8> at the split-K shapes.  Timed live: a
     CUDA graph of one launch per body layer on that layer's own fc2 weight (42 x 18.9 MB = 0.8 GB >> L2, i.e. cold
     weights, exactly as in the step), replayed; CUDA events on the launching stream.  Algorithmic bytes = weights +
-    activations in + the [B,E] fp32 result; the split-K partials are L2-resident scratch (ncu: 0 B written to DRAM)."""
+    activations in + the [B,E] fp32 result; the split-K partials are L2-resident scratch."""
     from rqvae import _native as N
     L = N.lib()
     blocks = ar.body_transformer.blocks
@@ -143,7 +144,7 @@ def gemm_kernel_roofline(ar, B, hbm_peak, peak_src):
     dt = N.fast_dtype()
     Ws = [b.mlp[2].weight.detach().to(dt).contiguous() for b in blocks]       # [E, 4E]
     X = torch.randn(B, 4 * E, device=Ws[0].device).to(dt)
-    splits = max(1, min(148 // (E // 128), 4 * E // 64))
+    splits = max(1, min(torch.cuda.get_device_properties(Ws[0].device).multi_processor_count // (E // 128), 4 * E // 64))
     part = torch.empty(splits, B, E, device=Ws[0].device)
     stream = torch.cuda.Stream()
     with torch.cuda.stream(stream):
@@ -251,7 +252,7 @@ def parity_record(name, dev):
     from tests.helpers import CodebookAux, build_ar, noise_tensor
     gold = os.path.join(ROOT, "tests", "golden")
     g, fixture = None, None
-    for fixture in ("ar.pt", "ar2.pt"):
+    for fixture in ("ar.pt", "ar2.pt", "ar3.pt"):
         g = torch.load(os.path.join(gold, fixture), weights_only=False)["ar"].get(name)
         if g is not None:
             break
@@ -299,6 +300,26 @@ def parity_record(name, dev):
             "free_running": free}
 
 
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir, codes, pix):
+    """codes [B,H,W,D] (exact in float64) and pixels [B,3,R,R] float32 of the last timed step.  Above the size limit, a fixed
+    seeded sample of whole images is written instead (pixels_index.npy names them)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"codes": codes.to(torch.float64)}
+    per_img = pix[0].numel() * 4
+    keep = (DUMP_LIMIT - arrays["codes"].numel() * 8) // per_img
+    if keep < pix.shape[0]:
+        idx = torch.randperm(pix.shape[0], generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        pix = pix[idx]
+        arrays["pixels_index"] = idx.to(torch.float64)
+    arrays["pixels"] = pix.to(torch.float32)
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v.numpy())
+    return {k: list(v.shape) for k, v in arrays.items()}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -313,6 +334,8 @@ def main():
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the exact_tier and strong records")
     ap.add_argument("--cpu-budget", type=float, default=25.0)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's codes and pixels as DIR/<name>.npy (float64 / float32, <= 64 MB)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -390,6 +413,7 @@ def main():
             if e2e:
                 io["pix_h"].copy_(pix, non_blocking=True)
             ev[i][2].record()
+            io["last"] = (codes, pix)
         t1.record()
         barrier()
         total = t0.elapsed_time(t1)
@@ -408,6 +432,7 @@ def main():
         clocks.start()
     total, ar_ms, dec_ms = timed(io, False, args.steps)
     clock_summary = clocks.summary() if rank == 0 else None
+    last_codes, last_pix = (t.cpu() for t in io["last"])
     launches = N.launch_count["total"] - launches0
     timed(io, True, 1)
     e_total, e_ar, e_dec = timed(io, True, args.steps)
@@ -417,7 +442,7 @@ def main():
     e2e_value = n_img / (e_total / 1e3)
     ar_ms_token = ar_ms / args.steps / (H * W * D)
     # P3 roofline: algorithmic bytes per spatial position / measured time per position (weights stream from HBM every
-    # position: 3.94 GB >> 126 MB L2)
+    # position: 3.94 GB >> 50 MB L2)
     wbytes = 2 if amp else 4
     peaks = {}
     try:
@@ -425,10 +450,10 @@ def main():
             peaks = json.load(f)
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
     pos_ms = ar_ms / args.steps / (H * W)
     ach = ar_bytes_per_position(name, B, wbytes) / 1e9 / (pos_ms / 1e3)
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "data sheet 3350 GB/s (H100 SXM HBM3)"
     roofline_step = {"bound": "hbm", "kernel": "AR spatial position (body stack + D x (head stack + classifier + sampler))",
                      "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "traffic": None,
                      "algorithmic_bytes_per_position": ar_bytes_per_position(name, B, wbytes), "ms_per_position": pos_ms,
@@ -437,14 +462,13 @@ def main():
     if rank == 0 and amp:
         try:
             roofline = gemm_kernel_roofline(ar, B, hbm_peak, peak_src)
-            roofline["traffic"] = TRAFFIC_NCU.get("gemm_tc_fc2") if name == "in1400m" and B == 64 else None
         except Exception as ex:
             roofline = dict(roofline_step, note="kernel-level measurement failed: %s" % str(ex)[:120])
     line = {"metric": metric_text(name), "value": value, "unit": "images/s", "n_gpus": max(world, 1), "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": total / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": (args.dtype if amp else "f32"), "data": "synthetic", "config": config,
             "ar_ms_per_token": ar_ms_token, "ar_ms_per_step": ar_ms / args.steps, "decode_ms_per_step": dec_ms / args.steps,
-            "clocks": clock_summary, "gpu_launches": launches,
+            "gpu": torch.cuda.get_device_name(dev), "clocks": clock_summary, "gpu_launches": launches,
             "e2e": {"value": e2e_value, "unit": "images/s",
                     "h2d_bytes_per_step": io["lab_h"].numel() * 8 + io["emp_h"].numel() * 8,
                     "d2h_bytes_per_step": io["pix_h"].numel() * 4},
@@ -497,6 +521,8 @@ def main():
                                         "sample": r["sample"], "ar_ms_per_token": r["ar_ms_per_token"]}
             except Exception as ex:   # the baseline is reported, never required
                 line["cpu_baseline"] = {"value": None, "error": str(ex)[:200]}
+        if args.dump_outputs:
+            line["dumped"] = dump_outputs(args.dump_outputs, last_codes, last_pix)
         print(json.dumps(line))
     if world > 1:
         dist.barrier()

@@ -1,5 +1,5 @@
 /*
- * rqb200 -- C ABI of the B200-native RQ-VAE / RQ-Transformer sampling engine (sm_100a).
+ * rqb200 -- C ABI of the H100-native RQ-VAE / RQ-Transformer sampling engine (sm_90a).
  *
  * The reference (kakaobrain/rq-vae-transformer @ 341395e) is pure Python/PyTorch and has no plugin / FFI
  * registry; its boundary for this path is the Python class surface of `rqvae.models` (SURVEY.md section 8b).  Each
@@ -35,7 +35,7 @@ extern "C" {
 
 /* arithmetic modes (DESIGN.md "two modes") */
 #define RQB200_MODE_EXACT 0  /* fp32 weights + fp32 FFMA: the bit-exact-indices gate                    */
-#define RQB200_MODE_FAST 1   /* fp16 (default) or bf16 operands on tcgen05, fp32 accumulate: throughput  */
+#define RQB200_MODE_FAST 1   /* fp16 (default) or bf16 operands on wgmma, fp32 accumulate: throughput  */
 
 /* rqb200_ar_config.flags (fast tier; scheduling only -- none of them changes a result bit, except SEQUENTIAL_PREFILL's
  * summation order) */
@@ -146,7 +146,7 @@ int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* c
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
                           void* workspace, size_t workspace_bytes, void* stream);
 /* RQTransformer.forward (transformers.py:113-188): teacher-forced logits of complete code maps, all positions at once (fast tier:
- * M = B*T row GEMMs on tcgen05 + causal attention; exact tier: returns RQB200_EINVAL -- use rqb200_ar_sample with force_codes and
+ * M = B*T row GEMMs on wgmma + causal attention; exact tier: returns RQB200_EINVAL -- use rqb200_ar_sample with force_codes and
  * logits_out, the sequential replay).  codes [B,H,W,D] int64, cond [B,cond_len] or NULL.
  * logits_out [D][H*W][B][V] f32 (token-major: logits of (b, pos, d) at ((d*H*W + pos)*B + b)*V); cond_logits_out (nullable,
  * cond_len > 1 and w_ccls given) [cond_len-1][B][Vc] f32 with Vc = vocab_cond rounded up to a multiple of 128. */
@@ -196,7 +196,7 @@ int64_t rqb200_vae_last_launches(const rqb200_vae* h);
 
 /* ------------------------------------------------------------------------------------------------ diagnostics
  * Single-kernel entry points used by tests/ and bench.py's roofline leg; not part of the reference-facing surface.
- * rqb200_dbg_gemm_tc: one launch of the tcgen05 weight-streaming GEMM (csrc/gemm_tc.cu):
+ * rqb200_dbg_gemm_tc: one launch of the wgmma weight-streaming GEMM (csrc/gemm_tc.cu):
  *   out[b, n] = act(sum_k W[n,k] X[b,k] + bias[n]) (+ residual[b,n]);  W [N_out,K], X [B,K] both 16-bit: fmt 0 = fp16, 1 = bf16;
  *   partial != NULL: partial [splits,B,N_out] f32 receives the per-split sums instead (no bias / act / residual; B <= 256).
  *   B > 256 (splits == 1) runs as row chunks of 256 (the batched-prefill / teacher-forced-forward shape). */
@@ -213,7 +213,7 @@ int rqb200_dbg_rq_quantize(int form, const float* x, const float* codebook, int6
 int rqb200_dbg_sample_logits(int algo, const float* logits, const float* q, int B, int V, float temperature, int top_k,
                              float top_p, int64_t* out_idx, void* stream);
 
-/* rqb200_dbg_conv_tc: one launch of the tcgen05 implicit-GEMM conv (csrc/conv_tc.cu): X NHWC fp16 [B,H,W,Cin], W OHWI fp16
+/* rqb200_dbg_conv_tc: one launch of the wgmma implicit-GEMM conv (csrc/conv_tc.cu): X NHWC fp16 [B,H,W,Cin], W OHWI fp16
  * [Cout,ks,ks,Cin], stride 1 "same" padding, out f32 NHWC (+bias, +residual) or NCHW when out_nchw.  X16lo / W16lo
  * (both or neither): the fp16 "lo" halves (value - fp16(value)) -> split-fp16, three products per conv. */
 int rqb200_dbg_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
@@ -234,7 +234,7 @@ int rqb200_dbg_chain2(int variant, int words, int n_stages, int ctas, int thread
                       size_t workspace_bytes, float* us_per_stage);
 
 /* rqb200_dbg_rows_gemm: the large-M GEMM of the batched prefill / forward passes (csrc/conv_tc.cu launch_rows_gemm_tc: persistent
- * 128 x BN tiles, double-buffered TMEM): out[m,n] = act(sum_k X[m,k] W[n,k] + bias[n]) (+ residual[m,n]).  X [ceil(M/128)*128, K] and
+ * 128 x BN tiles, wgmma): out[m,n] = act(sum_k X[m,k] W[n,k] + bias[n]) (+ residual[m,n]).  X [ceil(M/128)*128, K] and
  * W [N_out,K] 16-bit (fmt 0 fp16 / 1 bf16); exactly one of out_f32 / out_16; gelu applies to out_16 only. */
 int rqb200_dbg_rows_gemm(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                          int gelu, int fmt, int64_t M, int N_out, int K, void* stream);

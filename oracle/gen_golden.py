@@ -23,7 +23,7 @@ from oracle import synth                    # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden")
 
-from oracle.zoo import AR_ZOO, VAE_ZOO      # noqa: E402
+from oracle.zoo import AR_FIXTURE, AR_ZOO, VAE_ZOO      # noqa: E402
 
 
 def ar_cfg(name):
@@ -248,17 +248,33 @@ def gen_layouts(ns):
         json.dump(lay, f)
 
 
+def gen_init(ns, out):
+    """the reference's default initialisation under torch.manual_seed(0) (same constructor order => same weights)"""
+    E, nh, nb, nhl, V, bs, vc, cl = AR_ZOO["tiny"]
+    torch.manual_seed(0)
+    out["ar/tiny"] = synth.state_dict_sample(ns.RQTransformer(ar_cfg("tiny")).state_dict())
+    torch.manual_seed(0)
+    out["vae/tiny"] = synth.state_dict_sample(ns.RQVAE(**R.vae_kwargs(**VAE_ZOO["tiny"])).state_dict())
+
+
 def main():
     torch.set_grad_enabled(False)
     os.makedirs(GOLD, exist_ok=True)
     ns = R.load_reference()
     check_multinomial_identity()
-    which = sys.argv[1:] or ["rq", "sampler", "ar", "vae", "ar2", "layouts"]
-    for part, fn in (("rq", gen_rq), ("sampler", gen_sampler), ("ar", gen_ar), ("vae", gen_vae), ("ar2", gen_ar2)):
+    which = sys.argv[1:] or ["rq", "sampler", "ar", "vae", "ar2", "layouts", "init"]
+    for part, fn in (("rq", gen_rq), ("sampler", gen_sampler), ("ar", gen_ar), ("vae", gen_vae), ("ar2", gen_ar2),
+                     ("init", gen_init)):
         if part in which:
             out = {}
             t0 = time.time()
             fn(ns, out)
+            if part == "ar2":
+                # two files under 1 MB: cc3m654m (greedy run: logits of the first and last step only) | the other two shapes
+                lg = out["ar"]["cc3m654m"]["runs"][0]["logits"]
+                out["ar"]["cc3m654m"]["runs"][0]["logits"] = {k: v for k, v in lg.items() if k in (0, 255)}
+                torch.save({"ar": {n: out["ar"][n] for n in AR_FIXTURE if AR_FIXTURE[n] == "ar3"}}, os.path.join(GOLD, "ar3.pt"))
+                out = {"ar": {n: out["ar"][n] for n in AR_FIXTURE if AR_FIXTURE[n] == "ar2"}}
             torch.save(out, os.path.join(GOLD, part + ".pt"))
             print("%s done in %.1fs" % (part, time.time() - t0), flush=True)
     if "layouts" in which:

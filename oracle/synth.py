@@ -83,3 +83,16 @@ def exp_noise(seed, step, B, V):
     """per-token Exp(1) noise [B,V] from its own seeded generator (stream-independent of model/init RNG)."""
     g = torch.Generator().manual_seed(seed * 100003 + step)
     return torch.empty(B, V).exponential_(1, generator=g)
+
+
+def state_dict_sample(sd, n=64):
+    """{key: (shape, fp64 sum, n seeded sample values)} -- a small stand-in for a state_dict in a fixture; the positions
+    depend only on the tensor's size, so two state_dicts of one layout are sampled at the same places."""
+    out = {}
+    for k, v in sd.items():
+        flat = v.detach().reshape(-1).cpu()
+        if flat.numel() > n:
+            g = torch.Generator().manual_seed(flat.numel())
+            flat = flat[torch.randint(0, flat.numel(), (n,), generator=g)]
+        out[k] = (list(v.shape), float(v.double().sum()), flat.clone())
+    return out

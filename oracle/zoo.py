@@ -13,6 +13,8 @@ AR_ZOO = {
     "cc3m654m_16": (1280, 20, 26, 4, 16384, (16, 16, 4), 16384, 32),
     "t2i3900m": (2560, 40, 42, 6, 16384, (8, 8, 4), 16384, 32),
 }
+# fixture file (tests/golden/<name>.pt) holding the reference's AR trajectories of each shape
+AR_FIXTURE = {"cc3m654m": "ar2", "cc3m654m_16": "ar3", "t2i3900m": "ar3"}
 VAE_ZOO = {
     "tiny": dict(K=512, code_shape=(4, 4, 4), ch=32, ch_mult=(1, 2, 4), attn_resolutions=(4,), resolution=16),
     "tiny_attn_mid": dict(K=512, code_shape=(4, 4, 4), ch=32, ch_mult=(1, 1, 2, 4), attn_resolutions=(8,), resolution=32),

@@ -1,7 +1,7 @@
-// P3 "fast" tier -- the cached AR step as a PDL-chained, CUDA-graph-replayed sequence of sm_100a kernels.
+// P3 "fast" tier -- the cached AR step as a PDL-chained, CUDA-graph-replayed sequence of sm_90a kernels.
 //
 // Same semantics as ar_engine.cu's exact tier (reference: transformers.py:190-369, attentions.py:60-142), different
-// arithmetic class: 16-bit weights / activations / KV cache on tcgen05 (gemm_tc.cu) -- fp16 by default, the reference's own
+// arithmetic class: 16-bit weights / activations / KV cache on wgmma (gemm_tc.cu) -- fp16 by default, the reference's own
 // autocast class (transformers.py:114,206; main_sampling_fid.py:216), bf16 on request -- fp32 accumulation, fp32 residual
 // stream, fp32 LayerNorm / softmax / sampler.
 //
@@ -15,11 +15,9 @@
 //     gemm_tc    fc1 partials ; act_reduce h = gelu(sum + b1)
 //     gemm_tc    fc2 partials = W2 . h
 //
-// Every launch is one all-to-all exchange between the SMs (DESIGN.md section 8: the step is bound by the latency of these
-// dependent exchanges, not by HBM).  Forms with fewer LAUNCHES but the same number of EXCHANGES -- a persistent megakernel with
-// grid barriers (round 1), split-K reduced inside the GEMM behind an arrival counter with LayerNorm folded into the weights
-// (round 2: 5 launches per block) -- were built, parity-tested and measured slower (258 and 249-256 ms against 194 ms per 64
-// images); they are not kept in the tree.
+// Every launch is one all-to-all exchange between the SMs; the step is bound by the latency of these dependent exchanges before
+// it is bound by HBM.  Forms with fewer LAUNCHES but the same number of EXCHANGES (a persistent megakernel with grid barriers,
+// split-K reduced inside the GEMM behind an arrival counter) pay the same per exchange and are not kept in the tree.
 //
 // Every kernel starts with griddepcontrol.launch_dependents and reads upstream data only after griddepcontrol.wait, so
 // the NEXT kernel's prologue -- for the GEMMs: filling the shared-memory ring with weight tiles -- overlaps this one.
@@ -64,8 +62,8 @@ static int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem
 
 // ------------------------------------------------------------------------------------------------ kernels
 // The per-block small vectors (biases, LayerNorm parameters: ~80 KB per block, read once per token) are DRAM misses -- 2.8 GB of
-// weights and the KV cache pass through L2 between two uses -- and each sits on a stage's critical path (a shared copy for all
-// blocks made the step 2 % faster, profiles/dropped_r2/shared_params_r2.txt).  LN1 of block l therefore asks L2 for block l+1's.
+// weights and the KV cache pass through L2 between two uses -- and each sits on a stage's critical path.  LN1 of block l therefore
+// asks L2 for block l+1's.
 struct PrefetchList {
     const void* p[8];
     uint32_t bytes[8];
@@ -73,8 +71,7 @@ struct PrefetchList {
 };
 
 // x_out = x_in + bias + sum_s partial[s] (+ extra row) ; xn = LayerNorm(x_out) in 16-bit.  One CTA per row.
-// (instantiated as <384, 3> only: 192-thread CTAs with two chunks per thread, padded grids and a 2-CTA-cluster form all measured
-//  equal or slower, profiles/dropped_r2/ln_grid_threads_r2.txt)
+// (instantiated as <384, 3> only)
 template <int THREADS, int NCH>
 __global__ void __launch_bounds__(THREADS)
 ln_reduce_kernel(const float* __restrict__ x_in, const float* __restrict__ partial, int S, const float* __restrict__ bias,
@@ -239,9 +236,7 @@ act_reduce_kernel(const float* __restrict__ partial, int S, const float* __restr
 // instruction (a lane-per-key row read costs 8x the L1 wavefronts); the per-key dot products are finished with a 31-shuffle
 // transpose-reduce per 32 keys, after which lane j holds the score of key j.  Up to 64 K rows / 64 V rows are in flight at once
 // and the V rows are requested before the softmax arithmetic.  T <= 512.
-// (Measured and dropped in round 2: pulling the cached rows into L2 ahead of griddepcontrol.wait -- from this kernel or from the
-// previous layer's -- changes nothing (the two 64-row phases cost 4.4 us each at T = 64 either way); reading them into registers
-// ahead of the wait is a race in the head graph, where the producer of row d-1 is a kernel of the SAME graph that a chain of
+// (The cached rows are not read into registers ahead of griddepcontrol.wait: that is a race in the head graph, where the producer of row d-1 is a kernel of the SAME graph that a chain of
 // small launches does not keep from still being in flight.)
 constexpr int AF_MAXT = 512;
 
@@ -563,7 +558,7 @@ prefill_attn_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* __re
 // 16 query rows -- S = Q K^T as 8 n-tiles x 4 k-steps of mma.sync.m16n8k16 (fp32 accumulate), scale, causal mask, row softmax in
 // registers (quad shuffles), the probabilities repacked as 16-bit A fragments (the m16n8 accumulator pair of two adjacent key tiles IS
 // the m16k16 A fragment), O = P V with V through ldmatrix.trans.  ~100 tensor instructions per warp instead of ~270 k scalar FMAs per
-// CTA.  (Not the tcgen05 path: 64 x 64 x 64 per head is two orders of magnitude below a UMMA tile's worth of work.)
+// CTA.  (Not the wgmma path: 64 x 64 x 64 per head is two orders of magnitude below a wgmma tile's worth of work.)
 template <bool BF>
 __device__ __forceinline__ void pa_mma(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     if (BF)
@@ -1154,7 +1149,7 @@ static int stack_batched(ArFast& f, const std::vector<rqb200_block_weights>& blo
     const bool save_deep = f.deep;
     if (M > 256 && !f.batched_deep) f.deep = false;
     struct Restore { ArFast& f; bool d; ~Restore() { f.deep = d; } } restore{f, save_deep};
-    // M > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, double-buffered TMEM, epilogue overlapped with the next
+    // M > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue, like the next
     // tile); M <= 256: the weight streamer
     const bool rows = M > 256 && !f.batched_streamer;
     for (size_t l = 0; l < blocks.size(); l++) {

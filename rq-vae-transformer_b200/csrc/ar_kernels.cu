@@ -1,5 +1,5 @@
 // P3 building blocks, "exact" tier: fp32 activations, fp32 FFMA accumulate, weights fp32 (bit-exact-indices gate) or
-// bf16 (storage only).  These are the correctness anchors for the tcgen05 weight-streaming kernels in
+// bf16 (storage only).  These are the correctness anchors for the wgmma weight-streaming kernels in
 // ar_gemm_tc.cu: same interfaces, same epilogues.
 //
 // Reference sites (rqvae/models/rqtransformer/attentions.py unless noted):

@@ -1,4 +1,4 @@
-// rqb200 -- shared helpers for the sm_100a kernels (error plumbing, warp/block reductions, launch counter).
+// rqb200 -- shared helpers for the sm_90a kernels (error plumbing, warp/block reductions, launch counter).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -106,7 +106,7 @@ __device__ __forceinline__ float block_max(float v, float* scratch) {
 }
 
 // 16-bit tensor-core operand storage of the fast tier.  `bf` selects the format at run time (uniform per launch): 0 = IEEE fp16
-// (the reference's autocast class, transformers.py:114,206), 1 = bf16.  Same bytes, same tcgen05 kind::f16 rate.
+// (the reference's autocast class, transformers.py:114,206), 1 = bf16.  Same bytes, same wgmma rate.
 typedef uint16_t h16;
 __device__ __forceinline__ uint32_t pack_h16x2(float a, float b, int bf) {
     if (bf) {

@@ -1,5 +1,5 @@
 // P2 building blocks, "exact" tier (fp32 FFMA): NHWC implicit-GEMM convolution, GroupNorm(32)+SiLU, single-head
-// spatial attention.  Correctness anchors for the tcgen05 implicit-GEMM path (conv_tc.cu).
+// spatial attention.  Correctness anchors for the wgmma implicit-GEMM path (conv_tc.cu).
 //
 // Reference sites (rqvae/models/rqvae/layers.py): Normalize :16-17 (GroupNorm 32 groups, eps 1e-6, affine),
 // nonlinearity :11-13 (SiLU), ResnetBlock._forward :100-120 (3x3 s1 p1 convs, 1x1 nin_shortcut, x + h),

@@ -1,4 +1,4 @@
-// P2 "fast" tier -- NHWC implicit-GEMM convolution on tcgen05 tensor cores (fp16 operands, fp32 accumulate in TMEM).
+// P2 "fast" tier -- NHWC implicit-GEMM convolution on wgmma tensor cores (fp16 operands, fp32 accumulate in registers).
 //
 // Replaces cuDNN's conv behind ResnetBlock / AttnBlock / Upsample / conv_in / conv_out of the decoder (reference:
 // rqvae/models/rqvae/layers.py:100-120,158-182,31-35; modules.py:171-202).  The reference's own GPU path runs these convs
@@ -12,9 +12,10 @@
 //       no im2col buffer, no halo logic in the kernel.
 //   N = BN output channels (16 | 128 | 256), K = taps x Cin walked in 64-channel slabs (one 128 B swizzled row per pixel).
 //
-// Persistent CTAs (grid = #SMs) loop over (pixel tile, cout tile) pairs; warp 0 = TMA producer, warp 1 = single-thread
-// tcgen05.mma issuer, warps 2-5 = epilogue.  Two TMEM accumulators (2 x BN columns) are ping-ponged so the epilogue of
-// tile i (TMEM -> registers -> +bias (+residual) -> fp32 NHWC / NCHW stores) overlaps the main loop of tile i+1.
+// Persistent CTAs (grid = #SMs) loop over (pixel tile, cout tile) pairs; warp 8 = TMA producer, warps 0-7 = two consumer
+// warpgroups, each issuing wgmma m64nBNk16 for 64 of the tile's 128 pixels and then running the epilogue (registers -> shared
+// staging -> +bias (+residual) -> fp32 NHWC / NCHW stores).  The producer runs ahead across tiles, so the next tile's operands
+// load while this tile's epilogue runs.
 #include <cstdlib>
 
 #include "kernels.h"
@@ -44,7 +45,8 @@ struct ConvTcParams {
     int gn_chunks;                 // H * W / 32
 };
 
-constexpr int CT_THREADS = 192;
+constexpr int CT_THREADS = 288;            // warps 0-7: two consumer warpgroups (64 tile rows each), warp 8: TMA producer
+constexpr int CT_CONSUMERS = 256;
 constexpr int CT_A_BYTES = 128 * 64 * 2;
 
 // PASSES == 1: single fp16 product.  PASSES == 3: split-fp16 ("fp16x3") -- both operands are carried as hi + lo fp16 pairs and
@@ -96,6 +98,112 @@ __device__ __forceinline__ void gn_chunk_stats(const float (&wv)[16], bool valid
     writer = (lane & keep_mask) == 0;
 }
 
+// Epilogue of one thread: tile row r (one output pixel), output channels [n0, n0 + 16) in v.  Warp q of the four that share a column
+// half holds the tile's pixels [32 q, 32 q + 32) -- the layout the GroupNorm partial statistics are formed over.
+__device__ __forceinline__ void ct_epilogue16(const ConvTcParams& p, const float (&v)[16], int n0, int q, int lane, int tx, int ty, int tb,
+                                              int b, int y, int x, int64_t pix, bool valid) {
+    if (n0 >= p.Cout) return;                                           // (warp-uniform)
+    if (p.out_nchw) {
+        if (!valid) return;
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            const int n = n0 + i;
+            if (n < p.Cout) p.out[(((int64_t)b * p.Cout + n) * p.H + y) * p.W + x] = v[i] + p.bias[n];
+        }
+    } else if (p.out16 != nullptr) {
+        if (!valid) return;
+        float w[16];
+#pragma unroll
+        for (int i = 0; i < 16; i += 4) {
+            const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
+            w[i] = v[i] + bb.x; w[i + 1] = v[i + 1] + bb.y; w[i + 2] = v[i + 2] + bb.z; w[i + 3] = v[i + 3] + bb.w;
+        }
+        if (p.gelu) {
+#pragma unroll
+            for (int i = 0; i < 16; i++) w[i] = 0.5f * w[i] * (1.0f + erff(w[i] * 0.70710678118654752440f));
+        }
+        uint4 pk[2];
+        uint32_t* pw = reinterpret_cast<uint32_t*>(pk);
+#pragma unroll
+        for (int i = 0; i < 8; i++) pw[i] = pack_h16x2(w[2 * i], w[2 * i + 1], p.fmt);
+        uint4* o16 = reinterpret_cast<uint4*>(reinterpret_cast<h16*>(p.out16) + pix * p.Cout + n0);
+        o16[0] = pk[0];
+        o16[1] = pk[1];
+    } else {
+        float* o = p.out + pix * p.Cout + n0;
+        const float* rs = p.residual ? p.residual + pix * p.Cout + n0 : nullptr;
+        float wv[16];
+#pragma unroll
+        for (int i = 0; i < 16; i += 4) {
+            float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
+            float4 w = make_float4(v[i] + bb.x, v[i + 1] + bb.y, v[i + 2] + bb.z, v[i + 3] + bb.w);
+            if (rs && valid) {
+                float4 rr = *reinterpret_cast<const float4*>(rs + i);
+                w.x += rr.x; w.y += rr.y; w.z += rr.z; w.w += rr.w;
+            }
+            if (valid) *reinterpret_cast<float4*>(o + i) = w;
+            wv[i] = w.x; wv[i + 1] = w.y; wv[i + 2] = w.z; wv[i + 3] = w.w;
+        }
+        if (p.gn_part != nullptr) {
+            // this warp's 32 pixels belong to one image (TW*TH >= 32, checked by the host); cg = 4 | 8 | 16 channels
+            const int cg = p.Cout >> 5;
+            const int wpi = (p.TW * p.TH) >> 5;                      // warps (32-pixel chunks) per image within a tile
+            const int chunk = (ty * p.tiles_x + tx) * wpi + (q % wpi);
+            const int bw = tb * p.NB + (q * 32) / (p.TW * p.TH);      // image of this warp
+            float tot;
+            int vidx;
+            bool writer;
+            if (cg == 4) gn_chunk_stats<4>(wv, valid, lane, tot, vidx, writer);
+            else if (cg == 8) gn_chunk_stats<8>(wv, valid, lane, tot, vidx, writer);
+            else gn_chunk_stats<16>(wv, valid, lane, tot, vidx, writer);
+            const int ngr = 16 / cg;
+            if (writer && bw < p.B)                                    // vidx < ngr: sum of group vidx; else sum of squares
+                p.gn_part[(((int64_t)bw * p.gn_chunks + chunk) * 32 + (n0 / cg + (vidx % ngr))) * 2 + (vidx / ngr)] = (double)tot;
+        }
+    }
+}
+
+// accumulator columns [C0, BN) in chunks of CW through the staging buffer; thread t <-> tile row t % 128, columns 16 (t / 128) of the chunk
+template <int BN, int CW, int C0>
+__device__ __forceinline__ void ct_drain(const ConvTcParams& p, const float (&acc)[BN / 2], float* stage, int wg, int t, int nt, int tx,
+                                         int ty, int tb, int b, int y, int x, int64_t pix, bool valid) {
+    if constexpr (C0 < BN) {
+        tc::stage_acc<BN, CW, C0>(acc, stage, wg, t);
+        tc::bar_sync(1, CT_CONSUMERS);
+        const int r = t & 127, h = t >> 7;
+        if (h * 16 < CW) {
+            float v[16];
+            const float4* src = reinterpret_cast<const float4*>(stage + r * (CW + 4) + h * 16);
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const float4 z = src[i];
+                v[4 * i] = z.x; v[4 * i + 1] = z.y; v[4 * i + 2] = z.z; v[4 * i + 3] = z.w;
+            }
+            ct_epilogue16(p, v, nt * BN + C0 + h * 16, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
+        }
+        tc::bar_sync(1, CT_CONSUMERS);
+        ct_drain<BN, CW, C0 + CW>(p, acc, stage, wg, t, nt, tx, ty, tb, b, y, x, pix, valid);
+    }
+}
+
+template <int BN, int FMT, int PASSES>
+__device__ __forceinline__ void ct_mma_kblock(float (&acc)[BN / 2], uint32_t a, uint32_t b, bool first) {
+    constexpr int B_BYTES = BN * 64 * 2;
+    if (PASSES == 3) {                              // small terms first, the dominant product last
+#pragma unroll
+        for (int j = 0; j < 4; j++)
+            tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + CT_A_BYTES + j * 32), tc::gmma_desc_k128(b + j * 32),
+                                    (!first || j > 0) ? 1u : 0u);
+#pragma unroll
+        for (int j = 0; j < 4; j++)
+            tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32), tc::gmma_desc_k128(b + B_BYTES + j * 32), 1u);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; j++)
+        tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32), tc::gmma_desc_k128(b + j * 32),
+                                (PASSES == 3 || !first || j > 0) ? 1u : 0u);
+}
+
 template <int BN, int STAGES, int PASSES>
 __global__ void __launch_bounds__(CT_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -104,14 +212,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     constexpr int NOPS = PASSES == 3 ? 2 : 1;
     constexpr int STAGE_BYTES = NOPS * (CT_A_BYTES + B_BYTES);
     constexpr int OFF_B = NOPS * CT_A_BYTES;                 // [A_hi | A_lo | B_hi | B_lo]
-    constexpr uint32_t TMEM_COLS = (2 * BN) < 32 ? 32 : 2 * BN;
+    constexpr int CW = BN < 32 ? BN : 32;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+    float* stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);        // [128][CW + 4] epilogue staging
+    uint64_t* full = reinterpret_cast<uint64_t*>(stage + 128 * (CW + 4));
     uint64_t* empty = full + STAGES;
-    uint64_t* tfull = empty + STAGES;      // [2]
-    uint64_t* tempty = tfull + 2;          // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int cslabs = p.Cin / 64;
@@ -121,21 +227,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_b;
     const int total = m_tiles * p.n_tiles_n;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tc::prefetch_tmap(&tmA);
         tc::prefetch_tmap(&tmB);
-        for (int s = 0; s < STAGES; s++) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 1); }
-        for (int s = 0; s < 2; s++) { tc::mbar_init(&tfull[s], 1); tc::mbar_init(&tempty[s], 4); }
+        // empty[s]: one arrival per consumer warp once its warpgroup's MMAs of that slot have completed
+        for (int s = 0; s < STAGES; s++) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 8); }
         tc::fence_barrier_init();
     }
-    if (warp == 1) tc::tmem_alloc(tmem_slot, TMEM_COLS);
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
+            // ---- TMA producer: runs ahead across tiles, so the next tile's operands load during this tile's epilogue
             uint32_t it = 0;                                   // running k-block counter across tiles
             for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
                 const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
@@ -157,136 +260,46 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == 1) {
-        const uint32_t idesc = tc::umma_idesc(128, BN, p.fmt);
-        uint32_t it = 0, tcount = 0;
-        for (int tile = blockIdx.x; tile < total; tile += gridDim.x, tcount++) {
-            const uint32_t as = tcount & 1;
-            tc::mbar_wait(&tempty[as], ((tcount >> 1) & 1) ^ 1);      // epilogue has drained this accumulator
-            tc::tc_fence_after();
-            for (int kb = 0; kb < nkb; kb++, it++) {
-                const int s = it % STAGES;
-                tc::mbar_wait(&full[s], (it / STAGES) & 1);
-                tc::tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t a = tc::smem_u32(smem + s * STAGE_BYTES), b = a + OFF_B;
-                    if (PASSES == 3) {                              // small terms first, the dominant product last
-#pragma unroll
-                        for (int j = 0; j < 4; j++)
-                            tc::umma_f16(tmem_base + as * BN, tc::umma_desc_k128(a + CT_A_BYTES + j * 32), tc::umma_desc_k128(b + j * 32),
-                                         idesc, (kb > 0 || j > 0) ? 1u : 0u);
-#pragma unroll
-                        for (int j = 0; j < 4; j++)
-                            tc::umma_f16(tmem_base + as * BN, tc::umma_desc_k128(a + j * 32), tc::umma_desc_k128(b + B_BYTES + j * 32),
-                                         idesc, 1u);
-                    }
-#pragma unroll
-                    for (int j = 0; j < 4; j++)
-                        tc::umma_f16(tmem_base + as * BN, tc::umma_desc_k128(a + j * 32), tc::umma_desc_k128(b + j * 32), idesc,
-                                     (PASSES == 3 || kb > 0 || j > 0) ? 1u : 0u);
-                    tc::umma_commit(&empty[s]);
-                    if (kb == nkb - 1) tc::umma_commit(&tfull[as]);
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int r = q * 32 + lane;                                   // row of the tile == TMEM lane
-        const int rx = r % p.TW, ry = (r / p.TW) % p.TH, rb = r / (p.TW * p.TH);
-        uint32_t tcount = 0;
-        for (int tile = blockIdx.x; tile < total; tile += gridDim.x, tcount++) {
-            const uint32_t as = tcount & 1;
-            const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
-            const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
-            const int x = tx * p.TW + rx, y = ty * p.TH + ry, b = tb * p.NB + rb;
-            const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
-            const bool valid = (x < p.W) && (y < p.H) && (b < p.B) && (p.m_rows == 0 || pix < p.m_rows);
-            tc::mbar_wait(&tfull[as], (tcount >> 1) & 1);
-            tc::tc_fence_after();
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 16) {
-                uint32_t v[16];
-                tc::tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + as * BN + (uint32_t)c0, v);
-                tc::tmem_ld_wait();
-                const int n0 = nt * BN + c0;
-                if (n0 >= p.Cout) continue;                                 // (warp-uniform)
-                if (p.out_nchw) {
-                    if (!valid) continue;
-#pragma unroll
-                    for (int i = 0; i < 16; i++) {
-                        const int n = n0 + i;
-                        if (n < p.Cout)
-                            p.out[(((int64_t)b * p.Cout + n) * p.H + y) * p.W + x] = __uint_as_float(v[i]) + p.bias[n];
-                    }
-                } else if (p.out16 != nullptr) {
-                    if (!valid) continue;
-                    float w[16];
-#pragma unroll
-                    for (int i = 0; i < 16; i += 4) {
-                        const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
-                        w[i] = __uint_as_float(v[i]) + bb.x; w[i + 1] = __uint_as_float(v[i + 1]) + bb.y;
-                        w[i + 2] = __uint_as_float(v[i + 2]) + bb.z; w[i + 3] = __uint_as_float(v[i + 3]) + bb.w;
-                    }
-                    if (p.gelu) {
-#pragma unroll
-                        for (int i = 0; i < 16; i++) w[i] = 0.5f * w[i] * (1.0f + erff(w[i] * 0.70710678118654752440f));
-                    }
-                    uint4 pk[2];
-                    uint32_t* pw = reinterpret_cast<uint32_t*>(pk);
-#pragma unroll
-                    for (int i = 0; i < 8; i++) pw[i] = pack_h16x2(w[2 * i], w[2 * i + 1], p.fmt);
-                    uint4* o16 = reinterpret_cast<uint4*>(reinterpret_cast<h16*>(p.out16) + pix * p.Cout + n0);
-                    o16[0] = pk[0];
-                    o16[1] = pk[1];
-                } else {
-                    float* o = p.out + pix * p.Cout + n0;
-                    const float* rs = p.residual ? p.residual + pix * p.Cout + n0 : nullptr;
-                    float wv[16];
-#pragma unroll
-                    for (int i = 0; i < 16; i += 4) {
-                        float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
-                        float4 w = make_float4(__uint_as_float(v[i]) + bb.x, __uint_as_float(v[i + 1]) + bb.y,
-                                               __uint_as_float(v[i + 2]) + bb.z, __uint_as_float(v[i + 3]) + bb.w);
-                        if (rs && valid) {
-                            float4 rr = *reinterpret_cast<const float4*>(rs + i);
-                            w.x += rr.x; w.y += rr.y; w.z += rr.z; w.w += rr.w;
-                        }
-                        if (valid) *reinterpret_cast<float4*>(o + i) = w;
-                        wv[i] = w.x; wv[i + 1] = w.y; wv[i + 2] = w.z; wv[i + 3] = w.w;
-                    }
-                    if (p.gn_part != nullptr) {
-                        // this warp's 32 pixels belong to one image (TW*TH >= 32, checked by the host); cg = 4 | 8 | 16 channels
-                        const int cg = p.Cout >> 5;
-                        const int wpi = (p.TW * p.TH) >> 5;                      // warps (32-pixel chunks) per image within a tile
-                        const int chunk = (ty * p.tiles_x + tx) * wpi + (q % wpi);
-                        const int bw = tb * p.NB + (q * 32) / (p.TW * p.TH);      // image of this warp
-                        float tot;
-                        int vidx;
-                        bool writer;
-                        if (cg == 4) gn_chunk_stats<4>(wv, valid, lane, tot, vidx, writer);
-                        else if (cg == 8) gn_chunk_stats<8>(wv, valid, lane, tot, vidx, writer);
-                        else gn_chunk_stats<16>(wv, valid, lane, tot, vidx, writer);
-                        const int ngr = 16 / cg;
-                        if (writer && bw < p.B)                                    // vidx < ngr: sum of group vidx; else sum of squares
-                            p.gn_part[(((int64_t)bw * p.gn_chunks + chunk) * 32 + (n0 / cg + (vidx % ngr))) * 2 + (vidx / ngr)] = (double)tot;
-                    }
-                }
-            }
-            tc::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(&tempty[as]);               // 4 epilogue warps -> accumulator free
-        }
+        return;
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc(tmem_base, TMEM_COLS);
+
+    // ---- consumer warpgroups 0, 1: tile rows (pixels) [64 wg, 64 wg + 64) x BN output channels; one k block in flight
+    const int wg = warp >> 2, t = threadIdx.x;
+    const int r = t & 127;                                           // epilogue: row of the tile
+    const int rx = r % p.TW, ry = (r / p.TW) % p.TH, rb = r / (p.TW * p.TH);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+        for (int kb = 0; kb < nkb; kb++, it++) {
+            const int s = it % STAGES;
+            tc::mbar_wait(&full[s], (it / STAGES) & 1);
+            const uint32_t a = tc::smem_u32(smem + s * STAGE_BYTES) + wg * (64 * 128), b = tc::smem_u32(smem + s * STAGE_BYTES + OFF_B);
+            tc::wgmma_fence();
+            if (p.fmt) ct_mma_kblock<BN, 1, PASSES>(acc, a, b, kb == 0);
+            else ct_mma_kblock<BN, 0, PASSES>(acc, a, b, kb == 0);
+            tc::wgmma_commit();
+            tc::wgmma_wait<1>();
+            if (kb > 0 && lane == 0) tc::mbar_arrive(&empty[(it - 1) % STAGES]);
+        }
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc);
+        if (lane == 0) tc::mbar_arrive(&empty[(it - 1) % STAGES]);
+
+        const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
+        const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
+        const int x = tx * p.TW + rx, y = ty * p.TH + ry, b = tb * p.NB + rb;
+        const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
+        const bool valid = (x < p.W) && (y < p.H) && (b < p.B) && (p.m_rows == 0 || pix < p.m_rows);
+        ct_drain<BN, CW, 0>(p, acc, stage, wg, t, nt, tx, ty, tb, b, y, x, pix, valid);
+    }
 }
 
 template <int BN, int STAGES, int PASSES>
 static int launch_conv_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
                             const ConvTcParams& p, int n_sm, cudaStream_t st) {
-    constexpr size_t smem = (size_t)STAGES * (PASSES == 3 ? 2 : 1) * (CT_A_BYTES + BN * 128) + 1024 + 256;
+    constexpr size_t smem = (size_t)STAGES * (PASSES == 3 ? 2 : 1) * (CT_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 256;
     static_assert(smem <= 227 * 1024, "conv_tc: shared memory budget");
     RQB_ENSURE_SMEM(smem, conv_tc_kernel<BN, STAGES, PASSES>);
     const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
@@ -301,7 +314,7 @@ static int sm_count() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
@@ -369,18 +382,14 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
 
 // Rows GEMM through the persistent conv kernel: out[m, n] = act(sum_k X[m,k] W[n,k] + bias[n]) (+ residual[m,n]) for M token rows
 // -- a 1x1 "conv" over ceil(M/128) images of 16x8 pixels.  The batched prefill / teacher-forced forward passes of the AR tier
-// (csrc/ar_fast.cu) use it for M > 256: persistent CTAs, 128 x BN tiles, double-buffered TMEM accumulators whose epilogue
-// overlaps the next tile's main loop -- what gemm_tc_kernel (a weight streamer built for M <= 256) does not have.
+// (csrc/ar_fast.cu) use it for M > 256: persistent CTAs, 128 x BN tiles, operand loads of the next tile overlapped with
+// this tile's epilogue -- what gemm_tc_kernel (a weight streamer built for M <= 256) does not have.
 // X [M_alloc, K] 16-bit with M_alloc >= ceil(M/128)*128 rows readable; exactly one of out_f32 / out_16 non-null;
 // residual (f32, may alias out_f32) only with out_f32.  N_out % 128 == 0, K % 64 == 0.
 int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                         int gelu, int fmt, int64_t M, int N_out, int K, cudaStream_t st) {
     if (N_out % 128 != 0 || K % 64 != 0 || M < 1 || (out_f32 == nullptr) == (out_16 == nullptr) || bias == nullptr)
         return fail(RQB200_EINVAL, "rows_gemm_tc: need N_out % 128 == 0, K % 64 == 0, a bias and exactly one output");
-    // 256 x 256 tiles on CTA pairs when the shape allows (RQB200_ROWS_GEMM_1CTA=1, read once: this kernel for every shape)
-    static const bool one_cta = [] { const char* e = std::getenv("RQB200_ROWS_GEMM_1CTA"); return e && e[0] == '1'; }();
-    if (!one_cta && rows_gemm2_supported(M, N_out, K))
-        return launch_rows_gemm2_tc(X16, W16, bias, residual, out_f32, out_16, gelu, fmt, M, N_out, K, st);
     ConvTcParams p = {};
     p.B = (int)ceil_div(M, 128); p.H = 8; p.W = 16; p.Cin = K; p.Cout = N_out; p.ks = 1; p.stride = 1;
     p.TW = 16; p.TH = 8; p.NB = 1;
@@ -517,14 +526,14 @@ int launch_groupnorm_f16(const float* X, const float* gamma, const float* beta, 
 int launch_cast_f16(const float* X, void* Y16, void* Y16lo, int B, int H, int W, int C, int upsample, cudaStream_t st) {
     if (C % 4 != 0) return fail(RQB200_EINVAL, "cast_f16: C % 4 != 0");
     int64_t total4 = (int64_t)B * H * W * C / 4 * (upsample ? 4 : 1);
-    int gx = (int)std::min<int64_t>(ceil_div(total4, 256), 148 * 16);
+    int gx = (int)std::min<int64_t>(ceil_div(total4, 256), sm_count() * 16);
     cast_f16_kernel<<<gx, 256, 0, st>>>(X, (__half*)Y16, (__half*)Y16lo, B, H, W, C, upsample);
     return check_launch("cast_f16");
 }
 
 }  // namespace rqb
 
-// diagnostic entry point: one conv through the tcgen05 path (tests/test_gpu_tc.py)
+// diagnostic entry point: one conv through the wgmma path (tests/test_gpu_tc.py)
 // out_nchw bit 0: NCHW output; bits 8.. : stride (0/1 -> 1, 2 -> the Downsample conv; then H, W are the OUTPUT extent)
 extern "C" int rqb200_dbg_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                                   const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,

@@ -7,7 +7,7 @@
 //   mode 2  one persistent kernel, the same data flow, stages separated by a grid-wide barrier (release/acquire counter)
 //   mode 3  one persistent kernel, the same data flow, every CTA waits only for the epoch flags of the `fan` CTAs it reads from
 //   mode 4  mode 1 with all of a thread's loads in flight before its first store (threads * 8 float4 >= 16 KB)
-// Result: microseconds per stage.  tests/test_gpu_tc.py only checks that it runs; profiles/bench_chain.py prints the table.
+// Result: microseconds per stage.  tests/test_gpu_tc.py only checks that it runs.
 #include "kernels.h"
 #include "tc_common.cuh"
 

@@ -1,8 +1,8 @@
 // Diagnostic micro-benchmark (not on any product path): how fast does ONE SM pull L2-resident data into shared memory?
 //
-// The stage trace of the cached AR step (profiles/trace_ar.py) shows a GEMM's "dependency resolved -> accumulator ready" time
-// growing by ~0.3 us per 8 KB activation box (64 rows x 128 B, SWIZZLE_128B tensor-map load): ~14 B/clk per SM.  This kernel
-// measures the candidates for that load on all SMs at once:
+// The stage trace of the cached AR step (RQB200_TRACE=1) shows a GEMM's "dependency resolved -> accumulator ready" time growing
+// with the activation boxes it loads (64 rows x 128 B, SWIZZLE_128B tensor-map load).  This kernel measures the candidates for
+// that load on all SMs at once:
 //   mode 0  cp.async.bulk.tensor.2d boxes of `rows` x 128 B out of a row-major [rows_total, row_bytes] tensor (what gemm_tc does)
 //   mode 1  cp.async.bulk (1-D) copies of rows*128 contiguous bytes (what a pre-swizzled, tile-major operand would allow)
 // Every CTA issues `depth` loads back to back into distinct shared-memory slots, waits for all of them, and repeats `iters` times.

@@ -1,13 +1,13 @@
-// P3 "fast" tier workhorse -- weight-streaming skinny GEMM on tcgen05 tensor cores.
+// P3 "fast" tier workhorse -- weight-streaming skinny GEMM on wgmma tensor cores.
 //
 //   D[n, b] = sum_k W[n, k] * X[b, k]            W: [N_out, K] (nn.Linear layout), X: [B, K], both fp16 or both bf16
-//                                                (GemmTcParams.fmt; the reference's amp class is fp16), D fp32 in TMEM
+//                                                (GemmTcParams.fmt; the reference's amp class is fp16), D fp32 in registers
 //
 // Replaces every nn.Linear of the cached AR step (reference: attentions.py:69-71,99,117-122; transformers.py:94) at
 // M = batch rows.  At B <= 256 these GEMMs are HBM-bound on the *weights* (SURVEY.md finding 5), so the kernel is laid
-// out as a weight streamer with the operands SWAPPED: the weight tile is the UMMA "A" operand (M = 128 output features
-// per CTA, K-major -- exactly the [out,in] row-major layout checkpoints already have, no transpose), the activations are
-// the "B" operand (N = batch padded to 16).  One elected thread issues tcgen05.mma (128 x BN x 16, kind::f16 -> fp32 TMEM);
+// out as a weight streamer with the operands SWAPPED: the weight tile is the wgmma "A" operand (M = 128 output features
+// per CTA, 64 per consumer warpgroup, K-major -- exactly the [out,in] row-major layout checkpoints already have, no transpose), the activations are
+// the "B" operand (N = batch padded to 16).  Two consumer warpgroups issue wgmma (m64nBNk16 each, fp32 register accumulators);
 // weights and activations arrive through TMA (SWIZZLE_128B, 64-element K slabs) into a STAGES-deep mbarrier ring.
 //
 // Programmatic dependent launch: weight tiles do not depend on the previous kernel, so the producer warp fills the ring
@@ -15,12 +15,10 @@
 // for the upstream kernel.  Back-to-back kernels of the per-token chain thereby keep HBM busy across kernel boundaries.
 //
 // Split-K (blockIdx.x = tile * splits + split) spreads the N_out/128 tiles of the narrow GEMMs (proj, fc2: 12 tiles at
-// E = 1536) over all 148 SMs; partial tiles go to an fp32 workspace [split][B][N_out] and are summed in a FIXED order by
-// the consumer kernel (ln_reduce / attn_fast / act_reduce) -> deterministic, no atomics.  (A form that reduced inside this kernel --
-// partial tiles to L2, one arrival counter per tile, each split CTA reducing its slice of the rows -- was built and measured in
-// round 2: an in-kernel barrier costs what a kernel boundary costs and GEMM-after-GEMM loses the weight prefetch; 249 vs 194 ms.)
+// E = 1536) over all 132 SMs; partial tiles go to an fp32 workspace [split][B][N_out] and are summed in a FIXED order by
+// the consumer kernel (ln_reduce / attn_fast / act_reduce) -> deterministic, no atomics.
 //
-// More activation rows than one UMMA N (256) -- batched prefill, teacher-forced forward -- run as gridDim.y row chunks of BN.
+// More activation rows than one wgmma N (256) -- batched prefill, teacher-forced forward -- run as gridDim.y row chunks of BN.
 #include "kernels.h"
 #include "tc_common.cuh"
 #include <cudaTypedefs.h>
@@ -74,50 +72,37 @@ int make_tmap_4d_nhwc(CUtensorMap* out, const void* base, uint64_t C, uint64_t W
     return 0;
 }
 
-constexpr int GT_THREADS = 192;
+constexpr int GT_THREADS = 288;             // warps 0-7: two consumer warpgroups (64 output features each), warp 8: TMA producer
+constexpr int GT_CONSUMERS = 256;
 constexpr int GT_A_BYTES = 128 * 64 * 2;     // 128 output features x 64 k, 16-bit
 
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
-template <int BN, int MODE, bool FULL>
-__device__ __forceinline__ void gt_epilogue_cols(const GemmTcParams& p, uint32_t taddr, bool nvalid, float bias, const float* res,
-                                                 int64_t res_ld, int rdiv, float* out_f, h16* out_h, int64_t ld, int m0, int nb) {
-    // issue the TMEM loads of up to 64 columns back to back, wait once
-#pragma unroll 1
-    for (int cb = 0; cb < BN; cb += 64) {
-        uint32_t r4[4][16];
+// Epilogue of one thread for 16 accumulator columns [col0, col0 + 16) = activation rows m0 + col of output feature n.
+template <int MODE, bool FULL>
+__device__ __forceinline__ void gt_epilogue_cols(const GemmTcParams& p, const float* v, bool nvalid, float bias, const float* res,
+                                                 int64_t res_ld, int rdiv, float* out_f, h16* out_h, int64_t ld, int m0, int nb,
+                                                 int col0) {
+    if (!nvalid) return;
 #pragma unroll
-        for (int c = 0; c < 4; c++)
-            if (cb + c * 16 < BN) tc::tmem_ld16(taddr + (uint32_t)(cb + c * 16), r4[c]);
-        tc::tmem_ld_wait();
-        if (nvalid) {
-#pragma unroll
-            for (int c = 0; c < 4; c++) {
-                if (cb + c * 16 < BN) {
-#pragma unroll
-                    for (int i = 0; i < 16; i++) {
-                        const int col = cb + c * 16 + i;                    // activation row m0 + col
-                        if (FULL || col < nb) {
-                            float v = __uint_as_float(r4[c][i]);
-                            if (MODE != GT_PARTIAL) v += bias;
-                            if (MODE == GT_F32 && res != nullptr)
-                                v += res[(rdiv ? (int64_t)((m0 + col) / rdiv) : (int64_t)(m0 + col)) * res_ld];
-                            if (MODE == GT_PARTIAL || MODE == GT_F32) out_f[(int64_t)col * ld] = v;
-                            else if (MODE == GT_H16) out_h[(int64_t)col * ld] = pack_h16(v, p.fmt);
-                            else out_h[(int64_t)col * ld] = pack_h16(gelu_erf_f(v), p.fmt);
-                        }
-                    }
-                }
-            }
+    for (int i = 0; i < 16; i++) {
+        const int col = col0 + i;                                    // activation row m0 + col
+        if (FULL || col < nb) {
+            float x = v[i];
+            if (MODE != GT_PARTIAL) x += bias;
+            if (MODE == GT_F32 && res != nullptr) x += res[(rdiv ? (int64_t)((m0 + col) / rdiv) : (int64_t)(m0 + col)) * res_ld];
+            if (MODE == GT_PARTIAL || MODE == GT_F32) out_f[(int64_t)col * ld] = x;
+            else if (MODE == GT_H16) out_h[(int64_t)col * ld] = pack_h16(x, p.fmt);
+            else out_h[(int64_t)col * ld] = pack_h16(gelu_erf_f(x), p.fmt);
         }
     }
 }
 
-// Epilogue of one thread: accumulator columns [0, BN) of TMEM lane `taddr` = output feature n for the activation rows
-// m0 .. m0 + nb - 1.  One warp per scheduler here, so the instruction stream is kept short and branch-free: the mode is a
-// template parameter, row addresses are base + constant * stride, and the row bound is checked only for ragged chunks.
-template <int BN, int MODE>
-__device__ __forceinline__ void gt_epilogue(const GemmTcParams& p, uint32_t taddr, int n, int split, int m0, int nb) {
+// Epilogue of one thread: output feature n, accumulator columns [col0, col0 + 16) staged in shared memory (v), for the activation rows
+// m0 .. m0 + nb - 1.  The mode is a template parameter, row addresses are base + constant * stride, and the row bound is checked
+// only for ragged chunks.
+template <int MODE>
+__device__ __forceinline__ void gt_epilogue(const GemmTcParams& p, const float* v, int n, int split, int m0, int nb, int col0) {
     const bool nvalid = n < p.N_out;
     const float bias = (MODE != GT_PARTIAL && p.bias != nullptr && nvalid) ? p.bias[n] * p.bias_scale : 0.f;
     const float* res = nullptr;
@@ -140,23 +125,58 @@ __device__ __forceinline__ void gt_epilogue(const GemmTcParams& p, uint32_t tadd
         out_h = reinterpret_cast<h16*>(p.out) + (int64_t)m0 * p.ld_out + n;
         ld = p.ld_out;
     }
-    if (nb == BN) gt_epilogue_cols<BN, MODE, true>(p, taddr, nvalid, bias, res, res_ld, rdiv, out_f, out_h, ld, m0, nb);
-    else gt_epilogue_cols<BN, MODE, false>(p, taddr, nvalid, bias, res, res_ld, rdiv, out_f, out_h, ld, m0, nb);
+    if (col0 + 16 <= nb) gt_epilogue_cols<MODE, true>(p, v, nvalid, bias, res, res_ld, rdiv, out_f, out_h, ld, m0, nb, col0);
+    else if (col0 < nb) gt_epilogue_cols<MODE, false>(p, v, nvalid, bias, res, res_ld, rdiv, out_f, out_h, ld, m0, nb, col0);
+}
+
+// accumulator columns [C0, BN) in chunks of CW: stage, then every consumer thread finishes one (feature, 16 columns) piece
+template <int BN, int CW, int C0>
+__device__ __forceinline__ void gt_drain(const GemmTcParams& p, const float (&acc)[BN / 2], float* stage, int wg, int t, int n_base,
+                                         int split, int m0, int nb) {
+    if constexpr (C0 < BN) {
+        tc::stage_acc<BN, CW, C0>(acc, stage, wg, t);
+        tc::bar_sync(1, GT_CONSUMERS);
+        const int r = t & 127, h = t >> 7;                           // feature row of the tile, which 16 of the CW columns
+        if (h * 16 < CW) {
+            float v[16];
+            const float4* src = reinterpret_cast<const float4*>(stage + r * (CW + 4) + h * 16);
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const float4 x = src[i];
+                v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
+            }
+            const int n = n_base + r, col0 = C0 + h * 16;
+            switch (p.mode) {
+                case GT_PARTIAL: gt_epilogue<GT_PARTIAL>(p, v, n, split, m0, nb, col0); break;
+                case GT_F32: gt_epilogue<GT_F32>(p, v, n, split, m0, nb, col0); break;
+                case GT_H16: gt_epilogue<GT_H16>(p, v, n, split, m0, nb, col0); break;
+                default: gt_epilogue<GT_H16_GELU>(p, v, n, split, m0, nb, col0); break;
+            }
+        }
+        tc::bar_sync(1, GT_CONSUMERS);
+        gt_drain<BN, CW, C0 + CW>(p, acc, stage, wg, t, n_base, split, m0, nb);
+    }
+}
+
+template <int BN, int FMT>
+__device__ __forceinline__ void gt_mma_kblock(float (&acc)[BN / 2], uint32_t a, uint32_t b, bool first) {
+#pragma unroll
+    for (int j = 0; j < 4; j++)
+        tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32), tc::gmma_desc_k128(b + j * 32), (!first || j > 0) ? 1u : 0u);
 }
 
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(GT_THREADS)
+__global__ void __launch_bounds__(GT_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, GemmTcParams p) {
     constexpr int B_BYTES = BN * 64 * 2;
     constexpr int STAGE_BYTES = GT_A_BYTES + B_BYTES;
-    constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
+    constexpr int CW = BN < 32 ? BN : 32;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+    float* stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);          // [128][CW + 4] epilogue staging
+    uint64_t* full = reinterpret_cast<uint64_t*>(stage + 128 * (CW + 4));
     uint64_t* xfull = full + STAGES;              // activations land on their own barrier (weights: full[])
     uint64_t* empty = xfull + STAGES;
-    uint64_t* tmem_full = empty + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
@@ -167,21 +187,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
     const bool tr = p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0;
 
     tc::pdl_launch_dependents();             // let the next kernel of the chain start its own weight prefetch
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         if (tr && !p.trace_w) p.trace[0] = tc::gtimer();
         tc::prefetch_tmap(&tmW);
         tc::prefetch_tmap(&tmX);
-        for (int s = 0; s < STAGES; s++) { tc::mbar_init(&full[s], 1); tc::mbar_init(&xfull[s], 1); tc::mbar_init(&empty[s], 1); }
-        tc::mbar_init(tmem_full, 1);
+        // empty[s]: one arrival per consumer warp once its warpgroup's MMAs of that slot have completed
+        for (int s = 0; s < STAGES; s++) { tc::mbar_init(&full[s], 1); tc::mbar_init(&xfull[s], 1); tc::mbar_init(&empty[s], 8); }
         tc::fence_barrier_init();
     }
-    if (warp == 1) tc::tmem_alloc(tmem_slot, TMEM_COLS);     // (also relinquishes the allocation permit: co-resident CTAs do not wait)
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             // ---- TMA producer.  Weights first (independent of the upstream kernel), then wait, then activations.
             const int pre = nkb < STAGES ? nkb : STAGES;
@@ -193,6 +209,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
             }
             if (p.l2pf)
                 for (int i = pre; i < nkb; i++) tc::tma_prefetch_2d(&tmW, (kb0 + i) * 64, tile * 128);
+            if (tr && p.trace_w) {
+                // diagnostic: when did the weight tiles requested ahead of the dependency land?  (replaces the entry stamp)
+                for (int i = 0; i < pre; i++) tc::mbar_wait(&full[i], 0);
+                p.trace[0] = tc::gtimer();
+            }
             tc::pdl_wait();
             if (tr) p.trace[1] = tc::gtimer();
             for (int i = 0; i < pre; i++) {
@@ -208,58 +229,42 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
                 tc::tma_load_2d(smem + s * STAGE_BYTES + GT_A_BYTES, &tmX, &xfull[s], (kb0 + i) * 64, m0, tc::L2_EVICT_LAST);
             }
         }
-    } else if (warp == 1) {
-        // ---- MMA issuer
-        // one polling lane: 31 idle lanes spinning on the same mbarrier only add shared-memory traffic next to the TMA writes
-        const uint32_t idesc = tc::umma_idesc(128, BN, p.fmt);
-        if (lane == 0) {
-            if (tr && p.trace_w) {
-                // diagnostic: when did the weight tiles requested ahead of the dependency land?  (replaces the entry stamp)
-                for (int i = 0; i < (nkb < STAGES ? nkb : STAGES); i++) tc::mbar_wait(&full[i], 0);
-                p.trace[0] = tc::gtimer();
-            }
-            for (int i = 0; i < nkb; i++) {
-                const int s = i % STAGES;
-                tc::mbar_wait(&full[s], (i / STAGES) & 1);
-                tc::mbar_wait(&xfull[s], (i / STAGES) & 1);
-                tc::tc_fence_after();
-                const uint32_t a = tc::smem_u32(smem + s * STAGE_BYTES), b = a + GT_A_BYTES;
-#pragma unroll
-                for (int j = 0; j < 4; j++)
-                    tc::umma_f16(tmem_base, tc::umma_desc_k128(a + j * 32), tc::umma_desc_k128(b + j * 32), idesc,
-                                 (i > 0 || j > 0) ? 1u : 0u);
-                tc::umma_commit(&empty[s]);                    // frees the ring slot once these MMAs have read it
-                if (i == nkb - 1) tc::umma_commit(tmem_full);  // accumulator complete
-            }
-        }
-        __syncwarp();
-    } else {
-        // ---- epilogue warps 2..5: TMEM lane quarter = warp % 4, thread <-> one output feature n, all batch columns
-        tc::pdl_wait();
-        const int q = warp & 3;
-        const int n = tile * 128 + q * 32 + lane;
-        if (lane == 0) tc::mbar_wait(tmem_full, 0);              // (one polling lane per warp)
-        __syncwarp();
-        tc::tc_fence_after();
-        if (tr && warp == 2 && lane == 0) p.trace[2] = tc::gtimer();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-        const int nb = (p.B - m0) < BN ? (p.B - m0) : BN;          // valid activation rows of this chunk
-        switch (p.mode) {
-            case GT_PARTIAL: gt_epilogue<BN, GT_PARTIAL>(p, taddr, n, split, m0, nb); break;
-            case GT_F32: gt_epilogue<BN, GT_F32>(p, taddr, n, split, m0, nb); break;
-            case GT_H16: gt_epilogue<BN, GT_H16>(p, taddr, n, split, m0, nb); break;
-            default: gt_epilogue<BN, GT_H16_GELU>(p, taddr, n, split, m0, nb); break;
-        }
-        if (tr && warp == 2 && lane == 0) p.trace[3] = tc::gtimer();
+        return;
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc(tmem_base, TMEM_COLS);
+
+    // ---- consumer warpgroups 0, 1: weight rows [64 wg, 64 wg + 64) of the tile x all BN activation columns, k in 16-wide steps.
+    //      One k block stays in flight: the slot of block i - 1 is released once block i has been issued and i - 1 has completed.
+    const int wg = warp >> 2, t = threadIdx.x;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+    for (int i = 0; i < nkb; i++) {
+        const int s = i % STAGES;
+        tc::mbar_wait(&full[s], (i / STAGES) & 1);
+        tc::mbar_wait(&xfull[s], (i / STAGES) & 1);
+        const uint32_t a = tc::smem_u32(smem + s * STAGE_BYTES) + wg * (64 * 128), b = tc::smem_u32(smem + s * STAGE_BYTES + GT_A_BYTES);
+        tc::wgmma_fence();
+        if (p.fmt) gt_mma_kblock<BN, 1>(acc, a, b, i == 0);
+        else gt_mma_kblock<BN, 0>(acc, a, b, i == 0);
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+        if (i > 0 && lane == 0) tc::mbar_arrive(&empty[(i - 1) % STAGES]);
+    }
+    tc::wgmma_wait<0>();
+    tc::acc_fence(acc);
+    if (nkb > 0 && lane == 0) tc::mbar_arrive(&empty[(nkb - 1) % STAGES]);
+
+    tc::pdl_wait();
+    if (tr && t == 0) p.trace[2] = tc::gtimer();
+    const int nb = (p.B - m0) < BN ? (p.B - m0) : BN;          // valid activation rows of this chunk
+    gt_drain<BN, CW, 0>(p, acc, stage, wg, t, tile * 128, split, m0, nb);
+    if (tr && t == 0) p.trace[3] = tc::gtimer();
 }
 
 template <int BN, int STAGES>
 static int launch_gemm_tc_t(const CUtensorMap& tmW, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl, cudaStream_t st) {
-    constexpr size_t smem = (size_t)STAGES * (GT_A_BYTES + BN * 128) + 1024 + 512;
+    constexpr size_t smem = (size_t)STAGES * (GT_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 512;
+    static_assert(smem <= 227 * 1024, "gemm_tc: shared memory budget");
     RQB_ENSURE_SMEM(smem, gemm_tc_kernel<BN, STAGES>);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(ceil_div(p.N_out, 128) * p.splits), (unsigned)ceil_div(p.B, BN));
@@ -303,7 +308,7 @@ int make_tmap_weight(CUtensorMap* out, const void* W, int N_out, int K) {
 
 }  // namespace rqb
 
-// ---- diagnostic entry points (tests/test_gpu_tc.py, bench.py's roofline leg): one GEMM through the tcgen05 kernel
+// ---- diagnostic entry points (tests/test_gpu_tc.py, bench.py's roofline leg): one GEMM through the wgmma kernel
 
 extern "C" int rqb200_dbg_gemm_tc(const void* W16, const void* X16, const float* bias, const float* residual, void* out,
                                   int out_is_16, int gelu, float* partial, int N_out, int K, int B, int splits, int fmt,

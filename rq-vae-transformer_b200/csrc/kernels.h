@@ -52,16 +52,12 @@ int launch_groupnorm_silu(const float* X, const float* gamma, const float* beta,
 int launch_vae_attn(const float* qkv, float* out, int B, int HW, int C, cudaStream_t st);
 size_t groupnorm_ws_doubles(int B, int HW);
 int launch_gn_stats(const float* X, double* stats_ws, int B, int HW, int C, cudaStream_t st);
-// conv_tc.cu -- tcgen05 implicit-GEMM conv (fast tier) and its fp16 operand producers
+// conv_tc.cu -- wgmma implicit-GEMM conv (fast tier), the large-M rows GEMM on the same kernel, and the fp16 operand producers
 bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int in_nchw);
 int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                    const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                    cudaStream_t st, int stride = 1, double* gn_part = nullptr);
 bool conv_tc_gn_fusable(int H, int W, int Cout);
-// CTA-pair form (csrc/rows_gemm2.cu: cta_group::2, 256 x 256 tiles); launch_rows_gemm_tc dispatches to it when the shape allows
-bool rows_gemm2_supported(int64_t M, int N_out, int K);
-int launch_rows_gemm2_tc(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
-                         int gelu, int fmt, int64_t M, int N_out, int K, cudaStream_t st);
 int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                         int gelu, int fmt, int64_t M, int N_out, int K, cudaStream_t st);
 int launch_groupnorm_f16(const float* X, const float* gamma, const float* beta, void* Y16, void* Y16lo, double* stats_ws, int B,
@@ -70,7 +66,7 @@ int launch_cast_f16(const float* X, void* Y16, void* Y16lo, int B, int H, int W,
 int make_tmap_4d_nhwc(CUtensorMap* out, const void* base, uint64_t C, uint64_t W, uint64_t H, uint64_t B, uint32_t box_c,
                       uint32_t box_w, uint32_t box_h, uint32_t box_b, uint32_t stride = 1);
 
-// gemm_tc.cu -- tcgen05 weight-streaming GEMM (fast tier)
+// gemm_tc.cu -- wgmma weight-streaming GEMM (fast tier)
 enum GemmTcMode { GT_F32 = 0, GT_H16 = 1, GT_H16_GELU = 2, GT_PARTIAL = 3 };
 struct GemmTcParams {
     int N_out, K, B, splits, mode;   // B = activation rows (batch rows of the cached step, or B*T tokens of a prefill / forward pass)

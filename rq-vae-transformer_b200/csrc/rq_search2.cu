@@ -1,11 +1,11 @@
-// P1, second form of the fused residual-quantisation search (RQB200_RQ_V2=1; default off until it has run on a B200).
+// P1, second form of the fused residual-quantisation search (RQB200_RQ_V2=1).
 //
-// Why: ncu on rq_quantize_kernel (profiles/ncu_rq_quantize_r1) shows the 2x4 register tile is bound by shared-memory wavefronts
-// (6 LDS.128 = 24 wavefronts per 32 FFMA instructions; FMA pipe 30 % busy).  Balance needs F >= 16 L per thread, i.e. an 8x8
+// Why: the 2x4 register tile of rq_quantize_kernel is bound by shared-memory wavefronts (6 LDS.128 = 24 wavefronts per 32 FFMA
+// instructions).  Balance needs F >= 16 L per thread, i.e. an 8x8
 // register tile (16 LDS.128 per 256 FFMA), which needs a CTA tile of 64 vectors x 256 codewords for 8 warps; the 1 KB codeword
 // rows then no longer fit the shared memory whole, so the codebook is streamed in 32-channel slabs (TMA 2-D boxes of 256 rows x
 // 128 B, SWIZZLE_128B -> conflict-free 128-bit reads) while the 64 accumulators of a thread stay live over the 8 slabs of a
-// codeword block.  64 vectors per CTA would leave N=4096 with 64 CTAs for 148 SMs, so two CTAs of a cluster share one group of
+// codeword block.  64 vectors per CTA would leave N=4096 with 64 CTAs for 132 SMs, so two CTAs of a cluster share one group of
 // vectors and split the CODEBOOK; after every depth they exchange their 64 (distance, index) candidates through distributed
 // shared memory and both apply the same residual update.
 //

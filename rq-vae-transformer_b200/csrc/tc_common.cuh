@@ -1,10 +1,12 @@
-// sm_100a primitives written as inline PTX: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld),
-// UMMA shared-memory + instruction descriptors, PDL (griddepcontrol).  Bit layouts follow the PTX ISA tcgen05
-// descriptor tables (same fields CUTLASS' cute/arch/mma_sm100_desc.hpp names).
+// sm_90a primitives written as inline PTX: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / commit / wait, shared-memory
+// matrix descriptors; the mma_async wrappers themselves are in wgmma.cuh), PDL (griddepcontrol).  Bit layouts follow the PTX
+// ISA wgmma matrix-descriptor table.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace rqb {
 namespace tc {
@@ -79,61 +81,46 @@ __device__ __forceinline__ long long gtimer() {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// ---------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {   // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-    // every kernel here allocates once: give up the permit right away so a co-resident CTA's tcgen05.alloc does not wait for it
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {     // the same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; kind::f16 covers fp16 and bf16 operands with fp32 accumulate
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread (thread i <-> TMEM lane (warp%4)*32 + i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// named barrier over the `n` threads of the consumer warpgroups (id 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // K-major operand tile in shared memory, rows of 128 B (64 x 16-bit) written by TMA with SWIZZLE_128B, 8-row groups
 // 1024 B apart: start_address[0,14) = addr>>4, LBO[16,30) unused for swizzled K-major, SBO[32,46) = 1024>>4,
-// version[46,48) = 1 (sm_100), layout_type[61,64) = 2 (SWIZZLE_128B).  Tile base must be 1024 B aligned; stepping along
+// base_offset[49,52) = 0, layout_type[62,64) = 1 (SWIZZLE_128B).  Tile base must be 1024 B aligned; stepping along
 // K inside the 128 B row = adding the byte offset to the start address (hardware applies the XOR swizzle).
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t gmma_desc_k128(uint32_t smem_addr) {
     uint64_t d = (uint64_t)((smem_addr >> 4) & 0x3FFFu);
     d |= (uint64_t)1 << 16;                    // LBO = 1 (ignored)
     d |= (uint64_t)(1024 >> 4) << 32;          // SBO
-    d |= (uint64_t)1 << 46;                    // descriptor version
-    d |= (uint64_t)2 << 61;                    // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                    // SWIZZLE_128B
     return d;
 }
-// instruction descriptor, kind::f16: c_format[4,6)=1 (F32); a_format[7,10), b_format[10,13): 0 = F16, 1 = BF16;
-// a_major[15], b_major[16] = 0 (K-major); n_dim[17,23) = N>>3; m_dim[24,29) = M>>4
-__host__ __device__ constexpr uint32_t umma_idesc(int M, int N, int ab_format) {
-    return (1u << 4) | ((uint32_t)ab_format << 7) | ((uint32_t)ab_format << 10) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
+
+// Register accumulator of one consumer warpgroup (64 rows x N columns, wgmma D fragment) -> a row-major staging buffer in shared
+// memory holding columns [c0, c0 + CW) of the 128-row tile (two warpgroups): stage[row * (CW + 4) + col - c0].  The epilogue then
+// reads it back as "one thread <-> one row, 16 consecutive columns".
+template <int N, int CW, int C0>
+__device__ __forceinline__ void stage_acc(const float (&d)[N / 2], float* stage, int wg, int t) {
+    constexpr int SP = CW + 4;
+    const int w = (t >> 5) & 3, l = t & 31;
+    const int row = wg * 64 + w * 16 + (l >> 2);
+#pragma unroll
+    for (int j = C0 / 8; j < (C0 + CW) / 8; j++) {
+        const int col = 8 * j + 2 * (l & 3) - C0;
+        *reinterpret_cast<float2*>(stage + row * SP + col) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(stage + (row + 8) * SP + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
 }
 
 }  // namespace tc

@@ -24,7 +24,7 @@ struct rqb200_vae {
     bool finalized = false;
     bool fast_ok = false;     // FAST mode and every decoder channel count is a multiple of 128
     bool split = false;       // split-fp16 (3 products per conv): "<key>.weight_lo" tensors registered
-    bool enc_fast = false;    // the encoder's convs were registered in fp16 as well: encode on the tcgen05 path
+    bool enc_fast = false;    // the encoder's convs were registered in fp16 as well: encode on the wgmma path
     bool gn_fuse = true;      // conv epilogues emit the next GroupNorm's partial statistics (mode bit RQB200_VAE_NO_GN_FUSE clears it)
     int64_t last_launches = 0;
     int64_t max_act = 0;      // max H*W*C per image over all activations
@@ -45,7 +45,7 @@ struct VaeRun {
     __half* l16[2] = {nullptr, nullptr};      // their fp16 'lo' halves (split-fp16 products); null -> single product
     bool fast = false;
 
-    // ---- fast tier helpers (tcgen05 implicit GEMM; decoder only, C % 128 == 0 everywhere)
+    // ---- fast tier helpers (wgmma implicit GEMM; decoder only, C % 128 == 0 everywhere)
     // want_stats: the output feeds a GroupNorm next -> its epilogue emits the GroupNorm partial statistics (no gn_stats pass)
     const float* stats_buf = nullptr;         // conv output whose statistics sit in gn_ws
     int stats_chunks = 0;
@@ -235,7 +235,7 @@ struct VaeRun {
         return conv("decoder.conv_out", buf[a], out, nullptr, res, res, ch, c.out_ch, 3, 1, 0, 0, 1);
     }
 
-    // fast-tier encoder: every conv but conv_in on the tcgen05 path through the decoder's building blocks, the five stride-2
+    // fast-tier encoder: every conv but conv_in on the wgmma path through the decoder's building blocks, the five stride-2
     // Downsample convs included (tensor map with element stride 2); conv_in (Cin = 3, NCHW fp32 input, 0.3 % of the encoder's
     // flops) stays on the fp32 FFMA kernel
     int encode_fast(const float* x, float* z_e) {

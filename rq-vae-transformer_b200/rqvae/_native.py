@@ -155,7 +155,7 @@ def dtype_code(t):
 
 
 def default_precision():
-    """'exact' (fp32 FFMA, bit-exact-indices gate) or 'fast' (fp16/bf16 tcgen05).  RQB200_PRECISION overrides."""
+    """'exact' (fp32 FFMA, bit-exact-indices gate) or 'fast' (fp16/bf16 wgmma).  RQB200_PRECISION overrides."""
     return os.environ.get("RQB200_PRECISION", "auto")
 
 

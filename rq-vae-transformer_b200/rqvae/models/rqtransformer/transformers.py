@@ -7,7 +7,7 @@ Boundary kept (SURVEY.md section 8b): constructor from an ``RQTransformerConfig`
 ``rqb200_ar_sample`` (csrc/ar_engine.cu): one native call per ``sample``, no per-token host work.
 
 Arithmetic tiers: ``amp=False`` -> 'exact' (fp32 weights/activations, FFMA -- the tier the bit-exact-indices gate is
-defined on); ``amp=True`` -> 'fast' (fp16 weights / activations / KV on tcgen05 tensor cores, fp32 accumulate -- the
+defined on); ``amp=True`` -> 'fast' (fp16 weights / activations / KV on wgmma tensor cores, fp32 accumulate -- the
 reference's own amp class is fp16 autocast, transformers.py:114,206; RQB200_FAST_DTYPE=bf16 selects bf16 instead).
 ``self.precision`` ('exact' | 'fast') or RQB200_PRECISION overrides the ``amp`` mapping."""
 import ctypes as C
@@ -199,7 +199,7 @@ class RQTransformer(Stage2Model):
         w.cls_ln_w, w.cls_ln_b = f32(self.classifier.layer_norm.weight), f32(self.classifier.layer_norm.bias)
         w.codebook = f32(codebook)
         if hasattr(self, "cond_classifier") and mode == N.MODE_FAST:
-            pad = -self.vocab_size_cond % 128            # classifier rows padded with zeros up to the 128-feature tcgen05 tile
+            pad = -self.vocab_size_cond % 128            # classifier rows padded with zeros up to the 128-feature wgmma tile
             pw = torch.nn.functional.pad(self.cond_classifier.linear.weight.detach(), (0, 0, 0, pad))
             pb = torch.nn.functional.pad(self.cond_classifier.linear.bias.detach(), (0, pad))
             w.w_ccls, w.b_ccls = wt(pw), f32(pb)
@@ -272,7 +272,7 @@ class RQTransformer(Stage2Model):
             fc = None if force_codes is None else force_codes.to(torch.int64).contiguous()
             bounds = [(0, B)]
             if mode == N.MODE_FAST and B > 256:
-                # the tcgen05 tier takes at most 256 batch rows per call (UMMA N <= 256): run equal chunks back to back
+                # the wgmma tier takes at most 256 batch rows per call (wgmma N <= 256): run equal chunks back to back
                 if return_logits:
                     raise N.NativeError("rqb200: return_logits with B > 256 is not supported on the fast tier")
                 n_chunks = -(-B // 256)
@@ -360,7 +360,7 @@ class RQTransformer(Stage2Model):
         """transformers.py:113-188 -- teacher-forced logits [B,H,W,D,V]; with cond_len > 1 also the cond logits
         [B,cond_len-1,vocab_cond] (the reference's return convention :185-188).
         Fast tier (amp=True): all positions at once -- the body over B*(cond_len+H*W-1) rows, the head over B*H*W*D rows, as
-        large-M tcgen05 GEMMs + causal attention (rqb200_ar_forward).  Exact tier: the sequential teacher-forced replay."""
+        large-M wgmma GEMMs + causal attention (rqb200_ar_forward).  Exact tier: the sequential teacher-forced replay."""
         B, H, W, D = xs.shape
         if self._mode(amp) == N.MODE_FAST:
             return self._native_forward(xs, model_aux, cond)

@@ -2,7 +2,7 @@
 
 Boundary kept (SURVEY.md section 8b): ``encode`` :80, ``decode`` :85, ``forward`` :74, ``get_codes`` :91, ``decode_code`` :105,
 ``get_code_emb_with_depth`` :146, ``decode_partial_code`` :150, ``get_recon_imgs`` :111, attribute ``code_shape`` and the
-state_dict key layout.  ``precision``: 'exact' = fp32 FFMA kernels, 'fast' = fp16-operand / fp32-accumulate tcgen05
+state_dict key layout.  ``precision``: 'exact' = fp32 FFMA kernels, 'fast' = fp16-operand / fp32-accumulate wgmma
 implicit GEMM (the reference's own GPU decode runs cuDNN with TF32 allowed -- same 10-bit mantissa class)."""
 import ctypes as C
 import os
@@ -93,7 +93,7 @@ class RQVAE(Stage1Model):
         if not handle:
             raise N.NativeError("rqb200_vae_create: " + L.rqb200_last_error().decode())
         wdt = torch.float16 if mode == N.MODE_FAST else torch.float32
-        # fast tier: the encoder runs on the tcgen05 conv path as well (every conv but the Cin = 3 conv_in); RQB200_ENC_FAST=0 keeps
+        # fast tier: the encoder runs on the wgmma conv path as well (every conv but the Cin = 3 conv_in); RQB200_ENC_FAST=0 keeps
         # the encoder on the fp32 kernels
         enc_fast = mode == N.MODE_FAST and os.environ.get("RQB200_ENC_FAST", "1") == "1"
         keep = {}

@@ -1,4 +1,4 @@
-"""Fast tier (fp16 -- the reference's autocast class -- or bf16 operands on tcgen05, PDL chain, CUDA graphs) of the AR step
+"""Fast tier (fp16 -- the reference's autocast class -- or bf16 operands on wgmma, PDL chain, CUDA graphs) of the AR step
 against (a) the logits the unmodified reference stored in tests/golden/ar.pt and (b) the fp32 exact tier, which is itself
 pinned bit-exactly to the reference fixtures (tests/test_gpu_parity.py).  Protocol (SURVEY.md 8c / Appendix E):
 teacher-forced step parity -- logits within a 16-bit error bound, indices identical except where the fp32 decision margin is
@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from oracle import synth
-from oracle.zoo import AR_ZOO
+from oracle.zoo import AR_FIXTURE, AR_ZOO
 from tests.helpers import CodebookAux, build_ar, noise_tensor
 
 pytestmark = pytest.mark.gpu
@@ -19,7 +19,7 @@ DEV = "cuda"
 
 
 def _case(name, golden, layouts):
-    g = golden("ar2" if name in ("cc3m654m", "cc3m654m_16", "t2i3900m") else "ar")["ar"][name]
+    g = golden(AR_FIXTURE.get(name, "ar"))["ar"][name]
     E, nh, nb_, nhl, V, bs, vc, cl = AR_ZOO[name]
     model, sd = build_ar(name, layouts, g["weight_seed"])
     cb = synth.randn_seeded((V, 256), g["codebook_seed"]).to(DEV)

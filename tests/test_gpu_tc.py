@@ -1,4 +1,4 @@
-"""tcgen05 tier, kernel level: the weight-streaming GEMM against an fp32 matmul of the same 16-bit-rounded operands."""
+"""wgmma tier, kernel level: the weight-streaming GEMM against an fp32 matmul of the same 16-bit-rounded operands."""
 import pytest
 import torch
 
@@ -51,7 +51,7 @@ def test_gemm_tc_matches_fp32_matmul(N_out, K, B, splits, fmt):
 
 @pytest.mark.parametrize("N_out,K,M", [(1536, 1536, 257), (4608, 1536, 2048), (1280, 5120, 1000), (256, 256, 4096)])
 def test_gemm_tc_large_m_row_chunks(N_out, K, M):
-    """more activation rows than one UMMA N (batched prefill / teacher-forced forward): gridDim.y chunks of 256 rows"""
+    """more activation rows than one wgmma N (batched prefill / teacher-forced forward): gridDim.y chunks of 256 rows"""
     g = torch.Generator().manual_seed(N_out + K + M)
     W = (torch.randn(N_out, K, generator=g) / K ** 0.5).half().to(DEV)
     X = torch.randn(M, K, generator=g).half().to(DEV)

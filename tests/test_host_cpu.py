@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from oracle.zoo import AR_ZOO, VAE_ZOO, vae_ddconfig
-from oracle import ref_loader
+from oracle import synth
 
 from rqvae import _native as N
 from rqvae.models import create_model
@@ -56,23 +56,22 @@ def test_vae_state_dict_layout_matches_reference(layouts, name):
     assert mine == layouts["vae/" + name]
 
 
-@pytest.mark.skipif(not ref_loader.reference_available(), reason="reference tree not present")
-def test_seeded_default_init_equals_reference():
-    """same constructor order => same RNG consumption => torch.manual_seed(0) yields the reference's weights"""
-    ns = ref_loader.load_reference()
-    E, nh, nb, nhl, V, bs, vc, cl = AR_ZOO["tiny"]
+def _assert_matches_sample(sd, ref):
+    assert sorted(sd) == sorted(ref)
+    for k, (shape, total, values) in synth.state_dict_sample(sd).items():
+        assert shape == ref[k][0], k
+        assert torch.equal(values, ref[k][2]), k
+        assert abs(total - ref[k][1]) <= 1e-9 * (1.0 + abs(ref[k][1])), k     # fp64 sums: reduction order may differ
+
+
+def test_seeded_default_init_equals_reference(golden):
+    """same constructor order => same RNG consumption => torch.manual_seed(0) yields the reference's weights (a seeded sample and
+    the exact sum of every tensor the reference initialised, tests/golden/init.pt)"""
+    ref = golden("init")
     torch.manual_seed(0)
-    ref = ns.RQTransformer(ref_loader.transformer_cfg(E, nh, nb, nhl, V, block_size=bs, vocab_cond=vc, cond_len=cl))
+    _assert_matches_sample(make_ar("tiny").state_dict(), ref["ar/tiny"])
     torch.manual_seed(0)
-    mine = make_ar("tiny")
-    for k, v in ref.state_dict().items():
-        assert torch.equal(v, mine.state_dict()[k]), k
-    torch.manual_seed(0)
-    refv = ns.RQVAE(**ref_loader.vae_kwargs(**VAE_ZOO["tiny"]))
-    torch.manual_seed(0)
-    minev = make_vae("tiny")
-    for k, v in refv.state_dict().items():
-        assert torch.equal(v, minev.state_dict()[k]), k
+    _assert_matches_sample(make_vae("tiny").state_dict(), ref["vae/tiny"])
 
 
 def test_shared_codebook_aliases_one_tensor():
