@@ -42,14 +42,7 @@ extern "C" {
 #define RQB200_AR_NO_GRAPH 1            /* launch kernel by kernel instead of replaying CUDA graphs                        */
 #define RQB200_AR_NO_PDL 2              /* plain stream order instead of programmatic dependent launch                     */
 #define RQB200_AR_TRACE 4               /* record 4 globaltimer stamps per launch (rqb200_ar_trace)                        */
-#define RQB200_AR_L2_PREFETCH 8         /* GEMMs prefetch into L2 the weight boxes that do not fit their shared-memory ring */
-#define RQB200_AR_SHALLOW_RING 16       /* half-depth GEMM rings: two GEMM CTAs of consecutive launches share an SM        */
 #define RQB200_AR_SEQUENTIAL_PREFILL 32 /* prefill the prefix token by token with the single-step graph (the prefill oracle) */
-#define RQB200_AR_BATCHED_DEEP_RING 64  /* large-M passes (prefill / forward) keep the deep ring: one CTA per SM                  */
-#define RQB200_AR_ATTN_ONE_WARP 256    /* body attention: one warp per (b, head) (round-1/2 form) instead of four               */
-#define RQB200_AR_TRACE_WEIGHTS 512    /* with TRACE: GEMM stamp 0 = prefetched weight tiles landed (instead of kernel entry)    */
-#define RQB200_AR_NO_PARAM_PREFETCH 1024 /* LN1 of block l does not prefetch block l+1's small vectors into L2                  */
-#define RQB200_AR_BATCHED_STREAMER 128  /* large-M passes through the weight-streaming GEMM instead of the persistent rows GEMM    */
 
 const char* rqb200_last_error(void);
 int rqb200_version(void);
@@ -220,29 +213,11 @@ int rqb200_dbg_conv_tc(const void* X16, const void* W16, const void* X16lo, cons
                        const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                        void* stream);
 
-/* rqb200_dbg_chain: micro-benchmark of ONE dependent stage (csrc/dbg_chain.cu), the quantity that bounds the cached AR step.
- * mode 0: PDL chain of empty kernels in a CUDA graph; 1: PDL chain, every CTA reads 16 KB written by other CTAs of the previous
- * kernel and writes 16 KB; 2: one persistent kernel, same data flow, grid-wide barrier between stages; 3: persistent, every CTA
- * waits only for the `fan` producers it reads.  Runs `reps` timed repetitions of an `n_stages` chain on its own stream and
- * returns microseconds per stage.  workspace (device): >= 2*ctas*16 KB + 4 KB + 4*ctas bytes. */
-int rqb200_dbg_chain(int mode, int n_stages, int ctas, int threads, int smem_bytes, int fan, int reps, void* workspace,
-                     size_t workspace_bytes, float* us_per_stage);
-/* rqb200_dbg_chain2: the same PDL chain with the stage's two halves separable.  variant bit 0: every CTA reads `words` floats that
- * another CTA of the previous kernel wrote (all of a thread's loads in flight); bit 1: every CTA writes `words` floats; bit 2: the
- * reads go to lines nobody writes (clean) instead.  workspace (device) >= 3 * ctas * words * 4 bytes. */
-int rqb200_dbg_chain2(int variant, int words, int n_stages, int ctas, int threads, int smem_bytes, int reps, void* workspace,
-                      size_t workspace_bytes, float* us_per_stage);
-
 /* rqb200_dbg_rows_gemm: the large-M GEMM of the batched prefill / forward passes (csrc/conv_tc.cu launch_rows_gemm_tc: persistent
  * 128 x BN tiles, wgmma): out[m,n] = act(sum_k X[m,k] W[n,k] + bias[n]) (+ residual[m,n]).  X [ceil(M/128)*128, K] and
  * W [N_out,K] 16-bit (fmt 0 fp16 / 1 bf16); exactly one of out_f32 / out_16; gelu applies to out_16 only. */
 int rqb200_dbg_rows_gemm(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                          int gelu, int fmt, int64_t M, int N_out, int K, void* stream);
-/* rqb200_dbg_tma_rate: micro-benchmark of one SM's shared-memory fill rate from L2 (csrc/dbg_tma.cu).  mode 0: tensor-map boxes
- * of `rows` x 128 B (what the GEMM kernels issue); mode 1: 1-D bulk copies of rows*128 contiguous bytes.  `depth` loads in flight,
- * `iters` rounds, every CTA cycling over the same `boxes_total` boxes of `buffer` (>= boxes_total*rows*128 bytes). */
-int rqb200_dbg_tma_rate(int mode, int rows, int depth, int iters, int boxes_total, const void* buffer, int ctas,
-                        float* bytes_per_clk, float* us_per_iter);
 
 #ifdef __cplusplus
 }

@@ -796,11 +796,11 @@ struct ArFast {
     cudaGraphExec_t graphs[G_COUNT] = {nullptr, nullptr, nullptr, nullptr};
     int64_t n_nodes[G_COUNT] = {0, 0, 0, 0};   // kernels recorded in each graph (for the launch counter)
     cudaStream_t cap_stream = nullptr;   // capture never happens on the caller's stream (it may be the legacy default stream)
-    bool use_graph = true, use_pdl = true, attn4 = true, param_prefetch = true, deep = true, l2pf = false, batched_prefill = true, batched_deep = false, batched_streamer = false;
+    bool use_graph = true, use_pdl = true, batched_prefill = true;
     int split_qkv = 4, split_proj = 12, split_fc1 = 1, split_fc2 = 12;
     int n_sm = 148;
     // diagnostic stage trace (cfg.flags & RQB200_AR_TRACE)
-    bool trace = false, trace_w = false;
+    bool trace = false;
     mutable long long* tr_base = nullptr;
     mutable int tr_next = 0;
     mutable std::vector<std::string> tr_names;
@@ -873,7 +873,7 @@ static size_t fast_layout(const ArFast& f, int B, void* base, size_t cap, FastWs
 static GemmTcParams gemm_base(const ArFast& f, int N_out, int K, int rows, int splits, int mode) {
     GemmTcParams p = {};
     p.N_out = N_out; p.K = K; p.B = rows; p.splits = splits; p.mode = mode;
-    p.fmt = f.bf; p.deep = f.deep ? 1 : 0; p.l2pf = f.l2pf ? 1 : 0; p.bias_scale = 1.f; p.ld_out = N_out;
+    p.fmt = f.bf; p.bias_scale = 1.f; p.ld_out = N_out;
     return p;
 }
 
@@ -884,7 +884,6 @@ static int gemm(const ArFast& f, const char* name, const CUtensorMap& tw, const 
     p.bias = bias; p.bias_scale = bias_scale; p.out = out; p.partial = partial;
     p.residual = residual; p.ld_res = ld_res; p.res_row_ptr = res_row_ptr; p.res_row_stride = res_row_stride;
     p.trace = tr_slot(f, name);
-    p.trace_w = f.trace_w ? 1 : 0;
     return launch_gemm_tc(tw, tx, p, f.use_pdl, st);
 }
 
@@ -904,13 +903,13 @@ static int ln(const ArFast& f, const char* name, int rows, const float* x_in, co
     }
     PrefetchList none = {};
     return launch_pdl(ln_reduce_kernel<384, 3>, dim3((unsigned)rows), dim3(384), (size_t)0, st, f.use_pdl, x_in, partial, S, bias, extra, x_out,
-                      g, be, xn, rows, E, f.bf, tr_slot(f, name), (pf && f.param_prefetch) ? *pf : none);
+                      g, be, xn, rows, E, f.bf, tr_slot(f, name), pf ? *pf : none);
 }
 
 static int attn(const ArFast& f, FastWs& ws, const float* bqkv, h16* kc, h16* vc, int Tmax, const int* t_ptr, int t_host,
                 cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
-    if (f.attn4 && Tmax >= 16 && Tmax - 1 <= AF2_MAXROWS) {          // the body stack: four warps per (b, head)
+    if (Tmax >= 16 && Tmax - 1 <= AF2_MAXROWS) {          // the body stack: four warps per (b, head)
         const int rows = (Tmax - 1 + 7) & ~7;                        // cached rows a step can read (row t is the new token); 32 B-aligned float arrays behind them
         RQB_ENSURE_SMEM(attn2_smem(AF2_MAXROWS), attn_fast2_kernel);
         {   // 11 CTAs x 19.6 KB need the largest shared-memory carve-out (L1 is not used by this kernel)
@@ -1077,14 +1076,7 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
     f->use_graph = !(cfg.flags & RQB200_AR_NO_GRAPH);
     f->use_pdl = !(cfg.flags & RQB200_AR_NO_PDL);
     f->trace = (cfg.flags & RQB200_AR_TRACE) != 0;
-    f->trace_w = (cfg.flags & RQB200_AR_TRACE_WEIGHTS) != 0;
-    f->l2pf = (cfg.flags & RQB200_AR_L2_PREFETCH) != 0;
-    f->deep = !(cfg.flags & RQB200_AR_SHALLOW_RING);
-    f->attn4 = !(cfg.flags & RQB200_AR_ATTN_ONE_WARP);
-    f->param_prefetch = !(cfg.flags & RQB200_AR_NO_PARAM_PREFETCH);
     f->batched_prefill = !(cfg.flags & RQB200_AR_SEQUENTIAL_PREFILL);
-    f->batched_deep = (cfg.flags & RQB200_AR_BATCHED_DEEP_RING) != 0;
-    f->batched_streamer = (cfg.flags & RQB200_AR_BATCHED_STREAMER) != 0;
     {
         int dev = 0, n = 0;
         cudaGetDevice(&dev);
@@ -1131,7 +1123,7 @@ struct BatchBufs {
     h16 *XN, *QKV, *ATT, *H;     // [M,E], [M,3E], [M,E], [M,4E] scratch
 };
 
-static int stack_batched(ArFast& f, const std::vector<rqb200_block_weights>& blocks, const std::vector<FastLayer>& maps,
+static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights>& blocks, const std::vector<FastLayer>& maps,
                          const BatchBufs& bb, int G, int T, h16* kc, h16* vc, int64_t kv_per_layer, int Tmax, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const int E = c.embed_dim;
@@ -1145,13 +1137,9 @@ static int stack_batched(ArFast& f, const std::vector<rqb200_block_weights>& blo
     RQB_TRY(make_tmap_2d(&tx_h, bb.H, 1, 4 * E, M, (uint64_t)E * 8, 64, bn));
     RQB_ENSURE_SMEM(prefill_attn_smem(PA_MAXT), prefill_attn_kernel);
     const float* nof = nullptr;
-    // large-M launches: half-depth rings put two CTAs on an SM, so one tile's epilogue overlaps the other's main loop
-    const bool save_deep = f.deep;
-    if (M > 256 && !f.batched_deep) f.deep = false;
-    struct Restore { ArFast& f; bool d; ~Restore() { f.deep = d; } } restore{f, save_deep};
     // M > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue, like the next
     // tile); M <= 256: the weight streamer
-    const bool rows = M > 256 && !f.batched_streamer;
+    const bool rows = M > 256;
     for (size_t l = 0; l < blocks.size(); l++) {
         const rqb200_block_weights& bw = blocks[l];
         RQB_TRY(ln(f, "", (int)M, bb.X, nof, 0, nof, nof, nullptr, bw.ln1_w, bw.ln1_b, bb.XN, st));
@@ -1334,7 +1322,7 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
         CUtensorMap tx;
         RQB_TRY(make_tmap_2d(&tx, ws.XN, 1, E, Mh, (uint64_t)E * 2, 64, gemm_tc_bn((int)std::min<int64_t>(Mh, 256))));
         RQB_TRY(ln(*f, "", (int)Mh, ws.HX, nof, 0, nof, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, st));
-        if (Mh > 256 && !f->batched_streamer) {
+        if (Mh > 256) {
             RQB_TRY(launch_rows_gemm_tc(ws.XN, w.w_cls, w.b_cls, nullptr, logits_out, nullptr, 0, f->bf, Mh, V, E, st));
         } else {
             GemmTcParams p = gemm_base(*f, V, E, (int)Mh, 1, GT_F32);

@@ -165,9 +165,14 @@ __device__ __forceinline__ void gt_mma_kblock(float (&acc)[BN / 2], uint32_t a, 
         tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32), tc::gmma_desc_k128(b + j * 32), (!first || j > 0) ? 1u : 0u);
 }
 
-template <int BN, int STAGES>
+// ring depth: the deepest ring that fits (one CTA per SM, the whole K slice of a split prefetched ahead of the upstream kernel)
+template <int BN>
+constexpr int GT_STAGES = BN <= 64 ? 8 : BN == 128 ? 6 : 4;
+
+template <int BN>
 __global__ void __launch_bounds__(GT_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, GemmTcParams p) {
+    constexpr int STAGES = GT_STAGES<BN>;
     constexpr int B_BYTES = BN * 64 * 2;
     constexpr int STAGE_BYTES = GT_A_BYTES + B_BYTES;
     constexpr int CW = BN < 32 ? BN : 32;
@@ -188,7 +193,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
 
     tc::pdl_launch_dependents();             // let the next kernel of the chain start its own weight prefetch
     if (warp == 8 && lane == 0) {
-        if (tr && !p.trace_w) p.trace[0] = tc::gtimer();
+        if (tr) p.trace[0] = tc::gtimer();
         tc::prefetch_tmap(&tmW);
         tc::prefetch_tmap(&tmX);
         // empty[s]: one arrival per consumer warp once its warpgroup's MMAs of that slot have completed
@@ -206,13 +211,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
             for (int i = 0; i < pre; i++) {
                 tc::mbar_expect_tx(&full[i], GT_A_BYTES);
                 tc::tma_load_2d(smem + i * STAGE_BYTES, &tmW, &full[i], (kb0 + i) * 64, tile * 128, w_hint);
-            }
-            if (p.l2pf)
-                for (int i = pre; i < nkb; i++) tc::tma_prefetch_2d(&tmW, (kb0 + i) * 64, tile * 128);
-            if (tr && p.trace_w) {
-                // diagnostic: when did the weight tiles requested ahead of the dependency land?  (replaces the entry stamp)
-                for (int i = 0; i < pre; i++) tc::mbar_wait(&full[i], 0);
-                p.trace[0] = tc::gtimer();
             }
             tc::pdl_wait();
             if (tr) p.trace[1] = tc::gtimer();
@@ -261,11 +259,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
     if (tr && t == 0) p.trace[3] = tc::gtimer();
 }
 
-template <int BN, int STAGES>
+template <int BN>
 static int launch_gemm_tc_t(const CUtensorMap& tmW, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl, cudaStream_t st) {
-    constexpr size_t smem = (size_t)STAGES * (GT_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 512;
+    constexpr size_t smem = (size_t)GT_STAGES<BN> * (GT_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 512;
     static_assert(smem <= 227 * 1024, "gemm_tc: shared memory budget");
-    RQB_ENSURE_SMEM(smem, gemm_tc_kernel<BN, STAGES>);
+    RQB_ENSURE_SMEM(smem, gemm_tc_kernel<BN>);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(ceil_div(p.N_out, 128) * p.splits), (unsigned)ceil_div(p.B, BN));
     cfg.blockDim = dim3(GT_THREADS);
@@ -276,13 +274,11 @@ static int launch_gemm_tc_t(const CUtensorMap& tmW, const CUtensorMap& tmX, cons
     at[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    RQB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, STAGES>, tmW, tmX, p));
+    RQB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN>, tmW, tmX, p));
     g_launches++;
     return 0;
 }
 
-// ring depth: `deep` = the deepest ring that fits (one CTA per SM, the whole K slice of a split prefetched ahead of the upstream
-// kernel); otherwise half of it, so that two CTAs of consecutive launches share an SM.  Same k order -> same bits either way.
 int launch_gemm_tc(const CUtensorMap& tmW, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl, cudaStream_t st) {
     if (p.K % 64 != 0 || p.N_out % 128 != 0) return fail(RQB200_EINVAL, "gemm_tc: need K % 64 == 0 and N_out % 128 == 0");
     if (p.B < 1) return fail(RQB200_EINVAL, "gemm_tc: no activation rows");
@@ -291,13 +287,12 @@ int launch_gemm_tc(const CUtensorMap& tmW, const CUtensorMap& tmX, const GemmTcP
     const int bn = gemm_tc_bn(p.B);
     if (p.B > 256 && p.mode == GT_PARTIAL) return fail(RQB200_EINVAL, "gemm_tc: split-K takes at most 256 activation rows");
     if (p.mode != GT_PARTIAL && p.splits != 1) return fail(RQB200_EINVAL, "gemm_tc: direct epilogues need splits == 1");
-    const bool deep = p.deep != 0;
     switch (bn) {
-        case 16: return deep ? launch_gemm_tc_t<16, 8>(tmW, tmX, p, pdl, st) : launch_gemm_tc_t<16, 4>(tmW, tmX, p, pdl, st);
-        case 32: return deep ? launch_gemm_tc_t<32, 8>(tmW, tmX, p, pdl, st) : launch_gemm_tc_t<32, 4>(tmW, tmX, p, pdl, st);
-        case 64: return deep ? launch_gemm_tc_t<64, 8>(tmW, tmX, p, pdl, st) : launch_gemm_tc_t<64, 4>(tmW, tmX, p, pdl, st);
-        case 128: return deep ? launch_gemm_tc_t<128, 6>(tmW, tmX, p, pdl, st) : launch_gemm_tc_t<128, 3>(tmW, tmX, p, pdl, st);
-        default: return deep ? launch_gemm_tc_t<256, 4>(tmW, tmX, p, pdl, st) : launch_gemm_tc_t<256, 2>(tmW, tmX, p, pdl, st);
+        case 16: return launch_gemm_tc_t<16>(tmW, tmX, p, pdl, st);
+        case 32: return launch_gemm_tc_t<32>(tmW, tmX, p, pdl, st);
+        case 64: return launch_gemm_tc_t<64>(tmW, tmX, p, pdl, st);
+        case 128: return launch_gemm_tc_t<128>(tmW, tmX, p, pdl, st);
+        default: return launch_gemm_tc_t<256>(tmW, tmX, p, pdl, st);
     }
 }
 
@@ -319,7 +314,7 @@ extern "C" int rqb200_dbg_gemm_tc(const void* W16, const void* X16, const float*
     RQB_TRY(make_tmap_weight(&tw, W16, N_out, K));
     RQB_TRY(make_tmap_2d(&tx, X16, 1, (uint64_t)K, (uint64_t)B, (uint64_t)K * 2, 64, (uint32_t)bn));
     GemmTcParams p = {};
-    p.N_out = N_out; p.K = K; p.B = B; p.splits = splits; p.fmt = fmt; p.deep = 1;
+    p.N_out = N_out; p.K = K; p.B = B; p.splits = splits; p.fmt = fmt;
     p.bias = bias; p.bias_scale = 1.f; p.residual = residual; p.ld_res = N_out; p.out = out; p.ld_out = N_out; p.partial = partial;
     p.mode = (splits > 1 || partial != nullptr) ? GT_PARTIAL : (out_is_16 ? (gelu ? GT_H16_GELU : GT_H16) : GT_F32);
     if (p.mode == GT_PARTIAL && partial == nullptr) return fail(RQB200_EINVAL, "dbg_gemm_tc: splits > 1 needs a partial buffer");

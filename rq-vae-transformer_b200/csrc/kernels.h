@@ -71,8 +71,6 @@ enum GemmTcMode { GT_F32 = 0, GT_H16 = 1, GT_H16_GELU = 2, GT_PARTIAL = 3 };
 struct GemmTcParams {
     int N_out, K, B, splits, mode;   // B = activation rows (batch rows of the cached step, or B*T tokens of a prefill / forward pass)
     int fmt;                      // 16-bit operand / output format: 0 = fp16 (the reference's autocast class), 1 = bf16
-    int deep;                     // 1: deepest shared-memory ring (one CTA per SM); 0: half depth (two CTAs of consecutive launches per SM)
-    int l2pf;                     // 1: before waiting for the upstream kernel, prefetch into L2 the weight boxes that do not fit the ring
     const float* bias;            // [N_out] (nullable); added as bias * bias_scale
     float bias_scale;
     // GT_F32 only: out = acc + bias + residual[(row0 * res_row_stride) + b * ld_res + n], row0 = res_row_ptr ? *res_row_ptr : 0
@@ -85,7 +83,6 @@ struct GemmTcParams {
     int64_t ld_out;
     float* partial;               // GT_PARTIAL: [splits][B][N_out] f32 (no bias)
     long long* trace;             // diagnostics, nullable: 4 globaltimer stamps of CTA 0 (entry, dependency resolved, accumulator ready, done)
-    int trace_w;                  // diagnostics: stamp 0 = the weight tiles requested ahead of the dependency have landed (instead of entry)
 };
 inline int gemm_tc_bn(int B) { return B <= 16 ? 16 : B <= 32 ? 32 : B <= 64 ? 64 : B <= 128 ? 128 : 256; }
 int make_tmap_weight(CUtensorMap* out, const void* W, int N_out, int K);

@@ -1,4 +1,4 @@
-// P1, second form of the fused residual-quantisation search (RQB200_RQ_V2=1).
+// P1, second form of the fused residual-quantisation search.
 //
 // Why: the 2x4 register tile of rq_quantize_kernel is bound by shared-memory wavefronts (6 LDS.128 = 24 wavefronts per 32 FFMA
 // instructions).  Balance needs F >= 16 L per thread, i.e. an 8x8

@@ -92,7 +92,7 @@ sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise
     // 16-bit lanes (8 words), the warp reduces them with shuffles, one word per thread sums the 32 warps.
     bool kth_done = false;
     if (algo == 1 && top_k > 0 && top_k < V) {
-        // ---- 2'. bucket select (RQB200_SAMPLER_V2=1): the k-th largest VALUE through one 2048-bucket histogram over the row's
+        // ---- 2'. bucket select: the k-th largest VALUE through one 2048-bucket histogram over the row's
         // [min, max] range (a monotone linear map, so bucket order == value order), a suffix scan to find the bucket that holds
         // it, and an exact ranking of that bucket's few members.  Rows with non-finite entries, a degenerate range or an
         // overfull threshold bucket take the radix select below.  Same threshold value => identical masking.

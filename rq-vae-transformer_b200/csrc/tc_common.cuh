@@ -53,11 +53,6 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
         : "memory");
 }
-// L2-only prefetch of one box (no shared-memory destination, no barrier)
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, int c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1) : "memory");
-}
 // L2-only prefetch of a contiguous global range (bytes % 16 == 0, 16 B aligned)
 __device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");

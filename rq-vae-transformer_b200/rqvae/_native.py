@@ -10,8 +10,7 @@ LIB_PATH = os.environ.get("RQB200_LIB", os.path.join(os.path.dirname(_HERE), "cs
 OK, EINVAL, ECUDA, ENODEV, EWORKSPACE, ESTATE = 0, -1, -2, -3, -4, -5
 F32, BF16, F16 = 0, 1, 2
 MODE_EXACT, MODE_FAST = 0, 1
-AR_NO_GRAPH, AR_NO_PDL, AR_TRACE, AR_L2_PREFETCH, AR_SHALLOW_RING, AR_SEQUENTIAL_PREFILL, AR_BATCHED_DEEP_RING, AR_BATCHED_STREAMER = 1, 2, 4, 8, 16, 32, 64, 128
-AR_ATTN_ONE_WARP, AR_TRACE_WEIGHTS, AR_NO_PARAM_PREFETCH = 256, 512, 1024
+AR_NO_GRAPH, AR_NO_PDL, AR_TRACE, AR_SEQUENTIAL_PREFILL = 1, 2, 4, 32
 _DT = {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16}
 
 c_f32p, c_i64p, c_vp = C.c_void_p, C.c_void_p, C.c_void_p
@@ -72,8 +71,6 @@ def lib():
                                        C.c_void_p]
     L.rqb200_dbg_rows_gemm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64,
                                        C.c_int, C.c_int, C.c_void_p]
-    L.rqb200_dbg_tma_rate.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_float),
-                                      C.POINTER(C.c_float)]
     L.rqb200_dbg_rq_quantize.argtypes = [C.c_int] + L.rqb200_rq_quantize.argtypes
     L.rqb200_dbg_sample_logits.argtypes = [C.c_int] + L.rqb200_sample_logits.argtypes
     L.rqb200_ar_create.restype = C.c_void_p
@@ -111,10 +108,6 @@ def lib():
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     L.rqb200_dbg_conv_tc.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
-    L.rqb200_dbg_chain.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
-                                   C.POINTER(C.c_float)]
-    L.rqb200_dbg_chain2.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
-                                    C.POINTER(C.c_float)]
     _lib = L
     return L
 
@@ -125,8 +118,8 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_ar_forward_workspace_bytes", "rqb200_ar_trace", "rqb200_ar_last_launches", "rqb200_vae_create",
            "rqb200_vae_destroy", "rqb200_vae_set_tensor", "rqb200_vae_finalize", "rqb200_vae_workspace_bytes",
            "rqb200_vae_decode", "rqb200_vae_decode_code", "rqb200_vae_encode", "rqb200_vae_last_launches",
-           "rqb200_dbg_gemm_tc", "rqb200_dbg_conv_tc", "rqb200_dbg_chain", "rqb200_dbg_chain2", "rqb200_dbg_rq_quantize",
-           "rqb200_dbg_sample_logits", "rqb200_dbg_tma_rate", "rqb200_dbg_rows_gemm"]
+           "rqb200_dbg_gemm_tc", "rqb200_dbg_conv_tc", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
+           "rqb200_dbg_rows_gemm"]
 
 
 def check(rc, what=""):
@@ -170,15 +163,8 @@ def ar_engine_options():
     flags = 0
     flags |= AR_NO_GRAPH if env("RQB200_NO_GRAPH", "0") == "1" else 0
     flags |= AR_NO_PDL if env("RQB200_NO_PDL", "0") == "1" else 0
-    flags |= AR_TRACE if env("RQB200_TRACE", "0") in ("1", "2") else 0
-    flags |= AR_TRACE_WEIGHTS if env("RQB200_TRACE", "0") == "2" else 0
-    flags |= AR_L2_PREFETCH if env("RQB200_GEMM_L2PF", "0") == "1" else 0
-    flags |= AR_SHALLOW_RING if env("RQB200_GEMM_SHALLOW", "0") == "1" else 0
+    flags |= AR_TRACE if env("RQB200_TRACE", "0") == "1" else 0
     flags |= AR_SEQUENTIAL_PREFILL if env("RQB200_SEQ_PREFILL", "0") == "1" else 0
-    flags |= AR_BATCHED_DEEP_RING if env("RQB200_BATCHED_DEEP", "0") == "1" else 0
-    flags |= AR_BATCHED_STREAMER if env("RQB200_BATCHED_STREAMER", "0") == "1" else 0
-    flags |= AR_ATTN_ONE_WARP if env("RQB200_ATTN_ONE_WARP", "0") == "1" else 0
-    flags |= AR_NO_PARAM_PREFETCH if env("RQB200_NO_PARAM_PREFETCH", "0") == "1" else 0
     return {"flags": flags,
             "splits": [int(env("RQB200_SPLIT_" + k, "0")) for k in ("QKV", "PROJ", "FC1", "FC2")]}
 

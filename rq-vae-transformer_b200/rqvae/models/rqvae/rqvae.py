@@ -93,9 +93,6 @@ class RQVAE(Stage1Model):
         if not handle:
             raise N.NativeError("rqb200_vae_create: " + L.rqb200_last_error().decode())
         wdt = torch.float16 if mode == N.MODE_FAST else torch.float32
-        # fast tier: the encoder runs on the wgmma conv path as well (every conv but the Cin = 3 conv_in); RQB200_ENC_FAST=0 keeps
-        # the encoder on the fp32 kernels
-        enc_fast = mode == N.MODE_FAST and os.environ.get("RQB200_ENC_FAST", "1") == "1"
         keep = {}
 
         def reg(name, t):
@@ -106,16 +103,14 @@ class RQVAE(Stage1Model):
         def reg_conv(name, w_oihw):
             """conv weight OIHW -> OHWI in the engine's dtype; fast tier: fp16 hi + lo halves (split-fp16 products)"""
             w = w_oihw.detach().permute(0, 2, 3, 1).contiguous().float()
-            fast16 = name.startswith(("decoder.", "post_quant_conv"))
-            if enc_fast and name.startswith(("encoder.", "quant_conv")) and not name.startswith("encoder.conv_in"):
-                fast16 = True
-            if mode == N.MODE_FAST and fast16:
+            # fast tier: every conv but the encoder's Cin = 3 conv_in runs on the wgmma conv path
+            if mode == N.MODE_FAST and not name.startswith("encoder.conv_in"):
                 hi = w.to(torch.float16)
                 reg(name, hi)
                 if self.split_fp16:
                     reg(name + "_lo", (w - hi.float()).to(torch.float16))
             else:
-                reg(name, w)          # exact tier, and the encoder in every tier (fp32 FFMA kernels)
+                reg(name, w)          # exact tier, and the encoder's conv_in in every tier (fp32 FFMA kernels)
 
         sd = {k: v for k, v in self.state_dict().items()}
         for k, v in sd.items():

@@ -117,12 +117,13 @@ def test_c_abi_library_exports_every_declared_symbol():
     assert N.lib().rqb200_version() >= 100
 
 
-def test_engine_flag_constants_match_the_header():
-    """the binding's AR_* flag values are the header's RQB200_AR_* defines (one bit each, no overlap)"""
+def test_engine_flag_set_and_values_match_the_header():
+    """the header defines exactly the four RQB200_AR_* flags, and the binding's AR_* values are those defines (one bit each,
+    no overlap)"""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     hdr = open(os.path.join(root, "include", "rqb200.h")).read()
     flags = {n: int(v) for n, v in re.findall(r"#define\s+RQB200_(AR_[A-Z0-9_]+)\s+(\d+)", hdr)}
-    assert len(flags) >= 8
+    assert set(flags) == {"AR_NO_GRAPH", "AR_NO_PDL", "AR_TRACE", "AR_SEQUENTIAL_PREFILL"}
     for name, value in flags.items():
         assert value & (value - 1) == 0, name
         assert getattr(N, name) == value, name
