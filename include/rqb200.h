@@ -112,6 +112,9 @@ typedef struct rqb200_ar_weights {
 
 typedef struct rqb200_ar rqb200_ar;
 
+/* Both tiers: embed_dim == 64 * n_head, n_head_layers >= 0 (0: a head-less model, each depth's token goes straight to the
+ * classifier).  Fast tier (RQB200_MODE_FAST) also: cond_len + H*W <= 2048 (a 32x32 grid behind up to 1024 prefix tokens),
+ * n_body >= 1, E % 128 == 0, V % 128 == 0, code_dim % 64 == 0, D <= 8, E <= 4608.  NULL on failure (rqb200_last_error). */
 rqb200_ar* rqb200_ar_create(const rqb200_ar_config* cfg, const rqb200_ar_weights* w);
 void rqb200_ar_destroy(rqb200_ar* h);
 size_t rqb200_ar_workspace_bytes(const rqb200_ar* h, int B);

@@ -235,10 +235,11 @@ act_reduce_kernel(const float* __restrict__ partial, int S, const float* __restr
 // lane <-> dims (2*lane, 2*lane+1) for q/k/v/out everywhere: every cache row is read as ONE coalesced 128 B line per warp
 // instruction (a lane-per-key row read costs 8x the L1 wavefronts); the per-key dot products are finished with a 31-shuffle
 // transpose-reduce per 32 keys, after which lane j holds the score of key j.  Up to 64 K rows / 64 V rows are in flight at once
-// and the V rows are requested before the softmax arithmetic.  T <= 512.
+// and the V rows are requested before the softmax arithmetic.  T <= FAST_MAXT: the scores take 16 * T B of dynamic shared memory
+// (32 KB at 2048, under the 48 KB default).
 // (The cached rows are not read into registers ahead of griddepcontrol.wait: that is a race in the head graph, where the producer of row d-1 is a kernel of the SAME graph that a chain of
 // small launches does not keep from still being in flight.)
-constexpr int AF_MAXT = 512;
+constexpr int FAST_MAXT = 2048;          // the fast tier's longest body sequence, cond_len + H*W (a 32x32 grid behind a 1024-token prefix)
 
 // pv[u] = this lane's partial dot product for key u (u < 32); returns the full dot product of key `lane`
 __device__ __forceinline__ float af_transpose_reduce(float (&pv)[32], int lane) {
@@ -487,6 +488,7 @@ attn_fast2_kernel(const float* __restrict__ part, int S, const float* __restrict
 // single-step buffers).  One CTA per (group, head); the group's K and V rows are staged in shared memory (row stride 66 elements:
 // conflict-free for lane <-> key), warp <-> query, lane <-> key for the scores and lane <-> 2 dims for the output -- the same
 // arithmetic order as attn_fast_kernel's.  When kc != NULL the K / V rows are also written to the cache [g][head][t][64].
+// T <= PA_MAXT (~280 B of shared memory per token); longer prefixes run prefill_attn_flash_kernel.
 constexpr int PA_MAXT = 512;
 static size_t prefill_attn_smem(int T) { return ((size_t)2 * T * 33 + 4 * 64 + (size_t)4 * T) * 4; }
 __global__ void __launch_bounds__(128)
@@ -656,6 +658,141 @@ prefill_attn_mma_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* 
             pa_mma<BF>(oacc[2 * jp + 1], pa[kk], b[2], b[3]);
         }
     }
+    const float i0 = 1.0f / s0, i1 = 1.0f / s1;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const int d = 8 * j + (lane & 3) * 2;
+        if (r0 < T) *reinterpret_cast<uint32_t*>(att + ((int64_t)r0 * G + g) * E + h * 64 + d) = pack_h16x2(oacc[j][0] * i0, oacc[j][1] * i0, BF ? 1 : 0);
+        if (r1 < T) *reinterpret_cast<uint32_t*>(att + ((int64_t)r1 * G + g) * E + h * 64 + d) = pack_h16x2(oacc[j][2] * i1, oacc[j][3] * i1, BF ? 1 : 0);
+    }
+}
+
+// The same causal attention for prefixes longer than 512 tokens (the 32x32 grids: T up to cond_len + 1023), where a whole prefix no
+// longer fits in shared memory: prefill_attn_mma_kernel's mma.sync arithmetic tiled flash-attention style.  One CTA per (query tile
+// of 64 rows, group, head), query tiles launched heaviest (last) first; each of the four warps owns 16 query rows.  K / V are read
+// in 64-key tiles double-buffered through cp.async (the 144 B rows of the ldmatrix path); per tile S = Q K^T on mma.sync (fp32
+// accumulate), the causal mask on the diagonal tile only, an online softmax (running row max and sum in fp32, O rescaled between
+// tiles), P repacked as A fragments and O += P V through ldmatrix.trans.  Key tiles are visited in a fixed order: run-to-run
+// deterministic.  When kc != NULL the CTA of query tile i writes the cache rows of tile i (every row exactly once).
+template <bool BF>
+__global__ void __launch_bounds__(128)
+prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* __restrict__ vc, h16* __restrict__ att, int G, int T, int E,
+                          int nh, int Tmax) {
+    __shared__ __align__(16) uint8_t sm[5 * 64 * PM_ROW];         // Q | K[2] | V[2]
+    uint8_t* Qs = sm;
+    tc::pdl_launch_dependents();
+    tc::pdl_wait();
+    const int n_pairs = G * nh;
+    const int qt = (T + 63) / 64 - 1 - (int)(blockIdx.x / n_pairs);  // heaviest query tile first
+    const int pair = (int)(blockIdx.x % n_pairs);
+    const int g = pair / nh, h = pair % nh;
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    // tile `kt` of matrix `mat` (0 Q, 1 K, 2 V) -> dst; rows beyond T are zeros (their scores are masked, but P V must not see NaN)
+    auto load_tile = [&](int mat, int kt, uint8_t* dst) {
+        for (int i = threadIdx.x; i < 64 * 8; i += 128) {
+            const int r = i >> 3, c = i & 7, t = kt * 64 + r;
+            uint8_t* d = dst + r * PM_ROW + c * 16;
+            if (t < T)
+                cp_async16(tc::smem_u32(d), qkv + ((int64_t)t * G + g) * 3 * E + mat * E + h * 64 + c * 8);
+            else
+                *reinterpret_cast<uint4*>(d) = make_uint4(0u, 0u, 0u, 0u);
+        }
+    };
+    load_tile(0, qt, Qs);
+    load_tile(1, 0, sm + 64 * PM_ROW);
+    load_tile(2, 0, sm + 3 * 64 * PM_ROW);
+    asm volatile("cp.async.commit_group;" ::: "memory");
+    if (kc != nullptr) {                                  // this query tile's K / V rows -> the cache
+        for (int i = threadIdx.x; i < 2 * 64 * 8; i += 128) {
+            const int mat = 1 + (i >> 9), r = (i >> 3) & 63, c = i & 7, t = qt * 64 + r;
+            if (t < T)
+                *reinterpret_cast<uint4*>((mat == 1 ? kc : vc) + (((int64_t)g * nh + h) * Tmax + t) * 64 + c * 8) =
+                    *reinterpret_cast<const uint4*>(qkv + ((int64_t)t * G + g) * 3 * E + mat * E + h * 64 + c * 8);
+        }
+    }
+    const int r0 = qt * 64 + 16 * w + (lane >> 2), r1 = r0 + 8;
+    uint32_t qa[4][4];
+    float oacc[8][4];
+#pragma unroll
+    for (int j = 0; j < 8; j++) { oacc[j][0] = oacc[j][1] = oacc[j][2] = oacc[j][3] = 0.f; }
+    float m0 = -INFINITY, m1 = -INFINITY, s0 = 0.f, s1 = 0.f;      // running max; this lane's share of the running sum
+    for (int kt = 0; kt <= qt; kt++) {
+        if (kt < qt) {                                    // prefetch the next key tile into the other buffer
+            load_tile(1, kt + 1, sm + (1 + ((kt + 1) & 1)) * 64 * PM_ROW);
+            load_tile(2, kt + 1, sm + (3 + ((kt + 1) & 1)) * 64 * PM_ROW);
+            asm volatile("cp.async.commit_group;" ::: "memory");
+            asm volatile("cp.async.wait_group 1;" ::: "memory");
+        } else {
+            asm volatile("cp.async.wait_group 0;" ::: "memory");
+        }
+        __syncthreads();
+        const uint32_t ks = tc::smem_u32(sm + (1 + (kt & 1)) * 64 * PM_ROW), vs = tc::smem_u32(sm + (3 + (kt & 1)) * 64 * PM_ROW);
+        if (kt == 0) {
+#pragma unroll
+            for (int kk = 0; kk < 4; kk++)
+                pa_ldsm4(qa[kk], tc::smem_u32(Qs) + (uint32_t)((16 * w + (lane & 15)) * PM_ROW + kk * 32 + (lane >> 4) * 16));
+        }
+        // ---- S = Q K^T for this warp's 16 query rows x 64 keys
+        float sacc[8][4];
+#pragma unroll
+        for (int j = 0; j < 8; j++) { sacc[j][0] = sacc[j][1] = sacc[j][2] = sacc[j][3] = 0.f; }
+#pragma unroll
+        for (int kk = 0; kk < 4; kk++) {
+#pragma unroll
+            for (int jp = 0; jp < 4; jp++) {
+                uint32_t b[4];
+                pa_ldsm4(b, ks + (uint32_t)((16 * jp + (lane & 7) + ((lane >> 4) << 3)) * PM_ROW + kk * 32 + ((lane >> 3) & 1) * 16));
+                pa_mma<BF>(sacc[2 * jp], qa[kk], b[0], b[1]);
+                pa_mma<BF>(sacc[2 * jp + 1], qa[kk], b[2], b[3]);
+            }
+        }
+        // ---- scale (+ causal mask on the diagonal tile), new row maxima
+        const bool diag = kt == qt;
+        float t0 = m0, t1 = m1;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const int c0 = kt * 64 + 8 * j + (lane & 3) * 2;
+            sacc[j][0] = (!diag || c0 <= r0) ? sacc[j][0] * 0.125f : -INFINITY;
+            sacc[j][1] = (!diag || c0 + 1 <= r0) ? sacc[j][1] * 0.125f : -INFINITY;
+            sacc[j][2] = (!diag || c0 <= r1) ? sacc[j][2] * 0.125f : -INFINITY;
+            sacc[j][3] = (!diag || c0 + 1 <= r1) ? sacc[j][3] * 0.125f : -INFINITY;
+            t0 = fmaxf(t0, fmaxf(sacc[j][0], sacc[j][1]));
+            t1 = fmaxf(t1, fmaxf(sacc[j][2], sacc[j][3]));
+        }
+        t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 1)); t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 2));
+        t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 1)); t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 2));
+        // (every row sees at least one unmasked key in every tile it visits: t0 / t1 are finite, alpha of the first tile is 0)
+        const float a0 = __expf(m0 - t0), a1 = __expf(m1 - t1);
+        m0 = t0;
+        m1 = t1;
+        s0 *= a0;
+        s1 *= a1;
+#pragma unroll
+        for (int j = 0; j < 8; j++) { oacc[j][0] *= a0; oacc[j][1] *= a0; oacc[j][2] *= a1; oacc[j][3] *= a1; }
+        uint32_t pa[4][4];
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const float e0 = __expf(sacc[j][0] - m0), e1 = __expf(sacc[j][1] - m0), e2 = __expf(sacc[j][2] - m1), e3 = __expf(sacc[j][3] - m1);
+            s0 += e0 + e1;
+            s1 += e2 + e3;
+            pa[j >> 1][(j & 1) * 2] = pack_h16x2(e0, e1, BF ? 1 : 0);
+            pa[j >> 1][(j & 1) * 2 + 1] = pack_h16x2(e2, e3, BF ? 1 : 0);
+        }
+        // ---- O += P V
+#pragma unroll
+        for (int kk = 0; kk < 4; kk++) {
+#pragma unroll
+            for (int jp = 0; jp < 4; jp++) {
+                uint32_t b[4];
+                pa_ldsm4_t(b, vs + (uint32_t)((16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8) * PM_ROW + (2 * jp + (lane >> 4)) * 16));
+                pa_mma<BF>(oacc[2 * jp], pa[kk], b[0], b[1]);
+                pa_mma<BF>(oacc[2 * jp + 1], pa[kk], b[2], b[3]);
+            }
+        }
+        __syncthreads();                                  // (this buffer is refilled by the next iteration's prefetch)
+    }
+    s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
     const float i0 = 1.0f / s0, i1 = 1.0f / s1;
 #pragma unroll
     for (int j = 0; j < 8; j++) {
@@ -835,7 +972,7 @@ static long long* tr_slot(const ArFast& f, const char* name) {
     return f.tr_base + 4 * (int64_t)(f.tr_next++);
 }
 
-static int prefill_tmax(const rqb200_ar_config& c) { return std::min(PA_MAXT, c.cond_len + c.H * c.W - 1); }
+static int prefill_tmax(const rqb200_ar_config& c) { return c.cond_len + c.H * c.W - 1; }
 
 static size_t fast_layout(const ArFast& f, int B, void* base, size_t cap, FastWs* ws) {
     const rqb200_ar_config& c = f.cfg;
@@ -976,8 +1113,12 @@ static int fast_stack(const ArFast& f, const std::vector<rqb200_block_weights>& 
         RQB_TRY(gemm(f, "fc2", maps[l].fc2, f.tx_h, E, 4 * E, B, f.split_fc2, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0,
                      st));
     }
-    // fold the last block's pending fc2 reduction into x (x is final on return) -- and the caller's LayerNorm, if any
-    RQB_TRY(ln(f, "finalize", B, x, ws.P, f.split_fc2, blocks.back().b2, nof, x, fin_g, fin_b, fin_g ? ws.XN : nullptr, st));
+    // fold the last block's pending fc2 reduction into x (x is final on return) -- and the caller's LayerNorm, if any.  An empty
+    // stack (a head-less model) only forms its input token x = x_src + pending_extra.
+    if (blocks.empty())
+        RQB_TRY(ln(f, "finalize", B, x_src, nof, 0, nof, pending_extra, x, fin_g, fin_b, fin_g ? ws.XN : nullptr, st));
+    else
+        RQB_TRY(ln(f, "finalize", B, x, ws.P, f.split_fc2, blocks.back().b2, nof, x, fin_g, fin_b, fin_g ? ws.XN : nullptr, st));
     return 0;
 }
 
@@ -1066,8 +1207,12 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
                        const rqb200_block_weights* head_p) {
     std::vector<rqb200_block_weights> body(body_p, body_p + cfg.n_body), head(head_p, head_p + cfg.n_head_layers);
     const int E = cfg.embed_dim;
-    if (E % 128 != 0 || cfg.vocab % 128 != 0 || cfg.code_dim % 64 != 0 || cfg.D > 8 || cfg.cond_len + cfg.H * cfg.W > AF_MAXT || E > 4608) {
-        set_error("ar fast tier: need E % 128 == 0, V % 128 == 0, code_dim % 64 == 0, D <= 8, cond_len + H*W <= 512, E <= 4608");
+    if (E % 128 != 0 || cfg.vocab % 128 != 0 || cfg.code_dim % 64 != 0 || cfg.D > 8 || cfg.cond_len + cfg.H * cfg.W > FAST_MAXT || E > 4608) {
+        set_error("ar fast tier: need E % 128 == 0, V % 128 == 0, code_dim % 64 == 0, D <= 8, cond_len + H*W <= 2048, E <= 4608");
+        return nullptr;
+    }
+    if (cfg.n_body < 1) {
+        set_error("ar fast tier: need at least one body layer (n_body >= 1)");
         return nullptr;
     }
     ArFast* f = new ArFast();
@@ -1128,7 +1273,7 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
     const rqb200_ar_config& c = f.cfg;
     const int E = c.embed_dim;
     const int64_t M = (int64_t)G * T;
-    if (M > (int64_t)1 << 30 || T > PA_MAXT) return fail(RQB200_EINVAL, "ar fast tier: batched pass too large");
+    if (M > (int64_t)1 << 30 || T > FAST_MAXT) return fail(RQB200_EINVAL, "ar fast tier: batched pass too large");
     const bool pdl = true;               // the pass is a PDL chain too: a launch's set-up overlaps its predecessor's tail
     CUtensorMap tx_xn, tx_att, tx_h;
     const int bn = gemm_tc_bn((int)std::min<int64_t>(M, 256));
@@ -1166,9 +1311,18 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
                 RQB_TRY(launch_pdl(prefill_attn_mma_kernel<false>, dim3((unsigned)(G * c.n_head)), dim3(128), (size_t)0, st, pdl,
                                    (const h16*)bb.QKV, kcl, vcl, bb.ATT, G, T, E, c.n_head, Tmax));
             }
-        } else {
+        } else if (T <= PA_MAXT) {
             RQB_TRY(launch_pdl(prefill_attn_kernel, dim3((unsigned)(G * c.n_head)), dim3(128), prefill_attn_smem(T), st, pdl,
                                (const h16*)bb.QKV, kcl, vcl, bb.ATT, G, T, E, c.n_head, Tmax, f.bf));
+        } else {                                          // longer than the shared-memory prefix: 64-key tiles, online softmax
+            const dim3 grid((unsigned)((int64_t)ceil_div(T, 64) * G * c.n_head));
+            if (f.bf) {
+                RQB_TRY(launch_pdl(prefill_attn_flash_kernel<true>, grid, dim3(128), (size_t)0, st, pdl, (const h16*)bb.QKV, kcl, vcl, bb.ATT,
+                                   G, T, E, c.n_head, Tmax));
+            } else {
+                RQB_TRY(launch_pdl(prefill_attn_flash_kernel<false>, grid, dim3(128), (size_t)0, st, pdl, (const h16*)bb.QKV, kcl, vcl, bb.ATT,
+                                   G, T, E, c.n_head, Tmax));
+            }
         }
         if (rows) {
             RQB_TRY(launch_rows_gemm_tc(bb.ATT, bw.wproj, bw.bproj, bb.X, bb.X, nullptr, 0, f.bf, M, E, E, st));
@@ -1226,7 +1380,7 @@ static int prefill_batched(ArFast& f, FastWs& ws, int T, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const int E = c.embed_dim, B = f.B, HW = c.H * c.W, cl = c.cond_len, Tb = cl + HW;
     const int64_t M = (int64_t)B * T;
-    if (M > ws.Mmax || T > PA_MAXT) return fail(RQB200_EINVAL, "ar fast tier: prefix too long for the batched prefill");
+    if (M > ws.Mmax) return fail(RQB200_EINVAL, "ar fast tier: prefix too long for the batched prefill");
     const bool save_pdl = f.use_pdl, save_tr = f.trace;
     f.use_pdl = false;
     f.trace = false;
@@ -1278,7 +1432,6 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
     const rqb200_ar_weights& w = f->w;
     const int E = c.embed_dim, D = c.D, HW = c.H * c.W, cl = c.cond_len, V = c.vocab, Tb = cl + HW - 1;
     if (B < 1) return fail(RQB200_EINVAL, "ar_forward: B must be > 0");
-    if (Tb > PA_MAXT) return fail(RQB200_EINVAL, "ar_forward: sequence too long for the batched attention kernel");
     if (cond_logits_out && (cl < 2 || !w.w_ccls)) return fail(RQB200_EINVAL, "ar_forward: cond logits need cond_len > 1 and a cond classifier");
     FwdWs ws;
     if (forward_layout(*f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_forward: workspace too small");
@@ -1378,7 +1531,7 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
     if (!resume) {
         // prefill: cond tokens, then (start_loc resume) the code tokens of positions < idx_begin  (transformers.py:237-239)
         const int T0 = cl + idx_begin;
-        if (f->batched_prefill && T0 >= 4 && T0 <= PA_MAXT && (int64_t)B * T0 <= ws.Mmax) {
+        if (f->batched_prefill && T0 >= 4 && (int64_t)B * T0 <= ws.Mmax) {
             RQB_TRY(prefill_batched(*f, ws, T0, st));
             // state.idx must equal idx_begin for the first head graph
             if (idx_begin > 0) RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, idx_begin, 0));
