@@ -483,84 +483,7 @@ attn_fast2_kernel(const float* __restrict__ part, int S, const float* __restrict
     if (tr != nullptr && blockIdx.x == 0 && threadIdx.x == 0) tr[3] = tc::gtimer();
 }
 
-// Causal attention over a whole prefix in one launch (batched prefill / teacher-forced forward).  qkv [M, 3E] 16-bit (bias already
-// added by the GEMM epilogue), row of (group g, token t) = t * G + g  (token-major: the rows of one token are contiguous, like the
-// single-step buffers).  One CTA per (group, head); the group's K and V rows are staged in shared memory (row stride 66 elements:
-// conflict-free for lane <-> key), warp <-> query, lane <-> key for the scores and lane <-> 2 dims for the output -- the same
-// arithmetic order as attn_fast_kernel's.  When kc != NULL the K / V rows are also written to the cache [g][head][t][64].
-// T <= PA_MAXT (~280 B of shared memory per token); longer prefixes run prefill_attn_flash_kernel.
-constexpr int PA_MAXT = 512;
-static size_t prefill_attn_smem(int T) { return ((size_t)2 * T * 33 + 4 * 64 + (size_t)4 * T) * 4; }
-__global__ void __launch_bounds__(128)
-prefill_attn_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* __restrict__ vc, h16* __restrict__ att, int G, int T, int E,
-                    int nh, int Tmax, int bf) {
-    extern __shared__ uint32_t pa_smem[];
-    uint32_t (*ks)[33] = reinterpret_cast<uint32_t (*)[33]>(pa_smem);
-    uint32_t (*vs)[33] = reinterpret_cast<uint32_t (*)[33]>(pa_smem + (size_t)T * 33);
-    float (*qs)[64] = reinterpret_cast<float (*)[64]>(pa_smem + (size_t)2 * T * 33);
-    float* ps_all = reinterpret_cast<float*>(pa_smem + (size_t)2 * T * 33 + 4 * 64);
-    tc::pdl_launch_dependents();
-    tc::pdl_wait();
-    const int g = blockIdx.x / nh, h = blockIdx.x % nh;
-    const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
-    float* ps = ps_all + (size_t)wq * T;
-    for (int i = threadIdx.x; i < T * 32; i += 128) {
-        const int t = i >> 5, c2 = i & 31;
-        const h16* row = qkv + ((int64_t)t * G + g) * 3 * E + h * 64 + 2 * c2;
-        const uint32_t kk = *reinterpret_cast<const uint32_t*>(row + E), vv = *reinterpret_cast<const uint32_t*>(row + 2 * E);
-        ks[t][c2] = kk;
-        vs[t][c2] = vv;
-        if (kc) {
-            *reinterpret_cast<uint32_t*>(kc + (((int64_t)g * nh + h) * Tmax + t) * 64 + 2 * c2) = kk;
-            *reinterpret_cast<uint32_t*>(vc + (((int64_t)g * nh + h) * Tmax + t) * 64 + 2 * c2) = vv;
-        }
-    }
-    __syncthreads();
-    for (int t = wq; t < T; t += 4) {
-        const float2 qf = unpack_h16x2(*reinterpret_cast<const uint32_t*>(qkv + ((int64_t)t * G + g) * 3 * E + h * 64 + 2 * lane), bf);
-        __syncwarp();
-        qs[wq][2 * lane] = qf.x;
-        qs[wq][2 * lane + 1] = qf.y;
-        __syncwarp();
-        float m = -INFINITY;
-        for (int j = lane; j <= t; j += 32) {
-            float acc = 0.f;
-#pragma unroll
-            for (int u = 0; u < 32; u++) {
-                const float2 kk = unpack_h16x2(ks[j][u], bf);
-                acc = fmaf(qs[wq][2 * u], kk.x, acc);
-                acc = fmaf(qs[wq][2 * u + 1], kk.y, acc);
-            }
-            acc *= 0.125f;
-            ps[j] = acc;
-            m = fmaxf(m, acc);
-        }
-        m = warp_max(m);
-        float sum = 0.f;
-        for (int j = lane; j <= t; j += 32) {
-            const float e = __expf(ps[j] - m);
-            ps[j] = e;
-            sum += e;
-        }
-        sum = warp_sum(sum);
-        __syncwarp();
-        float2 o = make_float2(0.f, 0.f);
-        for (int j = 0; j <= t; j++) {
-            const float2 vv = unpack_h16x2(vs[j][lane], bf);
-            o.x = fmaf(ps[j], vv.x, o.x);
-            o.y = fmaf(ps[j], vv.y, o.y);
-        }
-        const float inv = 1.0f / sum;
-        *reinterpret_cast<uint32_t*>(att + ((int64_t)t * G + g) * E + h * 64 + 2 * lane) = pack_h16x2(o.x * inv, o.y * inv, bf);
-    }
-}
-
-// The same causal attention for prefixes of at most 64 tokens (the 8x8 grids' body pass: T = cond_len + 63) on the warp-level tensor
-// cores: Q, K, V of one (group, head) are staged in shared memory (144 B rows: conflict-free ldmatrix), each of the four warps owns
-// 16 query rows -- S = Q K^T as 8 n-tiles x 4 k-steps of mma.sync.m16n8k16 (fp32 accumulate), scale, causal mask, row softmax in
-// registers (quad shuffles), the probabilities repacked as 16-bit A fragments (the m16n8 accumulator pair of two adjacent key tiles IS
-// the m16k16 A fragment), O = P V with V through ldmatrix.trans.  ~100 tensor instructions per warp instead of ~270 k scalar FMAs per
-// CTA.  (Not the wgmma path: 64 x 64 x 64 per head is two orders of magnitude below a wgmma tile's worth of work.)
+// Warp-level tensor-core pieces of prefill_attn_flash_kernel: mma.sync.m16n8k16 (fp32 accumulate) and ldmatrix.x4 (plain, .trans).
 template <bool BF>
 __device__ __forceinline__ void pa_mma(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     if (BF)
@@ -577,103 +500,15 @@ __device__ __forceinline__ void pa_ldsm4_t(uint32_t (&r)[4], uint32_t addr) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
 constexpr int PM_ROW = 144;                           // bytes per staged row (64 x 16-bit + 16 B pad)
-template <bool BF>
-__global__ void __launch_bounds__(128)
-prefill_attn_mma_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* __restrict__ vc, h16* __restrict__ att, int G, int T, int E,
-                        int nh, int Tmax) {
-    __shared__ __align__(16) uint8_t sm[3 * 64 * PM_ROW];
-    uint8_t* Qs = sm;
-    uint8_t* Ks = sm + 64 * PM_ROW;
-    uint8_t* Vs = sm + 2 * 64 * PM_ROW;
-    tc::pdl_launch_dependents();
-    tc::pdl_wait();
-    const int g = blockIdx.x / nh, h = blockIdx.x % nh;
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    // ---- stage Q, K, V rows [0, T) (rows beyond T: zeros); K / V also go to the cache
-    for (int i = threadIdx.x; i < 3 * 64 * 8; i += 128) {
-        const int mat = i / 512, t = (i >> 3) & 63, c = i & 7;
-        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-        if (t < T) v = *reinterpret_cast<const uint4*>(qkv + ((int64_t)t * G + g) * 3 * E + mat * E + h * 64 + c * 8);
-        *reinterpret_cast<uint4*>(sm + mat * 64 * PM_ROW + t * PM_ROW + c * 16) = v;
-        if (kc != nullptr && mat > 0 && t < T)
-            *reinterpret_cast<uint4*>((mat == 1 ? kc : vc) + (((int64_t)g * nh + h) * Tmax + t) * 64 + c * 8) = v;
-    }
-    __syncthreads();
-    if (16 * w >= T) return;                              // (no query rows for this warp)
-    const uint32_t qs = tc::smem_u32(Qs), ks = tc::smem_u32(Ks), vs = tc::smem_u32(Vs);
-    // ---- S = Q K^T for this warp's 16 query rows
-    float sacc[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; j++) { sacc[j][0] = sacc[j][1] = sacc[j][2] = sacc[j][3] = 0.f; }
-#pragma unroll
-    for (int kk = 0; kk < 4; kk++) {
-        uint32_t a[4];
-        pa_ldsm4(a, qs + (uint32_t)((16 * w + (lane & 15)) * PM_ROW + kk * 32 + (lane >> 4) * 16));
-#pragma unroll
-        for (int jp = 0; jp < 4; jp++) {                 // two key tiles per ldmatrix.x4
-            uint32_t b[4];
-            pa_ldsm4(b, ks + (uint32_t)((16 * jp + (lane & 7) + ((lane >> 4) << 3)) * PM_ROW + kk * 32 + ((lane >> 3) & 1) * 16));
-            pa_mma<BF>(sacc[2 * jp], a, b[0], b[1]);
-            pa_mma<BF>(sacc[2 * jp + 1], a, b[2], b[3]);
-        }
-    }
-    // ---- scale, causal mask, softmax over the row (a row's 64 scores live in the 4 lanes of a quad: 16 each)
-    const int r0 = 16 * w + (lane >> 2), r1 = r0 + 8;
-    float m0 = -INFINITY, m1 = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-        const int c0 = 8 * j + (lane & 3) * 2;
-        sacc[j][0] = (c0 <= r0) ? sacc[j][0] * 0.125f : -INFINITY;
-        sacc[j][1] = (c0 + 1 <= r0) ? sacc[j][1] * 0.125f : -INFINITY;
-        sacc[j][2] = (c0 <= r1) ? sacc[j][2] * 0.125f : -INFINITY;
-        sacc[j][3] = (c0 + 1 <= r1) ? sacc[j][3] * 0.125f : -INFINITY;
-        m0 = fmaxf(m0, fmaxf(sacc[j][0], sacc[j][1]));
-        m1 = fmaxf(m1, fmaxf(sacc[j][2], sacc[j][3]));
-    }
-    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1)); m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
-    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-    float s0 = 0.f, s1 = 0.f;
-    uint32_t pa[4][4];                                    // probabilities as A fragments, one per 16-key step
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-        const float e0 = __expf(sacc[j][0] - m0), e1 = __expf(sacc[j][1] - m0), e2 = __expf(sacc[j][2] - m1), e3 = __expf(sacc[j][3] - m1);
-        s0 += e0 + e1;
-        s1 += e2 + e3;
-        pa[j >> 1][(j & 1) * 2] = pack_h16x2(e0, e1, BF ? 1 : 0);
-        pa[j >> 1][(j & 1) * 2 + 1] = pack_h16x2(e2, e3, BF ? 1 : 0);
-    }
-    s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
-    s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-    // ---- O = P V
-    float oacc[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; j++) { oacc[j][0] = oacc[j][1] = oacc[j][2] = oacc[j][3] = 0.f; }
-#pragma unroll
-    for (int kk = 0; kk < 4; kk++) {                      // 16 keys per step
-#pragma unroll
-        for (int jp = 0; jp < 4; jp++) {                 // two 8-dim output tiles per ldmatrix.x4.trans
-            uint32_t b[4];
-            pa_ldsm4_t(b, vs + (uint32_t)((16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8) * PM_ROW + (2 * jp + (lane >> 4)) * 16));
-            pa_mma<BF>(oacc[2 * jp], pa[kk], b[0], b[1]);
-            pa_mma<BF>(oacc[2 * jp + 1], pa[kk], b[2], b[3]);
-        }
-    }
-    const float i0 = 1.0f / s0, i1 = 1.0f / s1;
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-        const int d = 8 * j + (lane & 3) * 2;
-        if (r0 < T) *reinterpret_cast<uint32_t*>(att + ((int64_t)r0 * G + g) * E + h * 64 + d) = pack_h16x2(oacc[j][0] * i0, oacc[j][1] * i0, BF ? 1 : 0);
-        if (r1 < T) *reinterpret_cast<uint32_t*>(att + ((int64_t)r1 * G + g) * E + h * 64 + d) = pack_h16x2(oacc[j][2] * i1, oacc[j][3] * i1, BF ? 1 : 0);
-    }
-}
-
-// The same causal attention for prefixes longer than 512 tokens (the 32x32 grids: T up to cond_len + 1023), where a whole prefix no
-// longer fits in shared memory: prefill_attn_mma_kernel's mma.sync arithmetic tiled flash-attention style.  One CTA per (query tile
-// of 64 rows, group, head), query tiles launched heaviest (last) first; each of the four warps owns 16 query rows.  K / V are read
-// in 64-key tiles double-buffered through cp.async (the 144 B rows of the ldmatrix path); per tile S = Q K^T on mma.sync (fp32
-// accumulate), the causal mask on the diagonal tile only, an online softmax (running row max and sum in fp32, O rescaled between
-// tiles), P repacked as A fragments and O += P V through ldmatrix.trans.  Key tiles are visited in a fixed order: run-to-run
-// deterministic.  When kc != NULL the CTA of query tile i writes the cache rows of tile i (every row exactly once).
+// Causal attention over a whole prefix in one launch (batched prefill / teacher-forced forward) for groups of more than 8 tokens.
+// qkv [M, 3E] 16-bit (bias already added by the GEMM epilogue), row of (group g, token t) = t * G + g (token-major: the rows of one
+// token are contiguous, like the single-step buffers).  One CTA per (query tile of 64 rows, group, head), query tiles launched
+// heaviest (last) first; each of the four warps owns 16 query rows.  K / V are read in 64-key tiles double-buffered through cp.async
+// (144 B rows: conflict-free ldmatrix); per tile S = Q K^T on mma.sync (fp32 accumulate), the causal mask on the diagonal tile only,
+// an online softmax (running row max and sum in fp32, O rescaled between tiles), the probabilities repacked as 16-bit A fragments
+// (the m16n8 accumulator pair of two adjacent key tiles IS the m16k16 A fragment) and O += P V with V through ldmatrix.trans.  Key
+// tiles are visited in a fixed order: run-to-run deterministic.  When kc != NULL the CTA of query tile i writes the cache rows
+// [g][head][t][64] of tile i (every row exactly once).
 template <bool BF>
 __global__ void __launch_bounds__(128)
 prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* __restrict__ vc, h16* __restrict__ att, int G, int T, int E,
@@ -802,8 +637,9 @@ prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16
     }
 }
 
-// ... and for groups of at most 8 tokens (the head stack of the teacher-forced forward: D tokens per (position, batch row), ~10^5
-// (group, head) pairs): one WARP per pair, everything in registers, lane <-> dims (2*lane, 2*lane+1), scores by warp reductions.
+// The same causal attention for groups of at most 8 tokens (the head stack of the teacher-forced forward: D tokens per (position,
+// batch row), ~10^5 (group, head) pairs): one WARP per pair, everything in registers, lane <-> dims (2*lane, 2*lane+1), scores by
+// warp reductions.
 template <int TMAXS>
 __global__ void __launch_bounds__(128)
 prefill_attn_small_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* __restrict__ vc, h16* __restrict__ att, int G, int T, int E,
@@ -1280,7 +1116,6 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
     RQB_TRY(make_tmap_2d(&tx_xn, bb.XN, 1, E, M, (uint64_t)E * 2, 64, bn));
     RQB_TRY(make_tmap_2d(&tx_att, bb.ATT, 1, E, M, (uint64_t)E * 2, 64, bn));
     RQB_TRY(make_tmap_2d(&tx_h, bb.H, 1, 4 * E, M, (uint64_t)E * 8, 64, bn));
-    RQB_ENSURE_SMEM(prefill_attn_smem(PA_MAXT), prefill_attn_kernel);
     const float* nof = nullptr;
     // M > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue, like the next
     // tile); M <= 256: the weight streamer
@@ -1303,18 +1138,7 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
         } else if (T <= 8) {
             RQB_TRY(launch_pdl(prefill_attn_small_kernel<8>, dim3((unsigned)ceil_div((int64_t)G * c.n_head, 4)), dim3(128), (size_t)0, st, pdl,
                                (const h16*)bb.QKV, kcl, vcl, bb.ATT, G, T, E, c.n_head, Tmax, f.bf));
-        } else if (T >= 16 && T <= 64) {                  // one 64-key tile: the mma.sync form
-            if (f.bf) {
-                RQB_TRY(launch_pdl(prefill_attn_mma_kernel<true>, dim3((unsigned)(G * c.n_head)), dim3(128), (size_t)0, st, pdl,
-                                   (const h16*)bb.QKV, kcl, vcl, bb.ATT, G, T, E, c.n_head, Tmax));
-            } else {
-                RQB_TRY(launch_pdl(prefill_attn_mma_kernel<false>, dim3((unsigned)(G * c.n_head)), dim3(128), (size_t)0, st, pdl,
-                                   (const h16*)bb.QKV, kcl, vcl, bb.ATT, G, T, E, c.n_head, Tmax));
-            }
-        } else if (T <= PA_MAXT) {
-            RQB_TRY(launch_pdl(prefill_attn_kernel, dim3((unsigned)(G * c.n_head)), dim3(128), prefill_attn_smem(T), st, pdl,
-                               (const h16*)bb.QKV, kcl, vcl, bb.ATT, G, T, E, c.n_head, Tmax, f.bf));
-        } else {                                          // longer than the shared-memory prefix: 64-key tiles, online softmax
+        } else {                                          // 64-query tiles over 64-key tiles, online softmax
             const dim3 grid((unsigned)((int64_t)ceil_div(T, 64) * G * c.n_head));
             if (f.bf) {
                 RQB_TRY(launch_pdl(prefill_attn_flash_kernel<true>, grid, dim3(128), (size_t)0, st, pdl, (const h16*)bb.QKV, kcl, vcl, bb.ATT,
