@@ -55,6 +55,10 @@ int rqb200_device_count(void);
  * reference).  residual_out (nullable) [N,C] f32 = x - quant_list[D-1].  C must be 256 (quantizations.py:181). */
 int rqb200_rq_quantize(const float* x, const float* codebook, int64_t N, int K, int C, int D, int64_t* codes,
                        float* quant_list, float* residual_out, void* stream);
+/* The same search with one codebook per depth (RQBottleneck(shared_codebook=False)): depth d searches and subtracts with
+ * codebooks_host[d] [K_host[d],C] f32.  codebooks_host / K_host are HOST arrays of D entries, D <= 16; the K_d may differ. */
+int rqb200_rq_quantize_depthwise(const float* x, const float* const* codebooks_host, const int32_t* K_host, int64_t N, int C, int D,
+                                 int64_t* codes, float* quant_list, float* residual_out, void* stream);
 
 /* One depth of RQBottleneck.get_soft_codes (quantizations.py:371-399): residual [N,C] f32 -> soft_out [N,K] = softmax(-d/temp) with
  * d = VQEmbedding.compute_distances (:43-62); logits_out (nullable) [N,K] = -d/temp (what the stochastic variant samples from). */
@@ -67,6 +71,12 @@ int rqb200_rq_embed_sum(const int64_t* codes, const float* codebook, int64_t N, 
 /* RQBottleneck.embed_code_with_depth (quantizations.py:313-334): out[n,d,:] = codebook[codes[n,d],:]. */
 int rqb200_rq_embed_depth(const int64_t* codes, const float* codebook, int64_t N, int D, int K, int C, float* out,
                           void* stream);
+/* embed_code / embed_code_with_depth with one codebook per depth: code d is looked up in codebooks_host[d] [K_host[d],C]
+ * (HOST arrays of D entries, D <= 16). */
+int rqb200_rq_embed_sum_depthwise(const int64_t* codes, const float* const* codebooks_host, const int32_t* K_host, int64_t N, int D,
+                                  int C, float* out, void* stream);
+int rqb200_rq_embed_depth_depthwise(const int64_t* codes, const float* const* codebooks_host, const int32_t* K_host, int64_t N,
+                                    int D, int C, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ sampler
  * sample_from_logits (rqvae/utils/utils.py:82-123; top_k_logits :60-64, top_p_probs :67-79).  logits [B,V] f32.
@@ -94,6 +104,7 @@ typedef struct rqb200_ar_config {
     int32_t weight_dtype;                               /* RQB200_F32 (exact); RQB200_F16 or RQB200_BF16 (fast) */
     int32_t flags;                                      /* fast tier: RQB200_AR_* flags                         */
     int32_t split_qkv, split_proj, split_fc1, split_fc2; /* fast tier: split-K factors, 0 = fill the SMs        */
+    int32_t codebook_per_depth;                         /* 0: w.codebook is [K,C]; 1: [D,K,C], depth d's table at d*K*C */
 } rqb200_ar_config;
 
 typedef struct rqb200_ar_weights {
@@ -102,7 +113,7 @@ typedef struct rqb200_ar_weights {
     const void *w_in, *w_head, *w_cls;                    /* [E,C], [E,C], [V,E]; weight dtype                   */
     const float *b_in, *b_head, *b_cls;
     const float *cls_ln_w, *cls_ln_b;
-    const float* codebook;                                /* [K,C] f32 (model_aux.get_code_emb_with_depth)       */
+    const float* codebook;                                /* [K,C] or [D,K,C] f32 (model_aux.get_code_emb_with_depth) */
     const rqb200_block_weights* body;                     /* host array [n_body]                                 */
     const rqb200_block_weights* head;                     /* host array [n_head_layers]                          */
     /* optional (cond_len > 1): cond_classifier (transformers.py:100-104) -- only rqb200_ar_forward's cond_logits use it */
@@ -174,7 +185,9 @@ typedef struct rqb200_vae rqb200_vae;
 rqb200_vae* rqb200_vae_create(const rqb200_vae_config* cfg);
 void rqb200_vae_destroy(rqb200_vae* h);
 /* register one tensor under its reference state_dict key (SURVEY.md A.3).  Conv weights must be passed
- * re-laid-out as [Cout,KH,KW,Cin] (OHWI) in the engine's weight dtype; everything else f32 as stored. */
+ * re-laid-out as [Cout,KH,KW,Cin] (OHWI) in the engine's weight dtype; everything else f32 as stored.  The RQ codebook is
+ * either "codebook" ([K,C], shared by every depth) or "codebook.0" .. "codebook.<D-1>" (one [K_d,C] table per depth,
+ * K_d = numel / embed_dim); finalize requires exactly one of the two. */
 int rqb200_vae_set_tensor(rqb200_vae* h, const char* key, const void* ptr, int dtype, int64_t numel);
 /* resolves every layer of encoder+decoder against the registered tensors; fails listing the first missing key */
 int rqb200_vae_finalize(rqb200_vae* h);
@@ -204,6 +217,9 @@ int rqb200_dbg_gemm_tc(const void* W16, const void* X16, const float* bias, cons
  * take), 0 = what rqb200_rq_quantize picks.  Both forms are bit-identical (tests/test_gpu_parity.py). */
 int rqb200_dbg_rq_quantize(int form, const float* x, const float* codebook, int64_t N, int K, int C, int D, int64_t* codes,
                            float* quant_list, float* residual_out, void* stream);
+/* rqb200_rq_quantize_depthwise with the kernel form forced (form 2 takes every K_d <= 16384).  Both forms are bit-identical. */
+int rqb200_dbg_rq_quantize_depthwise(int form, const float* x, const float* const* codebooks_host, const int32_t* K_host, int64_t N,
+                                     int C, int D, int64_t* codes, float* quant_list, float* residual_out, void* stream);
 /* rqb200_dbg_sample_logits: rqb200_sample_logits with the top-k threshold search forced: 0 = 8-pass radix select, 1 = bucket
  * select (the default).  Identical indices. */
 int rqb200_dbg_sample_logits(int algo, const float* logits, const float* q, int B, int V, float temperature, int top_k,

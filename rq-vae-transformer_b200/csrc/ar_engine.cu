@@ -78,6 +78,7 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
     const rqb200_ar_weights& w = h->w;
     const int E = c.embed_dim, D = c.D, HW = c.H * c.W, C = c.code_dim, V = c.vocab, K = c.codebook_size;
     const int wd = c.weight_dtype, cl = c.cond_len, Tb = cl + HW;
+    const int64_t cbs = c.codebook_per_depth ? (int64_t)K * C : 0;     // floats between depth d's codebook and depth d+1's
     if (B <= 0) return fail(RQB200_EINVAL, "ar_sample: B must be > 0");
     if (idx0 < 0 || idx_end > HW || idx0 > idx_end) return fail(RQB200_EINVAL, "ar_sample: bad position span");
     ArWs ws;
@@ -92,7 +93,7 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
         const int Tn0 = cl + idx0;
         RQB_TRY(launch_cond_token(cond, w.cond_emb, w.pos_emb_cond, B, cl, c.vocab_cond, E, Tn0, ws.X, st));
         if (idx0 > 0) {
-            RQB_TRY(launch_code_emb(out, w.codebook, B, HW, D, K, C, 0, idx0, ws.EMB, st));
+            RQB_TRY(launch_code_emb(out, w.codebook, cbs, B, HW, D, K, C, 0, idx0, ws.EMB, st));
             RQB_TRY(launch_linear(ws.EMB, C, w.w_in, wd, w.b_in, nullptr, ws.LIN, E, B * idx0 * D, E, C, 0, st));
             RQB_TRY(launch_body_token(ws.LIN, w.pos_emb_hw, B, D, E, 0, idx0, cl, Tn0, ws.X, st));
         }
@@ -103,7 +104,7 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
     int64_t step = 0;
     for (int idx = idx0; idx < idx_end; idx++) {
         if (idx > idx0 || resume) {   // decode step on the token of position idx-1 (transformers.py:240-242)
-            RQB_TRY(launch_code_emb(out, w.codebook, B, HW, D, K, C, idx - 1, 1, ws.EMB, st));
+            RQB_TRY(launch_code_emb(out, w.codebook, cbs, B, HW, D, K, C, idx - 1, 1, ws.EMB, st));
             RQB_TRY(launch_linear(ws.EMB, C, w.w_in, wd, w.b_in, nullptr, ws.LIN, E, B * D, E, C, 0, st));
             RQB_TRY(launch_body_token(ws.LIN, w.pos_emb_hw, B, D, E, idx - 1, 1, 0, 1, ws.X, st));
             RQB_TRY(run_stack(h, h->body, ws, B, 1, cl + idx - 1, Tb, ws.kc_body, ws.vc_body, st));
@@ -113,7 +114,7 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
             if (d == 0) {
                 RQB_TRY(launch_row_add(ws.CTX, E, 0, w.pos_emb_d, B, E, ws.X, st));                         // ctx + pos_emb_d[0]
             } else {
-                RQB_TRY(launch_head_cumsum(out, w.codebook, B, HW, D, K, C, idx, d, ws.EMB, st));         // cumsum_{i<d} e_i
+                RQB_TRY(launch_head_cumsum(out, w.codebook, cbs, B, HW, D, K, C, idx, d, ws.EMB, st));         // cumsum_{i<d} e_i
                 RQB_TRY(launch_linear(ws.EMB, C, w.w_head, wd, w.b_head, nullptr, ws.TOK, E, B, E, C, 0, st));
                 RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
             }
@@ -138,7 +139,8 @@ extern "C" {
 rqb200_ar* rqb200_ar_create(const rqb200_ar_config* cfg, const rqb200_ar_weights* w) {
     if (!cfg || !w) { rqb::set_error("ar_create: null argument"); return nullptr; }
     if (cfg->embed_dim != cfg->n_head * 64) { rqb::set_error("ar_create: embed_dim must be n_head*64"); return nullptr; }
-    if (cfg->embed_dim % 64 || cfg->code_dim % 4 || cfg->vocab > 16384 || cfg->cond_len < 1 || cfg->D < 1) {
+    if (cfg->embed_dim % 64 || cfg->code_dim % 4 || cfg->vocab > 16384 || cfg->cond_len < 1 || cfg->D < 1 ||
+        (cfg->codebook_per_depth != 0 && cfg->codebook_per_depth != 1)) {
         rqb::set_error("ar_create: unsupported shape");
         return nullptr;
     }

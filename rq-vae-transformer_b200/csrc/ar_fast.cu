@@ -706,9 +706,11 @@ cond_tok_kernel(const StepState* __restrict__ stt, const float* __restrict__ con
 // summed code embeddings in 16-bit: mode 0 -> all D codes of position idx-1 (body input), mode d>=1 -> codes 0..d-1 of
 // position idx (head input, cumsum)                                              (transformers.py:219-225, 250-255)
 // mode < 0 (prefill / forward): grid (B, n_pos); the first -mode codes of position blockIdx.y + pos0, written to row blockIdx.y * B + b
+// code i is looked up in cb + i * cb_dstride (0: one shared codebook; K*C: per-depth codebooks stacked [D,K,C]).
+// stt is not __restrict__: the previous kernel writes it, and a read-only (non-coherent) load may be scheduled above pdl_wait().
 __global__ void __launch_bounds__(64)
-code_sum_kernel(const StepState* __restrict__ stt, const float* __restrict__ cb, int HW, int D, int K, int C, int mode, int pos0,
-                h16* __restrict__ out, int bf) {
+code_sum_kernel(const StepState* stt, const float* __restrict__ cb, int64_t cb_dstride, int HW, int D, int K, int C,
+                int mode, int pos0, h16* __restrict__ out, int bf) {
     tc::pdl_launch_dependents();
     tc::pdl_wait();
     const int b = blockIdx.x, B = gridDim.x;
@@ -720,11 +722,12 @@ code_sum_kernel(const StepState* __restrict__ stt, const float* __restrict__ cb,
         for (int i = 0; i < nd; i++) {
             int64_t k = stt->codes[((int64_t)b * HW + pos) * D + i];
             k = k < 0 ? 0 : (k >= K ? K - 1 : k);
-            a += cb[k * C + c];
+            a += cb[i * cb_dstride + k * C + c];
         }
         o[c] = pack_h16(a, bf);
     }
 }
+static int64_t cb_dstride(const rqb200_ar_config& c) { return c.codebook_per_depth ? (int64_t)c.codebook_size * c.code_dim : 0; }
 // bookkeeping: which graph just ran decides what advances
 __global__ void advance_kernel(StepState* stt, int ds, int didx, int dstep) {
     tc::pdl_launch_dependents();
@@ -966,8 +969,8 @@ static int record_body(ArFast& f, FastWs& ws, bool cond_token, cudaStream_t st) 
         RQB_TRY(launch_pdl(cond_tok_kernel, dim3(B, 1), dim3(256), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.cond_emb,
                            w.pos_emb_cond, c.cond_len, c.vocab_cond, E, ws.XB));
     } else {
-        RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook, HW,
-                           c.D, c.codebook_size, c.code_dim, 0, 0, ws.S, f.bf));
+        RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
+                           cb_dstride(c), HW, c.D, c.codebook_size, c.code_dim, 0, 0, ws.S, f.bf));
         // x = W_in (sum_d e_d) + D b_in + pos_emb_hw[idx-1]       (bias counted D times, transformers.py:220,225)
         RQB_TRY(gemm(f, "w_in", f.tm_win, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_in, (float)c.D, ws.XB, nullptr,
                      w.pos_emb_hw - E /* row idx-1 */, 0, &ws.state->idx, E, st));
@@ -988,7 +991,7 @@ static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st)
                                w.cls_ln_b, st));
         } else {
             RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
-                               HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf));
+                               cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf));
             RQB_TRY(gemm(f, "w_head", f.tm_whead, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
                          w.pos_emb_d + (int64_t)d * E, 0, nullptr, 0, st));
             RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, nullptr, ws.XH, ws.kc_head, ws.vc_head, D, nullptr, d, w.cls_ln_w,
@@ -1188,8 +1191,8 @@ static int body_tokens_batched(ArFast& f, const StepState* state, float* X, h16*
         const int64_t Mc = (int64_t)B * n_code;
         CUtensorMap tx_s;
         RQB_TRY(make_tmap_2d(&tx_s, S, 1, c.code_dim, Mc, (uint64_t)c.code_dim * 2, 64, gemm_tc_bn((int)std::min<int64_t>(Mc, 256))));
-        RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, n_code), dim3(64), (size_t)0, st, false, state, w.codebook, HW, c.D, c.codebook_size,
-                           c.code_dim, -c.D, 0, S, f.bf));
+        RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, n_code), dim3(64), (size_t)0, st, false, state, w.codebook, cb_dstride(c), HW, c.D,
+                           c.codebook_size, c.code_dim, -c.D, 0, S, f.bf));
         GemmTcParams p = gemm_base(f, E, c.code_dim, (int)Mc, 1, GT_F32);
         p.bias = w.b_in; p.bias_scale = (float)c.D; p.out = X + (int64_t)cl * B * E;
         p.residual = w.pos_emb_hw; p.ld_res = E; p.res_div = B;          // row (j, b) gets pos_emb_hw[j]
@@ -1287,8 +1290,8 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
         CUtensorMap tx_s;
         RQB_TRY(make_tmap_2d(&tx_s, ws.S, 1, c.code_dim, G, (uint64_t)c.code_dim * 2, 64, gemm_tc_bn(std::min(G, 256))));
         for (int d = 1; d < D; d++) {
-            RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, HW), dim3(64), (size_t)0, st, false, (const StepState*)ws.state, w.codebook, HW, D,
-                               c.codebook_size, c.code_dim, -d, 0, ws.S, f->bf));
+            RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, HW), dim3(64), (size_t)0, st, false, (const StepState*)ws.state, w.codebook,
+                               cb_dstride(c), HW, D, c.codebook_size, c.code_dim, -d, 0, ws.S, f->bf));
             GemmTcParams p = gemm_base(*f, E, c.code_dim, G, 1, GT_F32);
             p.bias = w.b_head; p.out = ws.HX + (int64_t)d * G * E; p.residual = w.pos_emb_d + (int64_t)d * E; p.ld_res = 0;
             RQB_TRY(launch_gemm_tc(f->tm_whead, tx_s, p, false, st));

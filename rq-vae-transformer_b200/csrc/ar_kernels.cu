@@ -181,14 +181,15 @@ int launch_attn_cached(const float* qkv, float* kc, float* vc, float* out, int B
 }
 
 // ------------------------------------------------------------------------------------------------ embedding glue
-// out[(b*J + (j-j0))*D + d, :] = codebook[codes[b, j, d], :]   for j in [j0, j0+J)
-__global__ void code_emb_kernel(const int64_t* __restrict__ codes, const float* __restrict__ cb, int HW, int D, int K, int C,
-                                int j0, int J, float* __restrict__ out) {
+// out[(b*J + (j-j0))*D + d, :] = codebook_d[codes[b, j, d], :]   for j in [j0, j0+J); codebook_d = cb + d * cb_dstride
+__global__ void code_emb_kernel(const int64_t* __restrict__ codes, const float* __restrict__ cb, int64_t cb_dstride, int HW, int D,
+                                int K, int C, int j0, int J, float* __restrict__ out) {
     int r = blockIdx.x;                         // over B*J*D
     int d = r % D, j = (r / D) % J, b = r / (D * J);
     int64_t k = codes[((int64_t)b * HW + j0 + j) * D + d];
     k = k < 0 ? 0 : (k >= K ? K - 1 : k);
-    for (int c = threadIdx.x; c < C; c += blockDim.x) out[(int64_t)r * C + c] = cb[k * C + c];
+    const float* e = cb + d * cb_dstride + k * C;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) out[(int64_t)r * C + c] = e[c];
 }
 // body tokens: X[b, s0 + (j-j0), :] = ((l0 + l1) + l2) + ... + pos_hw[j]   with l_d = lin[(b*J + (j-j0))*D + d, :]
 __global__ void body_token_kernel(const float* __restrict__ lin, const float* __restrict__ pos_hw, int D, int E, int j0, int J,
@@ -213,15 +214,15 @@ __global__ void cond_token_kernel(const int64_t* __restrict__ cond, const float*
         X[((int64_t)b * Tn + s) * E + e] = cond_emb[c * E + e] + pos_cond[(int64_t)s * E + e];
 }
 // head input for depth d >= 1: out[b,:] = e_0 + e_1 + ... + e_{d-1} (sequential, torch.cumsum order)
-__global__ void head_cumsum_kernel(const int64_t* __restrict__ codes, const float* __restrict__ cb, int HW, int D, int K, int C,
-                                   int j, int d, float* __restrict__ out) {
+__global__ void head_cumsum_kernel(const int64_t* __restrict__ codes, const float* __restrict__ cb, int64_t cb_dstride, int HW, int D,
+                                   int K, int C, int j, int d, float* __restrict__ out) {
     int b = blockIdx.x;
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
         float a = 0.f;
         for (int i = 0; i < d; i++) {
             int64_t k = codes[((int64_t)b * HW + j) * D + i];
             k = k < 0 ? 0 : (k >= K ? K - 1 : k);
-            float e = cb[k * C + c];
+            float e = cb[i * cb_dstride + k * C + c];
             a = (i == 0) ? e : a + e;
         }
         out[(int64_t)b * C + c] = a;
@@ -235,10 +236,10 @@ __global__ void row_add_kernel(const float* __restrict__ in, int64_t in_row_stri
     for (int e = threadIdx.x; e < E; e += blockDim.x) out[(int64_t)b * E + e] = x[e] + (pos ? pos[e] : 0.f);
 }
 
-int launch_code_emb(const int64_t* codes, const float* cb, int B, int HW, int D, int K, int C, int j0, int J, float* out,
-                    cudaStream_t st) {
+int launch_code_emb(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j0, int J,
+                    float* out, cudaStream_t st) {
     if (B * J * D <= 0) return 0;
-    code_emb_kernel<<<B * J * D, 64, 0, st>>>(codes, cb, HW, D, K, C, j0, J, out);
+    code_emb_kernel<<<B * J * D, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j0, J, out);
     return check_launch("code_emb");
 }
 int launch_body_token(const float* lin, const float* pos_hw, int B, int D, int E, int j0, int J, int s0, int Tn, float* X,
@@ -252,9 +253,9 @@ int launch_cond_token(const int64_t* cond, const float* cond_emb, const float* p
     cond_token_kernel<<<B * cond_len, 256, 0, st>>>(cond, cond_emb, pos_cond, cond_len, vocab_cond, E, Tn, X);
     return check_launch("cond_token");
 }
-int launch_head_cumsum(const int64_t* codes, const float* cb, int B, int HW, int D, int K, int C, int j, int d, float* out,
-                       cudaStream_t st) {
-    head_cumsum_kernel<<<B, 64, 0, st>>>(codes, cb, HW, D, K, C, j, d, out);
+int launch_head_cumsum(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j, int d,
+                       float* out, cudaStream_t st) {
+    head_cumsum_kernel<<<B, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j, d, out);
     return check_launch("head_cumsum");
 }
 int launch_row_add(const float* in, int64_t in_row_stride, int64_t in_off, const float* pos, int B, int E, float* out,

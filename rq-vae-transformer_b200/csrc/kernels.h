@@ -5,15 +5,26 @@
 #include "common.cuh"
 
 namespace rqb {
+// The codebooks of one RQ search / embedding launch, passed by value.  n == 1: one [K,C] table serves every depth (a shared
+// codebook); n == D: depth d uses table d ([K_d,C], shared_codebook=False).
+constexpr int RQ_MAX_TABLES = 16;
+struct RqTables {
+    const float* cb[RQ_MAX_TABLES];
+    int K[RQ_MAX_TABLES];
+    int n;
+    __host__ __device__ __forceinline__ int of(int depth) const { return n == 1 ? 0 : depth; }
+};
+// host arrays of n device pointers / sizes -> RqTables; fails unless 1 <= n <= RQ_MAX_TABLES, every K > 0 and no pointer is null
+int make_rq_tables(RqTables* out, const float* const* cb_host, const int32_t* K_host, int n);
+
 // rq_search.cu
-int launch_rq_quantize(const float* x, const float* cb, int64_t N, int K, int C, int D, int64_t* codes, float* quant_list,
+int launch_rq_quantize(const float* x, const RqTables& tabs, int64_t N, int C, int D, int64_t* codes, float* quant_list,
                        float* resid_out, cudaStream_t st, int form = 0);
 // rq_search2.cu -- 8x8 register tile, codebook streamed in 32-channel slabs, 2-CTA clusters splitting the codebook (the default form)
-bool rq_quantize2_supported(int64_t N, int K, int C);
-int launch_rq_quantize2(const float* x, const float* cb, int64_t N, int K, int C, int D, int64_t* codes, float* quant_list,
+bool rq_quantize2_supported(int64_t N, const RqTables& tabs, int C);
+int launch_rq_quantize2(const float* x, const RqTables& tabs, int64_t N, int C, int D, int64_t* codes, float* quant_list,
                         float* resid_out, cudaStream_t st);
-int launch_rq_embed(const int64_t* codes, const float* cb, int64_t N, int D, int K, int C, float* out, bool sum,
-                    cudaStream_t st);
+int launch_rq_embed(const int64_t* codes, const RqTables& tabs, int64_t N, int D, int C, float* out, bool sum, cudaStream_t st);
 // sampler.cu
 int launch_sample(const float* logits, const float* q, int B, int V, float temperature, int top_k, float top_p,
                   int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo = 1);
@@ -24,14 +35,15 @@ int launch_layernorm(const float* X, int64_t ldx, const float* g, const float* b
                      cudaStream_t st);
 int launch_attn_cached(const float* qkv, float* kc, float* vc, float* out, int B, int Tn, int T_past, int Tmax, int E,
                        int nh, cudaStream_t st);
-int launch_code_emb(const int64_t* codes, const float* cb, int B, int HW, int D, int K, int C, int j0, int J, float* out,
-                    cudaStream_t st);
+// cb_dstride: floats between depth d's table and depth d+1's (0: one shared [K,C] table; K*C: a [D,K,C] per-depth stack)
+int launch_code_emb(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j0, int J,
+                    float* out, cudaStream_t st);
 int launch_body_token(const float* lin, const float* pos_hw, int B, int D, int E, int j0, int J, int s0, int Tn, float* X,
                       cudaStream_t st);
 int launch_cond_token(const int64_t* cond, const float* cond_emb, const float* pos_cond, int B, int cond_len, int vocab_cond,
                       int E, int Tn, float* X, cudaStream_t st);
-int launch_head_cumsum(const int64_t* codes, const float* cb, int B, int HW, int D, int K, int C, int j, int d, float* out,
-                       cudaStream_t st);
+int launch_head_cumsum(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j, int d,
+                       float* out, cudaStream_t st);
 int launch_row_add(const float* in, int64_t in_row_stride, int64_t in_off, const float* pos, int B, int E, float* out,
                    cudaStream_t st);
 // conv_kernels.cu

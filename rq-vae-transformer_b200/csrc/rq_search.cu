@@ -65,16 +65,14 @@ struct RqSmem {
 };
 
 __global__ void __launch_bounds__(RQ_THREADS, 1)
-rq_quantize_kernel(const float* __restrict__ x, const float* __restrict__ cb, int64_t N, int K, int D,
-                   int64_t* __restrict__ codes, float* __restrict__ quant_list, float* __restrict__ resid_out) {
+rq_quantize_kernel(const float* __restrict__ x, const RqTables tabs, int64_t N, int D, int64_t* __restrict__ codes,
+                   float* __restrict__ quant_list, float* __restrict__ resid_out) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     RqSmem& s = *reinterpret_cast<RqSmem*>(smem_raw);
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const int tx = t & 15, ty = t >> 4;
     const int64_t n0 = (int64_t)blockIdx.x * RQ_TN;
     const int nvalid = (int)min((int64_t)RQ_TN, N - n0);
-    const int ntiles = (K + RQ_TK - 1) / RQ_TK;
-    const int total = ntiles * D;
 
     if (t == 0) {
         mbar_init(&s.bar[0], 1);
@@ -90,9 +88,10 @@ rq_quantize_kernel(const float* __restrict__ x, const float* __restrict__ cb, in
     }
     __syncthreads();
 
-    auto issue = [&](int it) {   // warp 0 only: stream codebook tile (it % ntiles) into ring slot (it & 1)
-        int tl = it % ntiles, slot = it & 1;
-        int k0 = tl * RQ_TK, rows = min(RQ_TK, K - k0);
+    auto issue = [&](int depth, int tl, int slot) {   // warp 0 only: stream tile tl of depth's codebook into ring slot `slot`
+        const int ti = tabs.of(depth);
+        const float* cb = tabs.cb[ti];
+        int k0 = tl * RQ_TK, rows = min(RQ_TK, tabs.K[ti] - k0);
         if (lane == 0) mbar_expect_tx(&s.bar[slot], (uint32_t)rows * RQ_C * 4);
         __syncwarp();
         for (int r = lane; r < rows; r += 32)
@@ -111,7 +110,7 @@ rq_quantize_kernel(const float* __restrict__ x, const float* __restrict__ cb, in
         }
     };
 
-    if (warp == 0) issue(0);
+    if (warp == 0) issue(0, 0, 0);
     norms_x();
     float agg[RQ_TN];            // thread t owns channel t of every vector's aggregate
 #pragma unroll
@@ -123,9 +122,15 @@ rq_quantize_kernel(const float* __restrict__ x, const float* __restrict__ cb, in
     uint32_t phase[2] = {0u, 0u};
     const int v0 = ty * 2;
 
-    for (int it = 0; it < total; it++) {
-        const int slot = it & 1, tl = it % ntiles, depth = it / ntiles;
-        if (warp == 0 && it + 1 < total) issue(it + 1);
+    // tiles are visited depth by depth; each depth has its own table and tile count
+    for (int it = 0, depth = 0, tl = 0; depth < D; it++) {
+        const int slot = it & 1;
+        const int ti = tabs.of(depth), K = tabs.K[ti], ntiles = (K + RQ_TK - 1) / RQ_TK;
+        const float* cb = tabs.cb[ti];
+        if (warp == 0) {          // the next tile; the next depth's first tile does not depend on this depth's argmin
+            if (tl + 1 < ntiles) issue(depth, tl + 1, slot ^ 1);
+            else if (depth + 1 < D) issue(depth + 1, 0, slot ^ 1);
+        }
         mbar_wait(&s.bar[slot], phase[slot]);
         phase[slot] ^= 1u;
         const int k0 = tl * RQ_TK, rows = min(RQ_TK, K - k0);
@@ -207,6 +212,10 @@ rq_quantize_kernel(const float* __restrict__ x, const float* __restrict__ cb, in
             __syncthreads();
             if (depth + 1 < D) norms_x();
             __syncthreads();
+            depth++;
+            tl = 0;
+        } else {
+            tl++;
         }
     }
     if (resid_out != nullptr) {
@@ -215,17 +224,19 @@ rq_quantize_kernel(const float* __restrict__ x, const float* __restrict__ cb, in
 }
 
 template <bool SUM>
-__global__ void rq_embed_kernel(const int64_t* __restrict__ codes, const float* __restrict__ cb, int64_t N, int D, int K,
-                                int C, float* __restrict__ out) {
-    // one CTA (C/4 threads, float4 each) per vector; SUM: cat(D rows).sum(-2) in depth order (quantizations.py:308)
+__global__ void rq_embed_kernel(const int64_t* __restrict__ codes, const RqTables tabs, int64_t N, int D, int C,
+                                float* __restrict__ out) {
+    // one CTA (C/4 threads, float4 each) per vector; SUM: cat(D rows).sum(-2) in depth order (quantizations.py:308).
+    // Depth d reads table tabs.of(d).
     int64_t n = blockIdx.x;
     int c4 = threadIdx.x;
     if (c4 * 4 >= C) return;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int d = 0; d < D; d++) {
+        const int ti = tabs.of(d), K = tabs.K[ti];
         int64_t k = codes[n * D + d];
         k = k < 0 ? 0 : (k >= K ? K - 1 : k);
-        float4 e = __ldg(reinterpret_cast<const float4*>(cb + k * C) + c4);
+        float4 e = __ldg(reinterpret_cast<const float4*>(tabs.cb[ti] + k * C) + c4);
         if (SUM) {
             acc.x += e.x; acc.y += e.y; acc.z += e.z; acc.w += e.w;
         } else {
@@ -295,42 +306,76 @@ int launch_rq_soft(const float* r, const float* cb, int64_t N, int K, int C, flo
     return check_launch("rq_soft_codes");
 }
 
-int launch_rq_embed(const int64_t* codes, const float* cb, int64_t N, int D, int K, int C, float* out, bool sum,
-                    cudaStream_t st) {
+int make_rq_tables(RqTables* out, const float* const* cb_host, const int32_t* K_host, int n) {
+    if (!cb_host || !K_host || n < 1 || n > RQ_MAX_TABLES) return fail(RQB200_EINVAL, "rq tables: need 1..16 tables");
+    *out = RqTables{};
+    out->n = n;
+    for (int i = 0; i < n; i++) {
+        if (!cb_host[i] || K_host[i] <= 0) return fail(RQB200_EINVAL, "rq tables: null table or K <= 0");
+        out->cb[i] = cb_host[i];
+        out->K[i] = K_host[i];
+    }
+    return 0;
+}
+
+int launch_rq_embed(const int64_t* codes, const RqTables& tabs, int64_t N, int D, int C, float* out, bool sum, cudaStream_t st) {
     if (C % 4 != 0 || C > 4096 || N < 0 || D <= 0) return fail(RQB200_EINVAL, "rq_embed: bad shape");
+    if (tabs.n != 1 && tabs.n != D) return fail(RQB200_EINVAL, "rq_embed: need one table or one per depth");
     if (N == 0) return 0;
     if (sum)
-        rq_embed_kernel<true><<<(unsigned)N, C / 4, 0, st>>>(codes, cb, N, D, K, C, out);
+        rq_embed_kernel<true><<<(unsigned)N, C / 4, 0, st>>>(codes, tabs, N, D, C, out);
     else
-        rq_embed_kernel<false><<<(unsigned)N, C / 4, 0, st>>>(codes, cb, N, D, K, C, out);
+        rq_embed_kernel<false><<<(unsigned)N, C / 4, 0, st>>>(codes, tabs, N, D, C, out);
     return check_launch("rq_embed");
 }
 
 // form: 0 = pick (the 8x8-register-tile cluster kernel of rq_search2.cu whenever the shape allows: 3.7 vs 7.6 ms at N = 4096,
 // K = 16384; bit-identical results), 1 = this file's 2x4-tile kernel, 2 = rq_search2.cu or fail
-int launch_rq_quantize(const float* x, const float* cb, int64_t N, int K, int C, int D, int64_t* codes, float* quant_list,
+int launch_rq_quantize(const float* x, const RqTables& tabs, int64_t N, int C, int D, int64_t* codes, float* quant_list,
                        float* resid_out, cudaStream_t st, int form) {
     if (C != RQ_C) return fail(RQB200_EINVAL, "rq_quantize: C must be 256");
-    if (N < 0 || K <= 0 || D <= 0) return fail(RQB200_EINVAL, "rq_quantize: bad shape");
+    if (N < 0 || D <= 0) return fail(RQB200_EINVAL, "rq_quantize: bad shape");
+    if (tabs.n != 1 && tabs.n != D) return fail(RQB200_EINVAL, "rq_quantize: need one codebook or one per depth");
     if (N == 0) return 0;   // empty input: nothing to do (reference returns empty tensors)
-    if (form != 1 && rq_quantize2_supported(N, K, C)) return launch_rq_quantize2(x, cb, N, K, C, D, codes, quant_list, resid_out, st);
+    if (form != 1 && rq_quantize2_supported(N, tabs, C)) return launch_rq_quantize2(x, tabs, N, C, D, codes, quant_list, resid_out, st);
     if (form == 2) return fail(RQB200_EINVAL, "rq_quantize: shape not supported by the cluster kernel");
     RQB_ENSURE_SMEM(sizeof(RqSmem), rq_quantize_kernel);
     unsigned grid = (unsigned)ceil_div(N, RQ_TN);
-    rq_quantize_kernel<<<grid, RQ_THREADS, sizeof(RqSmem), st>>>(x, cb, N, K, D, codes, quant_list, resid_out);
+    rq_quantize_kernel<<<grid, RQ_THREADS, sizeof(RqSmem), st>>>(x, tabs, N, D, codes, quant_list, resid_out);
     return check_launch("rq_quantize");
 }
 
 }  // namespace rqb
 
+static int rq_quantize_entry(int form, const float* x, const float* const* cb_host, const int32_t* K_host, int n, int64_t N, int C,
+                             int D, int64_t* codes, float* quant_list, float* residual_out, void* stream) {
+    rqb::RqTables tabs;
+    RQB_TRY(rqb::make_rq_tables(&tabs, cb_host, K_host, n));
+    return rqb::launch_rq_quantize(x, tabs, N, C, D, codes, quant_list, residual_out, (cudaStream_t)stream, form);
+}
+static int rq_embed_entry(const int64_t* codes, const float* const* cb_host, const int32_t* K_host, int n, int64_t N, int D, int C,
+                          float* out, bool sum, void* stream) {
+    rqb::RqTables tabs;
+    RQB_TRY(rqb::make_rq_tables(&tabs, cb_host, K_host, n));
+    return rqb::launch_rq_embed(codes, tabs, N, D, C, out, sum, (cudaStream_t)stream);
+}
+
 extern "C" {
 int rqb200_rq_quantize(const float* x, const float* codebook, int64_t N, int K, int C, int D, int64_t* codes,
                        float* quant_list, float* residual_out, void* stream) {
-    return rqb::launch_rq_quantize(x, codebook, N, K, C, D, codes, quant_list, residual_out, (cudaStream_t)stream, 0);
+    return rq_quantize_entry(0, x, &codebook, &K, 1, N, C, D, codes, quant_list, residual_out, stream);
+}
+int rqb200_rq_quantize_depthwise(const float* x, const float* const* codebooks_host, const int32_t* K_host, int64_t N, int C, int D,
+                                 int64_t* codes, float* quant_list, float* residual_out, void* stream) {
+    return rq_quantize_entry(0, x, codebooks_host, K_host, D, N, C, D, codes, quant_list, residual_out, stream);
 }
 int rqb200_dbg_rq_quantize(int form, const float* x, const float* codebook, int64_t N, int K, int C, int D, int64_t* codes,
                            float* quant_list, float* residual_out, void* stream) {
-    return rqb::launch_rq_quantize(x, codebook, N, K, C, D, codes, quant_list, residual_out, (cudaStream_t)stream, form);
+    return rq_quantize_entry(form, x, &codebook, &K, 1, N, C, D, codes, quant_list, residual_out, stream);
+}
+int rqb200_dbg_rq_quantize_depthwise(int form, const float* x, const float* const* codebooks_host, const int32_t* K_host, int64_t N,
+                                     int C, int D, int64_t* codes, float* quant_list, float* residual_out, void* stream) {
+    return rq_quantize_entry(form, x, codebooks_host, K_host, D, N, C, D, codes, quant_list, residual_out, stream);
 }
 int rqb200_rq_soft_codes(const float* residual, const float* codebook, int64_t N, int K, int C, float temp, float* soft_out,
                          float* logits_out, void* stream) {
@@ -338,10 +383,18 @@ int rqb200_rq_soft_codes(const float* residual, const float* codebook, int64_t N
 }
 int rqb200_rq_embed_sum(const int64_t* codes, const float* codebook, int64_t N, int D, int K, int C, float* out,
                         void* stream) {
-    return rqb::launch_rq_embed(codes, codebook, N, D, K, C, out, true, (cudaStream_t)stream);
+    return rq_embed_entry(codes, &codebook, &K, 1, N, D, C, out, true, stream);
 }
 int rqb200_rq_embed_depth(const int64_t* codes, const float* codebook, int64_t N, int D, int K, int C, float* out,
                           void* stream) {
-    return rqb::launch_rq_embed(codes, codebook, N, D, K, C, out, false, (cudaStream_t)stream);
+    return rq_embed_entry(codes, &codebook, &K, 1, N, D, C, out, false, stream);
+}
+int rqb200_rq_embed_sum_depthwise(const int64_t* codes, const float* const* codebooks_host, const int32_t* K_host, int64_t N, int D,
+                                  int C, float* out, void* stream) {
+    return rq_embed_entry(codes, codebooks_host, K_host, D, N, D, C, out, true, stream);
+}
+int rqb200_rq_embed_depth_depthwise(const int64_t* codes, const float* const* codebooks_host, const int32_t* K_host, int64_t N,
+                                    int D, int C, float* out, void* stream) {
+    return rq_embed_entry(codes, codebooks_host, K_host, D, N, D, C, out, false, stream);
 }
 }

@@ -28,7 +28,7 @@ constexpr int R2_NCH = R2_C / R2_CC;
 constexpr int R2_STAGES = 3;
 constexpr int R2_STAGE_BYTES = R2_KB * R2_CC * 4;     // 32 KB
 constexpr int R2_PITCH = 260;
-constexpr int R2_MAXEN = 8192;     // codewords per CTA whose ||e||^2 fit the shared table  (K <= 16384)
+constexpr int R2_MAXEN = 8192;     // codewords per CTA whose ||e||^2 fit the shared table  (every K_d <= 16384)
 constexpr int R2_CONSUMERS = 256;
 constexpr int R2_THREADS = R2_CONSUMERS;      // 8 warps = 2 per scheduler partition: the 8x8 tile needs ~200 registers per thread
 
@@ -76,13 +76,18 @@ __device__ __forceinline__ void r2_wait_cluster(uint64_t* bar, uint32_t parity) 
         "r"(parity)
         : "memory");
 }
+// one TMA descriptor per codebook table (RqTables order)
+struct Rq2Maps {
+    CUtensorMap m[RQ_MAX_TABLES];
+};
+
 __device__ __forceinline__ bool r2_before(float d, int k, float od, int ok) {   // (od, ok) < (d, k) lexicographically
     return od < d || (od == d && ok < k);
 }
 
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(R2_THREADS, 1)
-rq_quantize2_kernel(const __grid_constant__ CUtensorMap tmCB, const float* __restrict__ x, const float* __restrict__ cb, int64_t N,
-                    int K, int D, int64_t* __restrict__ codes, float* __restrict__ quant_list, float* __restrict__ resid_out) {
+rq_quantize2_kernel(const __grid_constant__ Rq2Maps tms, const RqTables tabs, const float* __restrict__ x, int64_t N, int D,
+                    int64_t* __restrict__ codes, float* __restrict__ quant_list, float* __restrict__ resid_out) {
     extern __shared__ uint8_t smem_raw[];
     // 1024 B alignment (swizzle atom) by an OFFSET into the shared array: keeps the pointers in the shared address space, so the
     // hot loop compiles to LDS.128 and not to generic LD
@@ -93,31 +98,46 @@ rq_quantize2_kernel(const __grid_constant__ CUtensorMap tmCB, const float* __res
     const uint32_t rank = blockIdx.x & 1u;                       // cluster = 2 consecutive CTAs along x
     const int64_t n0 = (int64_t)(blockIdx.x >> 1) * R2_TN;
     const int nvalid = (int)min((int64_t)R2_TN, N - n0);
-    const int nblk = (K + R2_KB - 1) / R2_KB;
-    const int nb0 = (nblk + 1) / 2;
-    const int blk0 = rank == 0 ? 0 : nb0;                        // this CTA's codeword blocks [blk0, blk0 + nb)
-    const int nb = rank == 0 ? nb0 : nblk - nb0;
-    const int kbase = blk0 * R2_KB;
+    // the codebook split of depth d: this CTA's codeword blocks [blk0, blk0 + nb) of table tabs.of(d)
+    auto split = [&](int d, int& blk0, int& nb) {
+        const int nblk = (tabs.K[tabs.of(d)] + R2_KB - 1) / R2_KB;
+        const int nb0 = (nblk + 1) / 2;
+        blk0 = rank == 0 ? 0 : nb0;
+        nb = rank == 0 ? nb0 : nblk - nb0;
+    };
 
     if (t == 0) {
         for (int i = 0; i < R2_STAGES; i++) { tc::mbar_init(&s.full[i], 1); tc::mbar_init(&s.empty[i], 8); }
         tc::mbar_init(&s.peer_bar[0], R2_TN);
         tc::mbar_init(&s.peer_bar[1], R2_TN);
         tc::fence_barrier_init();
-        tc::prefetch_tmap(&tmCB);
+        for (int i = 0; i < tabs.n; i++) tc::prefetch_tmap(&tms.m[i]);
     }
     __syncthreads();
     r2_cluster_sync();                                           // the peer's barriers exist before anything is pushed to them
 
     // producer duty: lane 0 of warp 0 keeps R2_STAGES - 1 slabs in flight; before chunk `it` it (re)fills the slot chunk it-1 used,
     // which blocks it only while another warp is still reading that slot (warp 0 is never more than one chunk ahead of the slowest)
-    const int total = D * nb * R2_NCH;
+    // slabs are streamed depth by depth; thread 0 keeps a cursor (pd, pb, pcc) = (depth, block, slab) of the next slab to issue
+    int total = 0;
+    for (int d = 0; d < D; d++) {
+        int b0, n;
+        split(d, b0, n);
+        total += n * R2_NCH;
+    }
+    int pd = 0, pb = 0, pcc = 0, p_blk0, p_nb;
+    split(0, p_blk0, p_nb);
     auto issue = [&](int nx) {
+        while (p_nb == 0) split(++pd, p_blk0, p_nb);             // a depth whose table leaves this CTA no block
         const int st = nx % R2_STAGES;
         tc::mbar_wait(&s.empty[st], ((nx / R2_STAGES) & 1) ^ 1);
         tc::mbar_expect_tx(&s.full[st], R2_STAGE_BYTES);
-        tc::tma_load_2d(ring + st * R2_STAGE_BYTES, &tmCB, &s.full[st], (nx % R2_NCH) * R2_CC, (blk0 + (nx / R2_NCH) % nb) * R2_KB,
+        tc::tma_load_2d(ring + st * R2_STAGE_BYTES, &tms.m[tabs.of(pd)], &s.full[st], pcc * R2_CC, (p_blk0 + pb) * R2_KB,
                         tc::L2_EVICT_LAST);
+        if (++pcc == R2_NCH) {
+            pcc = 0;
+            if (++pb == p_nb) { pb = 0; if (++pd < D) split(pd, p_blk0, p_nb); }
+        }
     };
     if (t == 0)
         for (int nx = 0; nx < R2_STAGES - 1 && nx < total; nx++) issue(nx);
@@ -132,9 +152,14 @@ rq_quantize2_kernel(const __grid_constant__ CUtensorMap tmCB, const float* __res
             if (v < nvalid) val = *reinterpret_cast<const float4*>(x + (n0 + v) * R2_C + c4 * 4);
             *reinterpret_cast<float4*>(&s.resid[v][c4 * 4]) = val;
         }
-        // ||e||^2 of this CTA's codewords, the partial-sum tree of rq_quantize_kernel: 4 lanes x 64 sequential fmaf, (p0+p1)+(p2+p3)
-        {
-            const int nk = min(nb * R2_KB, K - kbase);
+        // ||e||^2 of this CTA's codewords of depth d's table, the partial-sum tree of rq_quantize_kernel: 4 lanes x 64 sequential
+        // fmaf, (p0+p1)+(p2+p3)
+        auto fill_en = [&](int d) {
+            int blk0, nb;
+            split(d, blk0, nb);
+            const int ti = tabs.of(d), kbase = blk0 * R2_KB;
+            const float* cb = tabs.cb[ti];
+            const int nk = min(nb * R2_KB, tabs.K[ti] - kbase);
             const int part = t & 3;
             for (int r0 = 0; r0 < nk; r0 += R2_CONSUMERS / 4) {
                 const int r = r0 + (t >> 2);
@@ -154,7 +179,8 @@ rq_quantize2_kernel(const __grid_constant__ CUtensorMap tmCB, const float* __res
                 a += __shfl_xor_sync(0xffffffffu, a, 2);
                 if (part == 0 && r < nk) s.en[r] = a;
             }
-        }
+        };
+        fill_en(0);
         r2_consumer_sync();
         auto norms_x = [&]() {       // ||r||^2 per vector: lane sums channels lane, lane+32, ... then the xor butterfly (as rq_search.cu)
 #pragma unroll
@@ -176,6 +202,11 @@ rq_quantize2_kernel(const __grid_constant__ CUtensorMap tmCB, const float* __res
         for (int i = 0; i < 8; i++) { best_d[i] = INFINITY; best_k[i] = 0x7fffffff; }
         int it = 0;
         for (int depth = 0; depth < D; depth++) {
+            const int ti = tabs.of(depth), K = tabs.K[ti];
+            const float* cb = tabs.cb[ti];
+            int blk0, nb;
+            split(depth, blk0, nb);
+            const int kbase = blk0 * R2_KB;
             for (int b = 0; b < nb; b++) {
                 float acc[8][8];
 #pragma unroll
@@ -274,7 +305,11 @@ rq_quantize2_kernel(const __grid_constant__ CUtensorMap tmCB, const float* __res
                 }
             }
             r2_consumer_sync();
-            if (depth + 1 < D) norms_x();
+            if (depth + 1 < D) {
+                // a new table: refill ||e||^2 (en[] is no longer read: every thread passed the syncs since this depth's distances)
+                if (tabs.of(depth + 1) != ti) fill_en(depth + 1);
+                norms_x();
+            }
             r2_consumer_sync();
         }
         if (resid_out != nullptr && rank == 0)
@@ -284,17 +319,23 @@ rq_quantize2_kernel(const __grid_constant__ CUtensorMap tmCB, const float* __res
     r2_cluster_sync();                                           // nobody leaves while the peer may still push into this CTA
 }
 
-bool rq_quantize2_supported(int64_t N, int K, int C) { return C == R2_C && K <= 2 * R2_MAXEN && N > 0; }
+bool rq_quantize2_supported(int64_t N, const RqTables& tabs, int C) {
+    if (C != R2_C || N <= 0) return false;
+    for (int i = 0; i < tabs.n; i++)
+        if (tabs.K[i] > 2 * R2_MAXEN) return false;
+    return true;
+}
 
-int launch_rq_quantize2(const float* x, const float* cb, int64_t N, int K, int C, int D, int64_t* codes, float* quant_list,
+int launch_rq_quantize2(const float* x, const RqTables& tabs, int64_t N, int C, int D, int64_t* codes, float* quant_list,
                         float* resid_out, cudaStream_t st) {
-    if (!rq_quantize2_supported(N, K, C)) return fail(RQB200_EINVAL, "rq_quantize2: need C == 256 and K <= 16384");
-    CUtensorMap tm;
-    RQB_TRY(make_tmap_2d(&tm, cb, 2, (uint64_t)R2_C, (uint64_t)K, (uint64_t)R2_C * 4, R2_CC, R2_KB));
+    if (!rq_quantize2_supported(N, tabs, C)) return fail(RQB200_EINVAL, "rq_quantize2: need C == 256 and every K <= 16384");
+    Rq2Maps tms{};
+    for (int i = 0; i < tabs.n; i++)
+        RQB_TRY(make_tmap_2d(&tms.m[i], tabs.cb[i], 2, (uint64_t)R2_C, (uint64_t)tabs.K[i], (uint64_t)R2_C * 4, R2_CC, R2_KB));
     const size_t smem = (size_t)R2_STAGES * R2_STAGE_BYTES + sizeof(Rq2Smem) + 1024;
     RQB_ENSURE_SMEM(smem, rq_quantize2_kernel);
     const unsigned grid = 2u * (unsigned)ceil_div(N, R2_TN);
-    rq_quantize2_kernel<<<grid, R2_THREADS, smem, st>>>(tm, x, cb, N, K, D, codes, quant_list, resid_out);
+    rq_quantize2_kernel<<<grid, R2_THREADS, smem, st>>>(tms, tabs, x, N, D, codes, quant_list, resid_out);
     return check_launch("rq_quantize2");
 }
 

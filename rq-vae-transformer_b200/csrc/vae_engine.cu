@@ -29,6 +29,7 @@ struct rqb200_vae {
     int64_t last_launches = 0;
     int64_t max_act = 0;      // max H*W*C per image over all activations
     int64_t max_gn_hw = 0;
+    rqb::RqTables codebooks{};   // decode_code's embedding tables, resolved by finalize from "codebook" or "codebook.<d>"
 };
 
 namespace rqb {
@@ -378,7 +379,26 @@ int rqb200_vae_finalize(rqb200_vae* h) {
     run.fast = h->fast_ok && h->enc_fast;
     run.encode(nullptr, nullptr);
     if (!run.missing.empty()) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor " + run.missing);
-    if (h->t.find("codebook") == h->t.end()) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor codebook (missing)");
+    {
+        const rqb200_vae_config& c = h->cfg;
+        const bool shared = h->t.count("codebook") != 0, per_depth = h->t.count("codebook.0") != 0;
+        if (!shared && !per_depth) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor codebook (missing)");
+        if (shared && per_depth) return rqb::fail(RQB200_EINVAL, "vae_finalize: both codebook and codebook.<d> registered");
+        if (per_depth && (c.depth < 1 || c.depth > rqb::RQ_MAX_TABLES))
+            return rqb::fail(RQB200_EINVAL, "vae_finalize: per-depth codebooks need depth 1..16");
+        const float* ptrs[rqb::RQ_MAX_TABLES];
+        int32_t ks[rqb::RQ_MAX_TABLES];
+        const int n = shared ? 1 : c.depth;
+        for (int d = 0; d < n; d++) {
+            auto it = h->t.find(shared ? std::string("codebook") : "codebook." + std::to_string(d));
+            if (it == h->t.end()) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor codebook." + std::to_string(d) + " (missing)");
+            ptrs[d] = (const float*)it->second.ptr;
+            ks[d] = shared ? c.codebook_size : (int32_t)(it->second.numel / c.embed_dim);
+            if (!shared && (int64_t)ks[d] * c.embed_dim != it->second.numel)
+                return rqb::fail(RQB200_EINVAL, "vae_finalize: codebook." + std::to_string(d) + " is not [K, embed_dim]");
+        }
+        RQB_TRY(rqb::make_rq_tables(&h->codebooks, ptrs, ks, n));
+    }
     h->finalized = true;
     return 0;
 }
@@ -417,9 +437,7 @@ int rqb200_vae_decode_code(rqb200_vae* h, const int64_t* codes, int B, float* ou
     const rqb200_vae_config& c = h->cfg;
     int r = c.resolution >> (c.n_levels - 1);
     float* zq = rqb::vae_zq_buffer(h, B, workspace, workspace_bytes);
-    const VTensor& cb = h->t["codebook"];
-    RQB_TRY(rqb::launch_rq_embed(codes, (const float*)cb.ptr, (int64_t)B * r * r, c.depth, c.codebook_size, c.embed_dim, zq,
-                                 true, (cudaStream_t)stream));
+    RQB_TRY(rqb::launch_rq_embed(codes, h->codebooks, (int64_t)B * r * r, c.depth, c.embed_dim, zq, true, (cudaStream_t)stream));
     int rc = run.decode(zq, out);
     h->last_launches = rqb::g_launches;
     return rc;

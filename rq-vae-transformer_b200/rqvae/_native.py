@@ -24,7 +24,8 @@ class BlockWeights(C.Structure):
 class ArConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("embed_dim", "n_head", "n_body", "n_head_layers", "vocab", "H", "W", "D",
                                          "vocab_cond", "cond_len", "code_dim", "codebook_size", "mode", "weight_dtype",
-                                         "flags", "split_qkv", "split_proj", "split_fc1", "split_fc2")]
+                                         "flags", "split_qkv", "split_proj", "split_fc1", "split_fc2",
+                                         "codebook_per_depth")]
 
 
 class ArWeights(C.Structure):
@@ -67,6 +68,13 @@ def lib():
                                        C.c_void_p]
     L.rqb200_rq_embed_sum.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     L.rqb200_rq_embed_depth.argtypes = L.rqb200_rq_embed_sum.argtypes
+    # per-depth codebooks: host arrays of D device pointers and D sizes
+    L.rqb200_rq_quantize_depthwise.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_int64, C.c_int, C.c_int,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.rqb200_dbg_rq_quantize_depthwise.argtypes = [C.c_int] + L.rqb200_rq_quantize_depthwise.argtypes
+    L.rqb200_rq_embed_sum_depthwise.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_int64, C.c_int, C.c_int,
+                                                C.c_void_p, C.c_void_p]
+    L.rqb200_rq_embed_depth_depthwise.argtypes = L.rqb200_rq_embed_sum_depthwise.argtypes
     L.rqb200_sample_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_float, C.c_void_p,
                                        C.c_void_p]
     L.rqb200_dbg_rows_gemm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64,
@@ -119,7 +127,8 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_vae_destroy", "rqb200_vae_set_tensor", "rqb200_vae_finalize", "rqb200_vae_workspace_bytes",
            "rqb200_vae_decode", "rqb200_vae_decode_code", "rqb200_vae_encode", "rqb200_vae_last_launches",
            "rqb200_dbg_gemm_tc", "rqb200_dbg_conv_tc", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
-           "rqb200_dbg_rows_gemm"]
+           "rqb200_dbg_rows_gemm", "rqb200_rq_quantize_depthwise", "rqb200_rq_embed_sum_depthwise",
+           "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise"]
 
 
 def check(rc, what=""):

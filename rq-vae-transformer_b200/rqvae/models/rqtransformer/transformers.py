@@ -123,23 +123,37 @@ class RQTransformer(Stage2Model):
             p = "fast" if amp else "exact"
         return N.MODE_FAST if p == "fast" else N.MODE_EXACT
 
-    @staticmethod
-    def _codebook_of(model_aux, depth):
-        """the [K,C] table behind model_aux.get_code_emb_with_depth (transformers.py:109-111)"""
+    def _codebook_of(self, model_aux, depth):
+        """the table(s) behind model_aux.get_code_emb_with_depth (transformers.py:109-111): the [K,C] tensor of a shared codebook,
+        or the list of the D per-depth [K,C] tables, each K equal to the vocabulary"""
         q = getattr(model_aux, "quantizer", None)
+        if q is not None and hasattr(q, "_tables"):
+            tabs = q._tables()
+            if isinstance(tabs, list) and (len(tabs) != depth or any(t.shape[0] != self.vocab_size[0] for t in tabs)):
+                raise ValueError("rqb200: model_aux's per-depth codebooks must number %d, each of the vocabulary's size %d (got %s)"
+                                 % (depth, self.vocab_size[0], [t.shape[0] for t in tabs]))
+            return tabs
         if q is not None and hasattr(q, "_shared_table"):
             return q._shared_table()
         if q is not None and getattr(q, "shared_codebook", False):
             return q.codebooks[0].weight[:-1]
-        raise NotImplementedError("rqb200: model_aux must be an RQ-VAE with a shared codebook")
+        raise NotImplementedError("rqb200: model_aux must be an RQ-VAE (its quantizer holds the codebooks)")
 
     def _engine(self, codebook, mode, slot=0):
+        """codebook: one [K,C] table or a list of D per-depth tables.  Engines are keyed by the tables' storage and rebuilt when
+        any of them is written in place (per-depth tables are stacked into one [D,K,C] copy per engine build)."""
         dev = self.pos_emb_hw.device
-        fp = (N.param_fingerprint(self), codebook._version)
+        per_depth = isinstance(codebook, list)
+        if per_depth:
+            fp = (N.param_fingerprint(self), tuple(t._version for t in codebook))
+            cb_id = tuple(t.data_ptr() for t in codebook)
+        else:
+            fp = (N.param_fingerprint(self), codebook._version)
+            cb_id = codebook.data_ptr()
         if fp != self._eng_fp:               # weights changed behind the module's own hooks (wrapper load, in-place write)
             self._invalidate_native()
             self._eng_fp = fp
-        key = (str(dev), mode, codebook.data_ptr(), slot)
+        key = (str(dev), mode, cb_id, slot)
         if key not in self._eng and slot > 0:
             # engines of one model share the packed weights of slot 0; each slot owns its workspace, KV cache and graphs
             base = self._engine(codebook, mode, 0)
@@ -148,7 +162,7 @@ class RQTransformer(Stage2Model):
             return eng
         if key in self._eng:
             return self._eng[key]
-        N.require_cuda(self.pos_emb_hw, codebook)
+        N.require_cuda(self.pos_emb_hw, *(codebook if per_depth else [codebook]))
         L = N.lib()
         wdt = N.fast_dtype() if mode == N.MODE_FAST else torch.float32
         opts = N.ar_engine_options() if mode == N.MODE_FAST else {"flags": 0, "splits": [0, 0, 0, 0]}
@@ -184,7 +198,9 @@ class RQTransformer(Stage2Model):
         cfg.n_body, cfg.n_head_layers = len(self.body_transformer.blocks), len(self.head_transformer.blocks)
         cfg.vocab, cfg.H, cfg.W, cfg.D = self.vocab_size[0], self.block_size[0], self.block_size[1], self.block_size[2]
         cfg.vocab_cond, cfg.cond_len = self.vocab_size_cond, self.block_size_cond
-        cfg.code_dim, cfg.codebook_size = codebook.shape[1], codebook.shape[0]
+        table0 = codebook[0] if per_depth else codebook
+        cfg.code_dim, cfg.codebook_size = table0.shape[1], table0.shape[0]
+        cfg.codebook_per_depth = int(per_depth)
         cfg.mode, cfg.weight_dtype = mode, N._DT[wdt]
         cfg.flags = opts["flags"]
         cfg.split_qkv, cfg.split_proj, cfg.split_fc1, cfg.split_fc2 = opts["splits"]
@@ -197,7 +213,7 @@ class RQTransformer(Stage2Model):
         w.w_head, w.b_head = wt(self.head_mlp.weight), f32(self.head_mlp.bias)
         w.w_cls, w.b_cls = wt(self.classifier.linear.weight), f32(self.classifier.linear.bias)
         w.cls_ln_w, w.cls_ln_b = f32(self.classifier.layer_norm.weight), f32(self.classifier.layer_norm.bias)
-        w.codebook = f32(codebook)
+        w.codebook = f32(torch.stack(codebook)) if per_depth else f32(codebook)
         if hasattr(self, "cond_classifier") and mode == N.MODE_FAST:
             pad = -self.vocab_size_cond % 128            # classifier rows padded with zeros up to the 128-feature wgmma tile
             pw = torch.nn.functional.pad(self.cond_classifier.linear.weight.detach(), (0, 0, 0, pad))

@@ -2,7 +2,8 @@
 
 Parameters / buffers keep the reference's names and shapes (``codebooks.{i}.weight`` [K+1, C] with a zero padding row,
 ``cluster_size_ema``, ``embed_ema``) so checkpoints load unchanged; the numeric work is done by
-``rqb200_rq_quantize`` / ``rqb200_rq_embed_sum`` / ``rqb200_rq_embed_depth`` (csrc/rq_search.cu)."""
+``rqb200_rq_quantize`` / ``rqb200_rq_embed_sum`` / ``rqb200_rq_embed_depth`` (csrc/rq_search.cu), or their ``*_depthwise``
+forms when every depth has its own codebook (``shared_codebook=False``)."""
 from typing import Iterable
 
 import numpy as np
@@ -97,16 +98,22 @@ class RQBottleneck(nn.Module):
 
     def _shared_table(self):
         if not self.shared_codebook:
-            raise NotImplementedError("rqb200: per-depth codebooks are not supported by the fused kernels "
-                                      "(every shipped config uses shared_codebook: true)")
+            raise ValueError("rqb200: this quantizer has one codebook per depth (use _tables())")
         return self.codebooks[0].codebook()
+
+    def _tables(self):
+        """what the kernels search and embed with: the one [K,C] table of a shared codebook, else the list of the D per-depth
+        [K_d,C] tables (views of codebooks[d].weight without the padding row; no copies)"""
+        if self.shared_codebook:
+            return self.codebooks[0].codebook()
+        return [cb.codebook() for cb in self.codebooks]
 
     @torch.no_grad()
     def quantize(self, x):
         """quantizations.py:237-271.  x [B,h,w,C] -> (list of D cumulative aggregates [B,h,w,C], codes [B,h,w,D] int64)."""
         B, h, w, C = x.shape
         depth = self.code_shape[-1]
-        quants, codes = nb.rq_quantize(x.reshape(-1, C), self._shared_table(), depth)
+        quants, codes = nb.rq_quantize(x.reshape(-1, C), self._tables(), depth)
         return [quants[i].reshape(B, h, w, C) for i in range(depth)], codes.reshape(B, h, w, depth)
 
     def forward(self, x):
@@ -128,21 +135,24 @@ class RQBottleneck(nn.Module):
         x = self.to_code_shape(x)
         B, h, w, C = x.shape
         depth = self.code_shape[-1]
-        cb = self._shared_table()
+        tabs = self._tables()
+        cb = tabs if isinstance(tabs, list) else [tabs] * depth      # table of depth d
+        if len({t.shape[0] for t in cb}) != 1:
+            raise ValueError("get_soft_codes: the per-depth codebooks must have equal sizes (the soft codes are stacked)")
         flat = x.reshape(-1, C).float().contiguous()
         softs, codes = [], []
         if not stochastic:
-            ql, code = nb.rq_quantize(flat, cb, depth)
+            ql, code = nb.rq_quantize(flat, tabs, depth)
             for d in range(depth):
-                softs.append(nb.rq_soft(flat if d == 0 else flat - ql[d - 1], cb, temp))
+                softs.append(nb.rq_soft(flat if d == 0 else flat - ql[d - 1], cb[d], temp))
             codes = code
         else:
             res = flat.clone()
             for d in range(depth):
-                soft, logits = nb.rq_soft(res, cb, temp, want_logits=True)
+                soft, logits = nb.rq_soft(res, cb[d], temp, want_logits=True)
                 q = torch.empty_like(soft).exponential_(1)        # the draw torch.multinomial(soft, 1) makes
                 idx = nb.sample_logits(logits, 1.0, None, None, q=q)
-                res = res - nb.rq_embed(idx.reshape(-1, 1), cb, summed=True)
+                res = res - nb.rq_embed(idx.reshape(-1, 1), cb[d], summed=True)
                 softs.append(soft)
                 codes.append(idx.unsqueeze(-1))
             codes = torch.cat(codes, -1)
@@ -153,14 +163,14 @@ class RQBottleneck(nn.Module):
     def embed_code(self, code):
         """quantizations.py:297-311"""
         assert code.shape[1:] == self.code_shape
-        out = nb.rq_embed(code.reshape(-1, code.shape[-1]), self._shared_table(), summed=True)
+        out = nb.rq_embed(code.reshape(-1, code.shape[-1]), self._tables(), summed=True)
         return self.to_latent_shape(out.reshape(*code.shape[:-1], -1))
 
     @torch.no_grad()
     def embed_code_with_depth(self, code, to_latent_shape=False):
         """quantizations.py:313-334 -> ([..., D, C], None)"""
         assert code.shape[-1] == self.code_shape[-1]
-        out = nb.rq_embed(code.reshape(-1, code.shape[-1]), self._shared_table(), summed=False)
+        out = nb.rq_embed(code.reshape(-1, code.shape[-1]), self._tables(), summed=False)
         out = out.reshape(*code.shape, -1)
         if to_latent_shape:
             out = torch.stack([self.to_latent_shape(out[..., d, :]) for d in range(code.shape[-1])], dim=-2)
@@ -170,11 +180,16 @@ class RQBottleneck(nn.Module):
     def embed_partial_code(self, code, code_idx, decode_type="select"):
         """quantizations.py:336-369"""
         assert code.shape[1:] == self.code_shape and code_idx < code.shape[-1]
+        tabs = self._tables()
         if decode_type == "select":
             sub = code[..., code_idx:code_idx + 1]
+            if isinstance(tabs, list):
+                tabs = tabs[code_idx:code_idx + 1]
         elif decode_type == "add":
             sub = code[..., :code_idx + 1]
+            if isinstance(tabs, list):
+                tabs = tabs[:code_idx + 1]
         else:
             raise NotImplementedError(f"{decode_type} is not implemented in partial decoding")
-        out = nb.rq_embed(sub.reshape(-1, sub.shape[-1]).contiguous(), self._shared_table(), summed=True)
+        out = nb.rq_embed(sub.reshape(-1, sub.shape[-1]).contiguous(), tabs, summed=True)
         return self.to_latent_shape(out.reshape(*code.shape[:-1], -1))

@@ -132,7 +132,12 @@ class RQVAE(Stage1Model):
             b = torch.cat([sd[base + ".q.bias"], sd[base + ".k.bias"], sd[base + ".v.bias"]], 0)
             reg_conv(base + ".qkv.weight", w)
             reg(base + ".qkv.bias", b.float())
-        reg("codebook", self.quantizer._shared_table().float())
+        tabs = self.quantizer._tables()
+        if isinstance(tabs, list):                             # one table per depth (shared_codebook=False)
+            for d, t in enumerate(tabs):
+                reg("codebook.%d" % d, t.float())
+        else:
+            reg("codebook", tabs.float())
         N.check(L.rqb200_vae_finalize(handle), "vae_finalize")
         eng = {"handle": handle, "keep": keep, "ws": {}}
         self._eng[key] = eng
