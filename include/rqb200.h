@@ -227,10 +227,18 @@ int rqb200_dbg_sample_logits(int algo, const float* logits, const float* q, int 
 
 /* rqb200_dbg_conv_tc: one launch of the wgmma implicit-GEMM conv (csrc/conv_tc.cu): X NHWC fp16 [B,H,W,Cin], W OHWI fp16
  * [Cout,ks,ks,Cin], stride 1 "same" padding, out f32 NHWC (+bias, +residual) or NCHW when out_nchw.  X16lo / W16lo
- * (both or neither): the fp16 "lo" halves (value - fp16(value)) -> split-fp16, three products per conv. */
+ * (both or neither): the fp16 "lo" halves (value - fp16(value)) -> split-fp16, three products per conv.
+ * out_nchw bit 1: the operands are bf16 instead of fp16; bits 8..: stride (2: the Downsample conv, H, W the output extent). */
 int rqb200_dbg_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                        const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                        void* stream);
+
+/* rqb200_dbg_conv_tc_gn: rqb200_dbg_conv_tc (NHWC output only) whose epilogue also writes the GroupNorm(32) partial statistics
+ * of its output: gn_part[((b * (H*W/32) + chunk) * 32 + group) * 2 + {0: sum, 1: sum of squares}] as fp64, the chunks of one
+ * (image, group) summing to the group's totals. */
+int rqb200_dbg_conv_tc_gn(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
+                          const float* residual, float* out, double* gn_part, int B, int H, int W, int Cin, int Cout, int ks,
+                          int out_nchw, void* stream);
 
 /* rqb200_dbg_rows_gemm: the large-M GEMM of the batched prefill / forward passes (csrc/conv_tc.cu launch_rows_gemm_tc: persistent
  * 128 x BN tiles, wgmma): out[m,n] = act(sum_k X[m,k] W[n,k] + bias[n]) (+ residual[m,n]).  X [ceil(M/128)*128, K] and

@@ -7,10 +7,16 @@
 //   D[pixel, cout] = sum_{tap, cin} A[pixel + tap, cin] * W[cout, tap, cin]
 //
 //   M = 128 output pixels per tile: a TW x TH x NB box of the NHWC activation tensor (NB > 1 images per tile when the
-//       feature map is smaller than 128 pixels), fetched per filter tap by ONE 4-D TMA load whose coordinates are shifted
-//       by the tap offset -- out-of-range rows/columns are zero-filled by the TMA unit, which IS the conv's zero padding;
-//       no im2col buffer, no halo logic in the kernel.
-//   N = BN output channels (16 | 128 | 256), K = taps x Cin walked in 64-channel slabs (one 128 B swizzled row per pixel).
+//       feature map is smaller than 128 pixels).  Out-of-range rows/columns of a TMA box are zero-filled by the TMA unit,
+//       which IS the conv's zero padding; no im2col buffer.
+//   N = BN output channels (16 | 64 | 128 | 256), K = taps x Cin walked in 64-channel slabs (one 128 B swizzled row per pixel).
+//
+// Two kernels share the layout and the epilogue:
+//   conv3x3_tc_kernel  every 3x3 stride-1 conv.  Input-stationary within a channel slab: ONE TMA box brings the 8 x TH x NB
+//                      tile plus its one-pixel halo, and the nine taps read it as shifted wgmma operands; only the weight
+//                      slabs stream through the ring (see the comment above the kernel).
+//   conv_tc_kernel     1x1 convs, the encoder's stride-2 convs and the rows GEMM: one activation box and one weight slab per
+//                      (tap, slab) k block.
 //
 // Persistent CTAs (grid = #SMs) loop over (pixel tile, cout tile) pairs; warp 8 = TMA producer, warps 0-7 = two consumer
 // warpgroups, each issuing wgmma m64nBNk16 for 64 of the tile's 128 pixels and then running the epilogue (registers -> shared
@@ -26,8 +32,9 @@ namespace rqb {
 struct ConvTcParams {
     int B, H, W, Cin, Cout;        // H,W: OUTPUT extent; the input is H*stride x W*stride
     int ks;                        // 1 or 3
-    int stride;                    // 1: "same" zero padding; 2: no left/top pad, one zero column/row on the right/bottom (F.pad
-                                   // (0,1,0,1) + stride-2 conv, layers.py:50-57) -- both are the tensor map's out-of-bounds fill
+    int stride;                    // 3x3 stride 1: "same" zero padding (conv3x3_tc_kernel); 2: no left/top pad, one zero column/row
+                                   // on the right/bottom (F.pad(0,1,0,1) + stride-2 conv, layers.py:50-57) -- both are the tensor
+                                   // map's out-of-bounds fill
     int TW, TH, NB;                // tile box, TW*TH*NB == 128
     int tiles_x, tiles_y, tiles_b, n_tiles_n;
     const float* bias;
@@ -222,7 +229,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int cslabs = p.Cin / 64;
     const int nkb = p.ks * p.ks * cslabs;
-    const int pad = (p.ks == 3 && p.stride == 1) ? 1 : 0;
     const int sx = p.stride;
     const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_b;
     const int total = m_tiles * p.n_tiles_n;
@@ -251,10 +257,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     const int ky = tap / p.ks, kx = tap % p.ks;
                     tc::mbar_expect_tx(&full[s], STAGE_BYTES);
                     uint8_t* st = smem + s * STAGE_BYTES;
-                    tc::tma_load_4d(st, &tmA, &full[s], c0, x0 * sx + kx - pad, y0 * sx + ky - pad, b0, tc::L2_EVICT_NORMAL);
+                    tc::tma_load_4d(st, &tmA, &full[s], c0, x0 * sx + kx, y0 * sx + ky, b0, tc::L2_EVICT_NORMAL);
                     tc::tma_load_2d(st + OFF_B, &tmB, &full[s], tap * p.Cin + c0, nt * BN, tc::L2_EVICT_LAST);
                     if (PASSES == 3) {
-                        tc::tma_load_4d(st + CT_A_BYTES, &tmAlo, &full[s], c0, x0 * sx + kx - pad, y0 * sx + ky - pad, b0, tc::L2_EVICT_NORMAL);
+                        tc::tma_load_4d(st + CT_A_BYTES, &tmAlo, &full[s], c0, x0 * sx + kx, y0 * sx + ky, b0, tc::L2_EVICT_NORMAL);
                         tc::tma_load_2d(st + OFF_B + B_BYTES, &tmBlo, &full[s], tap * p.Cin + c0, nt * BN, tc::L2_EVICT_LAST);
                     }
                 }
@@ -308,6 +314,166 @@ static int launch_conv_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
     return check_launch("conv_tc");
 }
 
+// ------------------------------------------------------------------------------------------------ 3x3 stride-1 convs
+// The output tile is 8 pixels wide (TW = 8) and TH = 16 rows (TH = 8 and NB = 2 images below 16 rows), so each wgmma core-matrix
+// group -- 8 rows of 128 B -- is one output row.  Per 64-channel slab ONE TMA box loads the (TW + 2) x (TH + 2) x NB input
+// pixels the tile's nine taps touch, at (x0 - 1, y0 - 1): halo pixel (b, hy, hx) sits at ((b (TH + 2) + hy) 10 + hx) 128 B.
+// Tap (dy, dx) of output row oy is then the same smem image read from pixel ((oy + dy) 10 + dx), with a uniform 1280 B group
+// stride (SBO): a shifted descriptor, no reload.  Only the weight slabs [BN x 64] of the nine taps stream through the ring.
+// k order: slab-major, tap-minor.
+//
+// L2 -> smem bytes per 64-channel slab and 128-pixel tile (hi + lo operands): 46 KB halo + 9 x 32 KB weights at BN = 128 ->
+// 166 flop/B, against 96 flop/B (Cout = 128) and 128 flop/B (Cout >= 256, BN = 256) for per-tap A + W reloads; conv_out
+// (BN = 16, Cout = 3): 46 KB + 9 x 4 KB -> 85 flop/B of wgmma work (was 21).
+constexpr int C3_HALO_BYTES = 10 * 10 * 2 * 128;   // per operand; the largest box (TH = 8, NB = 2: 200 pixels; TH = 16: 180)
+
+template <int BN, int FMT, int PASSES>
+__device__ __forceinline__ void c3_mma_kblock(float (&acc)[BN / 2], uint32_t a, uint32_t b, bool first) {
+    constexpr int B_BYTES = BN * 64 * 2;
+    constexpr uint32_t SBO = 10 * 128;                 // one halo row per core-matrix group
+    if (PASSES == 3) {                                 // small terms first, the dominant product last
+#pragma unroll
+        for (int j = 0; j < 4; j++)
+            tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + C3_HALO_BYTES + j * 32, SBO), tc::gmma_desc_k128(b + j * 32),
+                                    (!first || j > 0) ? 1u : 0u);
+#pragma unroll
+        for (int j = 0; j < 4; j++)
+            tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32, SBO), tc::gmma_desc_k128(b + B_BYTES + j * 32), 1u);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; j++)
+        tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32, SBO), tc::gmma_desc_k128(b + j * 32),
+                                (PASSES == 3 || !first || j > 0) ? 1u : 0u);
+}
+
+// Two halo slots (the next slab's halo loads during this slab's taps) and STAGES weight stages.
+// smem: [halo slot: A_hi | A_lo] x 2, [B_hi | B_lo] x STAGES, epilogue staging, barriers.
+template <int BN, int STAGES, int PASSES>
+__global__ void __launch_bounds__(CT_THREADS, 1)
+conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, ConvTcParams p) {
+    constexpr int B_BYTES = BN * 64 * 2;
+    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr int HSLOTS = 2;
+    constexpr int SLOT_BYTES = NOPS * C3_HALO_BYTES;
+    constexpr int STAGE_BYTES = NOPS * B_BYTES;
+    constexpr int CW = BN < 32 ? BN : 32;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* wst = smem + HSLOTS * SLOT_BYTES;
+    float* stage = reinterpret_cast<float*>(wst + STAGES * STAGE_BYTES);           // [128][CW + 4] epilogue staging
+    uint64_t* full = reinterpret_cast<uint64_t*>(stage + 128 * (CW + 4));
+    uint64_t* empty = full + STAGES;
+    uint64_t* hfull = empty + STAGES;
+    uint64_t* hempty = hfull + HSLOTS;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int cslabs = p.Cin / 64;
+    const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_b;
+    const int total = m_tiles * p.n_tiles_n;
+
+    if (warp == 8 && lane == 0) {
+        tc::prefetch_tmap(&tmA);
+        tc::prefetch_tmap(&tmB);
+        // empty[s] / hempty[h]: one arrival per consumer warp once its warpgroup's MMAs reading that buffer have completed
+        for (int s = 0; s < STAGES; s++) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 8); }
+        for (int h = 0; h < HSLOTS; h++) { tc::mbar_init(&hfull[h], 1); tc::mbar_init(&hempty[h], 8); }
+        tc::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        if (lane == 0) {
+            const uint32_t halo_tx = NOPS * 10 * (p.TH + 2) * p.NB * 128;
+            uint32_t it = 0, hit = 0;                          // running weight-stage / halo counters across tiles
+            for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+                const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
+                const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
+                const int x0 = tx * 8, y0 = ty * p.TH, b0 = tb * p.NB;
+                for (int sl = 0; sl < cslabs; sl++, hit++) {
+                    const int c0 = sl * 64;
+                    for (int tap = 0; tap < 9; tap++, it++) {
+                        const int s = it % STAGES;
+                        tc::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+                        tc::mbar_expect_tx(&full[s], STAGE_BYTES);
+                        uint8_t* w = wst + s * STAGE_BYTES;
+                        tc::tma_load_2d(w, &tmB, &full[s], tap * p.Cin + c0, nt * BN, tc::L2_EVICT_LAST);
+                        if (PASSES == 3) tc::tma_load_2d(w + B_BYTES, &tmBlo, &full[s], tap * p.Cin + c0, nt * BN, tc::L2_EVICT_LAST);
+                        if (tap == 0) {                        // the slab's first weights go out before the wait for a halo slot
+                            const int h = hit % HSLOTS;
+                            tc::mbar_wait(&hempty[h], ((hit / HSLOTS) & 1) ^ 1);
+                            tc::mbar_expect_tx(&hfull[h], halo_tx);
+                            uint8_t* a = smem + h * SLOT_BYTES;
+                            tc::tma_load_4d(a, &tmA, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
+                            if (PASSES == 3) tc::tma_load_4d(a + C3_HALO_BYTES, &tmAlo, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
+                        }
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    // ---- consumer warpgroups 0, 1: tile rows [64 wg, 64 wg + 64) = output rows [8 wg, 8 wg + 8) of the tile, all in one image
+    const int wg = warp >> 2, t = threadIdx.x;
+    const int r = t & 127;                                           // epilogue: row of the tile
+    const int rx = r % 8, ry = (r / 8) % p.TH, rb = r / (8 * p.TH);
+    const uint32_t a_wg = (uint32_t)(((8 * wg / p.TH) * (p.TH + 2) + (8 * wg) % p.TH) * 10 * 128);   // tap (0, 0) of row 8 wg
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+    uint32_t it = 0, hit = 0;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+        for (int sl = 0; sl < cslabs; sl++, hit++) {
+            const int h = hit % HSLOTS;
+            tc::mbar_wait(&hfull[h], (hit / HSLOTS) & 1);
+            const uint32_t a0 = tc::smem_u32(smem + h * SLOT_BYTES) + a_wg;
+            for (int tap = 0; tap < 9; tap++, it++) {
+                const int s = it % STAGES;
+                tc::mbar_wait(&full[s], (it / STAGES) & 1);
+                const uint32_t a = a0 + ((tap / 3) * 10 + tap % 3) * 128, b = tc::smem_u32(wst + s * STAGE_BYTES);
+                const bool first = sl == 0 && tap == 0;
+                tc::wgmma_fence();
+                if (p.fmt) c3_mma_kblock<BN, 1, PASSES>(acc, a, b, first);
+                else c3_mma_kblock<BN, 0, PASSES>(acc, a, b, first);
+                tc::wgmma_commit();
+                tc::wgmma_wait<1>();
+                if (!first && lane == 0) {                   // the previous k block's MMAs are complete: free what only it read
+                    tc::mbar_arrive(&empty[(it - 1) % STAGES]);
+                    if (tap == 0) tc::mbar_arrive(&hempty[(hit - 1) % HSLOTS]);
+                }
+            }
+        }
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc);
+        if (lane == 0) {
+            tc::mbar_arrive(&empty[(it - 1) % STAGES]);
+            tc::mbar_arrive(&hempty[(hit - 1) % HSLOTS]);
+        }
+
+        const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
+        const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
+        const int x = tx * 8 + rx, y = ty * p.TH + ry, b = tb * p.NB + rb;
+        const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
+        const bool valid = (x < p.W) && (y < p.H) && (b < p.B);
+        ct_drain<BN, CW, 0>(p, acc, stage, wg, t, nt, tx, ty, tb, b, y, x, pix, valid);
+    }
+}
+
+template <int BN, int STAGES, int PASSES>
+static int launch_conv3x3_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
+                               const ConvTcParams& p, int n_sm, cudaStream_t st) {
+    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr size_t smem = (size_t)2 * NOPS * C3_HALO_BYTES + (size_t)STAGES * NOPS * BN * 128 +
+                            128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 256;
+    static_assert(smem <= 227 * 1024, "conv3x3_tc: shared memory budget");
+    RQB_ENSURE_SMEM(smem, conv3x3_tc_kernel<BN, STAGES, PASSES>);
+    const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
+    const int grid = total < n_sm ? total : n_sm;
+    conv3x3_tc_kernel<BN, STAGES, PASSES><<<grid, CT_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
+    return check_launch("conv3x3_tc");
+}
+
 static int sm_count() {
     static int n = 0;
     if (!n) {
@@ -327,44 +493,80 @@ bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int 
     return pow2(H) && pow2(W);
 }
 
-// the epilogue can emit the output's GroupNorm(32) partial statistics when every epilogue warp's 32 pixels lie in one image and
-// a 16-channel chunk holds whole groups
-bool conv_tc_gn_fusable(int H, int W, int Cout) {
-    const int TW = W < 16 ? W : 16, TH = (128 / TW) < H ? (128 / TW) : H;
-    const int cg = Cout / 32;
-    return Cout % 32 == 0 && (cg == 4 || cg == 8 || cg == 16) && TW * TH >= 32 && (H * W) % 32 == 0;
+// output tile of one CTA, TW x TH x NB = 128 pixels.  3x3 stride 1 (conv3x3_tc_kernel): 8 pixels wide, 16 rows, or 8 rows of
+// NB = 2 images below 16 rows; maps narrower or lower than the tile leave the out-of-range part of it unstored.
+static void conv_tile(int H, int W, int ks, int stride, int& TW, int& TH, int& NB) {
+    if (ks == 3 && stride == 1) {
+        TW = 8;
+        TH = H > 8 ? 16 : 8;
+    } else {
+        TW = W < 16 ? W : 16;
+        TH = (128 / TW) < H ? (128 / TW) : H;
+    }
+    NB = 128 / (TW * TH);
 }
 
-// X: NHWC fp16 [B,H*stride,W*stride,Cin]; Wt: [Cout, ks, ks, Cin] fp16; out fp32 [B,H,W,Cout].  X16lo/W16lo non-null -> split-fp16
-// (3 products).  H, W are the OUTPUT extent.
+// the epilogue can emit the output's GroupNorm(32) partial statistics when the tiles cover the map exactly, every epilogue warp's
+// 32 pixels lie in one image and a 16-channel chunk holds whole groups
+bool conv_tc_gn_fusable(int H, int W, int Cout, int ks, int stride) {
+    int TW, TH, NB;
+    conv_tile(H, W, ks, stride, TW, TH, NB);
+    const int cg = Cout / 32;
+    return Cout % 32 == 0 && (cg == 4 || cg == 8 || cg == 16) && W % TW == 0 && H % TH == 0 && TW * TH >= 32 && (H * W) % 32 == 0;
+}
+
+// X: NHWC 16-bit [B,H*stride,W*stride,Cin]; Wt: [Cout, ks, ks, Cin] 16-bit; out fp32 [B,H,W,Cout].  X16lo/W16lo non-null ->
+// split-fp16 (3 products).  H, W are the OUTPUT extent.  fmt: 0 fp16 operands, 1 bf16.
 int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                    const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
-                   cudaStream_t st, int stride, double* gn_part) {
+                   cudaStream_t st, int stride, double* gn_part, int fmt) {
     ConvTcParams p = {};
-    p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ks = ks; p.stride = stride;
-    p.TW = W < 16 ? W : 16;
-    p.TH = (128 / p.TW) < H ? (128 / p.TW) : H;
-    p.NB = 128 / (p.TW * p.TH);
+    p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ks = ks; p.stride = stride; p.fmt = fmt;
+    conv_tile(H, W, ks, stride, p.TW, p.TH, p.NB);
     if (p.TW * p.TH * p.NB != 128) return fail(RQB200_EINVAL, "conv_tc: feature map extent must be a power of two");
-    p.tiles_x = W / p.TW; p.tiles_y = H / p.TH; p.tiles_b = (int)ceil_div(B, p.NB);
-    const int BN = Cout <= 16 ? 16 : (Cout % 256 == 0 ? 256 : (Cout % 128 == 0 ? 128 : 64));
+    p.tiles_x = (int)ceil_div(W, p.TW); p.tiles_y = (int)ceil_div(H, p.TH); p.tiles_b = (int)ceil_div(B, p.NB);
+    // 3x3: at most 128 output channels per tile.  The weight slabs, not the halo, are most of its L2 traffic, so BN = 256 would
+    // save little (178 vs 166 flop/B) and its 128 accumulators per thread spill; BN = 128 also doubles the CTAs of the 8 x 8 maps.
+    const bool c3 = ks == 3 && stride == 1;
+    const int BN = Cout <= 16 ? 16 : (Cout % 256 == 0 && !c3 ? 256 : (Cout % 128 == 0 ? 128 : 64));
     p.n_tiles_n = (int)ceil_div(Cout, BN);
     p.bias = bias; p.residual = residual; p.out = out; p.out_nchw = out_nchw;
     if (gn_part != nullptr) {
-        if (!conv_tc_gn_fusable(H, W, Cout) || out_nchw) return fail(RQB200_EINVAL, "conv_tc: GroupNorm statistics cannot be fused for this shape");
+        if (!conv_tc_gn_fusable(H, W, Cout, ks, stride) || out_nchw)
+            return fail(RQB200_EINVAL, "conv_tc: GroupNorm statistics cannot be fused for this shape");
         p.gn_part = gn_part;
         p.gn_chunks = H * W / 32;
     }
-    CUtensorMap tmA, tmB;
+    const bool split = X16lo != nullptr && W16lo != nullptr;
+    CUtensorMap tmA, tmB, tmAlo, tmBlo;
+    RQB_TRY(make_tmap_2d(&tmB, W16, 1, (uint64_t)ks * ks * Cin, (uint64_t)Cout, (uint64_t)ks * ks * Cin * 2, 64, (uint32_t)BN));
+    if (split)
+        RQB_TRY(make_tmap_2d(&tmBlo, W16lo, 1, (uint64_t)ks * ks * Cin, (uint64_t)Cout, (uint64_t)ks * ks * Cin * 2, 64, (uint32_t)BN));
+    const int n_sm = sm_count();
+    if (c3) {
+        // the halo box: the tile plus one pixel on every side
+        RQB_TRY(make_tmap_4d_nhwc(&tmA, X16, (uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B, 64, (uint32_t)p.TW + 2,
+                                  (uint32_t)p.TH + 2, (uint32_t)p.NB, 1));
+        if (split) {
+            RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B, 64, (uint32_t)p.TW + 2,
+                                      (uint32_t)p.TH + 2, (uint32_t)p.NB, 1));
+            switch (BN) {
+                case 16: return launch_conv3x3_tc_t<16, 8, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+                case 64: return launch_conv3x3_tc_t<64, 4, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+                default: return launch_conv3x3_tc_t<128, 3, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+            }
+        }
+        switch (BN) {
+            case 16: return launch_conv3x3_tc_t<16, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
+            case 64: return launch_conv3x3_tc_t<64, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
+            default: return launch_conv3x3_tc_t<128, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
+        }
+    }
     RQB_TRY(make_tmap_4d_nhwc(&tmA, X16, (uint64_t)Cin, (uint64_t)W * stride, (uint64_t)H * stride, (uint64_t)B, 64, (uint32_t)p.TW,
                               (uint32_t)p.TH, (uint32_t)p.NB, (uint32_t)stride));
-    RQB_TRY(make_tmap_2d(&tmB, W16, 1, (uint64_t)ks * ks * Cin, (uint64_t)Cout, (uint64_t)ks * ks * Cin * 2, 64, (uint32_t)BN));
-    const int n_sm = sm_count();
-    if (X16lo != nullptr && W16lo != nullptr) {
-        CUtensorMap tmAlo, tmBlo;
+    if (split) {
         RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)W * stride, (uint64_t)H * stride, (uint64_t)B, 64,
                                   (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.NB, (uint32_t)stride));
-        RQB_TRY(make_tmap_2d(&tmBlo, W16lo, 1, (uint64_t)ks * ks * Cin, (uint64_t)Cout, (uint64_t)ks * ks * Cin * 2, 64, (uint32_t)BN));
         switch (BN) {
             case 16: return launch_conv_tc_t<16, 5, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
             case 64: return launch_conv_tc_t<64, 4, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
@@ -533,15 +735,27 @@ int launch_cast_f16(const float* X, void* Y16, void* Y16lo, int B, int H, int W,
 
 }  // namespace rqb
 
-// diagnostic entry point: one conv through the wgmma path (tests/test_gpu_tc.py)
-// out_nchw bit 0: NCHW output; bits 8.. : stride (0/1 -> 1, 2 -> the Downsample conv; then H, W are the OUTPUT extent)
+// diagnostic entry point: one conv through the wgmma path (tests/test_gpu_tc.py, tests/test_gpu_conv3x3.py)
+// out_nchw bit 0: NCHW output; bit 1: bf16 operands; bits 8.. : stride (0/1 -> 1, 2 -> the Downsample conv; then H, W are the
+// OUTPUT extent)
 extern "C" int rqb200_dbg_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                                   const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                                   void* stream) {
     const int stride = (out_nchw >> 8) > 1 ? (out_nchw >> 8) : 1;
     if (!rqb::conv_tc_supported(H, W, Cin, Cout, ks, stride, 0)) return rqb::fail(RQB200_EINVAL, "conv_tc: unsupported shape");
     return rqb::launch_conv_tc(X16, W16, X16lo, W16lo, bias, residual, out, B, H, W, Cin, Cout, ks, out_nchw & 1, (cudaStream_t)stream,
-                               stride, nullptr);
+                               stride, nullptr, (out_nchw >> 1) & 1);
+}
+
+// diagnostic entry point: one conv with the GroupNorm(32) partial statistics of its output emitted by the epilogue
+// (tests/test_gpu_conv3x3.py); gn_part holds B * (H * W / 32) * 32 * 2 doubles.  out_nchw bits as above (NCHW is rejected).
+extern "C" int rqb200_dbg_conv_tc_gn(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
+                                     const float* residual, float* out, double* gn_part, int B, int H, int W, int Cin, int Cout, int ks,
+                                     int out_nchw, void* stream) {
+    const int stride = (out_nchw >> 8) > 1 ? (out_nchw >> 8) : 1;
+    if (!rqb::conv_tc_supported(H, W, Cin, Cout, ks, stride, 0)) return rqb::fail(RQB200_EINVAL, "conv_tc: unsupported shape");
+    return rqb::launch_conv_tc(X16, W16, X16lo, W16lo, bias, residual, out, B, H, W, Cin, Cout, ks, out_nchw & 1, (cudaStream_t)stream,
+                               stride, gn_part, (out_nchw >> 1) & 1);
 }
 
 // diagnostic entry point: the rows GEMM (tests/test_gpu_tc.py).  X must have ceil(M/128)*128 readable rows.

@@ -94,10 +94,13 @@ __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync
 // 1024 B apart: start_address[0,14) = addr>>4, LBO[16,30) unused for swizzled K-major, SBO[32,46) = 1024>>4,
 // base_offset[49,52) = 0, layout_type[62,64) = 1 (SWIZZLE_128B).  Tile base must be 1024 B aligned; stepping along
 // K inside the 128 B row = adding the byte offset to the start address (hardware applies the XOR swizzle).
-__device__ __forceinline__ uint64_t gmma_desc_k128(uint32_t smem_addr) {
+// sbo != 1024: the 8-row groups are `sbo` bytes apart (a multiple of 128) -- conv3x3_tc_kernel reads one output row of a halo
+// tile per group.  The XOR swizzle is a function of the absolute shared-memory address, as in the TMA write, so a group may
+// start at any 128 B row of a 1024 B-aligned TMA box.
+__device__ __forceinline__ uint64_t gmma_desc_k128(uint32_t smem_addr, uint32_t sbo = 1024) {
     uint64_t d = (uint64_t)((smem_addr >> 4) & 0x3FFFu);
     d |= (uint64_t)1 << 16;                    // LBO = 1 (ignored)
-    d |= (uint64_t)(1024 >> 4) << 32;          // SBO
+    d |= (uint64_t)((sbo >> 4) & 0x3FFFu) << 32;   // SBO
     d |= (uint64_t)1 << 62;                    // SWIZZLE_128B
     return d;
 }

@@ -65,7 +65,7 @@ struct VaeRun {
             w_lo = wl->ptr;
             in_lo = in16 == h16[0] ? l16[0] : l16[1];
         }
-        const bool fuse = want_stats && h->gn_fuse && !out_nchw && conv_tc_gn_fusable(Hh, Ww, Cout);
+        const bool fuse = want_stats && h->gn_fuse && !out_nchw && conv_tc_gn_fusable(Hh, Ww, Cout, ks, stride);
         stats_buf = fuse ? out : nullptr;
         stats_chunks = fuse ? Hh * Ww / 32 : 0;
         return launch_conv_tc(in16, w->ptr, in_lo, w_lo, (const float*)b->ptr, resid, out, B, Hh, Ww, Cin, Cout, ks, out_nchw, st, stride,

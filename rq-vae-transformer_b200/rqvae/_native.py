@@ -116,6 +116,7 @@ def lib():
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     L.rqb200_dbg_conv_tc.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    L.rqb200_dbg_conv_tc_gn.argtypes = [C.c_void_p] * 8 + [C.c_int] * 7 + [C.c_void_p]
     _lib = L
     return L
 
@@ -126,7 +127,7 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_ar_forward_workspace_bytes", "rqb200_ar_trace", "rqb200_ar_last_launches", "rqb200_vae_create",
            "rqb200_vae_destroy", "rqb200_vae_set_tensor", "rqb200_vae_finalize", "rqb200_vae_workspace_bytes",
            "rqb200_vae_decode", "rqb200_vae_decode_code", "rqb200_vae_encode", "rqb200_vae_last_launches",
-           "rqb200_dbg_gemm_tc", "rqb200_dbg_conv_tc", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
+           "rqb200_dbg_gemm_tc", "rqb200_dbg_conv_tc", "rqb200_dbg_conv_tc_gn", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
            "rqb200_dbg_rows_gemm", "rqb200_rq_quantize_depthwise", "rqb200_rq_embed_sum_depthwise",
            "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise"]
 
