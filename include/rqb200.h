@@ -105,20 +105,34 @@ typedef struct rqb200_ar_config {
     int32_t flags;                                      /* fast tier: RQB200_AR_* flags                         */
     int32_t split_qkv, split_proj, split_fc1, split_fc2; /* fast tier: split-K factors, 0 = fill the SMs        */
     int32_t codebook_per_depth;                         /* 0: w.codebook is [K,C]; 1: [D,K,C], depth d's table at d*K*C */
+    int32_t embed_variant;                              /* RQB200_EMB_* bits; 0 = the shipped family (see below)  */
 } rqb200_ar_config;
+
+/* rqb200_ar_config.embed_variant: where the body / head tokens come from and which classifier serves depth d
+ * (RQTransformerConfig's input_emb_vqvae, head_emb_vqvae, cumsum_depth_ctx, shared_tok_emb, shared_cls_emb; transformers.py:63-99).
+ * 0 is the shipped family: body token = sum_d input_mlp(e_d) + pos_emb_hw, head token d = head_mlp(sum_{i<d} e_i) + pos_emb_d[d],
+ * one [V,E] classifier, e_i = the RQ-VAE codebook row of code i. */
+#define RQB200_EMB_TOK_INPUT 1        /* input_emb_vqvae = false: body token = sum_d tok_emb(code_d) + pos_emb_hw (no w_in / b_in)     */
+#define RQB200_EMB_TOK_HEAD 2         /* head_emb_vqvae = false: head token d = tok_emb(code_{d-1}) + pos_emb_d[d] (no w_head / b_head) */
+#define RQB200_EMB_NO_CUMSUM 4        /* cumsum_depth_ctx = false (with head_mlp): head token d = head_mlp(e_{d-1}) + pos_emb_d[d]      */
+#define RQB200_EMB_TUPLE 8            /* shared_tok_emb = false: tok_emb is [D*V,E], code d of depth d at row d*V + code (TupleEmbedding) */
+#define RQB200_EMB_CLS_PER_DEPTH 16   /* shared_cls_emb = false: w_cls [D,V,E], b_cls [D,V]; depth d uses slice d (BatchLinear)       */
 
 typedef struct rqb200_ar_weights {
     const float *pos_emb_cond, *pos_emb_hw, *pos_emb_d;  /* [cond_len,E], [H*W,E], [D,E] f32                    */
     const float* cond_emb;                                /* [vocab_cond,E] f32                                  */
-    const void *w_in, *w_head, *w_cls;                    /* [E,C], [E,C], [V,E]; weight dtype                   */
-    const float *b_in, *b_head, *b_cls;
+    const void *w_in, *w_head, *w_cls;                    /* [E,C], [E,C], [V,E] ([D,V,E] with EMB_CLS_PER_DEPTH); weight dtype;
+                                                             w_in / w_head NULL when EMB_TOK_INPUT / EMB_TOK_HEAD replace them */
+    const float *b_in, *b_head, *b_cls;                   /* b_cls [V] or [D,V]                                  */
     const float *cls_ln_w, *cls_ln_b;
-    const float* codebook;                                /* [K,C] or [D,K,C] f32 (model_aux.get_code_emb_with_depth) */
+    const float* codebook;                                /* [K,C] or [D,K,C] f32 (model_aux.get_code_emb_with_depth); NULL when
+                                                             both EMB_TOK_INPUT and EMB_TOK_HEAD are set */
     const rqb200_block_weights* body;                     /* host array [n_body]                                 */
     const rqb200_block_weights* head;                     /* host array [n_head_layers]                          */
     /* optional (cond_len > 1): cond_classifier (transformers.py:100-104) -- only rqb200_ar_forward's cond_logits use it */
     const void* w_ccls;                                   /* [Vc,E], Vc = vocab_cond rounded up to 128 (zero rows); weight dtype; NULL when absent */
     const float *b_ccls, *ccls_ln_w, *ccls_ln_b;
+    const float* tok_emb;                                 /* [V,E] or [D*V,E] (EMB_TUPLE) f32; NULL unless EMB_TOK_INPUT or EMB_TOK_HEAD */
 } rqb200_ar_weights;
 
 typedef struct rqb200_ar rqb200_ar;

@@ -69,6 +69,19 @@ static int run_stack(const rqb200_ar* h, const std::vector<rqb200_block_weights>
     return 0;
 }
 
+// ws.LIN[(b*J + j)*D + d, :] = the body input embedding of code d at position j0 + j: input_mlp(e_d) (transformers.py:219-220), or
+// the tok_emb row of the code (:222, EMB_TOK_INPUT)
+static int body_inputs(const rqb200_ar* h, const int64_t* codes, int B, int j0, int J, ArWs& ws, cudaStream_t st) {
+    const rqb200_ar_config& c = h->cfg;
+    const rqb200_ar_weights& w = h->w;
+    const int E = c.embed_dim, D = c.D, HW = c.H * c.W, C = c.code_dim, K = c.codebook_size;
+    if (c.embed_variant & RQB200_EMB_TOK_INPUT)
+        return launch_code_emb(codes, w.tok_emb, (c.embed_variant & RQB200_EMB_TUPLE) ? (int64_t)c.vocab * E : 0, B, HW, D, c.vocab, E,
+                               j0, J, ws.LIN, st);
+    RQB_TRY(launch_code_emb(codes, w.codebook, c.codebook_per_depth ? (int64_t)K * C : 0, B, HW, D, K, C, j0, J, ws.EMB, st));
+    return launch_linear(ws.EMB, C, w.w_in, c.weight_dtype, w.b_in, nullptr, ws.LIN, E, B * J * D, E, C, 0, st);
+}
+
 // positions [idx0, idx_end) of the raster; resume != 0: no prefill, continue on the caches / context left in this workspace
 static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx0, int idx_end, int resume,
                           float temperature, const int32_t* top_k, const float* top_p, const float* noise,
@@ -79,6 +92,9 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
     const int E = c.embed_dim, D = c.D, HW = c.H * c.W, C = c.code_dim, V = c.vocab, K = c.codebook_size;
     const int wd = c.weight_dtype, cl = c.cond_len, Tb = cl + HW;
     const int64_t cbs = c.codebook_per_depth ? (int64_t)K * C : 0;     // floats between depth d's codebook and depth d+1's
+    const int ev = c.embed_variant;
+    const int64_t tes = (ev & RQB200_EMB_TUPLE) ? (int64_t)V * E : 0;  // floats between depth d's token table and depth d+1's
+    const size_t wsz = wd == RQB200_F32 ? 4 : 2;
     if (B <= 0) return fail(RQB200_EINVAL, "ar_sample: B must be > 0");
     if (idx0 < 0 || idx_end > HW || idx0 > idx_end) return fail(RQB200_EINVAL, "ar_sample: bad position span");
     ArWs ws;
@@ -93,8 +109,7 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
         const int Tn0 = cl + idx0;
         RQB_TRY(launch_cond_token(cond, w.cond_emb, w.pos_emb_cond, B, cl, c.vocab_cond, E, Tn0, ws.X, st));
         if (idx0 > 0) {
-            RQB_TRY(launch_code_emb(out, w.codebook, cbs, B, HW, D, K, C, 0, idx0, ws.EMB, st));
-            RQB_TRY(launch_linear(ws.EMB, C, w.w_in, wd, w.b_in, nullptr, ws.LIN, E, B * idx0 * D, E, C, 0, st));
+            RQB_TRY(body_inputs(h, out, B, 0, idx0, ws, st));
             RQB_TRY(launch_body_token(ws.LIN, w.pos_emb_hw, B, D, E, 0, idx0, cl, Tn0, ws.X, st));
         }
         RQB_TRY(run_stack(h, h->body, ws, B, Tn0, 0, Tb, ws.kc_body, ws.vc_body, st));
@@ -104,8 +119,7 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
     int64_t step = 0;
     for (int idx = idx0; idx < idx_end; idx++) {
         if (idx > idx0 || resume) {   // decode step on the token of position idx-1 (transformers.py:240-242)
-            RQB_TRY(launch_code_emb(out, w.codebook, cbs, B, HW, D, K, C, idx - 1, 1, ws.EMB, st));
-            RQB_TRY(launch_linear(ws.EMB, C, w.w_in, wd, w.b_in, nullptr, ws.LIN, E, B * D, E, C, 0, st));
+            RQB_TRY(body_inputs(h, out, B, idx - 1, 1, ws, st));
             RQB_TRY(launch_body_token(ws.LIN, w.pos_emb_hw, B, D, E, idx - 1, 1, 0, 1, ws.X, st));
             RQB_TRY(run_stack(h, h->body, ws, B, 1, cl + idx - 1, Tb, ws.kc_body, ws.vc_body, st));
             RQB_CUDA(cudaMemcpyAsync(ws.CTX, ws.X, (size_t)B * E * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -113,15 +127,21 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
         for (int d = 0; d < D; d++) {
             if (d == 0) {
                 RQB_TRY(launch_row_add(ws.CTX, E, 0, w.pos_emb_d, B, E, ws.X, st));                         // ctx + pos_emb_d[0]
+            } else if (ev & RQB200_EMB_TOK_HEAD) {
+                RQB_TRY(launch_head_cumsum(out, w.tok_emb, tes, B, HW, D, V, E, idx, d, ws.TOK, st, true));    // tok_emb(code_{d-1})
+                RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
             } else {
-                RQB_TRY(launch_head_cumsum(out, w.codebook, cbs, B, HW, D, K, C, idx, d, ws.EMB, st));         // cumsum_{i<d} e_i
+                // head_mlp(cumsum_{i<d} e_i), or head_mlp(e_{d-1}) without cumsum_depth_ctx
+                RQB_TRY(launch_head_cumsum(out, w.codebook, cbs, B, HW, D, K, C, idx, d, ws.EMB, st, (ev & RQB200_EMB_NO_CUMSUM) != 0));
                 RQB_TRY(launch_linear(ws.EMB, C, w.w_head, wd, w.b_head, nullptr, ws.TOK, E, B, E, C, 0, st));
                 RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
             }
             RQB_TRY(run_stack(h, h->head, ws, B, 1, d, D, ws.kc_head, ws.vc_head, st));                   // head cache restarts at d==0
             RQB_TRY(launch_layernorm(ws.X, E, w.cls_ln_w, w.cls_ln_b, ws.XN, E, B, E, st));
             float* lg = logits_out ? logits_out + step * (int64_t)B * V : ws.LOGITS;
-            RQB_TRY(launch_linear(ws.XN, E, w.w_cls, wd, w.b_cls, nullptr, lg, V, B, V, E, 0, st));
+            // one shared classifier, or depth d's [V,E] slice of the per-depth stack (BatchLinear, transformers.py:278-283)
+            const int64_t cd = (ev & RQB200_EMB_CLS_PER_DEPTH) ? d : 0;
+            RQB_TRY(launch_linear(ws.XN, E, (const char*)w.w_cls + cd * V * E * wsz, wd, w.b_cls + cd * V, nullptr, lg, V, B, V, E, 0, st));
             const float* q = noise ? noise + step * noise_stride : nullptr;
             const int64_t off = (int64_t)idx * D + d;
             RQB_TRY(launch_sample(lg, q, B, V, temperature, top_k[d], top_p[d], out + off, force ? force + off : nullptr,
@@ -147,6 +167,18 @@ rqb200_ar* rqb200_ar_create(const rqb200_ar_config* cfg, const rqb200_ar_weights
     if (cfg->weight_dtype != RQB200_F32 && cfg->weight_dtype != RQB200_BF16 && cfg->weight_dtype != RQB200_F16) {
         rqb::set_error("ar_create: weight dtype");
         return nullptr;
+    }
+    {
+        const int ev = cfg->embed_variant;
+        const bool tok_in = ev & RQB200_EMB_TOK_INPUT, tok_head = ev & RQB200_EMB_TOK_HEAD;
+        const char* bad = nullptr;
+        if (ev & ~(RQB200_EMB_TOK_INPUT | RQB200_EMB_TOK_HEAD | RQB200_EMB_NO_CUMSUM | RQB200_EMB_TUPLE | RQB200_EMB_CLS_PER_DEPTH))
+            bad = "ar_create: unknown embed_variant bits";
+        else if ((tok_in || tok_head) && !w->tok_emb) bad = "ar_create: embed_variant needs tok_emb";
+        else if ((!tok_in && !w->w_in) || (!tok_head && cfg->D > 1 && !w->w_head)) bad = "ar_create: embed_variant needs w_in / w_head";
+        else if (!(tok_in && tok_head) && !w->codebook) bad = "ar_create: embed_variant needs the RQ-VAE codebook";
+        else if (!w->w_cls || !w->b_cls) bad = "ar_create: classifier missing";
+        if (bad) { rqb::set_error(bad); return nullptr; }
     }
     rqb200_ar* h = new rqb200_ar();
     h->cfg = *cfg;

@@ -707,10 +707,11 @@ cond_tok_kernel(const StepState* __restrict__ stt, const float* __restrict__ con
 // position idx (head input, cumsum)                                              (transformers.py:219-225, 250-255)
 // mode < 0 (prefill / forward): grid (B, n_pos); the first -mode codes of position blockIdx.y + pos0, written to row blockIdx.y * B + b
 // code i is looked up in cb + i * cb_dstride (0: one shared codebook; K*C: per-depth codebooks stacked [D,K,C]).
+// last_only: code nd-1 alone instead of codes 0..nd-1 (cumsum_depth_ctx = false: the head input of depth d is e_{d-1}, :250-255).
 // stt is not __restrict__: the previous kernel writes it, and a read-only (non-coherent) load may be scheduled above pdl_wait().
 __global__ void __launch_bounds__(64)
 code_sum_kernel(const StepState* stt, const float* __restrict__ cb, int64_t cb_dstride, int HW, int D, int K, int C,
-                int mode, int pos0, h16* __restrict__ out, int bf) {
+                int mode, int pos0, h16* __restrict__ out, int bf, int last_only) {
     tc::pdl_launch_dependents();
     tc::pdl_wait();
     const int b = blockIdx.x, B = gridDim.x;
@@ -719,7 +720,7 @@ code_sum_kernel(const StepState* stt, const float* __restrict__ cb, int64_t cb_d
     h16* o = out + ((int64_t)blockIdx.y * B + b) * C;
     for (int c = threadIdx.x; c < C; c += 64) {
         float a = 0.f;
-        for (int i = 0; i < nd; i++) {
+        for (int i = last_only ? nd - 1 : 0; i < nd; i++) {
             int64_t k = stt->codes[((int64_t)b * HW + pos) * D + i];
             k = k < 0 ? 0 : (k >= K ? K - 1 : k);
             a += cb[i * cb_dstride + k * C + c];
@@ -728,6 +729,46 @@ code_sum_kernel(const StepState* stt, const float* __restrict__ cb, int64_t cb_d
     }
 }
 static int64_t cb_dstride(const rqb200_ar_config& c) { return c.codebook_per_depth ? (int64_t)c.codebook_size * c.code_dim : 0; }
+
+// token embeddings straight into the fp32 residual stream (input_emb_vqvae / head_emb_vqvae = false, transformers.py:222,257):
+//   out[row, :] = ((tok_d0[k_d0] + tok_d0+1[k_d0+1]) + ...) + pos[p * pos_stride]      over the codes d0 .. d0+nd-1 of position p,
+// tok_i = tok + i * tok_dstride (0: one shared [V,E] table; V*E: the TupleEmbedding's per-depth blocks).  The position:
+//   where 0: stt->idx - 1 (the body step's token),  1: stt->idx (a head step's token),  2: pos0 + blockIdx.y (batched rows),
+// row = blockIdx.y * B + b (token-major, like code_sum_kernel).  The body token sums all D codes with pos = pos_emb_hw (pos_stride E);
+// the head token of depth d is code d-1 alone with pos = pos_emb_d + d*E (pos_stride 0).  E % 4 == 0.
+// stt is not __restrict__ (see code_sum_kernel).
+__global__ void __launch_bounds__(128)
+tok_gather_kernel(const StepState* stt, const float* __restrict__ tok, int64_t tok_dstride, int HW, int D, int V, int E, int d0, int nd,
+                  int where, int pos0, const float* __restrict__ pos, int64_t pos_stride, float* __restrict__ out) {
+    tc::pdl_launch_dependents();
+    tc::pdl_wait();
+    const int b = blockIdx.x, B = gridDim.x;
+    const int p = where == 2 ? pos0 + blockIdx.y : (where == 0 ? stt->idx - 1 : stt->idx);
+    const int64_t* kr = stt->codes + ((int64_t)b * HW + p) * D;
+    int64_t rows[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+        if (i < nd) {
+            int64_t k = kr[d0 + i];
+            k = k < 0 ? 0 : (k >= V ? V - 1 : k);
+            rows[i] = (d0 + i) * tok_dstride + k * E;
+        }
+    const float4* pr = reinterpret_cast<const float4*>(pos + (int64_t)p * pos_stride);
+    float4* o = reinterpret_cast<float4*>(out + ((int64_t)blockIdx.y * B + b) * E);
+    for (int e4 = threadIdx.x; e4 < E / 4; e4 += 128) {
+        float4 a = reinterpret_cast<const float4*>(tok + rows[0])[e4];
+#pragma unroll
+        for (int i = 1; i < 8; i++)
+            if (i < nd) {
+                const float4 t = reinterpret_cast<const float4*>(tok + rows[i])[e4];
+                a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
+            }
+        const float4 q = pr[e4];
+        a.x += q.x; a.y += q.y; a.z += q.z; a.w += q.w;
+        o[e4] = a;
+    }
+}
+static int64_t tok_dstride(const rqb200_ar_config& c) { return (c.embed_variant & RQB200_EMB_TUPLE) ? (int64_t)c.vocab * c.embed_dim : 0; }
 // bookkeeping: which graph just ran decides what advances
 __global__ void advance_kernel(StepState* stt, int ds, int didx, int dstep) {
     tc::pdl_launch_dependents();
@@ -764,6 +805,7 @@ struct ArFast {
     std::vector<rqb200_block_weights> body, head;
     std::vector<FastLayer> lbody, lhead;
     CUtensorMap tm_win, tm_whead, tm_cls, tm_ccls;
+    CUtensorMap tm_cls_d[8];             // RQB200_EMB_CLS_PER_DEPTH: depth d's [V,E] slice of w_cls
     int bf = 0;                          // 16-bit format: 0 fp16, 1 bf16
     // per (workspace, B) state
     void* ws_base = nullptr;
@@ -968,9 +1010,13 @@ static int record_body(ArFast& f, FastWs& ws, bool cond_token, cudaStream_t st) 
     if (cond_token) {
         RQB_TRY(launch_pdl(cond_tok_kernel, dim3(B, 1), dim3(256), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.cond_emb,
                            w.pos_emb_cond, c.cond_len, c.vocab_cond, E, ws.XB));
+    } else if (c.embed_variant & RQB200_EMB_TOK_INPUT) {
+        // x = sum_d tok_emb(code_d) + pos_emb_hw[idx-1]           (transformers.py:222,225)
+        RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, 1), dim3(128), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.tok_emb,
+                           tok_dstride(c), HW, c.D, c.vocab, E, 0, c.D, 0, 0, w.pos_emb_hw, (int64_t)E, ws.XB));
     } else {
         RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
-                           cb_dstride(c), HW, c.D, c.codebook_size, c.code_dim, 0, 0, ws.S, f.bf));
+                           cb_dstride(c), HW, c.D, c.codebook_size, c.code_dim, 0, 0, ws.S, f.bf, 0));
         // x = W_in (sum_d e_d) + D b_in + pos_emb_hw[idx-1]       (bias counted D times, transformers.py:220,225)
         RQB_TRY(gemm(f, "w_in", f.tm_win, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_in, (float)c.D, ws.XB, nullptr,
                      w.pos_emb_hw - E /* row idx-1 */, 0, &ws.state->idx, E, st));
@@ -990,15 +1036,27 @@ static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st)
             RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, w.pos_emb_d, ws.XB, ws.kc_head, ws.vc_head, D, nullptr, 0, w.cls_ln_w,
                                w.cls_ln_b, st));
         } else {
-            RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
-                               cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf));
-            RQB_TRY(gemm(f, "w_head", f.tm_whead, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
-                         w.pos_emb_d + (int64_t)d * E, 0, nullptr, 0, st));
+            if (c.embed_variant & RQB200_EMB_TOK_HEAD) {
+                // token = tok_emb(code_{d-1}) + pos_emb_d[d]                                    (transformers.py:257,267)
+                RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, 1), dim3(128), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
+                                   w.tok_emb, tok_dstride(c), HW, D, c.vocab, E, d - 1, 1, 1, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
+                                   ws.XH));
+            } else {
+                // token = head_mlp(sum_{i<d} e_i, or e_{d-1} alone) + pos_emb_d[d]              (transformers.py:250-255,267)
+                RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
+                                   cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf,
+                                   (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
+                RQB_TRY(gemm(f, "w_head", f.tm_whead, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
+                             w.pos_emb_d + (int64_t)d * E, 0, nullptr, 0, st));
+            }
             RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, nullptr, ws.XH, ws.kc_head, ws.vc_head, D, nullptr, d, w.cls_ln_w,
                                w.cls_ln_b, st));
         }
         // classifier: LN(x) (fused into the stack's last launch) -> logits                       (transformers.py:278-285)
-        RQB_TRY(gemm(f, "cls", f.tm_cls, f.tx_xn, V, E, B, 1, GT_F32, w.b_cls, 1.f, ws.LOGITS, nullptr, nullptr, 0, nullptr, 0, st));
+        // per-depth classifiers (BatchLinear): depth d's [V,E] slice and bias row
+        const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
+        RQB_TRY(gemm(f, "cls", pd ? f.tm_cls_d[d] : f.tm_cls, f.tx_xn, V, E, B, 1, GT_F32, w.b_cls + (pd ? (int64_t)d * V : 0), 1.f,
+                     ws.LOGITS, nullptr, nullptr, 0, nullptr, 0, st));
         if (with_logits)
             RQB_TRY(launch_pdl(logits_copy_kernel, dim3(64), dim3(256), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
                                (const float*)ws.LOGITS, d, (int64_t)B * V));
@@ -1083,9 +1141,12 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
     };
     int rc = mk(body, f->lbody);
     if (!rc) rc = mk(head, f->lhead);
-    if (!rc) rc = make_tmap_weight(&f->tm_win, w.w_in, E, cfg.code_dim);
-    if (!rc) rc = make_tmap_weight(&f->tm_whead, w.w_head, E, cfg.code_dim);
+    if (!rc && w.w_in) rc = make_tmap_weight(&f->tm_win, w.w_in, E, cfg.code_dim);
+    if (!rc && w.w_head) rc = make_tmap_weight(&f->tm_whead, w.w_head, E, cfg.code_dim);
     if (!rc) rc = make_tmap_weight(&f->tm_cls, w.w_cls, cfg.vocab, E);
+    if (cfg.embed_variant & RQB200_EMB_CLS_PER_DEPTH)
+        for (int d = 0; d < cfg.D && !rc; d++)
+            rc = make_tmap_weight(&f->tm_cls_d[d], (const char*)w.w_cls + (size_t)d * cfg.vocab * E * 2, cfg.vocab, E);
     if (!rc && w.w_ccls) rc = make_tmap_weight(&f->tm_ccls, w.w_ccls, (cfg.vocab_cond + 127) / 128 * 128, E);
     if (rc) { delete f; return nullptr; }
     for (int i = 0; i <= G_COUNT; i++) f->tr_graph_base[i] = i * (TR_CAP / G_COUNT);
@@ -1187,12 +1248,16 @@ static int body_tokens_batched(ArFast& f, const StepState* state, float* X, h16*
     RQB_TRY(launch_pdl(cond_tok_kernel, dim3(B, std::min(T, cl)), dim3(256), (size_t)0, st, false, state, w.cond_emb, w.pos_emb_cond, cl,
                        c.vocab_cond, E, X));
     const int n_code = T - cl;       // code tokens of positions 0 .. n_code-1
-    if (n_code > 0) {
+    if (n_code > 0 && (c.embed_variant & RQB200_EMB_TOK_INPUT)) {
+        // row (j, b) = sum_d tok_emb(code_d of position j) + pos_emb_hw[j]                   (:222,225)
+        RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, n_code), dim3(128), (size_t)0, st, false, state, w.tok_emb, tok_dstride(c), HW, c.D,
+                           c.vocab, E, 0, c.D, 2, 0, w.pos_emb_hw, (int64_t)E, X + (int64_t)cl * B * E));
+    } else if (n_code > 0) {
         const int64_t Mc = (int64_t)B * n_code;
         CUtensorMap tx_s;
         RQB_TRY(make_tmap_2d(&tx_s, S, 1, c.code_dim, Mc, (uint64_t)c.code_dim * 2, 64, gemm_tc_bn((int)std::min<int64_t>(Mc, 256))));
         RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, n_code), dim3(64), (size_t)0, st, false, state, w.codebook, cb_dstride(c), HW, c.D,
-                           c.codebook_size, c.code_dim, -c.D, 0, S, f.bf));
+                           c.codebook_size, c.code_dim, -c.D, 0, S, f.bf, 0));
         GemmTcParams p = gemm_base(f, E, c.code_dim, (int)Mc, 1, GT_F32);
         p.bias = w.b_in; p.bias_scale = (float)c.D; p.out = X + (int64_t)cl * B * E;
         p.residual = w.pos_emb_hw; p.ld_res = E; p.res_div = B;          // row (j, b) gets pos_emb_hw[j]
@@ -1290,8 +1355,15 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
         CUtensorMap tx_s;
         RQB_TRY(make_tmap_2d(&tx_s, ws.S, 1, c.code_dim, G, (uint64_t)c.code_dim * 2, 64, gemm_tc_bn(std::min(G, 256))));
         for (int d = 1; d < D; d++) {
+            if (c.embed_variant & RQB200_EMB_TOK_HEAD) {        // tok_emb(code_{d-1}) + pos_emb_d[d]        (:164,177)
+                RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, HW), dim3(128), (size_t)0, st, false, (const StepState*)ws.state, w.tok_emb,
+                                   tok_dstride(c), HW, D, V, E, d - 1, 1, 2, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
+                                   ws.HX + (int64_t)d * G * E));
+                continue;
+            }
             RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, HW), dim3(64), (size_t)0, st, false, (const StepState*)ws.state, w.codebook,
-                               cb_dstride(c), HW, D, c.codebook_size, c.code_dim, -d, 0, ws.S, f->bf));
+                               cb_dstride(c), HW, D, c.codebook_size, c.code_dim, -d, 0, ws.S, f->bf,
+                               (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
             GemmTcParams p = gemm_base(*f, E, c.code_dim, G, 1, GT_F32);
             p.bias = w.b_head; p.out = ws.HX + (int64_t)d * G * E; p.residual = w.pos_emb_d + (int64_t)d * E; p.ld_res = 0;
             RQB_TRY(launch_gemm_tc(f->tm_whead, tx_s, p, false, st));
@@ -1299,15 +1371,28 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
         BatchBufs hb = {ws.HX, ws.XN, ws.QKV, ws.ATT, ws.H};
         RQB_TRY(stack_batched(*f, f->head, f->lhead, hb, G, D, nullptr, nullptr, 0, D, st));
         // classifier                                                                                   (:181-183)
-        CUtensorMap tx;
-        RQB_TRY(make_tmap_2d(&tx, ws.XN, 1, E, Mh, (uint64_t)E * 2, 64, gemm_tc_bn((int)std::min<int64_t>(Mh, 256))));
         RQB_TRY(ln(*f, "", (int)Mh, ws.HX, nof, 0, nof, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, st));
-        if (Mh > 256) {
-            RQB_TRY(launch_rows_gemm_tc(ws.XN, w.w_cls, w.b_cls, nullptr, logits_out, nullptr, 0, f->bf, Mh, V, E, st));
-        } else {
-            GemmTcParams p = gemm_base(*f, V, E, (int)Mh, 1, GT_F32);
-            p.bias = w.b_cls; p.out = logits_out;
-            RQB_TRY(launch_gemm_tc(f->tm_cls, tx, p, false, st));
+        // one launch over all Mh rows, or (per-depth classifiers) one per depth over that depth's G rows d*G .. (d+1)*G-1, the rows
+        // GEMM or the weight streamer picked by the rows each launch covers.  (The rows GEMM reads whole 128-row tiles -- past a
+        // slice into the next depth's rows, past the last one into forward_layout's +128 -- and stores only the slice's rows.)
+        const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
+        const int n_cls = pd ? D : 1;
+        const int64_t Mc = pd ? G : Mh;
+        const size_t wsz = 2;
+        for (int d = 0; d < n_cls; d++) {
+            const h16* xn = ws.XN + (int64_t)d * Mc * E;
+            const void* wc = (const char*)w.w_cls + (size_t)d * V * E * wsz;
+            const float* bc = w.b_cls + (int64_t)d * V;
+            float* lo = logits_out + (int64_t)d * Mc * V;
+            if (Mc > 256) {
+                RQB_TRY(launch_rows_gemm_tc(xn, wc, bc, nullptr, lo, nullptr, 0, f->bf, Mc, V, E, st));
+            } else {
+                CUtensorMap tx;
+                RQB_TRY(make_tmap_2d(&tx, xn, 1, E, Mc, (uint64_t)E * 2, 64, gemm_tc_bn((int)Mc)));
+                GemmTcParams p = gemm_base(*f, V, E, (int)Mc, 1, GT_F32);
+                p.bias = bc; p.out = lo;
+                RQB_TRY(launch_gemm_tc(pd ? f->tm_cls_d[d] : f->tm_cls, tx, p, false, st));
+            }
         }
         return 0;
     }();

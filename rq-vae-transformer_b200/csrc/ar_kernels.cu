@@ -213,17 +213,19 @@ __global__ void cond_token_kernel(const int64_t* __restrict__ cond, const float*
     for (int e = threadIdx.x; e < E; e += blockDim.x)
         X[((int64_t)b * Tn + s) * E + e] = cond_emb[c * E + e] + pos_cond[(int64_t)s * E + e];
 }
-// head input for depth d >= 1: out[b,:] = e_0 + e_1 + ... + e_{d-1} (sequential, torch.cumsum order)
+// head input for depth d >= 1: out[b,:] = e_0 + e_1 + ... + e_{d-1} (sequential, torch.cumsum order); last_only: e_{d-1} alone
+// (cumsum_depth_ctx = false, or the row of a token embedding table when cb is tok_emb)
 __global__ void head_cumsum_kernel(const int64_t* __restrict__ codes, const float* __restrict__ cb, int64_t cb_dstride, int HW, int D,
-                                   int K, int C, int j, int d, float* __restrict__ out) {
+                                   int K, int C, int j, int d, int last_only, float* __restrict__ out) {
     int b = blockIdx.x;
+    const int i0 = last_only ? d - 1 : 0;
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
         float a = 0.f;
-        for (int i = 0; i < d; i++) {
+        for (int i = i0; i < d; i++) {
             int64_t k = codes[((int64_t)b * HW + j) * D + i];
             k = k < 0 ? 0 : (k >= K ? K - 1 : k);
             float e = cb[i * cb_dstride + k * C + c];
-            a = (i == 0) ? e : a + e;
+            a = (i == i0) ? e : a + e;
         }
         out[(int64_t)b * C + c] = a;
     }
@@ -254,8 +256,8 @@ int launch_cond_token(const int64_t* cond, const float* cond_emb, const float* p
     return check_launch("cond_token");
 }
 int launch_head_cumsum(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j, int d,
-                       float* out, cudaStream_t st) {
-    head_cumsum_kernel<<<B, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j, d, out);
+                       float* out, cudaStream_t st, bool last_only) {
+    head_cumsum_kernel<<<B, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j, d, last_only ? 1 : 0, out);
     return check_launch("head_cumsum");
 }
 int launch_row_add(const float* in, int64_t in_row_stride, int64_t in_off, const float* pos, int B, int E, float* out,

@@ -42,8 +42,9 @@ int launch_body_token(const float* lin, const float* pos_hw, int B, int D, int E
                       cudaStream_t st);
 int launch_cond_token(const int64_t* cond, const float* cond_emb, const float* pos_cond, int B, int cond_len, int vocab_cond,
                       int E, int Tn, float* X, cudaStream_t st);
+// last_only: code d-1 alone instead of the sum over codes 0..d-1
 int launch_head_cumsum(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j, int d,
-                       float* out, cudaStream_t st);
+                       float* out, cudaStream_t st, bool last_only = false);
 int launch_row_add(const float* in, int64_t in_row_stride, int64_t in_off, const float* pos, int B, int E, float* out,
                    cudaStream_t st);
 // conv_kernels.cu

@@ -11,6 +11,8 @@ OK, EINVAL, ECUDA, ENODEV, EWORKSPACE, ESTATE = 0, -1, -2, -3, -4, -5
 F32, BF16, F16 = 0, 1, 2
 MODE_EXACT, MODE_FAST = 0, 1
 AR_NO_GRAPH, AR_NO_PDL, AR_TRACE, AR_SEQUENTIAL_PREFILL = 1, 2, 4, 32
+# rqb200_ar_config.embed_variant bits (0 = the shipped family)
+EMB_TOK_INPUT, EMB_TOK_HEAD, EMB_NO_CUMSUM, EMB_TUPLE, EMB_CLS_PER_DEPTH = 1, 2, 4, 8, 16
 _DT = {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16}
 
 c_f32p, c_i64p, c_vp = C.c_void_p, C.c_void_p, C.c_void_p
@@ -25,14 +27,14 @@ class ArConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("embed_dim", "n_head", "n_body", "n_head_layers", "vocab", "H", "W", "D",
                                          "vocab_cond", "cond_len", "code_dim", "codebook_size", "mode", "weight_dtype",
                                          "flags", "split_qkv", "split_proj", "split_fc1", "split_fc2",
-                                         "codebook_per_depth")]
+                                         "codebook_per_depth", "embed_variant")]
 
 
 class ArWeights(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("pos_emb_cond", "pos_emb_hw", "pos_emb_d", "cond_emb", "w_in", "w_head", "w_cls",
                                           "b_in", "b_head", "b_cls", "cls_ln_w", "cls_ln_b", "codebook")] + \
                [("body", C.POINTER(BlockWeights)), ("head", C.POINTER(BlockWeights))] + \
-               [(n, C.c_void_p) for n in ("w_ccls", "b_ccls", "ccls_ln_w", "ccls_ln_b")]
+               [(n, C.c_void_p) for n in ("w_ccls", "b_ccls", "ccls_ln_w", "ccls_ln_b", "tok_emb")]
 
 
 class VaeConfig(C.Structure):

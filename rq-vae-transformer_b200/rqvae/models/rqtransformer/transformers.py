@@ -20,6 +20,7 @@ import torch.nn as nn
 
 from ... import _native as N
 from ..interfaces import Stage2Model
+from .primitives import BatchLinear, LogitMask, TupleEmbedding
 
 
 class _Holder(nn.Module):
@@ -65,20 +66,22 @@ class RQTransformer(Stage2Model):
         if isinstance(config.vocab_size, int):
             config.vocab_size = [config.vocab_size] * config.block_size[2]
         vs = list(config.vocab_size)
-        if not (config.shared_tok_emb and config.shared_cls_emb and config.input_emb_vqvae and config.head_emb_vqvae
-                and config.cumsum_depth_ctx):
-            raise NotImplementedError("rqb200: only the shipped configuration family is implemented (shared_tok_emb, "
-                                      "shared_cls_emb, input_emb_vqvae, head_emb_vqvae, cumsum_depth_ctx all true)")
-        assert [vs[0]] * len(vs) == vs
+        if config.shared_tok_emb or config.shared_cls_emb:
+            assert [vs[0]] * len(vs) == vs, "shared token / classifier embeddings need one vocabulary size for every depth"
         self.vocab_size = vs
         E = config.embed_dim
         self.vocab_size_cond = max(config.vocab_size_cond, 1)
         self.block_size_cond = max(config.block_size_cond, 1)
         assert not (self.block_size_cond > 1 and self.vocab_size_cond == 1)
+        # modules in the reference's order (transformers.py:60-105): same state_dict order, same draws under a seed
         self.cond_emb = nn.Embedding(self.vocab_size_cond, E)
-        self.tok_emb = None
-        self.input_mlp = nn.Linear(config.input_embed_dim, E)
-        self.head_mlp = nn.Linear(config.input_embed_dim, E)
+        self.tok_emb, self.input_mlp, self.head_mlp = None, None, None
+        if config.input_emb_vqvae:
+            self.input_mlp = nn.Linear(config.input_embed_dim, E)
+        if config.head_emb_vqvae:
+            self.head_mlp = nn.Linear(config.input_embed_dim, E)
+        if not (config.input_emb_vqvae and config.head_emb_vqvae):
+            self.tok_emb = nn.Embedding(vs[0], E) if config.shared_tok_emb else TupleEmbedding(vs, E)
         self.pos_emb_cond = nn.Parameter(torch.zeros(1, self.block_size_cond, E))
         self.pos_emb_hw = nn.Parameter(torch.zeros(1, self.block_size[0] * self.block_size[1], E))
         self.pos_emb_d = nn.Parameter(torch.zeros(1, self.block_size[2], E))
@@ -86,7 +89,9 @@ class RQTransformer(Stage2Model):
             p.data.normal_(mean=0.0, std=0.02)
         self.body_transformer = _Stack(config.body)
         self.head_transformer = _Stack(config.head)
-        self.classifier = nn.Sequential(OrderedDict([("layer_norm", nn.LayerNorm(E)), ("linear", nn.Linear(E, vs[0]))]))
+        cls = nn.Linear(E, vs[0]) if config.shared_cls_emb else BatchLinear(self.block_size[2], E, max(vs))
+        self.classifier = nn.Sequential(OrderedDict([("layer_norm", nn.LayerNorm(E)), ("linear", cls),
+                                                     ("logit_mask", LogitMask(vs, value=-1e6))]))
         if config.block_size_cond > 1:
             self.cond_classifier = nn.Sequential(OrderedDict([("layer_norm", nn.LayerNorm(E)),
                                                               ("linear", nn.Linear(E, config.vocab_size_cond))]))
@@ -123,9 +128,32 @@ class RQTransformer(Stage2Model):
             p = "fast" if amp else "exact"
         return N.MODE_FAST if p == "fast" else N.MODE_EXACT
 
+    def _embed_variant(self):
+        """rqb200_ar_config.embed_variant of this model's five embedding / classifier switches (0: the shipped family)"""
+        c = self.config
+        v = 0 if c.input_emb_vqvae else N.EMB_TOK_INPUT
+        v |= 0 if c.head_emb_vqvae else N.EMB_TOK_HEAD
+        v |= N.EMB_NO_CUMSUM if (c.head_emb_vqvae and not c.cumsum_depth_ctx) else 0
+        v |= N.EMB_TUPLE if (self.tok_emb is not None and not c.shared_tok_emb) else 0
+        v |= 0 if c.shared_cls_emb else N.EMB_CLS_PER_DEPTH
+        return v
+
+    def _check_computable(self):
+        if [self.vocab_size[0]] * len(self.vocab_size) != self.vocab_size:
+            raise NotImplementedError("rqb200: per-depth vocabularies of different sizes (%s) can be built and loaded but not sampled "
+                                      "or evaluated: the reference's LogitMask indexes the logits of one depth as if they held all "
+                                      "depths and raises IndexError in both sample and forward, so there is no behaviour to "
+                                      "reproduce" % (self.vocab_size,))
+
     def _codebook_of(self, model_aux, depth):
         """the table(s) behind model_aux.get_code_emb_with_depth (transformers.py:109-111): the [K,C] tensor of a shared codebook,
-        or the list of the D per-depth [K,C] tables, each K equal to the vocabulary"""
+        or the list of the D per-depth [K,C] tables, each K equal to the vocabulary.  None when the model embeds its codes with its
+        own tok_emb only (input_emb_vqvae and head_emb_vqvae both false): model_aux is not needed then."""
+        if self.input_mlp is None and self.head_mlp is None:
+            return None
+        if model_aux is None:
+            raise ValueError("rqb200: this model embeds codes through model_aux's codebooks (input_emb_vqvae or head_emb_vqvae "
+                             "is true): pass the RQ-VAE as model_aux")
         q = getattr(model_aux, "quantizer", None)
         if q is not None and hasattr(q, "_tables"):
             tabs = q._tables()
@@ -140,11 +168,15 @@ class RQTransformer(Stage2Model):
         raise NotImplementedError("rqb200: model_aux must be an RQ-VAE (its quantizer holds the codebooks)")
 
     def _engine(self, codebook, mode, slot=0):
-        """codebook: one [K,C] table or a list of D per-depth tables.  Engines are keyed by the tables' storage and rebuilt when
-        any of them is written in place (per-depth tables are stacked into one [D,K,C] copy per engine build)."""
+        """codebook: one [K,C] table, a list of D per-depth tables, or None (a model that needs none).  Engines are keyed by the
+        tables' storage and rebuilt when any of them is written in place (per-depth tables are stacked into one [D,K,C] copy per
+        engine build)."""
         dev = self.pos_emb_hw.device
         per_depth = isinstance(codebook, list)
-        if per_depth:
+        if codebook is None:
+            fp = (N.param_fingerprint(self), None)
+            cb_id = None
+        elif per_depth:
             fp = (N.param_fingerprint(self), tuple(t._version for t in codebook))
             cb_id = tuple(t.data_ptr() for t in codebook)
         else:
@@ -163,6 +195,7 @@ class RQTransformer(Stage2Model):
         if key in self._eng:
             return self._eng[key]
         N.require_cuda(self.pos_emb_hw, *(codebook if per_depth else [codebook]))
+        self._check_computable()
         L = N.lib()
         wdt = N.fast_dtype() if mode == N.MODE_FAST else torch.float32
         opts = N.ar_engine_options() if mode == N.MODE_FAST else {"flags": 0, "splits": [0, 0, 0, 0]}
@@ -198,22 +231,41 @@ class RQTransformer(Stage2Model):
         cfg.n_body, cfg.n_head_layers = len(self.body_transformer.blocks), len(self.head_transformer.blocks)
         cfg.vocab, cfg.H, cfg.W, cfg.D = self.vocab_size[0], self.block_size[0], self.block_size[1], self.block_size[2]
         cfg.vocab_cond, cfg.cond_len = self.vocab_size_cond, self.block_size_cond
-        table0 = codebook[0] if per_depth else codebook
-        cfg.code_dim, cfg.codebook_size = table0.shape[1], table0.shape[0]
+        if codebook is None:
+            cfg.code_dim, cfg.codebook_size = 64, self.vocab_size[0]        # (unused: no code goes through a codebook)
+        else:
+            table0 = codebook[0] if per_depth else codebook
+            cfg.code_dim, cfg.codebook_size = table0.shape[1], table0.shape[0]
         cfg.codebook_per_depth = int(per_depth)
         cfg.mode, cfg.weight_dtype = mode, N._DT[wdt]
         cfg.flags = opts["flags"]
         cfg.split_qkv, cfg.split_proj, cfg.split_fc1, cfg.split_fc2 = opts["splits"]
+        cfg.embed_variant = self._embed_variant()
         if c.head.block.n_head != c.body.block.n_head:
             raise NotImplementedError("rqb200: body and head stacks must share n_head")
         w = N.ArWeights()
         w.pos_emb_cond, w.pos_emb_hw, w.pos_emb_d = f32(self.pos_emb_cond), f32(self.pos_emb_hw), f32(self.pos_emb_d)
         w.cond_emb = f32(self.cond_emb.weight)
-        w.w_in, w.b_in = wt(self.input_mlp.weight), f32(self.input_mlp.bias)
-        w.w_head, w.b_head = wt(self.head_mlp.weight), f32(self.head_mlp.bias)
-        w.w_cls, w.b_cls = wt(self.classifier.linear.weight), f32(self.classifier.linear.bias)
+        if self.input_mlp is not None:
+            w.w_in, w.b_in = wt(self.input_mlp.weight), f32(self.input_mlp.bias)
+        if self.head_mlp is not None:
+            w.w_head, w.b_head = wt(self.head_mlp.weight), f32(self.head_mlp.bias)
+        if self.tok_emb is not None:
+            te = self.tok_emb
+            if isinstance(te, TupleEmbedding):
+                V, D = self.vocab_size[0], self.block_size[2]
+                if te.offsets.tolist() != [d * V for d in range(D)]:
+                    raise ValueError("rqb200: tok_emb.offsets must be [0, V, 2V, ...] (got %s)" % te.offsets.tolist())
+            w.tok_emb = f32(te.weight)
+        lin = self.classifier.linear
+        if isinstance(lin, BatchLinear):
+            # [D,E,V] (input-major) -> one [D,V,E] copy per engine build: depth d's classifier is a row-major [V,E] slice
+            w.w_cls, w.b_cls = wt(lin.weight.detach().transpose(1, 2)), f32(lin.bias)
+        else:
+            w.w_cls, w.b_cls = wt(lin.weight), f32(lin.bias)
         w.cls_ln_w, w.cls_ln_b = f32(self.classifier.layer_norm.weight), f32(self.classifier.layer_norm.bias)
-        w.codebook = f32(torch.stack(codebook)) if per_depth else f32(codebook)
+        if codebook is not None:
+            w.codebook = f32(torch.stack(codebook)) if per_depth else f32(codebook)
         if hasattr(self, "cond_classifier") and mode == N.MODE_FAST:
             pad = -self.vocab_size_cond % 128            # classifier rows padded with zeros up to the 128-feature wgmma tile
             pw = torch.nn.functional.pad(self.cond_classifier.linear.weight.detach(), (0, 0, 0, pad))
@@ -267,6 +319,7 @@ class RQTransformer(Stage2Model):
         H, W, D = self.block_size
         B = partial.shape[0]
         dev = self.pos_emb_hw.device
+        self._check_computable()
         N.require_cuda(partial, cond, self.pos_emb_hw)
         ks, ps = self._lists(top_k, top_p)
         codebook = self._codebook_of(model_aux, D)
@@ -378,6 +431,7 @@ class RQTransformer(Stage2Model):
         Fast tier (amp=True): all positions at once -- the body over B*(cond_len+H*W-1) rows, the head over B*H*W*D rows, as
         large-M wgmma GEMMs + causal attention (rqb200_ar_forward).  Exact tier: the sequential teacher-forced replay."""
         B, H, W, D = xs.shape
+        self._check_computable()
         if self._mode(amp) == N.MODE_FAST:
             return self._native_forward(xs, model_aux, cond)
         if self.block_size_cond > 1:
