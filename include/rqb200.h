@@ -225,6 +225,13 @@ int64_t rqb200_vae_last_launches(const rqb200_vae* h);
  *   B > 256 (splits == 1) runs as row chunks of 256 (the batched-prefill / teacher-forced-forward shape). */
 int rqb200_dbg_gemm_tc(const void* W16, const void* X16, const float* bias, const float* residual, void* out,
                        int out_is_16, int gelu, float* partial, int N_out, int K, int B, int splits, int fmt, void* stream);
+/* rqb200_dbg_gemm_tc_fp8: the same GEMM with FP8 (E4M3) weights and fp16 activations:
+ *   out[b, n] = act(scale[n] * sum_k q[n,k] X[b,k] + bias[n]) (+ residual[b,n]);  partial != NULL: scale[n] * the per-split sums.
+ *   W8_packed: q [N_out,K] (float8_e4m3fn) rearranged into 128 x 64 tiles of 8 KB in wgmma A-fragment order, 16-byte aligned
+ *   (rqvae._native.pack_fp8_tiles); scale [N_out] f32.  X16 [B,K] fp16, 16-bit outputs fp16.  B > 128 (splits == 1) runs as row
+ *   chunks of 128. */
+int rqb200_dbg_gemm_tc_fp8(const void* W8_packed, const float* scale, const void* X16, const float* bias, const float* residual,
+                           void* out, int out_is_16, int gelu, float* partial, int N_out, int K, int B, int splits, void* stream);
 
 /* rqb200_dbg_rq_quantize: rqb200_rq_quantize with the kernel form forced: 1 = csrc/rq_search.cu (2x4 register tile), 2 =
  * csrc/rq_search2.cu (8x8 register tile, 2-CTA clusters splitting the codebook; fails with RQB200_EINVAL for shapes it does not

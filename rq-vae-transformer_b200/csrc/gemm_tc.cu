@@ -301,6 +301,192 @@ int make_tmap_weight(CUtensorMap* out, const void* W, int N_out, int K) {
     return make_tmap_2d(out, W, 1, (uint64_t)K, (uint64_t)N_out, (uint64_t)K * 2, 64, 128);
 }
 
+// ---------------------------------------------------------------- FP8 (E4M3) weights, fp16 activations
+//
+//   D[n, b] = s[n] * sum_k q[n, k] * X[b, k]       q: E4M3, one fp32 scale per output row; X fp16
+//
+// The same weight streamer with half the weight bytes.  wgmma has no mixed e4m3 x f16 form, so the weight tile is the
+// REGISTER A operand: every consumer thread loads its bytes from shared memory, widens them with cvt.rn.f16x2.e4m3x2 (exact:
+// every E4M3 value is an fp16 value) and issues the register-A m64nBNk16 f16 wgmma against the activations' descriptor.
+//
+// Packed weights (rqvae._native.pack_fp8_tiles): tile (row block T, k block kb) is 8 KB at ((T * K/64) + kb) * 8192, laid out
+// [warpgroup 2][half 2][thread 128][16 B]; the 16 bytes of (half h, thread t) are the A fragments of k16 steps 2h and 2h + 1,
+// 8 bytes each, byte e = element e of the fragment (WgmmaRA: register e / 2, lower byte = lower half).  A thread's k block is
+// two 16 B shared loads, consecutive threads on consecutive 16 B (conflict-free), and a tile arrives by one bulk copy.
+// The scale multiplies the accumulator before the common epilogue (bias, residual, GELU, partial sums): x = s[n] acc + bias.
+constexpr int G8_A_BYTES = 128 * 64;          // one packed E4M3 tile
+// the freed half of every stage deepens the ring
+template <int BN>
+constexpr int G8_STAGES = BN <= 32 ? 16 : BN == 64 ? 12 : 8;
+
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t v) {
+    uint32_t r;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"((unsigned short)v));
+    return r;
+}
+
+__device__ __forceinline__ void lds128(uint32_t (&v)[4], uint32_t addr) {
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr) : "memory");
+}
+
+// one 64-k block: widen this thread's 32 weight bytes into the four k16 A fragments, then issue the four wgmmas.  `a` must not be
+// the fragment set of the (possibly still running) previous block.
+template <int BN>
+__device__ __forceinline__ void g8_kblock(float (&acc)[BN / 2], uint32_t (&a)[4][4], uint32_t wt, uint32_t b, bool first) {
+    uint32_t lo[4], hi[4];
+    lds128(lo, wt);
+    lds128(hi, wt + 2048);
+    const uint32_t w[8] = {lo[0], lo[1], lo[2], lo[3], hi[0], hi[1], hi[2], hi[3]};
+#pragma unroll
+    for (int kk = 0; kk < 4; kk++) {
+        a[kk][0] = e4m3x2_to_f16x2(w[2 * kk]);
+        a[kk][1] = e4m3x2_to_f16x2(w[2 * kk] >> 16);
+        a[kk][2] = e4m3x2_to_f16x2(w[2 * kk + 1]);
+        a[kk][3] = e4m3x2_to_f16x2(w[2 * kk + 1] >> 16);
+    }
+    tc::wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; kk++) tc::WgmmaRA<BN>::mma(acc, a[kk], tc::gmma_desc_k128(b + kk * 32), (!first || kk > 0) ? 1u : 0u);
+}
+
+template <int BN>
+__global__ void __launch_bounds__(GT_THREADS, 1)
+gemm_tc_fp8_kernel(const uint8_t* __restrict__ W8, const float* __restrict__ scale, const __grid_constant__ CUtensorMap tmX,
+                   GemmTcParams p) {
+    constexpr int STAGES = G8_STAGES<BN>;
+    constexpr int B_BYTES = BN * 64 * 2;
+    constexpr int STAGE_BYTES = G8_A_BYTES + B_BYTES;
+    constexpr int CW = BN < 32 ? BN : 32;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    float* stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(stage + 128 * (CW + 4));
+    uint64_t* xfull = full + STAGES;
+    uint64_t* empty = xfull + STAGES;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tile = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
+    const int m0 = blockIdx.y * BN;
+    const int nkb_total = p.K / 64;
+    const int kb0 = (int)((int64_t)nkb_total * split / p.splits), kb1 = (int)((int64_t)nkb_total * (split + 1) / p.splits);
+    const int nkb = kb1 - kb0;
+    const bool tr = p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0;
+
+    tc::pdl_launch_dependents();
+    if (warp == 8 && lane == 0) {
+        if (tr) p.trace[0] = tc::gtimer();
+        tc::prefetch_tmap(&tmX);
+        for (int s = 0; s < STAGES; s++) { tc::mbar_init(&full[s], 1); tc::mbar_init(&xfull[s], 1); tc::mbar_init(&empty[s], 8); }
+        tc::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        if (lane == 0) {
+            const uint8_t* wsrc = W8 + ((size_t)tile * nkb_total + kb0) * G8_A_BYTES;
+            const int pre = nkb < STAGES ? nkb : STAGES;
+            const uint64_t w_hint = gridDim.y > 1 ? tc::L2_EVICT_LAST : tc::L2_EVICT_FIRST;
+            for (int i = 0; i < pre; i++) {
+                tc::mbar_expect_tx(&full[i], G8_A_BYTES);
+                tc::bulk_load(smem + i * STAGE_BYTES, wsrc + (size_t)i * G8_A_BYTES, G8_A_BYTES, &full[i], w_hint);
+            }
+            tc::pdl_wait();
+            if (tr) p.trace[1] = tc::gtimer();
+            for (int i = 0; i < pre; i++) {
+                tc::mbar_expect_tx(&xfull[i], B_BYTES);
+                tc::tma_load_2d(smem + i * STAGE_BYTES + G8_A_BYTES, &tmX, &xfull[i], (kb0 + i) * 64, m0, tc::L2_EVICT_LAST);
+            }
+            for (int i = pre; i < nkb; i++) {
+                const int s = i % STAGES;
+                tc::mbar_wait(&empty[s], ((i / STAGES) & 1) ^ 1);
+                tc::mbar_expect_tx(&full[s], G8_A_BYTES);
+                tc::bulk_load(smem + s * STAGE_BYTES, wsrc + (size_t)i * G8_A_BYTES, G8_A_BYTES, &full[s], w_hint);
+                tc::mbar_expect_tx(&xfull[s], B_BYTES);
+                tc::tma_load_2d(smem + s * STAGE_BYTES + G8_A_BYTES, &tmX, &xfull[s], (kb0 + i) * 64, m0, tc::L2_EVICT_LAST);
+            }
+        }
+        return;
+    }
+
+    // ---- consumers: as gemm_tc_kernel, with two fragment sets alternating so that the block in flight keeps its A registers
+    const int wg = warp >> 2, t = threadIdx.x;
+    const int frow = tile * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2);     // output features of this thread's accumulators
+    const float s_lo = scale[frow], s_hi = scale[frow + 8];
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+    uint32_t fa[4][4], fb[4][4];
+    auto kblock = [&](int i, uint32_t(&a)[4][4]) {
+        const int s = i % STAGES;
+        tc::mbar_wait(&full[s], (i / STAGES) & 1);
+        tc::mbar_wait(&xfull[s], (i / STAGES) & 1);
+        const uint32_t st0 = tc::smem_u32(smem + s * STAGE_BYTES);
+        g8_kblock<BN>(acc, a, st0 + wg * 4096 + (t & 127) * 16, st0 + G8_A_BYTES, i == 0);
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+        if (i > 0 && lane == 0) tc::mbar_arrive(&empty[(i - 1) % STAGES]);
+    };
+    int i = 0;
+    for (; i + 1 < nkb; i += 2) {
+        kblock(i, fa);
+        kblock(i + 1, fb);
+    }
+    if (i < nkb) kblock(i, fa);
+    tc::wgmma_wait<0>();
+    tc::acc_fence(acc);
+    if (nkb > 0 && lane == 0) tc::mbar_arrive(&empty[(nkb - 1) % STAGES]);
+    // accumulator d[4 j + i] is output feature frow + 8 (i / 2)
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+        acc[4 * j] *= s_lo; acc[4 * j + 1] *= s_lo;
+        acc[4 * j + 2] *= s_hi; acc[4 * j + 3] *= s_hi;
+    }
+
+    tc::pdl_wait();
+    if (tr && t == 0) p.trace[2] = tc::gtimer();
+    const int nb = (p.B - m0) < BN ? (p.B - m0) : BN;
+    gt_drain<BN, CW, 0>(p, acc, stage, wg, t, tile * 128, split, m0, nb);
+    if (tr && t == 0) p.trace[3] = tc::gtimer();
+}
+
+template <int BN>
+static int launch_gemm_tc_fp8_t(const void* W8, const float* scale, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl,
+                                cudaStream_t st) {
+    constexpr size_t smem = (size_t)G8_STAGES<BN> * (G8_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 512;
+    static_assert(smem <= 227 * 1024, "gemm_tc_fp8: shared memory budget");
+    RQB_ENSURE_SMEM(smem, gemm_tc_fp8_kernel<BN>);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(ceil_div(p.N_out, 128) * p.splits), (unsigned)ceil_div(p.B, BN));
+    cfg.blockDim = dim3(GT_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    RQB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_fp8_kernel<BN>, (const uint8_t*)W8, scale, tmX, p));
+    g_launches++;
+    return 0;
+}
+
+int launch_gemm_tc_fp8(const void* W8, const float* scale, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl, cudaStream_t st) {
+    if (p.K % 64 != 0 || p.N_out % 128 != 0) return fail(RQB200_EINVAL, "gemm_tc_fp8: need K % 64 == 0 and N_out % 128 == 0");
+    if (p.B < 1) return fail(RQB200_EINVAL, "gemm_tc_fp8: no activation rows");
+    if (p.splits < 1 || p.splits > p.K / 64) return fail(RQB200_EINVAL, "gemm_tc_fp8: bad split count");
+    if (p.fmt != 0) return fail(RQB200_EINVAL, "gemm_tc_fp8: FP8 weights take fp16 activations only");
+    if (W8 == nullptr || scale == nullptr || (reinterpret_cast<uintptr_t>(W8) & 15) != 0)
+        return fail(RQB200_EINVAL, "gemm_tc_fp8: packed weights must be 16-byte aligned, scales non-null");
+    if (p.B > 256 && p.mode == GT_PARTIAL) return fail(RQB200_EINVAL, "gemm_tc_fp8: split-K takes at most 256 activation rows");
+    if (p.mode != GT_PARTIAL && p.splits != 1) return fail(RQB200_EINVAL, "gemm_tc_fp8: direct epilogues need splits == 1");
+    switch (gemm_tc_fp8_bn(p.B)) {
+        case 16: return launch_gemm_tc_fp8_t<16>(W8, scale, tmX, p, pdl, st);
+        case 32: return launch_gemm_tc_fp8_t<32>(W8, scale, tmX, p, pdl, st);
+        case 64: return launch_gemm_tc_fp8_t<64>(W8, scale, tmX, p, pdl, st);
+        default: return launch_gemm_tc_fp8_t<128>(W8, scale, tmX, p, pdl, st);
+    }
+}
+
 }  // namespace rqb
 
 // ---- diagnostic entry points (tests/test_gpu_tc.py, bench.py's roofline leg): one GEMM through the wgmma kernel
@@ -319,4 +505,18 @@ extern "C" int rqb200_dbg_gemm_tc(const void* W16, const void* X16, const float*
     p.mode = (splits > 1 || partial != nullptr) ? GT_PARTIAL : (out_is_16 ? (gelu ? GT_H16_GELU : GT_H16) : GT_F32);
     if (p.mode == GT_PARTIAL && partial == nullptr) return fail(RQB200_EINVAL, "dbg_gemm_tc: splits > 1 needs a partial buffer");
     return launch_gemm_tc(tw, tx, p, false, (cudaStream_t)stream);
+}
+
+extern "C" int rqb200_dbg_gemm_tc_fp8(const void* W8_packed, const float* scale, const void* X16, const float* bias,
+                                      const float* residual, void* out, int out_is_16, int gelu, float* partial, int N_out, int K, int B,
+                                      int splits, void* stream) {
+    using namespace rqb;
+    CUtensorMap tx;
+    RQB_TRY(make_tmap_2d(&tx, X16, 1, (uint64_t)K, (uint64_t)B, (uint64_t)K * 2, 64, (uint32_t)gemm_tc_fp8_bn(B)));
+    GemmTcParams p = {};
+    p.N_out = N_out; p.K = K; p.B = B; p.splits = splits; p.fmt = 0;
+    p.bias = bias; p.bias_scale = 1.f; p.residual = residual; p.ld_res = N_out; p.out = out; p.ld_out = N_out; p.partial = partial;
+    p.mode = (splits > 1 || partial != nullptr) ? GT_PARTIAL : (out_is_16 ? (gelu ? GT_H16_GELU : GT_H16) : GT_F32);
+    if (p.mode == GT_PARTIAL && partial == nullptr) return fail(RQB200_EINVAL, "dbg_gemm_tc_fp8: splits > 1 needs a partial buffer");
+    return launch_gemm_tc_fp8(W8_packed, scale, tx, p, false, (cudaStream_t)stream);
 }

@@ -100,6 +100,11 @@ struct GemmTcParams {
 inline int gemm_tc_bn(int B) { return B <= 16 ? 16 : B <= 32 ? 32 : B <= 64 ? 64 : B <= 128 ? 128 : 256; }
 int make_tmap_weight(CUtensorMap* out, const void* W, int N_out, int K);
 int launch_gemm_tc(const CUtensorMap& tmW, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl, cudaStream_t st);
+// E4M3 weights packed in 128 x 64 fragment-order tiles (16 B aligned), one fp32 scale per output row; p.fmt must be 0 (fp16 X).
+// Row chunks are at most 128 activation rows (BN = 256 would need both A fragment sets beside 128 accumulators per thread): the
+// activation tensor map's box is gemm_tc_fp8_bn(B) rows.
+inline int gemm_tc_fp8_bn(int B) { return B <= 64 ? gemm_tc_bn(B) : 128; }
+int launch_gemm_tc_fp8(const void* W8, const float* scale, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl, cudaStream_t st);
 int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes_log2, uint64_t inner, uint64_t outer,
                  uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer);
 

@@ -53,6 +53,13 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
         : "memory");
 }
+// contiguous global -> shared copy through the TMA unit (bytes % 16 == 0, both ends 16 B aligned), completing on `bar`
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t hint) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar)), "l"(hint)
+        : "memory");
+}
 // L2-only prefetch of a contiguous global range (bytes % 16 == 0, 16 B aligned)
 __device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");

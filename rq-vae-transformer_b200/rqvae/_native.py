@@ -116,6 +116,7 @@ def lib():
     L.rqb200_vae_last_launches.argtypes = [C.c_void_p]
     L.rqb200_dbg_gemm_tc.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    L.rqb200_dbg_gemm_tc_fp8.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p] + [C.c_int] * 4 + [C.c_void_p]
     L.rqb200_dbg_conv_tc.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     L.rqb200_dbg_conv_tc_gn.argtypes = [C.c_void_p] * 8 + [C.c_int] * 7 + [C.c_void_p]
@@ -129,7 +130,7 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_ar_forward_workspace_bytes", "rqb200_ar_trace", "rqb200_ar_last_launches", "rqb200_vae_create",
            "rqb200_vae_destroy", "rqb200_vae_set_tensor", "rqb200_vae_finalize", "rqb200_vae_workspace_bytes",
            "rqb200_vae_decode", "rqb200_vae_decode_code", "rqb200_vae_encode", "rqb200_vae_last_launches",
-           "rqb200_dbg_gemm_tc", "rqb200_dbg_conv_tc", "rqb200_dbg_conv_tc_gn", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
+           "rqb200_dbg_gemm_tc", "rqb200_dbg_gemm_tc_fp8", "rqb200_dbg_conv_tc", "rqb200_dbg_conv_tc_gn", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
            "rqb200_dbg_rows_gemm", "rqb200_rq_quantize_depthwise", "rqb200_rq_embed_sum_depthwise",
            "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise"]
 
@@ -167,6 +168,57 @@ def default_precision():
 def fast_dtype():
     """16-bit operand format of the fast AR tier: fp16 (the reference's autocast class) unless RQB200_FAST_DTYPE=bf16"""
     return torch.bfloat16 if os.environ.get("RQB200_FAST_DTYPE", "fp16").lower() in ("bf16", "bfloat16") else torch.float16
+
+
+FP8_MAX = 448.0                  # largest finite float8_e4m3fn
+
+
+def quantize_fp8_rows(w):
+    """FP8 (E4M3) weight format: one fp32 scale per output row, s = amax|w[n]| / 448 (s = 1 for an all-zero row), q = w / s
+    clamped to +-448 and rounded to float8_e4m3fn.  Returns (q [N,K] float8_e4m3fn, s [N] f32) on w's device; q * s is the weight
+    the fp8 kernels compute with.  Every step is correctly rounded, so the CPU and the GPU give the same bits (both divisions take
+    a tensor divisor: CUDA torch divides by a Python scalar as a multiplication by its reciprocal)."""
+    w = w.detach().float()
+    amax = w.abs().amax(dim=1)
+    s = amax / torch.full_like(amax, FP8_MAX)
+    s = torch.where(s > 0, s, torch.ones_like(s))
+    q = (w / s[:, None]).clamp(-FP8_MAX, FP8_MAX).to(torch.float8_e4m3fn)
+    return q, s
+
+
+_FP8_TILE = None
+
+
+def fp8_tile_order():
+    """[8192] int64: element (row * 64 + k) of a 128 x 64 weight tile stored at each byte of its packed form.  Packed byte
+    ((wg * 2 + h) * 128 + t) * 16 + b belongs to consumer thread t of warpgroup wg, k16 step kk = 2 h + b / 8, element e = b % 8
+    of the wgmma m64k16 A fragment: row 64 wg + 16 (t / 32) + (t % 32) / 4 + 8 ((e / 2) % 2), k 16 kk + 2 (t % 4) + 8 (e / 4) + e % 2."""
+    global _FP8_TILE
+    if _FP8_TILE is None:
+        p = torch.arange(8192)
+        wg, h, t, b = p // 4096, (p // 2048) % 2, (p // 16) % 128, p % 16
+        kk, e, lane = 2 * h + b // 8, b % 8, t % 32
+        row = 64 * wg + 16 * (t // 32) + lane // 4 + 8 * ((e // 2) % 2)
+        col = 16 * kk + 2 * (lane % 4) + 8 * (e // 4) + e % 2
+        _FP8_TILE = row * 64 + col
+    return _FP8_TILE
+
+
+def pack_fp8_tiles(q):
+    """q [N,K] float8_e4m3fn (N % 128 == 0, K % 64 == 0) -> the packed uint8 weight stream of the fp8 GEMM: tile (T, kb) of rows
+    [128 T, 128 T + 128) x k [64 kb, 64 kb + 64) is 8 KB at byte (T * K / 64 + kb) * 8192, in fp8_tile_order()."""
+    N_out, K = q.shape
+    if N_out % 128 or K % 64:
+        raise ValueError("pack_fp8_tiles: need N %% 128 == 0 and K %% 64 == 0, got [%d, %d]" % (N_out, K))
+    t = q.view(torch.uint8).reshape(N_out // 128, 128, K // 64, 64).permute(0, 2, 1, 3).reshape(-1, 8192)
+    return t[:, fp8_tile_order().to(q.device)].reshape(-1).contiguous()
+
+
+def unpack_fp8_tiles(packed, N_out, K):
+    """inverse of pack_fp8_tiles: -> q [N_out,K] float8_e4m3fn"""
+    t = torch.empty(N_out // 128 * (K // 64), 8192, dtype=torch.uint8, device=packed.device)
+    t[:, fp8_tile_order().to(packed.device)] = packed.reshape(-1, 8192)
+    return t.reshape(N_out // 128, K // 64, 128, 64).permute(0, 2, 1, 3).reshape(N_out, K).view(torch.float8_e4m3fn)
 
 
 def ar_engine_options():
