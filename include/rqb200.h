@@ -32,6 +32,10 @@ extern "C" {
 #define RQB200_F32 0
 #define RQB200_BF16 1
 #define RQB200_F16 2
+/* FP8 weights (fast tier only): every streamed weight ([N,K] row-major in the other formats) is given as its E4M3 values q packed in
+ * 128 x 64 tiles of 8 KB in wgmma A-fragment order (rqvae._native.pack_fp8_tiles), 16-byte aligned, plus one fp32 scale per output
+ * row (the s* fields below); the weight is q * s.  Activations and the KV cache are fp16. */
+#define RQB200_E4M3 3
 
 /* arithmetic modes (DESIGN.md "two modes") */
 #define RQB200_MODE_EXACT 0  /* fp32 weights + fp32 FFMA: the bit-exact-indices gate                    */
@@ -93,6 +97,9 @@ typedef struct rqb200_block_weights {
     const void *wqkv, *wproj, *w1, *w2;            /* [3E,E] (rows: query|key|value), [E,E], [4E,E], [E,4E]; weight dtype */
     const float *bqkv, *bproj, *b1, *b2;           /* f32 biases */
     const float *ln1_w, *ln1_b, *ln2_w, *ln2_b;    /* f32 */
+    /* RQB200_E4M3 only (ignored otherwise): fp32 row scales of wqkv, wproj, w1, w2 -- [3E], [E], [4E], [E].  ABI 106 appended these
+     * four pointers, so arrays of this struct built against an older header have the wrong stride: rebuild them. */
+    const float *sqkv, *sproj, *s1, *s2;
 } rqb200_block_weights;
 
 typedef struct rqb200_ar_config {
@@ -101,7 +108,7 @@ typedef struct rqb200_ar_config {
     int32_t vocab_cond, cond_len;                       /* cond_emb rows, block_size_cond (>=1)                */
     int32_t code_dim, codebook_size;                    /* C (=256) and K of the RQ-VAE codebook               */
     int32_t mode;                                       /* RQB200_MODE_*                                       */
-    int32_t weight_dtype;                               /* RQB200_F32 (exact); RQB200_F16 or RQB200_BF16 (fast) */
+    int32_t weight_dtype;                               /* RQB200_F32 (exact); RQB200_F16, RQB200_BF16 or RQB200_E4M3 (fast) */
     int32_t flags;                                      /* fast tier: RQB200_AR_* flags                         */
     int32_t split_qkv, split_proj, split_fc1, split_fc2; /* fast tier: split-K factors, 0 = fill the SMs        */
     int32_t codebook_per_depth;                         /* 0: w.codebook is [K,C]; 1: [D,K,C], depth d's table at d*K*C */
@@ -133,13 +140,18 @@ typedef struct rqb200_ar_weights {
     const void* w_ccls;                                   /* [Vc,E], Vc = vocab_cond rounded up to 128 (zero rows); weight dtype; NULL when absent */
     const float *b_ccls, *ccls_ln_w, *ccls_ln_b;
     const float* tok_emb;                                 /* [V,E] or [D*V,E] (EMB_TUPLE) f32; NULL unless EMB_TOK_INPUT or EMB_TOK_HEAD */
+    /* RQB200_E4M3 only: fp32 row scales of w_in [E], w_head [E], w_cls ([V], or [D,V] with EMB_CLS_PER_DEPTH: depth d's packed [V,E]
+     * slice starts at byte d*V*E of w_cls) and w_ccls [Vc] (the zero padding rows: s = 1, q = 0).  Read only when weight_dtype is
+     * RQB200_E4M3, so a caller built against the struct without them is never read past its end. */
+    const float *s_in, *s_head, *s_cls, *s_ccls;
 } rqb200_ar_weights;
 
 typedef struct rqb200_ar rqb200_ar;
 
 /* Both tiers: embed_dim == 64 * n_head, n_head_layers >= 0 (0: a head-less model, each depth's token goes straight to the
  * classifier).  Fast tier (RQB200_MODE_FAST) also: cond_len + H*W <= 2048 (a 32x32 grid behind up to 1024 prefix tokens),
- * n_body >= 1, E % 128 == 0, V % 128 == 0, code_dim % 64 == 0, D <= 8, E <= 4608.  NULL on failure (rqb200_last_error). */
+ * n_body >= 1, E % 128 == 0, V % 128 == 0, code_dim % 64 == 0, D <= 8, E <= 4608.  RQB200_E4M3 weights: fast tier only, every
+ * present weight needs its scales and a 16-byte aligned packed stream.  NULL on failure (rqb200_last_error). */
 rqb200_ar* rqb200_ar_create(const rqb200_ar_config* cfg, const rqb200_ar_weights* w);
 void rqb200_ar_destroy(rqb200_ar* h);
 size_t rqb200_ar_workspace_bytes(const rqb200_ar* h, int B);

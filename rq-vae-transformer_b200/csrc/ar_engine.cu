@@ -8,6 +8,8 @@
 //     token, transformers.py:217-220,249-255 -- row-wise identical values);
 //   * the sampled code is written on the device and consumed by the next step's kernels; nothing returns to the host.
 #include <algorithm>
+#include <cstddef>
+#include <cstring>
 #include <vector>
 
 #include "kernels.h"
@@ -80,6 +82,26 @@ static int body_inputs(const rqb200_ar* h, const int64_t* codes, int B, int j0, 
                                j0, J, ws.LIN, st);
     RQB_TRY(launch_code_emb(codes, w.codebook, c.codebook_per_depth ? (int64_t)K * C : 0, B, HW, D, K, C, j0, J, ws.EMB, st));
     return launch_linear(ws.EMB, C, w.w_in, c.weight_dtype, w.b_in, nullptr, ws.LIN, E, B * J * D, E, C, 0, st);
+}
+
+// RQB200_E4M3: every weight the fast tier streams needs its fp32 row scales and a 16-byte aligned packed stream (the tiles arrive by
+// bulk copies).  nullptr when they do, else the reason.
+static const char* check_e4m3_weights(const rqb200_ar_config& c, const rqb200_ar_weights& w) {
+    auto bad = [](const void* q, const float* s) { return q != nullptr && (s == nullptr || (reinterpret_cast<uintptr_t>(q) & 15) != 0); };
+    for (int st = 0; st < 2; st++) {
+        const rqb200_block_weights* bl = st == 0 ? w.body : w.head;
+        const int n = st == 0 ? c.n_body : c.n_head_layers;
+        for (int l = 0; l < n; l++)
+            if (bad(bl[l].wqkv, bl[l].sqkv) || bad(bl[l].wproj, bl[l].sproj) || bad(bl[l].w1, bl[l].s1) || bad(bl[l].w2, bl[l].s2) ||
+                !bl[l].wqkv || !bl[l].wproj || !bl[l].w1 || !bl[l].w2)
+                return st == 0 ? "ar_create: E4M3 body block weights need their row scales (sqkv/sproj/s1/s2) and 16-byte aligned packed tiles"
+                               : "ar_create: E4M3 head block weights need their row scales (sqkv/sproj/s1/s2) and 16-byte aligned packed tiles";
+    }
+    if (bad(w.w_in, w.s_in)) return "ar_create: E4M3 w_in needs s_in and 16-byte aligned packed tiles";
+    if (bad(w.w_head, w.s_head)) return "ar_create: E4M3 w_head needs s_head and 16-byte aligned packed tiles";
+    if (bad(w.w_cls, w.s_cls)) return "ar_create: E4M3 w_cls needs s_cls and 16-byte aligned packed tiles";
+    if (bad(w.w_ccls, w.s_ccls)) return "ar_create: E4M3 w_ccls needs s_ccls and 16-byte aligned packed tiles";
+    return nullptr;
 }
 
 // positions [idx0, idx_end) of the raster; resume != 0: no prefill, continue on the caches / context left in this workspace
@@ -164,10 +186,13 @@ rqb200_ar* rqb200_ar_create(const rqb200_ar_config* cfg, const rqb200_ar_weights
         rqb::set_error("ar_create: unsupported shape");
         return nullptr;
     }
-    if (cfg->weight_dtype != RQB200_F32 && cfg->weight_dtype != RQB200_BF16 && cfg->weight_dtype != RQB200_F16) {
+    if (cfg->weight_dtype != RQB200_F32 && cfg->weight_dtype != RQB200_BF16 && cfg->weight_dtype != RQB200_F16 &&
+        cfg->weight_dtype != RQB200_E4M3) {
         rqb::set_error("ar_create: weight dtype");
         return nullptr;
     }
+    const bool e4m3 = cfg->weight_dtype == RQB200_E4M3;
+    if (e4m3 && cfg->mode != RQB200_MODE_FAST) { rqb::set_error("ar_create: E4M3 weights are a fast-tier format (mode RQB200_MODE_FAST)"); return nullptr; }
     {
         const int ev = cfg->embed_variant;
         const bool tok_in = ev & RQB200_EMB_TOK_INPUT, tok_head = ev & RQB200_EMB_TOK_HEAD;
@@ -180,15 +205,24 @@ rqb200_ar* rqb200_ar_create(const rqb200_ar_config* cfg, const rqb200_ar_weights
         else if (!w->w_cls || !w->b_cls) bad = "ar_create: classifier missing";
         if (bad) { rqb::set_error(bad); return nullptr; }
     }
+    if (e4m3) {
+        const char* bad = rqb::check_e4m3_weights(*cfg, *w);
+        if (bad) { rqb::set_error(bad); return nullptr; }
+    }
     rqb200_ar* h = new rqb200_ar();
     h->cfg = *cfg;
-    h->w = *w;
+    // the scale fields trail the struct: read them only for E4M3 (a caller built against the older struct ends before them)
+    h->w = rqb200_ar_weights{};
+    std::memcpy(&h->w, w, e4m3 ? sizeof(rqb200_ar_weights) : offsetof(rqb200_ar_weights, s_in));
     h->body.assign(w->body, w->body + cfg->n_body);
     h->head.assign(w->head, w->head + cfg->n_head_layers);
+    if (!e4m3)
+        for (auto* v : {&h->body, &h->head})
+            for (rqb200_block_weights& b : *v) b.sqkv = b.sproj = b.s1 = b.s2 = nullptr;
     h->w.body = h->body.data();
     h->w.head = h->head.data();
     if (cfg->mode == RQB200_MODE_FAST) {
-        if (cfg->weight_dtype == RQB200_F32) { rqb::set_error("ar_create: fast tier needs fp16 or bf16 weights"); delete h; return nullptr; }
+        if (cfg->weight_dtype == RQB200_F32) { rqb::set_error("ar_create: fast tier needs fp16, bf16 or E4M3 weights"); delete h; return nullptr; }
         h->fast = rqb::ar_fast_create(h->cfg, h->w, h->body.data(), h->head.data());
         if (!h->fast) { delete h; return nullptr; }
     }

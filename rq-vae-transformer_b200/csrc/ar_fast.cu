@@ -3,7 +3,8 @@
 // Same semantics as ar_engine.cu's exact tier (reference: transformers.py:190-369, attentions.py:60-142), different
 // arithmetic class: 16-bit weights / activations / KV cache on wgmma (gemm_tc.cu) -- fp16 by default, the reference's own
 // autocast class (transformers.py:114,206; main_sampling_fid.py:216), bf16 on request -- fp32 accumulation, fp32 residual
-// stream, fp32 LayerNorm / softmax / sampler.
+// stream, fp32 LayerNorm / softmax / sampler.  RQB200_E4M3: E4M3 weights with fp32 row scales on the fp8 weight streamer
+// (gemm_tc_fp8_kernel) in every GEMM, fp16 activations / KV cache; everything else as with fp16.
 //
 // One transformer block on the single new token of every batch row (M = batch rows):
 //
@@ -793,8 +794,16 @@ __global__ void init_state_kernel(StepState* dst, StepState v, int keep_pos) {
 }
 
 // ------------------------------------------------------------------------------------------------ engine
+// One streamed weight in the engine's format: a TMA tensor map of the [N,K] 16-bit matrix, or (RQB200_E4M3) the packed E4M3 tiles and
+// their fp32 row scales.  gemm_w() is the only place that tells the two apart.
+struct FastW {
+    CUtensorMap tm;
+    const void* q8 = nullptr;
+    const float* s8 = nullptr;
+};
+
 struct FastLayer {
-    CUtensorMap qkv, proj, fc1, fc2;
+    FastW qkv, proj, fc1, fc2;
 };
 
 enum { G_COND = 0, G_CODE = 1, G_HEAD = 2, G_HEAD_LOGITS = 3, G_COUNT = 4 };
@@ -804,9 +813,10 @@ struct ArFast {
     rqb200_ar_weights w;
     std::vector<rqb200_block_weights> body, head;
     std::vector<FastLayer> lbody, lhead;
-    CUtensorMap tm_win, tm_whead, tm_cls, tm_ccls;
-    CUtensorMap tm_cls_d[8];             // RQB200_EMB_CLS_PER_DEPTH: depth d's [V,E] slice of w_cls
-    int bf = 0;                          // 16-bit format: 0 fp16, 1 bf16
+    FastW w_in, w_head, w_cls, w_ccls;
+    FastW w_cls_d[8];                    // RQB200_EMB_CLS_PER_DEPTH: depth d's [V,E] slice of w_cls
+    int bf = 0;                          // 16-bit activation format: 0 fp16, 1 bf16
+    bool fp8 = false;                    // RQB200_E4M3 weights (fp16 activations)
     // per (workspace, B) state
     void* ws_base = nullptr;
     int B = 0;
@@ -895,14 +905,34 @@ static GemmTcParams gemm_base(const ArFast& f, int N_out, int K, int rows, int s
     return p;
 }
 
-static int gemm(const ArFast& f, const char* name, const CUtensorMap& tw, const CUtensorMap& tx, int N_out, int K, int B, int splits,
+// rows per box of an activation tensor map: the row chunk of the weight streamer that reads it (at most 128 rows for E4M3 weights)
+static uint32_t act_box(const ArFast& f, int64_t rows) {
+    const int r = (int)std::min<int64_t>(rows, 256);
+    return (uint32_t)(f.fp8 ? gemm_tc_fp8_bn(r) : gemm_tc_bn(r));
+}
+
+// the weight streamer on one engine weight, in the engine's format
+static int gemm_w(const ArFast& f, const FastW& w, const CUtensorMap& tx, const GemmTcParams& p, bool pdl, cudaStream_t st) {
+    if (!f.fp8) return launch_gemm_tc(w.tm, tx, p, pdl, st);
+    if (ceil_div(p.B, gemm_tc_fp8_bn(p.B)) > 65535) return fail(RQB200_EINVAL, "ar fast tier: too many activation rows for one E4M3 GEMM");
+    return launch_gemm_tc_fp8(w.q8, w.s8, tx, p, pdl, st);
+}
+
+static int make_w(const ArFast& f, FastW* out, const void* w, const float* s, int N_out, int K) {
+    if (!f.fp8) return make_tmap_weight(&out->tm, w, N_out, K);
+    out->q8 = w;
+    out->s8 = s;
+    return 0;
+}
+
+static int gemm(const ArFast& f, const char* name, const FastW& w, const CUtensorMap& tx, int N_out, int K, int B, int splits,
                 int mode, const float* bias, float bias_scale, void* out, float* partial, const float* residual, int64_t ld_res,
                 const int* res_row_ptr, int64_t res_row_stride, cudaStream_t st) {
     GemmTcParams p = gemm_base(f, N_out, K, B, splits, mode);
     p.bias = bias; p.bias_scale = bias_scale; p.out = out; p.partial = partial;
     p.residual = residual; p.ld_res = ld_res; p.res_row_ptr = res_row_ptr; p.res_row_stride = res_row_stride;
     p.trace = tr_slot(f, name);
-    return launch_gemm_tc(tw, tx, p, f.use_pdl, st);
+    return gemm_w(f, w, tx, p, f.use_pdl, st);
 }
 
 static int ln(const ArFast& f, const char* name, int rows, const float* x_in, const float* partial, int S, const float* bias,
@@ -1018,7 +1048,7 @@ static int record_body(ArFast& f, FastWs& ws, bool cond_token, cudaStream_t st) 
         RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
                            cb_dstride(c), HW, c.D, c.codebook_size, c.code_dim, 0, 0, ws.S, f.bf, 0));
         // x = W_in (sum_d e_d) + D b_in + pos_emb_hw[idx-1]       (bias counted D times, transformers.py:220,225)
-        RQB_TRY(gemm(f, "w_in", f.tm_win, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_in, (float)c.D, ws.XB, nullptr,
+        RQB_TRY(gemm(f, "w_in", f.w_in, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_in, (float)c.D, ws.XB, nullptr,
                      w.pos_emb_hw - E /* row idx-1 */, 0, &ws.state->idx, E, st));
     }
     RQB_TRY(fast_stack(f, f.body, f.lbody, ws, ws.XB, nullptr, ws.XB, ws.kc_body, ws.vc_body, Tb, &ws.state->s, 0, nullptr, nullptr, st));
@@ -1046,7 +1076,7 @@ static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st)
                 RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
                                    cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf,
                                    (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
-                RQB_TRY(gemm(f, "w_head", f.tm_whead, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
+                RQB_TRY(gemm(f, "w_head", f.w_head, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
                              w.pos_emb_d + (int64_t)d * E, 0, nullptr, 0, st));
             }
             RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, nullptr, ws.XH, ws.kc_head, ws.vc_head, D, nullptr, d, w.cls_ln_w,
@@ -1055,7 +1085,7 @@ static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st)
         // classifier: LN(x) (fused into the stack's last launch) -> logits                       (transformers.py:278-285)
         // per-depth classifiers (BatchLinear): depth d's [V,E] slice and bias row
         const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
-        RQB_TRY(gemm(f, "cls", pd ? f.tm_cls_d[d] : f.tm_cls, f.tx_xn, V, E, B, 1, GT_F32, w.b_cls + (pd ? (int64_t)d * V : 0), 1.f,
+        RQB_TRY(gemm(f, "cls", pd ? f.w_cls_d[d] : f.w_cls, f.tx_xn, V, E, B, 1, GT_F32, w.b_cls + (pd ? (int64_t)d * V : 0), 1.f,
                      ws.LOGITS, nullptr, nullptr, 0, nullptr, 0, st));
         if (with_logits)
             RQB_TRY(launch_pdl(logits_copy_kernel, dim3(64), dim3(256), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
@@ -1115,6 +1145,7 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
     ArFast* f = new ArFast();
     f->cfg = cfg; f->w = w; f->body = body; f->head = head;
     f->bf = cfg.weight_dtype == RQB200_BF16 ? 1 : 0;
+    f->fp8 = cfg.weight_dtype == RQB200_E4M3;
     f->use_graph = !(cfg.flags & RQB200_AR_NO_GRAPH);
     f->use_pdl = !(cfg.flags & RQB200_AR_NO_PDL);
     f->trace = (cfg.flags & RQB200_AR_TRACE) != 0;
@@ -1132,22 +1163,23 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
     auto mk = [&](const std::vector<rqb200_block_weights>& bl, std::vector<FastLayer>& out) -> int {
         out.resize(bl.size());
         for (size_t l = 0; l < bl.size(); l++) {
-            RQB_TRY(make_tmap_weight(&out[l].qkv, bl[l].wqkv, 3 * E, E));
-            RQB_TRY(make_tmap_weight(&out[l].proj, bl[l].wproj, E, E));
-            RQB_TRY(make_tmap_weight(&out[l].fc1, bl[l].w1, 4 * E, E));
-            RQB_TRY(make_tmap_weight(&out[l].fc2, bl[l].w2, E, 4 * E));
+            RQB_TRY(make_w(*f, &out[l].qkv, bl[l].wqkv, bl[l].sqkv, 3 * E, E));
+            RQB_TRY(make_w(*f, &out[l].proj, bl[l].wproj, bl[l].sproj, E, E));
+            RQB_TRY(make_w(*f, &out[l].fc1, bl[l].w1, bl[l].s1, 4 * E, E));
+            RQB_TRY(make_w(*f, &out[l].fc2, bl[l].w2, bl[l].s2, E, 4 * E));
         }
         return 0;
     };
     int rc = mk(body, f->lbody);
     if (!rc) rc = mk(head, f->lhead);
-    if (!rc && w.w_in) rc = make_tmap_weight(&f->tm_win, w.w_in, E, cfg.code_dim);
-    if (!rc && w.w_head) rc = make_tmap_weight(&f->tm_whead, w.w_head, E, cfg.code_dim);
-    if (!rc) rc = make_tmap_weight(&f->tm_cls, w.w_cls, cfg.vocab, E);
-    if (cfg.embed_variant & RQB200_EMB_CLS_PER_DEPTH)
+    if (!rc && w.w_in) rc = make_w(*f, &f->w_in, w.w_in, w.s_in, E, cfg.code_dim);
+    if (!rc && w.w_head) rc = make_w(*f, &f->w_head, w.w_head, w.s_head, E, cfg.code_dim);
+    if (!rc) rc = make_w(*f, &f->w_cls, w.w_cls, w.s_cls, cfg.vocab, E);
+    if (cfg.embed_variant & RQB200_EMB_CLS_PER_DEPTH)       // depth d's [V,E] slice: V*E weight bytes per depth (2 per element in 16 bits)
         for (int d = 0; d < cfg.D && !rc; d++)
-            rc = make_tmap_weight(&f->tm_cls_d[d], (const char*)w.w_cls + (size_t)d * cfg.vocab * E * 2, cfg.vocab, E);
-    if (!rc && w.w_ccls) rc = make_tmap_weight(&f->tm_ccls, w.w_ccls, (cfg.vocab_cond + 127) / 128 * 128, E);
+            rc = make_w(*f, &f->w_cls_d[d], (const char*)w.w_cls + (size_t)d * cfg.vocab * E * (f->fp8 ? 1 : 2),
+                        f->fp8 ? w.s_cls + (size_t)d * cfg.vocab : nullptr, cfg.vocab, E);
+    if (!rc && w.w_ccls) rc = make_w(*f, &f->w_ccls, w.w_ccls, w.s_ccls, (cfg.vocab_cond + 127) / 128 * 128, E);
     if (rc) { delete f; return nullptr; }
     for (int i = 0; i <= G_COUNT; i++) f->tr_graph_base[i] = i * (TR_CAP / G_COUNT);
     return f;
@@ -1176,14 +1208,15 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
     if (M > (int64_t)1 << 30 || T > FAST_MAXT) return fail(RQB200_EINVAL, "ar fast tier: batched pass too large");
     const bool pdl = true;               // the pass is a PDL chain too: a launch's set-up overlaps its predecessor's tail
     CUtensorMap tx_xn, tx_att, tx_h;
-    const int bn = gemm_tc_bn((int)std::min<int64_t>(M, 256));
+    const uint32_t bn = act_box(f, M);
     RQB_TRY(make_tmap_2d(&tx_xn, bb.XN, 1, E, M, (uint64_t)E * 2, 64, bn));
     RQB_TRY(make_tmap_2d(&tx_att, bb.ATT, 1, E, M, (uint64_t)E * 2, 64, bn));
     RQB_TRY(make_tmap_2d(&tx_h, bb.H, 1, 4 * E, M, (uint64_t)E * 8, 64, bn));
     const float* nof = nullptr;
-    // M > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue, like the next
-    // tile); M <= 256: the weight streamer
-    const bool rows = M > 256;
+    // 16-bit weights, M > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue, like
+    // the next tile); M <= 256, and E4M3 weights at every M: the weight streamer (E4M3: 128-row chunks, faster than the fp16 rows GEMM
+    // at the forward's shapes)
+    const bool rows = !f.fp8 && M > 256;
     for (size_t l = 0; l < blocks.size(); l++) {
         const rqb200_block_weights& bw = blocks[l];
         RQB_TRY(ln(f, "", (int)M, bb.X, nof, 0, nof, nof, nullptr, bw.ln1_w, bw.ln1_b, bb.XN, st));
@@ -1192,7 +1225,7 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
         } else {
             GemmTcParams p = gemm_base(f, 3 * E, E, (int)M, 1, GT_H16);
             p.bias = bw.bqkv; p.out = bb.QKV;
-            RQB_TRY(launch_gemm_tc(maps[l].qkv, tx_xn, p, pdl, st));
+            RQB_TRY(gemm_w(f, maps[l].qkv, tx_xn, p, pdl, st));
         }
         h16* kcl = kc ? kc + kv_per_layer * l : nullptr;
         h16* vcl = vc ? vc + kv_per_layer * l : nullptr;
@@ -1217,7 +1250,7 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
         } else {
             GemmTcParams p = gemm_base(f, E, E, (int)M, 1, GT_F32);
             p.bias = bw.bproj; p.out = bb.X; p.residual = bb.X; p.ld_res = E;
-            RQB_TRY(launch_gemm_tc(maps[l].proj, tx_att, p, pdl, st));
+            RQB_TRY(gemm_w(f, maps[l].proj, tx_att, p, pdl, st));
         }
         RQB_TRY(ln(f, "", (int)M, bb.X, nof, 0, nof, nof, nullptr, bw.ln2_w, bw.ln2_b, bb.XN, st));
         if (rows) {
@@ -1227,12 +1260,12 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
             {
                 GemmTcParams p = gemm_base(f, 4 * E, E, (int)M, 1, GT_H16_GELU);
                 p.bias = bw.b1; p.out = bb.H;
-                RQB_TRY(launch_gemm_tc(maps[l].fc1, tx_xn, p, pdl, st));
+                RQB_TRY(gemm_w(f, maps[l].fc1, tx_xn, p, pdl, st));
             }
             {
                 GemmTcParams p = gemm_base(f, E, 4 * E, (int)M, 1, GT_F32);
                 p.bias = bw.b2; p.out = bb.X; p.residual = bb.X; p.ld_res = E;
-                RQB_TRY(launch_gemm_tc(maps[l].fc2, tx_h, p, pdl, st));
+                RQB_TRY(gemm_w(f, maps[l].fc2, tx_h, p, pdl, st));
             }
         }
     }
@@ -1255,13 +1288,13 @@ static int body_tokens_batched(ArFast& f, const StepState* state, float* X, h16*
     } else if (n_code > 0) {
         const int64_t Mc = (int64_t)B * n_code;
         CUtensorMap tx_s;
-        RQB_TRY(make_tmap_2d(&tx_s, S, 1, c.code_dim, Mc, (uint64_t)c.code_dim * 2, 64, gemm_tc_bn((int)std::min<int64_t>(Mc, 256))));
+        RQB_TRY(make_tmap_2d(&tx_s, S, 1, c.code_dim, Mc, (uint64_t)c.code_dim * 2, 64, act_box(f, Mc)));
         RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, n_code), dim3(64), (size_t)0, st, false, state, w.codebook, cb_dstride(c), HW, c.D,
                            c.codebook_size, c.code_dim, -c.D, 0, S, f.bf, 0));
         GemmTcParams p = gemm_base(f, E, c.code_dim, (int)Mc, 1, GT_F32);
         p.bias = w.b_in; p.bias_scale = (float)c.D; p.out = X + (int64_t)cl * B * E;
         p.residual = w.pos_emb_hw; p.ld_res = E; p.res_div = B;          // row (j, b) gets pos_emb_hw[j]
-        RQB_TRY(launch_gemm_tc(f.tm_win, tx_s, p, false, st));
+        RQB_TRY(gemm_w(f, f.w_in, tx_s, p, false, st));
     }
     return 0;
 }
@@ -1344,16 +1377,16 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
         if (cond_logits_out) {                                  // cond_classifier(latents[:, :cond_len-1])        (:153-156)
             const int64_t Mc = (int64_t)(cl - 1) * B;
             CUtensorMap tx;
-            RQB_TRY(make_tmap_2d(&tx, ws.XN, 1, E, Mc, (uint64_t)E * 2, 64, gemm_tc_bn((int)std::min<int64_t>(Mc, 256))));
+            RQB_TRY(make_tmap_2d(&tx, ws.XN, 1, E, Mc, (uint64_t)E * 2, 64, act_box(*f, Mc)));
             RQB_TRY(ln(*f, "", (int)Mc, ws.BX, nof, 0, nof, nof, nullptr, w.ccls_ln_w, w.ccls_ln_b, ws.XN, st));
             GemmTcParams p = gemm_base(*f, (c.vocab_cond + 127) / 128 * 128, E, (int)Mc, 1, GT_F32);
             p.bias = w.b_ccls; p.out = cond_logits_out;
-            RQB_TRY(launch_gemm_tc(f->tm_ccls, tx, p, false, st));
+            RQB_TRY(gemm_w(*f, f->w_ccls, tx, p, false, st));
         }
         // head tokens: d = 0 rows = spatial ctx (body rows of tokens cond_len-1 ..) + pos_emb_d[0]; d >= 1 rows = head_mlp(cumsum)
         RQB_TRY(ln(*f, "", G, ws.BX + (int64_t)(cl - 1) * B * E, nof, 0, nof, w.pos_emb_d, ws.HX, nof, nof, nullptr, st));
         CUtensorMap tx_s;
-        RQB_TRY(make_tmap_2d(&tx_s, ws.S, 1, c.code_dim, G, (uint64_t)c.code_dim * 2, 64, gemm_tc_bn(std::min(G, 256))));
+        RQB_TRY(make_tmap_2d(&tx_s, ws.S, 1, c.code_dim, G, (uint64_t)c.code_dim * 2, 64, act_box(*f, G)));
         for (int d = 1; d < D; d++) {
             if (c.embed_variant & RQB200_EMB_TOK_HEAD) {        // tok_emb(code_{d-1}) + pos_emb_d[d]        (:164,177)
                 RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, HW), dim3(128), (size_t)0, st, false, (const StepState*)ws.state, w.tok_emb,
@@ -1366,15 +1399,16 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
                                (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
             GemmTcParams p = gemm_base(*f, E, c.code_dim, G, 1, GT_F32);
             p.bias = w.b_head; p.out = ws.HX + (int64_t)d * G * E; p.residual = w.pos_emb_d + (int64_t)d * E; p.ld_res = 0;
-            RQB_TRY(launch_gemm_tc(f->tm_whead, tx_s, p, false, st));
+            RQB_TRY(gemm_w(*f, f->w_head, tx_s, p, false, st));
         }
         BatchBufs hb = {ws.HX, ws.XN, ws.QKV, ws.ATT, ws.H};
         RQB_TRY(stack_batched(*f, f->head, f->lhead, hb, G, D, nullptr, nullptr, 0, D, st));
         // classifier                                                                                   (:181-183)
         RQB_TRY(ln(*f, "", (int)Mh, ws.HX, nof, 0, nof, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, st));
         // one launch over all Mh rows, or (per-depth classifiers) one per depth over that depth's G rows d*G .. (d+1)*G-1, the rows
-        // GEMM or the weight streamer picked by the rows each launch covers.  (The rows GEMM reads whole 128-row tiles -- past a
-        // slice into the next depth's rows, past the last one into forward_layout's +128 -- and stores only the slice's rows.)
+        // GEMM or the weight streamer picked by the rows each launch covers (E4M3 weights: always the streamer).  (The rows GEMM reads
+        // whole 128-row tiles -- past a slice into the next depth's rows, past the last one into forward_layout's +128 -- and stores
+        // only the slice's rows.)
         const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
         const int n_cls = pd ? D : 1;
         const int64_t Mc = pd ? G : Mh;
@@ -1384,14 +1418,14 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
             const void* wc = (const char*)w.w_cls + (size_t)d * V * E * wsz;
             const float* bc = w.b_cls + (int64_t)d * V;
             float* lo = logits_out + (int64_t)d * Mc * V;
-            if (Mc > 256) {
+            if (!f->fp8 && Mc > 256) {
                 RQB_TRY(launch_rows_gemm_tc(xn, wc, bc, nullptr, lo, nullptr, 0, f->bf, Mc, V, E, st));
             } else {
                 CUtensorMap tx;
-                RQB_TRY(make_tmap_2d(&tx, xn, 1, E, Mc, (uint64_t)E * 2, 64, gemm_tc_bn((int)Mc)));
+                RQB_TRY(make_tmap_2d(&tx, xn, 1, E, Mc, (uint64_t)E * 2, 64, act_box(*f, Mc)));
                 GemmTcParams p = gemm_base(*f, V, E, (int)Mc, 1, GT_F32);
                 p.bias = bc; p.out = lo;
-                RQB_TRY(launch_gemm_tc(pd ? f->tm_cls_d[d] : f->tm_cls, tx, p, false, st));
+                RQB_TRY(gemm_w(*f, pd ? f->w_cls_d[d] : f->w_cls, tx, p, false, st));
             }
         }
         return 0;
@@ -1419,7 +1453,7 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
         drop_graphs(*f);
         f->ws_base = wsp;
         f->B = B;
-        const int bn = gemm_tc_bn(B);
+        const uint32_t bn = act_box(*f, B);
         RQB_TRY(make_tmap_2d(&f->tx_xn, ws.XN, 1, E, B, (uint64_t)E * 2, 64, bn));
         RQB_TRY(make_tmap_2d(&f->tx_att, ws.ATT, 1, E, B, (uint64_t)E * 2, 64, bn));
         RQB_TRY(make_tmap_2d(&f->tx_h, ws.Hh, 1, 4 * E, B, (uint64_t)E * 8, 64, bn));

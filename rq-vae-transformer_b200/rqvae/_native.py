@@ -8,7 +8,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RQB200_LIB", os.path.join(os.path.dirname(_HERE), "csrc", "librqb200.so"))
 
 OK, EINVAL, ECUDA, ENODEV, EWORKSPACE, ESTATE = 0, -1, -2, -3, -4, -5
-F32, BF16, F16 = 0, 1, 2
+F32, BF16, F16, E4M3 = 0, 1, 2, 3
 MODE_EXACT, MODE_FAST = 0, 1
 AR_NO_GRAPH, AR_NO_PDL, AR_TRACE, AR_SEQUENTIAL_PREFILL = 1, 2, 4, 32
 # rqb200_ar_config.embed_variant bits (0 = the shipped family)
@@ -20,7 +20,7 @@ c_f32p, c_i64p, c_vp = C.c_void_p, C.c_void_p, C.c_void_p
 
 class BlockWeights(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("wqkv", "wproj", "w1", "w2", "bqkv", "bproj", "b1", "b2",
-                                          "ln1_w", "ln1_b", "ln2_w", "ln2_b")]
+                                          "ln1_w", "ln1_b", "ln2_w", "ln2_b", "sqkv", "sproj", "s1", "s2")]
 
 
 class ArConfig(C.Structure):
@@ -34,7 +34,7 @@ class ArWeights(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("pos_emb_cond", "pos_emb_hw", "pos_emb_d", "cond_emb", "w_in", "w_head", "w_cls",
                                           "b_in", "b_head", "b_cls", "cls_ln_w", "cls_ln_b", "codebook")] + \
                [("body", C.POINTER(BlockWeights)), ("head", C.POINTER(BlockWeights))] + \
-               [(n, C.c_void_p) for n in ("w_ccls", "b_ccls", "ccls_ln_w", "ccls_ln_b", "tok_emb")]
+               [(n, C.c_void_p) for n in ("w_ccls", "b_ccls", "ccls_ln_w", "ccls_ln_b", "tok_emb", "s_in", "s_head", "s_cls", "s_ccls")]
 
 
 class VaeConfig(C.Structure):
@@ -166,8 +166,16 @@ def default_precision():
 
 
 def fast_dtype():
-    """16-bit operand format of the fast AR tier: fp16 (the reference's autocast class) unless RQB200_FAST_DTYPE=bf16"""
+    """16-bit activation format of the fast AR tier: fp16 (the reference's autocast class) unless RQB200_FAST_DTYPE=bf16
+    (RQB200_FAST_DTYPE=fp8 keeps fp16 activations)"""
     return torch.bfloat16 if os.environ.get("RQB200_FAST_DTYPE", "fp16").lower() in ("bf16", "bfloat16") else torch.float16
+
+
+def fast_weight_format():
+    """weight format of the fast AR tier, read from RQB200_FAST_DTYPE (case-insensitive): 'fp8' (E4M3 values with one fp32 scale
+    per output row, fp16 activations), 'bf16', or 'fp16' -- the default, also for any value it does not know"""
+    v = os.environ.get("RQB200_FAST_DTYPE", "fp16").lower()
+    return "fp8" if v == "fp8" else ("bf16" if v in ("bf16", "bfloat16") else "fp16")
 
 
 FP8_MAX = 448.0                  # largest finite float8_e4m3fn
@@ -219,6 +227,18 @@ def unpack_fp8_tiles(packed, N_out, K):
     t = torch.empty(N_out // 128 * (K // 64), 8192, dtype=torch.uint8, device=packed.device)
     t[:, fp8_tile_order().to(packed.device)] = packed.reshape(-1, 8192)
     return t.reshape(N_out // 128, K // 64, 128, 64).permute(0, 2, 1, 3).reshape(N_out, K).view(torch.float8_e4m3fn)
+
+
+def pack_fp8_weight(w):
+    """the AR engine's E4M3 form of one streamed weight, on w's device (CPU or GPU: the same bits).  w [N,K] (nn.Linear layout):
+    -> (packed uint8 [N*K] in pack_fp8_tiles' order, s [N] f32).  w [D,N,K] (one [N,K] weight per depth, e.g. the per-depth
+    classifiers of a BatchLinear transposed): each depth quantised by its own rows and packed on its own, the D streams concatenated
+    (depth d's at byte d*N*K) -> (packed [D*N*K], s [D,N])."""
+    if w.dim() == 2:
+        q, s = quantize_fp8_rows(w)
+        return pack_fp8_tiles(q), s
+    packed, scales = zip(*(pack_fp8_weight(w[d]) for d in range(w.shape[0])))
+    return torch.cat(packed), torch.stack(scales)
 
 
 def ar_engine_options():

@@ -8,7 +8,8 @@ Boundary kept (SURVEY.md section 8b): constructor from an ``RQTransformerConfig`
 
 Arithmetic tiers: ``amp=False`` -> 'exact' (fp32 weights/activations, FFMA -- the tier the bit-exact-indices gate is
 defined on); ``amp=True`` -> 'fast' (fp16 weights / activations / KV on wgmma tensor cores, fp32 accumulate -- the
-reference's own amp class is fp16 autocast, transformers.py:114,206; RQB200_FAST_DTYPE=bf16 selects bf16 instead).
+reference's own amp class is fp16 autocast, transformers.py:114,206; RQB200_FAST_DTYPE=bf16 selects bf16 instead,
+RQB200_FAST_DTYPE=fp8 E4M3 weights with one fp32 scale per output row and fp16 activations / KV).
 ``self.precision`` ('exact' | 'fast') or RQB200_PRECISION overrides the ``amp`` mapping."""
 import ctypes as C
 import os
@@ -189,7 +190,7 @@ class RQTransformer(Stage2Model):
         if key not in self._eng and slot > 0:
             # engines of one model share the packed weights of slot 0; each slot owns its workspace, KV cache and graphs
             base = self._engine(codebook, mode, 0)
-            eng = {"handle": base["make"](), "keep": base["keep"], "ws": None, "make": base["make"]}
+            eng = dict(base, handle=base["make"](), ws=None)
             self._eng[key] = eng
             return eng
         if key in self._eng:
@@ -197,9 +198,29 @@ class RQTransformer(Stage2Model):
         N.require_cuda(self.pos_emb_hw, *(codebook if per_depth else [codebook]))
         self._check_computable()
         L = N.lib()
-        wdt = N.fast_dtype() if mode == N.MODE_FAST else torch.float32
+        cfg, w, keep, streamed = self._engine_structs(codebook, mode)
+
+        def make():
+            hnd = L.rqb200_ar_create(C.byref(cfg), C.byref(w))
+            if not hnd:
+                raise N.NativeError("rqb200_ar_create: " + L.rqb200_last_error().decode())
+            return hnd
+
+        handle = make()
+        eng = {"handle": handle, "keep": keep, "ws": None, "make": make, "weight_dtype": cfg.weight_dtype, "streamed": streamed}
+        self._eng[key] = eng
+        return eng
+
+    def _engine_structs(self, codebook, mode):
+        """the rqb200_ar_config / rqb200_ar_weights of one engine build and the tensors they point into: (cfg, w, keep, streamed),
+        streamed = the tensors of the streamed weights (a subset of keep).  The fast tier's streamed weights (every nn.Linear / BatchLinear weight) are copied in its weight format:
+        fp16 or bf16, or (RQB200_FAST_DTYPE=fp8) packed E4M3 tiles plus fp32 row scales and no 16-bit copy; everything else is
+        read as fp32.  Host-only: runs on CPU tensors too."""
+        per_depth = isinstance(codebook, list)
+        fmt = N.fast_weight_format() if mode == N.MODE_FAST else "fp32"
+        wdt = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16, "fp8": None}[fmt]
         opts = N.ar_engine_options() if mode == N.MODE_FAST else {"flags": 0, "splits": [0, 0, 0, 0]}
-        keep = []
+        keep, streamed = [], []
 
         def f32(t):
             t = t.detach().float().contiguous()
@@ -207,9 +228,16 @@ class RQTransformer(Stage2Model):
             return t.data_ptr()
 
         def wt(t):
+            """one streamed weight ([N,K], or [D,N,K] per-depth) -> (weight pointer, row-scale pointer or None)"""
+            if fmt == "fp8":
+                q, sc = N.pack_fp8_weight(t.detach())
+                keep.extend([q, sc])
+                streamed.extend([q, sc])
+                return q.data_ptr(), sc.data_ptr()
             t = t.detach().to(wdt).contiguous()
             keep.append(t)
-            return t.data_ptr()
+            streamed.append(t)
+            return t.data_ptr(), None
 
         def blocks(stack):
             arr = (N.BlockWeights * len(stack.blocks))()
@@ -217,10 +245,11 @@ class RQTransformer(Stage2Model):
                 a = b.attn
                 wqkv = torch.cat([a.query.weight, a.key.weight, a.value.weight], 0)
                 bqkv = torch.cat([a.query.bias, a.key.bias, a.value.bias], 0)
-                arr[i].wqkv, arr[i].bqkv = wt(wqkv), f32(bqkv)
-                arr[i].w1, arr[i].b1 = wt(b.mlp[0].weight), f32(b.mlp[0].bias)
-                arr[i].wproj, arr[i].bproj = wt(a.proj.weight), f32(a.proj.bias)
-                arr[i].w2, arr[i].b2 = wt(b.mlp[2].weight), f32(b.mlp[2].bias)
+                (arr[i].wqkv, arr[i].sqkv), arr[i].bqkv = wt(wqkv), f32(bqkv)
+                del wqkv
+                (arr[i].w1, arr[i].s1), arr[i].b1 = wt(b.mlp[0].weight), f32(b.mlp[0].bias)
+                (arr[i].wproj, arr[i].sproj), arr[i].bproj = wt(a.proj.weight), f32(a.proj.bias)
+                (arr[i].w2, arr[i].s2), arr[i].b2 = wt(b.mlp[2].weight), f32(b.mlp[2].bias)
                 arr[i].ln1_w, arr[i].ln1_b = f32(b.ln1.weight), f32(b.ln1.bias)
                 arr[i].ln2_w, arr[i].ln2_b = f32(b.ln2.weight), f32(b.ln2.bias)
             return arr
@@ -237,7 +266,7 @@ class RQTransformer(Stage2Model):
             table0 = codebook[0] if per_depth else codebook
             cfg.code_dim, cfg.codebook_size = table0.shape[1], table0.shape[0]
         cfg.codebook_per_depth = int(per_depth)
-        cfg.mode, cfg.weight_dtype = mode, N._DT[wdt]
+        cfg.mode, cfg.weight_dtype = mode, N.E4M3 if fmt == "fp8" else N._DT[wdt]
         cfg.flags = opts["flags"]
         cfg.split_qkv, cfg.split_proj, cfg.split_fc1, cfg.split_fc2 = opts["splits"]
         cfg.embed_variant = self._embed_variant()
@@ -247,9 +276,9 @@ class RQTransformer(Stage2Model):
         w.pos_emb_cond, w.pos_emb_hw, w.pos_emb_d = f32(self.pos_emb_cond), f32(self.pos_emb_hw), f32(self.pos_emb_d)
         w.cond_emb = f32(self.cond_emb.weight)
         if self.input_mlp is not None:
-            w.w_in, w.b_in = wt(self.input_mlp.weight), f32(self.input_mlp.bias)
+            (w.w_in, w.s_in), w.b_in = wt(self.input_mlp.weight), f32(self.input_mlp.bias)
         if self.head_mlp is not None:
-            w.w_head, w.b_head = wt(self.head_mlp.weight), f32(self.head_mlp.bias)
+            (w.w_head, w.s_head), w.b_head = wt(self.head_mlp.weight), f32(self.head_mlp.bias)
         if self.tok_emb is not None:
             te = self.tok_emb
             if isinstance(te, TupleEmbedding):
@@ -259,10 +288,11 @@ class RQTransformer(Stage2Model):
             w.tok_emb = f32(te.weight)
         lin = self.classifier.linear
         if isinstance(lin, BatchLinear):
-            # [D,E,V] (input-major) -> one [D,V,E] copy per engine build: depth d's classifier is a row-major [V,E] slice
-            w.w_cls, w.b_cls = wt(lin.weight.detach().transpose(1, 2)), f32(lin.bias)
+            # [D,E,V] (input-major) -> one [D,V,E] copy per engine build: depth d's classifier is a row-major [V,E] slice (E4M3:
+            # quantised by its own V rows, scales [D,V])
+            (w.w_cls, w.s_cls), w.b_cls = wt(lin.weight.detach().transpose(1, 2)), f32(lin.bias)
         else:
-            w.w_cls, w.b_cls = wt(lin.weight), f32(lin.bias)
+            (w.w_cls, w.s_cls), w.b_cls = wt(lin.weight), f32(lin.bias)
         w.cls_ln_w, w.cls_ln_b = f32(self.classifier.layer_norm.weight), f32(self.classifier.layer_norm.bias)
         if codebook is not None:
             w.codebook = f32(torch.stack(codebook)) if per_depth else f32(codebook)
@@ -270,22 +300,27 @@ class RQTransformer(Stage2Model):
             pad = -self.vocab_size_cond % 128            # classifier rows padded with zeros up to the 128-feature wgmma tile
             pw = torch.nn.functional.pad(self.cond_classifier.linear.weight.detach(), (0, 0, 0, pad))
             pb = torch.nn.functional.pad(self.cond_classifier.linear.bias.detach(), (0, pad))
-            w.w_ccls, w.b_ccls = wt(pw), f32(pb)
+            (w.w_ccls, w.s_ccls), w.b_ccls = wt(pw), f32(pb)      # (E4M3: the zero rows get s = 1, q = 0)
             w.ccls_ln_w, w.ccls_ln_b = f32(self.cond_classifier.layer_norm.weight), f32(self.cond_classifier.layer_norm.bias)
         body, head = blocks(self.body_transformer), blocks(self.head_transformer)
         w.body, w.head = C.cast(body, C.POINTER(N.BlockWeights)), C.cast(head, C.POINTER(N.BlockWeights))
         keep.extend([body, head, cfg, w])
+        return cfg, w, keep, streamed
 
-        def make():
-            hnd = L.rqb200_ar_create(C.byref(cfg), C.byref(w))
-            if not hnd:
-                raise N.NativeError("rqb200_ar_create: " + L.rqb200_last_error().decode())
-            return hnd
-
-        handle = make()
-        eng = {"handle": handle, "keep": keep, "ws": None, "make": make, "dtype": wdt}
-        self._eng[key] = eng
-        return eng
+    def native_weight_bytes(self):
+        """bytes of the tensors the native engines of this model hold, each build counted once (engine slots share one):
+        {"streamed": the weight copies the fast tier streams, in its format (E4M3: packed bytes + 4 per row scale), "fp32": the
+        fp32 tensors they read (embeddings, biases, LayerNorms, codebook; mostly the module's own parameters)}"""
+        seen, out = set(), {"streamed": 0, "fp32": 0}
+        for eng in self._eng.values():
+            if id(eng["keep"]) in seen:
+                continue
+            seen.add(id(eng["keep"]))
+            sids = {id(t) for t in eng["streamed"]}
+            for t in eng["keep"]:
+                if isinstance(t, torch.Tensor):
+                    out["streamed" if id(t) in sids else "fp32"] += t.numel() * t.element_size()
+        return out
 
     # ------------------------------------------------------------------ reference surface
     def init_cache(self):
