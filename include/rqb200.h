@@ -178,6 +178,19 @@ int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* c
                           float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
                           void* workspace, size_t workspace_bytes, void* stream);
+/* RQTransformer.cached_forward (transformers.py:190-287): the logits of ONE token (h, w, d) into logits_out [B,V] f32.
+ *   xs: the caller's code map, int64, batch row b at xs + b*xs_batch_stride, positions in raster order, D codes each
+ *       (only the codes this step consumes are read: position idx-1 when d == 0, codes 0..d-1 of position idx when d > 0;
+ *       idx = pos_h*W + pos_w);
+ *   restart != 0: a new sequence -- d must be 0; prefill cond + positions [0, idx) from xs (batched prefill as in
+ *       rqb200_ar_sample), then head depth 0;
+ *   restart == 0: continue on the KV / context state the previous step left in the SAME workspace; (h,w,d) must be the
+ *       token after the previous step's, else RQB200_ESTATE.  A rqb200_ar_sample / _span call on the handle ends the sequence.
+ * The launches are those of the sampling loop (split-K factors included) minus the sampler: under teacher forcing the logits
+ * equal rqb200_ar_sample's logits_out bit for bit.  Fast tier: B <= 256 per call.  Arguments are checked before any CUDA
+ * call. */
+int rqb200_ar_step(rqb200_ar* h, const int64_t* xs, int64_t xs_batch_stride, const int64_t* cond, int B, int pos_h, int pos_w,
+                   int d, int restart, float* logits_out, void* workspace, size_t workspace_bytes, void* stream);
 /* RQTransformer.forward (transformers.py:113-188): teacher-forced logits of complete code maps, all positions at once (fast tier:
  * M = B*T row GEMMs on wgmma + causal attention; exact tier: returns RQB200_EINVAL -- use rqb200_ar_sample with force_codes and
  * logits_out, the sequential replay).  codes [B,H,W,D] int64, cond [B,cond_len] or NULL.
@@ -190,7 +203,7 @@ int rqb200_ar_forward(rqb200_ar* h, const int64_t* codes, const int64_t* cond, i
  * launch slot of the last graph replays to out_host[cap_launches][4] and the slot names ('\n'-separated) to names; returns the
  * number of slots (0 when tracing is off).  Synchronises the device. */
 int rqb200_ar_trace(rqb200_ar* h, long long* out_host, int cap_launches, char* names, int names_cap);
-/* number of kernels the last rqb200_ar_sample call launched (bench.py's gpu_launches) */
+/* number of kernels the last rqb200_ar_sample / _step / _forward call launched (bench.py's gpu_launches) */
 int64_t rqb200_ar_last_launches(const rqb200_ar* h);
 
 /* ------------------------------------------------------------------------------------------------ P2

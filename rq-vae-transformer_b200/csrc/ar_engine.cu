@@ -20,6 +20,10 @@ struct rqb200_ar {
     std::vector<rqb200_block_weights> body, head;
     int64_t last_launches = 0;
     rqb::ArFast* fast = nullptr;
+    // rqb200_ar_step: the workspace / batch of the stepped sequence and its next token ((pos_h*W + pos_w)*D + d), -1 when none
+    const void* step_ws = nullptr;
+    int step_B = 0;
+    int64_t step_next = -1;
 };
 
 namespace rqb {
@@ -27,6 +31,7 @@ namespace rqb {
 struct ArWs {
     float *X, *XN, *QKV, *ATT, *H, *CTX, *TOK, *EMB, *LIN, *LOGITS;
     float *kc_body, *vc_body, *kc_head, *vc_head;
+    int64_t* CODES;              // [B, HW, D] rqb200_ar_step's copy of the caller's codes
 };
 
 static size_t ar_layout(const rqb200_ar_config& c, int B, void* base, size_t cap, ArWs* ws) {
@@ -48,7 +53,8 @@ static size_t ar_layout(const rqb200_ar_config& c, int B, void* base, size_t cap
     float* vcb = a.take<float>(per_body * c.n_body);
     float* kch = a.take<float>(per_head * c.n_head_layers);
     float* vch = a.take<float>(per_head * c.n_head_layers);
-    if (ws) *ws = ArWs{X, XN, QKV, ATT, H, CTX, TOK, EMB, LIN, LOGITS, kcb, vcb, kch, vch};
+    int64_t* codes = a.take<int64_t>((int64_t)B * HW * D);
+    if (ws) *ws = ArWs{X, XN, QKV, ATT, H, CTX, TOK, EMB, LIN, LOGITS, kcb, vcb, kch, vch, codes};
     return a.off + 256;
 }
 
@@ -104,19 +110,66 @@ static const char* check_e4m3_weights(const rqb200_ar_config& c, const rqb200_ar
     return nullptr;
 }
 
+// prefill: tokens [cond (cl) | xs_emb[0 .. idx0-1]] through the body (transformers.py:224-239); ws.CTX = the last token's output
+static int prefill_prefix(const rqb200_ar* h, const int64_t* codes, const int64_t* cond, int B, int idx0, ArWs& ws, cudaStream_t st) {
+    const rqb200_ar_config& c = h->cfg;
+    const rqb200_ar_weights& w = h->w;
+    const int E = c.embed_dim, D = c.D, cl = c.cond_len, Tb = cl + c.H * c.W;
+    const int Tn0 = cl + idx0;
+    RQB_TRY(launch_cond_token(cond, w.cond_emb, w.pos_emb_cond, B, cl, c.vocab_cond, E, Tn0, ws.X, st));
+    if (idx0 > 0) {
+        RQB_TRY(body_inputs(h, codes, B, 0, idx0, ws, st));
+        RQB_TRY(launch_body_token(ws.LIN, w.pos_emb_hw, B, D, E, 0, idx0, cl, Tn0, ws.X, st));
+    }
+    RQB_TRY(run_stack(h, h->body, ws, B, Tn0, 0, Tb, ws.kc_body, ws.vc_body, st));
+    return launch_row_add(ws.X, (int64_t)Tn0 * E, (int64_t)(Tn0 - 1) * E, nullptr, B, E, ws.CTX, st);   // latents[:, -1]
+}
+
+// decode step of the body on the token of position idx-1 (transformers.py:240-242); ws.CTX = its output
+static int body_step(const rqb200_ar* h, const int64_t* codes, int B, int idx, ArWs& ws, cudaStream_t st) {
+    const rqb200_ar_config& c = h->cfg;
+    const int E = c.embed_dim, cl = c.cond_len, Tb = cl + c.H * c.W;
+    RQB_TRY(body_inputs(h, codes, B, idx - 1, 1, ws, st));
+    RQB_TRY(launch_body_token(ws.LIN, h->w.pos_emb_hw, B, c.D, E, idx - 1, 1, 0, 1, ws.X, st));
+    RQB_TRY(run_stack(h, h->body, ws, B, 1, cl + idx - 1, Tb, ws.kc_body, ws.vc_body, st));
+    RQB_CUDA(cudaMemcpyAsync(ws.CTX, ws.X, (size_t)B * E * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+// head depth d of position idx: its token, the head stack (cache rows [0, d) from the earlier depths) and the classifier -> lg [B,V]
+static int head_depth(const rqb200_ar* h, const int64_t* codes, int B, int idx, int d, ArWs& ws, float* lg, cudaStream_t st) {
+    const rqb200_ar_config& c = h->cfg;
+    const rqb200_ar_weights& w = h->w;
+    const int E = c.embed_dim, D = c.D, HW = c.H * c.W, C = c.code_dim, V = c.vocab, K = c.codebook_size, wd = c.weight_dtype;
+    const int64_t cbs = c.codebook_per_depth ? (int64_t)K * C : 0;     // floats between depth d's codebook and depth d+1's
+    const int ev = c.embed_variant;
+    const int64_t tes = (ev & RQB200_EMB_TUPLE) ? (int64_t)V * E : 0;  // floats between depth d's token table and depth d+1's
+    const size_t wsz = wd == RQB200_F32 ? 4 : 2;
+    if (d == 0) {
+        RQB_TRY(launch_row_add(ws.CTX, E, 0, w.pos_emb_d, B, E, ws.X, st));                         // ctx + pos_emb_d[0]
+    } else if (ev & RQB200_EMB_TOK_HEAD) {
+        RQB_TRY(launch_head_cumsum(codes, w.tok_emb, tes, B, HW, D, V, E, idx, d, ws.TOK, st, true));  // tok_emb(code_{d-1})
+        RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
+    } else {
+        // head_mlp(cumsum_{i<d} e_i), or head_mlp(e_{d-1}) without cumsum_depth_ctx
+        RQB_TRY(launch_head_cumsum(codes, w.codebook, cbs, B, HW, D, K, C, idx, d, ws.EMB, st, (ev & RQB200_EMB_NO_CUMSUM) != 0));
+        RQB_TRY(launch_linear(ws.EMB, C, w.w_head, wd, w.b_head, nullptr, ws.TOK, E, B, E, C, 0, st));
+        RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
+    }
+    RQB_TRY(run_stack(h, h->head, ws, B, 1, d, D, ws.kc_head, ws.vc_head, st));                   // head cache restarts at d==0
+    RQB_TRY(launch_layernorm(ws.X, E, w.cls_ln_w, w.cls_ln_b, ws.XN, E, B, E, st));
+    // one shared classifier, or depth d's [V,E] slice of the per-depth stack (BatchLinear, transformers.py:278-283)
+    const int64_t cd = (ev & RQB200_EMB_CLS_PER_DEPTH) ? d : 0;
+    return launch_linear(ws.XN, E, (const char*)w.w_cls + cd * V * E * wsz, wd, w.b_cls + cd * V, nullptr, lg, V, B, V, E, 0, st);
+}
+
 // positions [idx0, idx_end) of the raster; resume != 0: no prefill, continue on the caches / context left in this workspace
 static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx0, int idx_end, int resume,
                           float temperature, const int32_t* top_k, const float* top_p, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force, int64_t* out, void* wsp,
                           size_t ws_bytes, cudaStream_t st) {
     const rqb200_ar_config& c = h->cfg;
-    const rqb200_ar_weights& w = h->w;
-    const int E = c.embed_dim, D = c.D, HW = c.H * c.W, C = c.code_dim, V = c.vocab, K = c.codebook_size;
-    const int wd = c.weight_dtype, cl = c.cond_len, Tb = cl + HW;
-    const int64_t cbs = c.codebook_per_depth ? (int64_t)K * C : 0;     // floats between depth d's codebook and depth d+1's
-    const int ev = c.embed_variant;
-    const int64_t tes = (ev & RQB200_EMB_TUPLE) ? (int64_t)V * E : 0;  // floats between depth d's token table and depth d+1's
-    const size_t wsz = wd == RQB200_F32 ? 4 : 2;
+    const int D = c.D, HW = c.H * c.W, V = c.vocab;
     if (B <= 0) return fail(RQB200_EINVAL, "ar_sample: B must be > 0");
     if (idx0 < 0 || idx_end > HW || idx0 > idx_end) return fail(RQB200_EINVAL, "ar_sample: bad position span");
     ArWs ws;
@@ -126,44 +179,13 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
     if (!resume && out != partial) RQB_CUDA(cudaMemcpyAsync(out, partial, code_bytes, cudaMemcpyDeviceToDevice, st));   // xs = partial_sample.clone()
     if (idx0 >= idx_end) return 0;
 
-    if (!resume) {
-        // ---- prefill: tokens [cond (cl) | xs_emb[0 .. idx0-1]]  (transformers.py:224-239)
-        const int Tn0 = cl + idx0;
-        RQB_TRY(launch_cond_token(cond, w.cond_emb, w.pos_emb_cond, B, cl, c.vocab_cond, E, Tn0, ws.X, st));
-        if (idx0 > 0) {
-            RQB_TRY(body_inputs(h, out, B, 0, idx0, ws, st));
-            RQB_TRY(launch_body_token(ws.LIN, w.pos_emb_hw, B, D, E, 0, idx0, cl, Tn0, ws.X, st));
-        }
-        RQB_TRY(run_stack(h, h->body, ws, B, Tn0, 0, Tb, ws.kc_body, ws.vc_body, st));
-        RQB_TRY(launch_row_add(ws.X, (int64_t)Tn0 * E, (int64_t)(Tn0 - 1) * E, nullptr, B, E, ws.CTX, st));   // latents[:, -1]
-    }
-
+    if (!resume) RQB_TRY(prefill_prefix(h, out, cond, B, idx0, ws, st));
     int64_t step = 0;
     for (int idx = idx0; idx < idx_end; idx++) {
-        if (idx > idx0 || resume) {   // decode step on the token of position idx-1 (transformers.py:240-242)
-            RQB_TRY(body_inputs(h, out, B, idx - 1, 1, ws, st));
-            RQB_TRY(launch_body_token(ws.LIN, w.pos_emb_hw, B, D, E, idx - 1, 1, 0, 1, ws.X, st));
-            RQB_TRY(run_stack(h, h->body, ws, B, 1, cl + idx - 1, Tb, ws.kc_body, ws.vc_body, st));
-            RQB_CUDA(cudaMemcpyAsync(ws.CTX, ws.X, (size_t)B * E * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        }
+        if (idx > idx0 || resume) RQB_TRY(body_step(h, out, B, idx, ws, st));   // decode step on the token of position idx-1
         for (int d = 0; d < D; d++) {
-            if (d == 0) {
-                RQB_TRY(launch_row_add(ws.CTX, E, 0, w.pos_emb_d, B, E, ws.X, st));                         // ctx + pos_emb_d[0]
-            } else if (ev & RQB200_EMB_TOK_HEAD) {
-                RQB_TRY(launch_head_cumsum(out, w.tok_emb, tes, B, HW, D, V, E, idx, d, ws.TOK, st, true));    // tok_emb(code_{d-1})
-                RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
-            } else {
-                // head_mlp(cumsum_{i<d} e_i), or head_mlp(e_{d-1}) without cumsum_depth_ctx
-                RQB_TRY(launch_head_cumsum(out, w.codebook, cbs, B, HW, D, K, C, idx, d, ws.EMB, st, (ev & RQB200_EMB_NO_CUMSUM) != 0));
-                RQB_TRY(launch_linear(ws.EMB, C, w.w_head, wd, w.b_head, nullptr, ws.TOK, E, B, E, C, 0, st));
-                RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
-            }
-            RQB_TRY(run_stack(h, h->head, ws, B, 1, d, D, ws.kc_head, ws.vc_head, st));                   // head cache restarts at d==0
-            RQB_TRY(launch_layernorm(ws.X, E, w.cls_ln_w, w.cls_ln_b, ws.XN, E, B, E, st));
             float* lg = logits_out ? logits_out + step * (int64_t)B * V : ws.LOGITS;
-            // one shared classifier, or depth d's [V,E] slice of the per-depth stack (BatchLinear, transformers.py:278-283)
-            const int64_t cd = (ev & RQB200_EMB_CLS_PER_DEPTH) ? d : 0;
-            RQB_TRY(launch_linear(ws.XN, E, (const char*)w.w_cls + cd * V * E * wsz, wd, w.b_cls + cd * V, nullptr, lg, V, B, V, E, 0, st));
+            RQB_TRY(head_depth(h, out, B, idx, d, ws, lg, st));
             const float* q = noise ? noise + step * noise_stride : nullptr;
             const int64_t off = (int64_t)idx * D + d;
             RQB_TRY(launch_sample(lg, q, B, V, temperature, top_k[d], top_p[d], out + off, force ? force + off : nullptr,
@@ -172,6 +194,27 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
         }
     }
     return 0;
+}
+
+// rqb200_ar_step on the exact tier: the launches of ar_sample_impl, split at the depth boundary, on the workspace's copy of the
+// caller's codes (ws.CODES) and without the sampler
+static int ar_step_impl(rqb200_ar* h, const int64_t* xs, int64_t xs_stride, const int64_t* cond, int B, int idx, int d, int restart,
+                        float* logits_out, void* wsp, size_t ws_bytes, cudaStream_t st) {
+    const rqb200_ar_config& c = h->cfg;
+    const int D = c.D, HW = c.H * c.W;
+    ArWs ws;
+    if (ar_layout(c, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_step: workspace too small");
+    // the codes this step consumes (as in ar_fast_step)
+    const int64_t lo = restart ? 0 : (d == 0 ? (int64_t)(idx - 1) * D : (int64_t)idx * D);
+    const int64_t hi = d == 0 ? (int64_t)idx * D : (int64_t)idx * D + d;
+    if (hi > lo)
+        RQB_CUDA(cudaMemcpy2DAsync(ws.CODES + lo, (size_t)HW * D * sizeof(int64_t), xs + lo, (size_t)xs_stride * sizeof(int64_t),
+                                   (size_t)(hi - lo) * sizeof(int64_t), (size_t)B, cudaMemcpyDeviceToDevice, st));
+    if (restart)
+        RQB_TRY(prefill_prefix(h, ws.CODES, cond, B, idx, ws, st));
+    else if (d == 0)
+        RQB_TRY(body_step(h, ws.CODES, B, idx, ws, st));
+    return head_depth(h, ws.CODES, B, idx, d, ws, logits_out, st);
 }
 
 }  // namespace rqb
@@ -245,6 +288,7 @@ int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* c
         return rqb::fail(RQB200_EINVAL, "ar_sample: null argument");
     if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "ar_sample: no CUDA device");
     if (h->cfg.weight_dtype != RQB200_F32 && !h->fast) return rqb::fail(RQB200_EINVAL, "ar_sample: 16-bit weights need the fast tier");
+    h->step_next = -1;                   // sampling reuses the caches a stepped sequence keeps: that sequence ends here
     rqb::g_launches = 0;
     int rc;
     if (h->fast)
@@ -265,6 +309,39 @@ int rqb200_ar_sample(rqb200_ar* h, const int64_t* partial, const int64_t* cond, 
     const int HW = h->cfg.H * h->cfg.W;
     return rqb200_ar_sample_span(h, partial, cond, B, std::min(start_h * h->cfg.W + start_w, HW), HW, 0, temperature, top_k_host,
                                  top_p_host, noise, noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, stream);
+}
+int rqb200_ar_step(rqb200_ar* h, const int64_t* xs, int64_t xs_batch_stride, const int64_t* cond, int B, int pos_h, int pos_w,
+                   int d, int restart, float* logits_out, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h || !xs || !logits_out || !workspace) return rqb::fail(RQB200_EINVAL, "ar_step: null argument");
+    const rqb200_ar_config& c = h->cfg;
+    if (B <= 0) return rqb::fail(RQB200_EINVAL, "ar_step: B must be > 0");
+    if (pos_h < 0 || pos_h >= c.H || pos_w < 0 || pos_w >= c.W || d < 0 || d >= c.D)
+        return rqb::fail(RQB200_EINVAL, "ar_step: position (h, w, d) out of range");
+    if (restart && d != 0) return rqb::fail(RQB200_EINVAL, "ar_step: a restart begins a position: d must be 0");
+    const int idx = pos_h * c.W + pos_w;
+    const int64_t token = (int64_t)idx * c.D + d;
+    const int64_t reads = d > 0 ? token : (int64_t)idx * c.D;      // codes of each batch row this step reads: [0, reads) at most
+    if (xs_batch_stride < reads) return rqb::fail(RQB200_EINVAL, "ar_step: xs_batch_stride is shorter than the codes this step reads");
+    if (!restart && (h->step_ws != workspace || h->step_B != B || h->step_next != token))
+        return rqb::fail(RQB200_ESTATE, "ar_step: not the token after the previous step on this workspace and batch (restart the sequence)");
+    if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "ar_step: no CUDA device");
+    if (c.weight_dtype != RQB200_F32 && !h->fast) return rqb::fail(RQB200_EINVAL, "ar_step: 16-bit weights need the fast tier");
+    h->step_next = -1;
+    rqb::g_launches = 0;
+    int rc;
+    if (h->fast)
+        rc = rqb::ar_fast_step(h->fast, xs, xs_batch_stride, cond, B, idx, d, restart, logits_out, workspace, workspace_bytes,
+                               (cudaStream_t)stream);
+    else
+        rc = rqb::ar_step_impl(h, xs, xs_batch_stride, cond, B, idx, d, restart, logits_out, workspace, workspace_bytes,
+                               (cudaStream_t)stream);
+    h->last_launches = rqb::g_launches;
+    if (rc == 0) {
+        h->step_ws = workspace;
+        h->step_B = B;
+        h->step_next = token + 1;
+    }
+    return rc;
 }
 size_t rqb200_ar_forward_workspace_bytes(const rqb200_ar* h, int B) {
     if (!h || !h->fast || B <= 0) return 0;

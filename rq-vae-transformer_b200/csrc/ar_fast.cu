@@ -24,7 +24,7 @@
 // the NEXT kernel's prologue -- for the GEMMs: filling the shared-memory ring with weight tiles -- overlaps this one.
 // Position-dependent scalars (sequence index, spatial index, token counter) live in a device-side StepState that the
 // last kernel of each graph advances, so a handful of captured graphs (cond-token body step, code-token body step, head
-// steps + sampling) are replayed for all positions without host involvement.
+// steps + sampling; for rqb200_ar_step one head depth without sampling) are replayed for all positions without host involvement.
 //
 // The prefix (cond tokens, and on a start_loc resume the code tokens before it) is prefilled in ONE pass of M = B*T row
 // GEMMs + a causal attention kernel that writes the KV cache (reference: transformers.py:237-239, attentions.py:60-104 with
@@ -793,6 +793,26 @@ __global__ void init_state_kernel(StepState* dst, StepState v, int keep_pos) {
     }
 }
 
+// Single-token step (rqb200_ar_step): the codes [lo, hi) of every batch row (flat index pos * D + depth) from the caller's xs
+// (row b at xs + b * xs_stride) into the engine's code buffer, and the step's counters into the StepState, so that the captured
+// graphs replay unchanged.  restart: the whole StepState is v (prefill from position 0); else s / idx / logits_out only.  One CTA per
+// batch row.  The caller's pointers reach the graphs only through the StepState (logits_out) or not at all (xs is read here).
+__global__ void __launch_bounds__(128)
+step_ingest_kernel(StepState* stt, StepState v, int restart, const int64_t* __restrict__ xs, int64_t xs_stride, int64_t lo, int64_t hi,
+                   int64_t row_codes) {
+    tc::pdl_launch_dependents();
+    tc::pdl_wait();
+    const int b = blockIdx.x;
+    for (int64_t i = lo + threadIdx.x; i < hi; i += 128) v.codes[(int64_t)b * row_codes + i] = xs[(int64_t)b * xs_stride + i];
+    if (b == 0 && threadIdx.x == 0) {
+        if (restart) {
+            *stt = v;
+        } else {
+            stt->s = v.s; stt->idx = v.idx; stt->step = 0; stt->logits_out = v.logits_out;
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ engine
 // One streamed weight in the engine's format: a TMA tensor map of the [N,K] 16-bit matrix, or (RQB200_E4M3) the packed E4M3 tiles and
 // their fp32 row scales.  gemm_w() is the only place that tells the two apart.
@@ -806,7 +826,8 @@ struct FastLayer {
     FastW qkv, proj, fc1, fc2;
 };
 
-enum { G_COND = 0, G_CODE = 1, G_HEAD = 2, G_HEAD_LOGITS = 3, G_COUNT = 4 };
+// G_HEAD_STEP + d: head depth d alone with its logits copied out (rqb200_ar_step), d < 8
+enum { G_COND = 0, G_CODE = 1, G_HEAD = 2, G_HEAD_LOGITS = 3, G_HEAD_STEP = 4, G_COUNT = G_HEAD_STEP + 8 };
 
 struct ArFast {
     rqb200_ar_config cfg;
@@ -821,8 +842,8 @@ struct ArFast {
     void* ws_base = nullptr;
     int B = 0;
     CUtensorMap tx_xn, tx_att, tx_h, tx_s;
-    cudaGraphExec_t graphs[G_COUNT] = {nullptr, nullptr, nullptr, nullptr};
-    int64_t n_nodes[G_COUNT] = {0, 0, 0, 0};   // kernels recorded in each graph (for the launch counter)
+    cudaGraphExec_t graphs[G_COUNT] = {};
+    int64_t n_nodes[G_COUNT] = {};       // kernels recorded in each graph (for the launch counter)
     cudaStream_t cap_stream = nullptr;   // capture never happens on the caller's stream (it may be the legacy default stream)
     bool use_graph = true, use_pdl = true, batched_prefill = true;
     int split_qkv = 4, split_proj = 12, split_fc1 = 1, split_fc2 = 12;
@@ -832,14 +853,16 @@ struct ArFast {
     mutable long long* tr_base = nullptr;
     mutable int tr_next = 0;
     mutable std::vector<std::string> tr_names;
-    int tr_graph_base[G_COUNT + 1] = {0, 0, 0, 0, 0};
+    int tr_graph_base[G_COUNT + 1] = {};
 };
 
-constexpr int TR_CAP = 4096;             // launches per trace buffer
+constexpr int TR_PER_GRAPH = 1024;                 // trace slots owned by each graph
+constexpr int TR_CAP = TR_PER_GRAPH * G_COUNT;     // launches per trace buffer
 
 struct FastWs {
     StepState* state;
     long long* trace;
+    int64_t* CODES;              // [B, HW, D] the single-token step's copy of the caller's codes (sampling writes its own `out`)
     float *XB, *XH, *P, *LOGITS;
     h16 *XN, *ATT, *Hh, *S;
     h16 *kc_body, *vc_body, *kc_head, *vc_head;
@@ -872,6 +895,7 @@ static size_t fast_layout(const ArFast& f, int B, void* base, size_t cap, FastWs
     FastWs w;
     w.state = a.take<StepState>(1);
     w.trace = a.take<long long>(4 * TR_CAP);
+    w.CODES = a.take<int64_t>((int64_t)B * HW * c.D);
     w.XB = a.take<float>(B * E);
     w.XH = a.take<float>(B * E);
     int maxs = std::max(std::max(f.split_qkv * 3, f.split_proj), std::max(f.split_fc2, f.split_fc1 * 4));
@@ -1056,37 +1080,46 @@ static int record_body(ArFast& f, FastWs& ws, bool cond_token, cudaStream_t st) 
     return 0;
 }
 
-static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st) {
+// head depth d of the position stt->idx: its token, the head stack (cache rows [0, d) from the earlier depths of this position) and
+// the classifier -> ws.LOGITS
+static int record_head_depth(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const rqb200_ar_weights& w = f.w;
     const int E = c.embed_dim, B = f.B, HW = c.H * c.W, D = c.D, V = c.vocab;
-    for (int d = 0; d < D; d++) {
-        if (d == 0) {
-            // token = spatial ctx (body output) + pos_emb_d[0]                                   (transformers.py:259-270)
-            RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, w.pos_emb_d, ws.XB, ws.kc_head, ws.vc_head, D, nullptr, 0, w.cls_ln_w,
-                               w.cls_ln_b, st));
+    if (d == 0) {
+        // token = spatial ctx (body output) + pos_emb_d[0]                                   (transformers.py:259-270)
+        RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, w.pos_emb_d, ws.XB, ws.kc_head, ws.vc_head, D, nullptr, 0, w.cls_ln_w,
+                           w.cls_ln_b, st));
+    } else {
+        if (c.embed_variant & RQB200_EMB_TOK_HEAD) {
+            // token = tok_emb(code_{d-1}) + pos_emb_d[d]                                    (transformers.py:257,267)
+            RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, 1), dim3(128), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
+                               w.tok_emb, tok_dstride(c), HW, D, c.vocab, E, d - 1, 1, 1, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
+                               ws.XH));
         } else {
-            if (c.embed_variant & RQB200_EMB_TOK_HEAD) {
-                // token = tok_emb(code_{d-1}) + pos_emb_d[d]                                    (transformers.py:257,267)
-                RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, 1), dim3(128), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
-                                   w.tok_emb, tok_dstride(c), HW, D, c.vocab, E, d - 1, 1, 1, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
-                                   ws.XH));
-            } else {
-                // token = head_mlp(sum_{i<d} e_i, or e_{d-1} alone) + pos_emb_d[d]              (transformers.py:250-255,267)
-                RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
-                                   cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf,
-                                   (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
-                RQB_TRY(gemm(f, "w_head", f.w_head, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
-                             w.pos_emb_d + (int64_t)d * E, 0, nullptr, 0, st));
-            }
-            RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, nullptr, ws.XH, ws.kc_head, ws.vc_head, D, nullptr, d, w.cls_ln_w,
-                               w.cls_ln_b, st));
+            // token = head_mlp(sum_{i<d} e_i, or e_{d-1} alone) + pos_emb_d[d]              (transformers.py:250-255,267)
+            RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
+                               cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf,
+                               (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
+            RQB_TRY(gemm(f, "w_head", f.w_head, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
+                         w.pos_emb_d + (int64_t)d * E, 0, nullptr, 0, st));
         }
-        // classifier: LN(x) (fused into the stack's last launch) -> logits                       (transformers.py:278-285)
-        // per-depth classifiers (BatchLinear): depth d's [V,E] slice and bias row
-        const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
-        RQB_TRY(gemm(f, "cls", pd ? f.w_cls_d[d] : f.w_cls, f.tx_xn, V, E, B, 1, GT_F32, w.b_cls + (pd ? (int64_t)d * V : 0), 1.f,
-                     ws.LOGITS, nullptr, nullptr, 0, nullptr, 0, st));
+        RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, nullptr, ws.XH, ws.kc_head, ws.vc_head, D, nullptr, d, w.cls_ln_w,
+                           w.cls_ln_b, st));
+    }
+    // classifier: LN(x) (fused into the stack's last launch) -> logits                       (transformers.py:278-285)
+    // per-depth classifiers (BatchLinear): depth d's [V,E] slice and bias row
+    const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
+    RQB_TRY(gemm(f, "cls", pd ? f.w_cls_d[d] : f.w_cls, f.tx_xn, V, E, B, 1, GT_F32, w.b_cls + (pd ? (int64_t)d * V : 0), 1.f,
+                 ws.LOGITS, nullptr, nullptr, 0, nullptr, 0, st));
+    return 0;
+}
+
+static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st) {
+    const rqb200_ar_config& c = f.cfg;
+    const int B = f.B, HW = c.H * c.W, D = c.D, V = c.vocab;
+    for (int d = 0; d < D; d++) {
+        RQB_TRY(record_head_depth(f, ws, d, st));
         if (with_logits)
             RQB_TRY(launch_pdl(logits_copy_kernel, dim3(64), dim3(256), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
                                (const float*)ws.LOGITS, d, (int64_t)B * V));
@@ -1096,12 +1129,23 @@ static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st)
     return 0;
 }
 
+// the single-token step's head graph: depth d only, its logits to stt->logits_out (stt->step == 0), no sampler; the code of depth d
+// comes from the caller at the next step.  Launch for launch the depth-d part of record_head: the same logits, bit for bit.
+static int record_head_step(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
+    RQB_TRY(record_head_depth(f, ws, d, st));
+    RQB_TRY(launch_pdl(logits_copy_kernel, dim3(64), dim3(256), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
+                       (const float*)ws.LOGITS, 0, (int64_t)f.B * f.cfg.vocab));
+    if (d == f.cfg.D - 1) RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, f.use_pdl, ws.state, 0, 1, 0));
+    return 0;
+}
+
 static int record(ArFast& f, FastWs& ws, int which, cudaStream_t st) {
     f.tr_base = ws.trace;
     f.tr_next = f.tr_graph_base[which];
     int rc = which == G_COND ? record_body(f, ws, true, st) : which == G_CODE ? record_body(f, ws, false, st)
-                                                                                : record_head(f, ws, which == G_HEAD_LOGITS, st);
-    // trace slots: every graph owns a quarter of the buffer
+           : which >= G_HEAD_STEP ? record_head_step(f, ws, which - G_HEAD_STEP, st)
+                                  : record_head(f, ws, which == G_HEAD_LOGITS, st);
+    // trace slots: every graph owns TR_PER_GRAPH of the buffer
     return rc;
 }
 
@@ -1435,11 +1479,56 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
     return rc;
 }
 
+// (re)binds the activation tensor maps + graphs to the workspace wsp at batch B
+static int bind(ArFast& f, const FastWs& ws, void* wsp, int B) {
+    const rqb200_ar_config& c = f.cfg;
+    const int E = c.embed_dim;
+    drop_graphs(f);
+    f.ws_base = nullptr;
+    const uint32_t bn = act_box(f, B);
+    RQB_TRY(make_tmap_2d(&f.tx_xn, ws.XN, 1, E, B, (uint64_t)E * 2, 64, bn));
+    RQB_TRY(make_tmap_2d(&f.tx_att, ws.ATT, 1, E, B, (uint64_t)E * 2, 64, bn));
+    RQB_TRY(make_tmap_2d(&f.tx_h, ws.Hh, 1, 4 * E, B, (uint64_t)E * 8, 64, bn));
+    RQB_TRY(make_tmap_2d(&f.tx_s, ws.S, 1, c.code_dim, B, (uint64_t)c.code_dim * 2, 64, bn));
+    f.ws_base = wsp;
+    f.B = B;
+    return 0;
+}
+
+// one captured graph (captured on first use), or its launches recorded straight onto the stream (RQB200_AR_NO_GRAPH)
+static int run_graph(ArFast& f, FastWs& ws, int which, cudaStream_t st) {
+    if (!f.use_graph) return record(f, ws, which, st);
+    if (!f.graphs[which]) RQB_TRY(capture(f, ws, which, &f.graphs[which]));
+    RQB_CUDA(cudaGraphLaunch(f.graphs[which], st));
+    g_launches += f.n_nodes[which];      // kernels executed by this replay
+    return 0;
+}
+
+// prefill: cond tokens, then (start_loc resume) the code tokens of positions < idx_begin (transformers.py:237-239), from a StepState
+// with s = idx = 0.  Leaves state.idx = idx_begin, state.s = cond_len + idx_begin, ws.XB = the last prefix token's output rows.
+static int prefill_prefix(ArFast& f, FastWs& ws, int idx_begin, cudaStream_t st) {
+    const int T0 = f.cfg.cond_len + idx_begin;
+    if (f.batched_prefill && T0 >= 4 && (int64_t)f.B * T0 <= ws.Mmax) {
+        RQB_TRY(prefill_batched(f, ws, T0, st));
+        // state.idx must equal idx_begin for the first head graph
+        if (idx_begin > 0) RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, idx_begin, 0));
+    } else {
+        // one cached step each -- causal, so identical to the batched form
+        for (int s = 0; s < f.cfg.cond_len; s++) RQB_TRY(run_graph(f, ws, G_COND, st));
+        // state.idx must equal (position whose codes feed the body) + 1 while replaying the code-token graph
+        for (int j = 1; j <= idx_begin; j++) {
+            RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, 1, 0));
+            RQB_TRY(run_graph(f, ws, G_CODE, st));
+        }
+    }
+    return 0;
+}
+
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
                    float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st) {
     const rqb200_ar_config& c = f->cfg;
-    const int E = c.embed_dim, D = c.D, HW = c.H * c.W, cl = c.cond_len;
+    const int D = c.D, HW = c.H * c.W;
     if (B < 1 || B > 256) return fail(RQB200_EINVAL, "ar fast tier: batch must be in [1,256] per call");
     if (idx_begin < 0 || idx_end > HW || idx_begin > idx_end) return fail(RQB200_EINVAL, "ar_sample: bad position span");
     FastWs ws;
@@ -1448,16 +1537,9 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
     if (!resume && out != partial)
         RQB_CUDA(cudaMemcpyAsync(out, partial, (size_t)B * HW * D * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
     if (idx_begin >= idx_end) return 0;
-    if (f->ws_base != wsp || f->B != B) {        // (re)bind activation tensor maps + graphs to this workspace
+    if (f->ws_base != wsp || f->B != B) {
         if (resume) return fail(RQB200_ESTATE, "ar_sample: resume on a workspace / batch the engine is not bound to");
-        drop_graphs(*f);
-        f->ws_base = wsp;
-        f->B = B;
-        const uint32_t bn = act_box(*f, B);
-        RQB_TRY(make_tmap_2d(&f->tx_xn, ws.XN, 1, E, B, (uint64_t)E * 2, 64, bn));
-        RQB_TRY(make_tmap_2d(&f->tx_att, ws.ATT, 1, E, B, (uint64_t)E * 2, 64, bn));
-        RQB_TRY(make_tmap_2d(&f->tx_h, ws.Hh, 1, 4 * E, B, (uint64_t)E * 8, 64, bn));
-        RQB_TRY(make_tmap_2d(&f->tx_s, ws.S, 1, c.code_dim, B, (uint64_t)c.code_dim * 2, 64, bn));
+        RQB_TRY(bind(*f, ws, wsp, B));
     }
     StepState h = {};
     h.s = 0; h.idx = 0; h.step = 0;
@@ -1466,36 +1548,43 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
     for (int d = 0; d < D; d++) { h.top_k[d] = top_k[d]; h.top_p[d] = top_p[d]; }
     RQB_TRY(launch_pdl(init_state_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, h, resume ? 1 : 0));
     if (f->trace && !resume) RQB_CUDA(cudaMemsetAsync(ws.trace, 0, (size_t)4 * TR_CAP * sizeof(long long), st));
-    auto run = [&](int which) -> int {
-        if (!f->use_graph) return record(*f, ws, which, st);
-        if (!f->graphs[which]) RQB_TRY(capture(*f, ws, which, &f->graphs[which]));
-        RQB_CUDA(cudaGraphLaunch(f->graphs[which], st));
-        g_launches += f->n_nodes[which];     // kernels executed by this replay
-        return 0;
-    };
     const int head_graph = logits_out ? G_HEAD_LOGITS : G_HEAD;
-    if (!resume) {
-        // prefill: cond tokens, then (start_loc resume) the code tokens of positions < idx_begin  (transformers.py:237-239)
-        const int T0 = cl + idx_begin;
-        if (f->batched_prefill && T0 >= 4 && (int64_t)B * T0 <= ws.Mmax) {
-            RQB_TRY(prefill_batched(*f, ws, T0, st));
-            // state.idx must equal idx_begin for the first head graph
-            if (idx_begin > 0) RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, idx_begin, 0));
-        } else {
-            // one cached step each -- causal, so identical to the batched form
-            for (int s = 0; s < cl; s++) RQB_TRY(run(G_COND));
-            // state.idx must equal (position whose codes feed the body) + 1 while replaying the code-token graph
-            for (int j = 1; j <= idx_begin; j++) {
-                RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, 1, 0));
-                RQB_TRY(run(G_CODE));
-            }
-        }
-    }
+    if (!resume) RQB_TRY(prefill_prefix(*f, ws, idx_begin, st));
     for (int idx = idx_begin; idx < idx_end; idx++) {
-        if (idx > idx_begin || resume) RQB_TRY(run(G_CODE));   // body step on the token of position idx-1 (state.idx == idx)
-        RQB_TRY(run(head_graph));                              // D head steps + sampling; advances idx, step
+        if (idx > idx_begin || resume) RQB_TRY(run_graph(*f, ws, G_CODE, st));   // body step on the token of position idx-1 (state.idx == idx)
+        RQB_TRY(run_graph(*f, ws, head_graph, st));                              // D head steps + sampling; advances idx, step
     }
     return 0;
+}
+
+int ar_fast_step(ArFast* f, const int64_t* xs, int64_t xs_stride, const int64_t* cond, int B, int idx, int d, int restart,
+                 float* logits_out, void* wsp, size_t ws_bytes, cudaStream_t st) {
+    const rqb200_ar_config& c = f->cfg;
+    const int D = c.D, HW = c.H * c.W, cl = c.cond_len;
+    if (B < 1 || B > 256) return fail(RQB200_EINVAL, "ar fast tier: batch must be in [1,256] per call");
+    FastWs ws;
+    if (fast_layout(*f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_step: workspace too small");
+    if (f->ws_base != wsp || f->B != B) {
+        if (!restart) return fail(RQB200_ESTATE, "ar_step: continuing on a workspace / batch the engine is not bound to");
+        RQB_TRY(bind(*f, ws, wsp, B));
+    }
+    // the codes this step consumes: restart -> positions [0, idx) for the prefill; d == 0 -> position idx-1 for the body step;
+    // d > 0 -> codes 0 .. d-1 of position idx for the head token
+    const int64_t lo = restart ? 0 : (d == 0 ? (int64_t)(idx - 1) * D : (int64_t)idx * D);
+    const int64_t hi = d == 0 ? (int64_t)idx * D : (int64_t)idx * D + d;
+    StepState v = {};
+    v.cond = cond; v.codes = ws.CODES; v.logits_out = logits_out;
+    v.s = restart ? 0 : (d == 0 ? cl + idx - 1 : cl + idx);   // body keys cached before the token the next body step appends
+    v.idx = restart ? 0 : idx;                                  // (a restart's prefill advances idx itself, as in ar_fast_sample)
+    RQB_TRY(launch_pdl(step_ingest_kernel, dim3(B), dim3(128), (size_t)0, st, false, ws.state, v, restart, xs, xs_stride, lo, hi,
+                       (int64_t)HW * D));
+    if (restart) {
+        if (f->trace) RQB_CUDA(cudaMemsetAsync(ws.trace, 0, (size_t)4 * TR_CAP * sizeof(long long), st));
+        RQB_TRY(prefill_prefix(*f, ws, idx, st));
+    } else if (d == 0) {
+        RQB_TRY(run_graph(*f, ws, G_CODE, st));                  // body step on the codes of position idx-1
+    }
+    return run_graph(*f, ws, G_HEAD_STEP + d, st);
 }
 
 int ar_fast_trace(ArFast* f, long long* out_host, int cap_launches, char* names, int names_cap) {

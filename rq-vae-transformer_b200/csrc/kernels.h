@@ -112,7 +112,7 @@ int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes_log2, uint64
 struct StepState {
     int s;          // body sequence index of the token being processed (= cached body keys before it)
     int idx;        // spatial position whose codes are being sampled
-    int step;       // tokens sampled so far in this call (indexes noise / logits_out)
+    int step;       // tokens sampled so far in this call (indexes noise / logits_out); 0 in a single-token step
     int pad;
     const int64_t* cond;      // [B, cond_len] or null
     int64_t* codes;           // [B, HW, D] working copy (xs)
@@ -135,6 +135,9 @@ size_t ar_fast_workspace_bytes(const ArFast* f, int B);
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
                    float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st);
+// the logits of ONE token (idx, d) into logits_out [B,V] (rqb200_ar_step; arguments already checked by the caller)
+int ar_fast_step(ArFast* f, const int64_t* xs, int64_t xs_stride, const int64_t* cond, int B, int idx, int d, int restart,
+                 float* logits_out, void* wsp, size_t ws_bytes, cudaStream_t st);
 size_t ar_fast_forward_workspace_bytes(const ArFast* f, int B);
 int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B, float* logits_out, float* cond_logits_out, void* wsp,
                     size_t ws_bytes, cudaStream_t st);

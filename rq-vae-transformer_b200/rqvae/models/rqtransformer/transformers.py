@@ -2,7 +2,7 @@
 
 Boundary kept (SURVEY.md section 8b): constructor from an ``RQTransformerConfig``-shaped object, parameter names
 (state_dict layout A.3), ``sample`` :294-307 (same signature; ``fast``/``cached``/``is_tqdm``/``desc`` accepted),
-``cached_forward`` :191, ``init_cache`` :289, ``get_block_size``, attributes ``block_size`` / ``block_size_cond`` /
+``cached_forward`` :191 (stateful after ``init_cache``: one native token step per call, ``rqb200_ar_step``), ``init_cache`` :289, ``get_block_size``, attributes ``block_size`` / ``block_size_cond`` /
 ``vocab_size``.  The (h,w,d) loop, KV caches, embedding glue, classifier and ``sample_from_logits`` all run inside
 ``rqb200_ar_sample`` (csrc/ar_engine.cu): one native call per ``sample``, no per-token host work.
 
@@ -101,6 +101,7 @@ class RQTransformer(Stage2Model):
         self._eng = {}
         self._eng_fp = None
         self._cache = None
+        self._step = None                        # the stepped cached_forward sequence (init_cache / _step_route)
         self.last_launches = 0
 
     # ------------------------------------------------------------------ native engine plumbing
@@ -108,6 +109,7 @@ class RQTransformer(Stage2Model):
         for e in self._eng.values():
             N.lib().rqb200_ar_destroy(e["handle"])
         self._eng = {}
+        self._step = None                        # its KV caches lived in the engines' workspaces
 
     def _apply(self, fn, *a, **k):
         self._invalidate_native()
@@ -187,7 +189,7 @@ class RQTransformer(Stage2Model):
             self._invalidate_native()
             self._eng_fp = fp
         key = (str(dev), mode, cb_id, slot)
-        if key not in self._eng and slot > 0:
+        if key not in self._eng and slot != 0:
             # engines of one model share the packed weights of slot 0; each slot owns its workspace, KV cache and graphs
             base = self._engine(codebook, mode, 0)
             eng = dict(base, handle=base["make"](), ws=None)
@@ -324,8 +326,10 @@ class RQTransformer(Stage2Model):
 
     # ------------------------------------------------------------------ reference surface
     def init_cache(self):
-        """transformers.py:289-292 -- KV state lives inside one native call; nothing persists between calls"""
+        """transformers.py:289-292 -- ends any stepped cached_forward sequence; the next cached_forward at some (h, w, 0) starts a
+        new one (sample() keeps its KV state inside its own native call)"""
         self._cache = {"spatial_ctx_hw": None}
+        self._step = {"armed": True}
 
     def _lists(self, top_k, top_p):
         D = self.block_size[2]
@@ -427,7 +431,7 @@ class RQTransformer(Stage2Model):
         slot of the last replay of each captured graph -- where the time of one AR position goes"""
         rows = []
         for key, eng in self._eng.items():
-            cap = 4096
+            cap = 12288                          # TR_CAP of csrc/ar_fast.cu: 1024 slots for each of its 12 graphs
             buf = (C.c_longlong * (4 * cap))()
             names = C.create_string_buffer(cap * 16)
             n = N.lib().rqb200_ar_trace(eng["handle"], buf, cap, names, len(names))
@@ -447,10 +451,70 @@ class RQTransformer(Stage2Model):
         self.init_cache()
         return out
 
+    def _step_key(self, B, mode, codebook, cond, device):
+        """what a stepped sequence must keep from call to call: batch, tier, the codebook tables and the cond tensor (compared by
+        storage, not by value: reading them back would synchronise every call)"""
+        tabs = None if codebook is None else (tuple(t.data_ptr() for t in codebook) if isinstance(codebook, list) else codebook.data_ptr())
+        cnd = None if cond is None else (cond.data_ptr(), tuple(cond.shape), cond.dtype)
+        return (B, mode, tabs, cnd, str(device))
+
+    def _step_route(self, key, loc, n_codes):
+        """'restart', 'continue' or None (stateless evaluation) for a cached_forward at loc = (h, w, d) with the sequence key `key`
+        over xs holding n_codes codes per batch row; updates the sequence record.
+          restart:  the first call after init_cache(), at some (h, w, 0) -- the reference prefills the prefix then (:237-239);
+          continue: the token after the previous call's, in raster order, with the same key.
+        Any other call is evaluated statelessly.  One with the sequence's key ends the sequence (the reference would append a
+        duplicate or misplaced KV entry, or fail); one with another key (another batch, tier, cond or codebook) leaves it alone."""
+        H, W, D = self.block_size
+        h, w, d = loc
+        st = self._step
+        if st is None:
+            return None
+        if not (0 <= h < H and 0 <= w < W and 0 <= d < D):
+            return None
+        t = (h * W + w) * D + d
+        if n_codes < (t if d > 0 else (h * W + w) * D):          # xs lacks codes the step reads: let the stateless path zero-pad
+            if not st.get("armed") and st["key"] == key:
+                self._step = None
+            return None
+        if st.get("armed"):
+            if d != 0:
+                self._step = None
+                return None
+            self._step = {"key": key, "next": t + 1, "engines": None}
+            return "restart"
+        if st["key"] != key:
+            return None
+        if st["next"] != t:
+            self._step = None
+            return None
+        st["next"] = t + 1
+        return "continue"
+
     @torch.no_grad()
     def cached_forward(self, xs, model_aux=None, cond=None, amp=False, sample_loc=(0, 0, 0)):
-        """transformers.py:190-287 -- logits [B,V] for one (h,w,d).  Stateless re-evaluation: the prefix in ``xs`` is
-        teacher-forced through the native loop and the requested step's logits are returned."""
+        """transformers.py:190-287 -- logits [B,V] for one (h,w,d).
+        After init_cache(), calls in raster order from some (h, w, 0) (the reference's own loop) run one native token step each
+        (rqb200_ar_step): the first prefills cond and the positions before it from ``xs``, every later one appends one body token
+        (d == 0) and runs one head depth, on KV caches kept in engine slots of their own.  Like the reference, ``cond`` is read by
+        the first call only and later calls read only the codes the step consumes.  Any other call pattern is evaluated
+        statelessly: the prefix in ``xs`` is teacher-forced through the native loop and the requested step's logits returned."""
+        h, w, d = (int(v) for v in sample_loc)
+        H, W, D = self.block_size
+        B = xs.shape[0]
+        route = None
+        if self._step is not None and xs.dim() == 4 and tuple(xs.shape[2:]) == (W, D):
+            codebook = self._codebook_of(model_aux, D)
+            mode = self._mode(amp)
+            key = self._step_key(B, mode, codebook, cond, xs.device)
+            route = self._step_route(key, (h, w, d), xs.shape[1] * W * D)
+        if route is not None:
+            out = self._native_step(route, xs, codebook, cond, mode, (h, w, d))
+            if out is not None:
+                return out
+        return self._stateless_cached_forward(xs, model_aux, cond, amp, (h, w, d))
+
+    def _stateless_cached_forward(self, xs, model_aux, cond, amp, sample_loc):
         h, w, d = sample_loc
         H, W, D = self.block_size
         B = xs.shape[0]
@@ -459,6 +523,59 @@ class RQTransformer(Stage2Model):
         _, logits = self._native_sample(full, model_aux, cond, (0, 0), 1.0, None, None, amp, noise=False,
                                         return_logits=True, force_codes=full)
         return logits[(h * W + w) * D + d]
+
+    @torch.no_grad()
+    def _native_step(self, route, xs, codebook, cond, mode, loc):
+        """one rqb200_ar_step per batch chunk (fast tier: equal chunks of at most 256 rows, as _native_sample), each on its own
+        engine slot ("step", chunk).  None when the slots were rebuilt since the sequence began (weights written, .to(...)): the
+        stale caches are gone and the caller evaluates statelessly."""
+        H, W, D = self.block_size
+        h, w, d = loc
+        B, V, cl = xs.shape[0], self.vocab_size[0], self.block_size_cond
+        dev = self.pos_emb_hw.device
+        N.require_cuda(xs, cond, self.pos_emb_hw)
+        bounds = [(0, B)]
+        if mode == N.MODE_FAST and B > 256:
+            n_chunks = -(-B // 256)
+            bounds = [(i * B // n_chunks, (i + 1) * B // n_chunks) for i in range(n_chunks)]
+        st = self._step
+        restart = route == "restart"
+        try:
+            engines = [self._engine(codebook, mode, ("step", i)) for i in range(len(bounds))]
+            if self._step is not st:                 # _engine found the weights changed and dropped every engine and the sequence
+                if not restart:
+                    return None
+                self._step = st                      # (a sequence that begins now has no stale state)
+            if restart:
+                st["engines"] = engines
+            elif any(a is not b for a, b in zip(engines, st["engines"])):
+                self._step = None
+                return None
+            if xs.dtype != torch.int64 or xs.stride()[1:] != (W * D, D, 1):
+                xs = xs.to(torch.int64).contiguous()
+            stride = xs.stride(0) if B > 1 else xs.shape[1] * W * D
+            cond_t = None if (cond is None or not restart) else cond.reshape(B, cl).to(torch.int64).contiguous()
+            out = torch.empty(B, V, dtype=torch.float32, device=dev)
+            L = N.lib()
+            launches = 0
+            with torch.cuda.device(dev):
+                stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+                for eng, (lo, hi) in zip(engines, bounds):
+                    if restart:                      # (sized when a sequence begins; its batch stays until the next one)
+                        need = L.rqb200_ar_workspace_bytes(eng["handle"], hi - lo)
+                        if eng["ws"] is None or eng["ws"].numel() < need:
+                            eng["ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+                    N.check(L.rqb200_ar_step(
+                        eng["handle"], C.c_void_p(xs.data_ptr() + lo * stride * 8), stride,
+                        C.c_void_p(cond_t.data_ptr() + lo * cl * 8) if cond_t is not None else C.c_void_p(0), hi - lo, h, w, d,
+                        int(restart), C.c_void_p(out.data_ptr() + lo * V * 4), N.ptr(eng["ws"]), eng["ws"].numel(), stream), "ar_step")
+                    launches += L.rqb200_ar_last_launches(eng["handle"])
+        except BaseException:
+            self._step = None
+            raise
+        self.last_launches = launches
+        N.launch_count["total"] += launches
+        return out
 
     def forward(self, xs, model_aux=None, cond=None, amp=False):
         """transformers.py:113-188 -- teacher-forced logits [B,H,W,D,V]; with cond_len > 1 also the cond logits
