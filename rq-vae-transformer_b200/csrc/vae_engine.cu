@@ -34,6 +34,18 @@ struct rqb200_vae {
 
 namespace rqb {
 
+// What a conv reads: an fp32 activation for the exact-tier kernel, which folds the nearest x2 upsample and an NCHW layout into
+// its indexing, or, for the wgmma kernel, the fp16 hi/lo copy in h16[slot] / l16[slot], already upsampled by the cast.
+struct Operand {
+    const float* x;
+    int slot;                 // -1: the fp32 activation x
+    int upsample;
+    int nchw;
+};
+
+// One walk per network serves both tiers: the tier lives in operand / norm / conv, each of which branches on `fast`.  The
+// exact tier runs every conv and GroupNorm on the fp32 FFMA kernels; the fast tier (fast_ok: every channel count a multiple of
+// 128) runs them on the wgmma implicit GEMM with fp16 operands.
 struct VaeRun {
     rqb200_vae* h;
     cudaStream_t st;
@@ -42,104 +54,14 @@ struct VaeRun {
     float* buf[4];
     double* gn_ws;
     std::string missing;
-    __half* h16[2] = {nullptr, nullptr};      // fast tier: fp16 conv operands (GN output / cast / upsampled cast)
+    __half* h16[2] = {nullptr, nullptr};      // fp16 conv operands (GN output / cast / upsampled cast)
     __half* l16[2] = {nullptr, nullptr};      // their fp16 'lo' halves (split-fp16 products); null -> single product
-    bool fast = false;
+    float* zq = nullptr;                      // decode_code's staging buffer for the embedded codes
+    bool fast = false;                        // the walk's tier, set by decode / encode
 
-    // ---- fast tier helpers (wgmma implicit GEMM; decoder only, C % 128 == 0 everywhere)
-    // want_stats: the output feeds a GroupNorm next -> its epilogue emits the GroupNorm partial statistics (no gn_stats pass)
+    // fast tier: a conv whose output feeds a GroupNorm emits that GroupNorm's partial statistics from its epilogue
     const float* stats_buf = nullptr;         // conv output whose statistics sit in gn_ws
     int stats_chunks = 0;
-    int conv_f(const std::string& name, const __half* in16, float* out, const float* resid, int Hh, int Ww, int Cin, int Cout,
-               int ks, int out_nchw, int stride = 1, bool want_stats = false) {
-        const VTensor* w = get(name + ".weight", (int64_t)Cout * ks * ks * Cin);
-        const VTensor* b = get(name + ".bias", Cout);
-        note_act((int64_t)Hh * Ww, Cout);
-        if (dry || !w || !b) return 0;
-        if (w->dtype != RQB200_F16) return fail(RQB200_ESTATE, "vae fast tier: conv weights must be fp16: " + name);
-        const __half* in_lo = nullptr;
-        const void* w_lo = nullptr;
-        if (h->split) {
-            const VTensor* wl = get(name + ".weight_lo", (int64_t)Cout * ks * ks * Cin);
-            if (!wl) return 0;
-            w_lo = wl->ptr;
-            in_lo = in16 == h16[0] ? l16[0] : l16[1];
-        }
-        const bool fuse = want_stats && h->gn_fuse && !out_nchw && conv_tc_gn_fusable(Hh, Ww, Cout, ks, stride);
-        stats_buf = fuse ? out : nullptr;
-        stats_chunks = fuse ? Hh * Ww / 32 : 0;
-        return launch_conv_tc(in16, w->ptr, in_lo, w_lo, (const float*)b->ptr, resid, out, B, Hh, Ww, Cin, Cout, ks, out_nchw, st, stride,
-                              fuse ? gn_ws : nullptr);
-    }
-    int gn_f(const std::string& name, const float* in, __half* out16, int HW, int C, int silu) {
-        const VTensor* g = get(name + ".weight", C);
-        const VTensor* b = get(name + ".bias", C);
-        if (HW > h->max_gn_hw) h->max_gn_hw = HW;
-        if (dry || !g || !b) return 0;
-        const int fused = (in == stats_buf) ? stats_chunks : 0;
-        stats_buf = nullptr;
-        return launch_groupnorm_f16(in, (const float*)g->ptr, (const float*)b->ptr, out16, out16 == h16[0] ? l16[0] : l16[1], gn_ws, B, HW, C, silu, st,
-                                    fused);
-    }
-    int resblock_f(const std::string& p, int cur, int Hh, int Ww, int Cin, int Cout, int* rc) {
-        int a = (cur + 1) & 3, b = (cur + 2) & 3, c = (cur + 3) & 3;
-        (void)a;
-        *rc = gn_f(p + ".norm1", buf[cur], h16[0], Hh * Ww, Cin, 1); if (*rc) return cur;
-        *rc = conv_f(p + ".conv1", h16[0], buf[b], nullptr, Hh, Ww, Cin, Cout, 3, 0, 1, true); if (*rc) return cur;
-        *rc = gn_f(p + ".norm2", buf[b], h16[0], Hh * Ww, Cout, 1); if (*rc) return cur;
-        const float* res = buf[cur];
-        if (Cin != Cout) {
-            if (!dry) { *rc = launch_cast_f16(buf[cur], h16[1], l16[1], B, Hh, Ww, Cin, 0, st); if (*rc) return cur; }
-            *rc = conv_f(p + ".nin_shortcut", h16[1], buf[c], nullptr, Hh, Ww, Cin, Cout, 1, 0); if (*rc) return cur;
-            res = buf[c];
-        }
-        *rc = conv_f(p + ".conv2", h16[0], buf[b], res, Hh, Ww, Cout, Cout, 3, 0, 1, true);
-        return b;
-    }
-    int attnblock_f(const std::string& p, int cur, int Hh, int Ww, int C, int* rc) {
-        int a = (cur + 1) & 3, b = (cur + 2) & 3, c = (cur + 3) & 3;
-        *rc = gn_f(p + ".norm", buf[cur], h16[0], Hh * Ww, C, 0); if (*rc) return cur;
-        *rc = conv_f(p + ".qkv", h16[0], buf[b], nullptr, Hh, Ww, C, 3 * C, 1, 0); if (*rc) return cur;
-        if (!dry && missing.empty()) {
-            *rc = launch_vae_attn(buf[b], buf[a], B, Hh * Ww, C, st); if (*rc) return cur;
-            *rc = launch_cast_f16(buf[a], h16[0], l16[0], B, Hh, Ww, C, 0, st); if (*rc) return cur;
-        }
-        *rc = conv_f(p + ".proj_out", h16[0], buf[c], buf[cur], Hh, Ww, C, C, 1, 0, 1, true);
-        return c;
-    }
-    int decode_fast(const float* z, float* out) {
-        const rqb200_vae_config& c = h->cfg;
-        const int nl = c.n_levels, nb = c.num_res_blocks;
-        int res = c.resolution >> (nl - 1), rc = 0;
-        int ch = c.ch * c.ch_mult[nl - 1];
-        int cur = 0;
-        if (!dry) { rc = launch_cast_f16(z, h16[0], l16[0], B, res, res, c.embed_dim, 0, st); if (rc) return rc; }
-        rc = conv_f("post_quant_conv", h16[0], buf[1], nullptr, res, res, c.embed_dim, c.z_channels, 1, 0); if (rc) return rc;
-        if (!dry) { rc = launch_cast_f16(buf[1], h16[0], l16[0], B, res, res, c.z_channels, 0, st); if (rc) return rc; }
-        rc = conv_f("decoder.conv_in", h16[0], buf[0], nullptr, res, res, c.z_channels, ch, 3, 0, 1, true); if (rc) return rc;
-        cur = resblock_f("decoder.mid.block_1", cur, res, res, ch, ch, &rc); if (rc) return rc;
-        cur = attnblock_f("decoder.mid.attn_1", cur, res, res, ch, &rc); if (rc) return rc;
-        cur = resblock_f("decoder.mid.block_2", cur, res, res, ch, ch, &rc); if (rc) return rc;
-        for (int lvl = nl - 1; lvl >= 0; lvl--) {
-            int cout = c.ch * c.ch_mult[lvl];
-            for (int b = 0; b <= nb; b++) {
-                std::string p = "decoder.up." + std::to_string(lvl);
-                cur = resblock_f(p + ".block." + std::to_string(b), cur, res, res, ch, cout, &rc); if (rc) return rc;
-                ch = cout;
-                if (has_attn(res)) { cur = attnblock_f(p + ".attn." + std::to_string(b), cur, res, res, ch, &rc); if (rc) return rc; }
-            }
-            if (lvl != 0) {
-                int nxt = (cur + 1) & 3;
-                if (!dry) { rc = launch_cast_f16(buf[cur], h16[1], l16[1], B, res, res, ch, 1, st); if (rc) return rc; }   // x2 nearest, fp16
-                rc = conv_f("decoder.up." + std::to_string(lvl) + ".upsample.conv", h16[1], buf[nxt], nullptr, 2 * res, 2 * res, ch, ch, 3, 0, 1, true);
-                if (rc) return rc;
-                cur = nxt;
-                res *= 2;
-            }
-        }
-        rc = gn_f("decoder.norm_out", buf[cur], h16[0], res * res, ch, 1); if (rc) return rc;
-        return conv_f("decoder.conv_out", h16[0], out, nullptr, res, res, ch, c.out_ch, 3, 1);
-    }
 
     const VTensor* get(const std::string& k, int64_t numel) {
         auto it = h->t.find(k);
@@ -151,51 +73,90 @@ struct VaeRun {
     }
     void note_act(int64_t hw, int64_t c) { if (hw * c > h->max_act) h->max_act = hw * c; }
 
-    int conv(const std::string& name, const float* in, float* out, const float* resid, int Hi, int Wi, int Cin, int Cout,
-             int ks, int stride, int upsample, int in_nchw, int out_nchw) {
-        ConvGeom g;
-        g.B = B; g.Hi = Hi; g.Wi = Wi; g.Cin = Cin; g.Cout = Cout; g.KH = g.KW = ks; g.stride = stride;
-        g.upsample = upsample; g.in_nchw = in_nchw; g.out_nchw = out_nchw;
-        g.pad = (ks == 3 && stride == 1) ? 1 : 0;
-        int Hv = upsample ? 2 * Hi : Hi, Wv = upsample ? 2 * Wi : Wi;
-        g.Ho = stride == 2 ? Hv / 2 : Hv;
-        g.Wo = stride == 2 ? Wv / 2 : Wv;
-        const VTensor* w = get(name + ".weight", (int64_t)Cout * ks * ks * Cin);
-        const VTensor* b = get(name + ".bias", Cout);
-        note_act((int64_t)g.Ho * g.Wo, Cout);
-        if (dry || !w || !b) return 0;
-        return launch_conv(in, w->ptr, w->dtype, (const float*)b->ptr, resid, out, g, st);
+    // x as a conv operand: itself on the exact tier; on the fast tier its fp16 copy, cast into slot (x2 nearest upsampled if asked)
+    int operand(const float* x, int H, int W, int C, int slot, int upsample, Operand* o) {
+        *o = fast ? Operand{nullptr, slot, upsample, 0} : Operand{x, -1, upsample, 0};
+        if (!fast || dry) return 0;
+        return launch_cast_f16(x, h16[slot], l16[slot], B, H, W, C, upsample, st);
     }
-    int gn(const std::string& name, const float* in, float* out, int HW, int C, int silu) {
+    // GroupNorm (+ SiLU) of in: into out on the exact tier, into slot 0 on the fast tier (from fused statistics where the
+    // producing conv emitted them)
+    int norm(const std::string& name, const float* in, float* out, int HW, int C, int silu, Operand* o) {
         const VTensor* g = get(name + ".weight", C);
         const VTensor* b = get(name + ".bias", C);
         if (HW > h->max_gn_hw) h->max_gn_hw = HW;
         note_act(HW, C);
+        *o = fast ? Operand{nullptr, 0, 0, 0} : Operand{out, -1, 0, 0};
         if (dry || !g || !b) return 0;
-        return launch_groupnorm_silu(in, (const float*)g->ptr, (const float*)b->ptr, out, gn_ws, B, HW, C, silu, st);
+        if (!fast) return launch_groupnorm_silu(in, (const float*)g->ptr, (const float*)b->ptr, out, gn_ws, B, HW, C, silu, st);
+        const int fused = (in == stats_buf) ? stats_chunks : 0;
+        stats_buf = nullptr;
+        return launch_groupnorm_f16(in, (const float*)g->ptr, (const float*)b->ptr, h16[0], l16[0], gn_ws, B, HW, C, silu, st, fused);
     }
-    // buffers: cur = index of the live activation; returns new cur
-    int resblock(const std::string& p, int cur, int Hh, int Ww, int Cin, int Cout, int* rc) {
-        int a = (cur + 1) & 3, b = (cur + 2) & 3, c = (cur + 3) & 3;
-        *rc = gn(p + ".norm1", buf[cur], buf[a], Hh * Ww, Cin, 1); if (*rc) return cur;
-        *rc = conv(p + ".conv1", buf[a], buf[b], nullptr, Hh, Ww, Cin, Cout, 3, 1, 0, 0, 0); if (*rc) return cur;
-        *rc = gn(p + ".norm2", buf[b], buf[a], Hh * Ww, Cout, 1); if (*rc) return cur;
+    // H, W: the operand's extent before its upsample; a stride-2 conv is the Downsample's (0,1,0,1) pad + 3x3 conv
+    // (layers.py:50-57), which the wgmma kernel runs through a tensor map that samples every other pixel.  feeds_gn: the output
+    // goes to a GroupNorm next, so the wgmma epilogue emits its partial statistics.
+    int conv(const std::string& name, const Operand& in, float* out, const float* resid, int H, int W, int Cin, int Cout, int ks,
+             int stride, bool feeds_gn, int out_nchw) {
+        const int Ho = (in.upsample ? 2 * H : H) / stride, Wo = (in.upsample ? 2 * W : W) / stride;
+        const VTensor* w = get(name + ".weight", (int64_t)Cout * ks * ks * Cin);
+        const VTensor* b = get(name + ".bias", Cout);
+        note_act((int64_t)Ho * Wo, Cout);
+        if (dry || !w || !b) return 0;
+        if (in.slot < 0) {
+            ConvGeom g;
+            g.B = B; g.Hi = H; g.Wi = W; g.Cin = Cin; g.Cout = Cout; g.KH = g.KW = ks; g.stride = stride;
+            g.upsample = in.upsample; g.in_nchw = in.nchw; g.out_nchw = out_nchw;
+            g.pad = (ks == 3 && stride == 1) ? 1 : 0;
+            g.Ho = Ho;
+            g.Wo = Wo;
+            return launch_conv(in.x, w->ptr, w->dtype, (const float*)b->ptr, resid, out, g, st);
+        }
+        if (w->dtype != RQB200_F16) return fail(RQB200_ESTATE, "vae fast tier: conv weights must be fp16: " + name);
+        const __half* in_lo = nullptr;
+        const void* w_lo = nullptr;
+        if (h->split) {
+            const VTensor* wl = get(name + ".weight_lo", (int64_t)Cout * ks * ks * Cin);
+            if (!wl) return 0;
+            w_lo = wl->ptr;
+            in_lo = l16[in.slot];
+        }
+        const bool fuse = feeds_gn && h->gn_fuse && !out_nchw && conv_tc_gn_fusable(Ho, Wo, Cout, ks, stride);
+        stats_buf = fuse ? out : nullptr;
+        stats_chunks = fuse ? Ho * Wo / 32 : 0;
+        return launch_conv_tc(h16[in.slot], w->ptr, in_lo, w_lo, (const float*)b->ptr, resid, out, B, Ho, Wo, Cin, Cout, ks, out_nchw, st,
+                              stride, fuse ? gn_ws : nullptr);
+    }
+
+    // buffers: cur = index of the live activation, advanced past the block
+    int resblock(const std::string& p, int& cur, int H, int W, int Cin, int Cout) {
+        const int a = (cur + 1) & 3, b = (cur + 2) & 3, c = (cur + 3) & 3;
+        Operand x;
+        RQB_TRY(norm(p + ".norm1", buf[cur], buf[a], H * W, Cin, 1, &x));
+        RQB_TRY(conv(p + ".conv1", x, buf[b], nullptr, H, W, Cin, Cout, 3, 1, true, 0));
+        RQB_TRY(norm(p + ".norm2", buf[b], buf[a], H * W, Cout, 1, &x));
         const float* res = buf[cur];
         if (Cin != Cout) {
-            *rc = conv(p + ".nin_shortcut", buf[cur], buf[c], nullptr, Hh, Ww, Cin, Cout, 1, 1, 0, 0, 0); if (*rc) return cur;
+            Operand s;
+            RQB_TRY(operand(buf[cur], H, W, Cin, 1, 0, &s));
+            RQB_TRY(conv(p + ".nin_shortcut", s, buf[c], nullptr, H, W, Cin, Cout, 1, 1, false, 0));
             res = buf[c];
         }
-        *rc = conv(p + ".conv2", buf[a], buf[b], res, Hh, Ww, Cout, Cout, 3, 1, 0, 0, 0);
-        return b;
+        RQB_TRY(conv(p + ".conv2", x, buf[b], res, H, W, Cout, Cout, 3, 1, true, 0));
+        cur = b;
+        return 0;
     }
-    int attnblock(const std::string& p, int cur, int Hh, int Ww, int C, int* rc) {
-        int a = (cur + 1) & 3, b = (cur + 2) & 3, c = (cur + 3) & 3;
-        *rc = gn(p + ".norm", buf[cur], buf[a], Hh * Ww, C, 0); if (*rc) return cur;
+    int attnblock(const std::string& p, int& cur, int H, int W, int C) {
+        const int a = (cur + 1) & 3, b = (cur + 2) & 3, c = (cur + 3) & 3;
+        Operand x;
+        RQB_TRY(norm(p + ".norm", buf[cur], buf[a], H * W, C, 0, &x));
         // fused q|k|v 1x1 conv: key "<p>.qkv" registered by the host binding ([3C,1,1,C] / [3C])
-        *rc = conv(p + ".qkv", buf[a], buf[b], nullptr, Hh, Ww, C, 3 * C, 1, 1, 0, 0, 0); if (*rc) return cur;
-        if (!dry && missing.empty()) { *rc = launch_vae_attn(buf[b], buf[a], B, Hh * Ww, C, st); if (*rc) return cur; }
-        *rc = conv(p + ".proj_out", buf[a], buf[c], buf[cur], Hh, Ww, C, C, 1, 1, 0, 0, 0);
-        return c;
+        RQB_TRY(conv(p + ".qkv", x, buf[b], nullptr, H, W, C, 3 * C, 1, 1, false, 0));
+        if (!dry && missing.empty()) RQB_TRY(launch_vae_attn(buf[b], buf[a], B, H * W, C, st));
+        RQB_TRY(operand(buf[a], H, W, C, 0, 0, &x));
+        RQB_TRY(conv(p + ".proj_out", x, buf[c], buf[cur], H, W, C, C, 1, 1, true, 0));
+        cur = c;
+        return 0;
     }
     bool has_attn(int res) const {
         for (int i = 0; i < h->cfg.n_attn_res; i++) if (h->cfg.attn_resolutions[i] == res) return true;
@@ -204,103 +165,72 @@ struct VaeRun {
 
     // Decoder.forward (modules.py:171-202) preceded by post_quant_conv (rqvae.py:87).  z NHWC [B,r,r,embed_dim].
     int decode(const float* z, float* out) {
-        if (fast) return decode_fast(z, out);
+        fast = h->fast_ok;
         const rqb200_vae_config& c = h->cfg;
         const int nl = c.n_levels, nb = c.num_res_blocks;
-        int res = c.resolution >> (nl - 1), rc = 0;
-        int ch = c.ch * c.ch_mult[nl - 1];
-        int cur = 0;
-        rc = conv("post_quant_conv", z, buf[1], nullptr, res, res, c.embed_dim, c.z_channels, 1, 1, 0, 0, 0); if (rc) return rc;
-        rc = conv("decoder.conv_in", buf[1], buf[0], nullptr, res, res, c.z_channels, ch, 3, 1, 0, 0, 0); if (rc) return rc;
-        cur = resblock("decoder.mid.block_1", cur, res, res, ch, ch, &rc); if (rc) return rc;
-        cur = attnblock("decoder.mid.attn_1", cur, res, res, ch, &rc); if (rc) return rc;
-        cur = resblock("decoder.mid.block_2", cur, res, res, ch, ch, &rc); if (rc) return rc;
+        int res = c.resolution >> (nl - 1), ch = c.ch * c.ch_mult[nl - 1], cur = 0;
+        Operand x;
+        RQB_TRY(operand(z, res, res, c.embed_dim, 0, 0, &x));
+        RQB_TRY(conv("post_quant_conv", x, buf[1], nullptr, res, res, c.embed_dim, c.z_channels, 1, 1, false, 0));
+        RQB_TRY(operand(buf[1], res, res, c.z_channels, 0, 0, &x));
+        RQB_TRY(conv("decoder.conv_in", x, buf[0], nullptr, res, res, c.z_channels, ch, 3, 1, true, 0));
+        RQB_TRY(resblock("decoder.mid.block_1", cur, res, res, ch, ch));
+        RQB_TRY(attnblock("decoder.mid.attn_1", cur, res, res, ch));
+        RQB_TRY(resblock("decoder.mid.block_2", cur, res, res, ch, ch));
         for (int lvl = nl - 1; lvl >= 0; lvl--) {
-            int cout = c.ch * c.ch_mult[lvl];
+            const int cout = c.ch * c.ch_mult[lvl];
+            const std::string p = "decoder.up." + std::to_string(lvl);
             for (int b = 0; b <= nb; b++) {
-                std::string p = "decoder.up." + std::to_string(lvl);
-                cur = resblock(p + ".block." + std::to_string(b), cur, res, res, ch, cout, &rc); if (rc) return rc;
+                RQB_TRY(resblock(p + ".block." + std::to_string(b), cur, res, res, ch, cout));
                 ch = cout;
-                if (has_attn(res)) { cur = attnblock(p + ".attn." + std::to_string(b), cur, res, res, ch, &rc); if (rc) return rc; }
+                if (has_attn(res)) RQB_TRY(attnblock(p + ".attn." + std::to_string(b), cur, res, res, ch));
             }
             if (lvl != 0) {
-                int nxt = (cur + 1) & 3;
-                rc = conv("decoder.up." + std::to_string(lvl) + ".upsample.conv", buf[cur], buf[nxt], nullptr, res, res, ch, ch, 3, 1, 1, 0, 0);
-                if (rc) return rc;
+                const int nxt = (cur + 1) & 3;
+                RQB_TRY(operand(buf[cur], res, res, ch, 1, 1, &x));
+                RQB_TRY(conv(p + ".upsample.conv", x, buf[nxt], nullptr, res, res, ch, ch, 3, 1, true, 0));
                 cur = nxt;
                 res *= 2;
             }
         }
-        int a = (cur + 1) & 3;
-        rc = gn("decoder.norm_out", buf[cur], buf[a], res * res, ch, 1); if (rc) return rc;
-        return conv("decoder.conv_out", buf[a], out, nullptr, res, res, ch, c.out_ch, 3, 1, 0, 0, 1);
+        RQB_TRY(norm("decoder.norm_out", buf[cur], buf[(cur + 1) & 3], res * res, ch, 1, &x));
+        return conv("decoder.conv_out", x, out, nullptr, res, res, ch, c.out_ch, 3, 1, false, 1);
     }
 
-    // fast-tier encoder: every conv but conv_in on the wgmma path through the decoder's building blocks, the five stride-2
-    // Downsample convs included (tensor map with element stride 2); conv_in (Cin = 3, NCHW fp32 input, 0.3 % of the encoder's
-    // flops) stays on the fp32 FFMA kernel
-    int encode_fast(const float* x, float* z_e) {
-        const rqb200_vae_config& c = h->cfg;
-        const int nl = c.n_levels, nb = c.num_res_blocks;
-        int res = c.resolution, rc = 0, ch = c.ch, cur = 0;
-        rc = conv("encoder.conv_in", x, buf[0], nullptr, res, res, c.in_channels, ch, 3, 1, 0, 1, 0); if (rc) return rc;
-        for (int lvl = 0; lvl < nl; lvl++) {
-            int cout = c.ch * c.ch_mult[lvl];
-            std::string p = "encoder.down." + std::to_string(lvl);
-            for (int b = 0; b < nb; b++) {
-                cur = resblock_f(p + ".block." + std::to_string(b), cur, res, res, ch, cout, &rc); if (rc) return rc;
-                ch = cout;
-                if (has_attn(res)) { cur = attnblock_f(p + ".attn." + std::to_string(b), cur, res, res, ch, &rc); if (rc) return rc; }
-            }
-            if (lvl != nl - 1) {
-                int nxt = (cur + 1) & 3;
-                // Downsample (layers.py:50-57): pad (0,1,0,1) + 3x3 stride 2 = the same implicit GEMM through a tensor map that
-                // samples every other pixel; the one-pixel right/bottom pad is its out-of-bounds fill
-                if (!dry) { rc = launch_cast_f16(buf[cur], h16[1], l16[1], B, res, res, ch, 0, st); if (rc) return rc; }
-                rc = conv_f(p + ".downsample.conv", h16[1], buf[nxt], nullptr, res / 2, res / 2, ch, ch, 3, 0, 2, true); if (rc) return rc;
-                cur = nxt;
-                res /= 2;
-            }
-        }
-        cur = resblock_f("encoder.mid.block_1", cur, res, res, ch, ch, &rc); if (rc) return rc;
-        cur = attnblock_f("encoder.mid.attn_1", cur, res, res, ch, &rc); if (rc) return rc;
-        cur = resblock_f("encoder.mid.block_2", cur, res, res, ch, ch, &rc); if (rc) return rc;
-        int b2 = (cur + 2) & 3;
-        rc = gn_f("encoder.norm_out", buf[cur], h16[0], res * res, ch, 1); if (rc) return rc;
-        rc = conv_f("encoder.conv_out", h16[0], buf[b2], nullptr, res, res, ch, c.z_channels, 3, 0); if (rc) return rc;
-        if (!dry) { rc = launch_cast_f16(buf[b2], h16[0], l16[0], B, res, res, c.z_channels, 0, st); if (rc) return rc; }
-        return conv_f("quant_conv", h16[0], z_e, nullptr, res, res, c.z_channels, c.embed_dim, 1, 0);
-    }
-
-    // Encoder.forward (modules.py:73-98) followed by quant_conv (rqvae.py:82).  x NCHW -> z_e NHWC.
+    // Encoder.forward (modules.py:73-98) followed by quant_conv (rqvae.py:82).  x NCHW -> z_e NHWC.  The fast tier needs the
+    // encoder's convs registered in fp16 (enc_fast); conv_in (Cin = 3, NCHW fp32 input, 0.3 % of the encoder's flops) runs the
+    // fp32 FFMA kernel on both tiers.
     int encode(const float* x, float* z_e) {
-        if (fast && h->enc_fast) return encode_fast(x, z_e);
+        fast = h->fast_ok && h->enc_fast;
         const rqb200_vae_config& c = h->cfg;
         const int nl = c.n_levels, nb = c.num_res_blocks;
-        int res = c.resolution, rc = 0, ch = c.ch, cur = 0;
-        rc = conv("encoder.conv_in", x, buf[0], nullptr, res, res, c.in_channels, ch, 3, 1, 0, 1, 0); if (rc) return rc;
+        int res = c.resolution, ch = c.ch, cur = 0;
+        RQB_TRY(conv("encoder.conv_in", Operand{x, -1, 0, 1}, buf[0], nullptr, res, res, c.in_channels, ch, 3, 1, false, 0));
+        Operand o;
         for (int lvl = 0; lvl < nl; lvl++) {
-            int cout = c.ch * c.ch_mult[lvl];
-            std::string p = "encoder.down." + std::to_string(lvl);
+            const int cout = c.ch * c.ch_mult[lvl];
+            const std::string p = "encoder.down." + std::to_string(lvl);
             for (int b = 0; b < nb; b++) {
-                cur = resblock(p + ".block." + std::to_string(b), cur, res, res, ch, cout, &rc); if (rc) return rc;
+                RQB_TRY(resblock(p + ".block." + std::to_string(b), cur, res, res, ch, cout));
                 ch = cout;
-                if (has_attn(res)) { cur = attnblock(p + ".attn." + std::to_string(b), cur, res, res, ch, &rc); if (rc) return rc; }
+                if (has_attn(res)) RQB_TRY(attnblock(p + ".attn." + std::to_string(b), cur, res, res, ch));
             }
             if (lvl != nl - 1) {
-                int nxt = (cur + 1) & 3;
-                rc = conv(p + ".downsample.conv", buf[cur], buf[nxt], nullptr, res, res, ch, ch, 3, 2, 0, 0, 0); if (rc) return rc;
+                const int nxt = (cur + 1) & 3;
+                RQB_TRY(operand(buf[cur], res, res, ch, 1, 0, &o));
+                RQB_TRY(conv(p + ".downsample.conv", o, buf[nxt], nullptr, res, res, ch, ch, 3, 2, true, 0));
                 cur = nxt;
                 res /= 2;
             }
         }
-        cur = resblock("encoder.mid.block_1", cur, res, res, ch, ch, &rc); if (rc) return rc;
-        cur = attnblock("encoder.mid.attn_1", cur, res, res, ch, &rc); if (rc) return rc;
-        cur = resblock("encoder.mid.block_2", cur, res, res, ch, ch, &rc); if (rc) return rc;
-        int a = (cur + 1) & 3, b2 = (cur + 2) & 3;
-        rc = gn("encoder.norm_out", buf[cur], buf[a], res * res, ch, 1); if (rc) return rc;
-        rc = conv("encoder.conv_out", buf[a], buf[b2], nullptr, res, res, ch, c.z_channels, 3, 1, 0, 0, 0); if (rc) return rc;
-        return conv("quant_conv", buf[b2], z_e, nullptr, res, res, c.z_channels, c.embed_dim, 1, 1, 0, 0, 0);
+        RQB_TRY(resblock("encoder.mid.block_1", cur, res, res, ch, ch));
+        RQB_TRY(attnblock("encoder.mid.attn_1", cur, res, res, ch));
+        RQB_TRY(resblock("encoder.mid.block_2", cur, res, res, ch, ch));
+        float* zc = buf[(cur + 2) & 3];
+        RQB_TRY(norm("encoder.norm_out", buf[cur], buf[(cur + 1) & 3], res * res, ch, 1, &o));
+        RQB_TRY(conv("encoder.conv_out", o, zc, nullptr, res, res, ch, c.z_channels, 3, 1, false, 0));
+        RQB_TRY(operand(zc, res, res, c.z_channels, 0, 0, &o));
+        return conv("quant_conv", o, z_e, nullptr, res, res, c.z_channels, c.embed_dim, 1, 1, false, 0);
     }
 };
 
@@ -314,8 +244,8 @@ static size_t vae_layout(const rqb200_vae* h, int B, void* base, size_t cap, Vae
     if (run) run->gn_ws = g;
     const rqb200_vae_config& c = h->cfg;
     int r = c.resolution >> (c.n_levels - 1);
-    float* zq = a.take<float>((size_t)B * r * r * c.embed_dim);      // decode_code staging
-    (void)zq;
+    float* zq = a.take<float>((size_t)B * r * r * c.embed_dim);
+    if (run) run->zq = zq;
     for (int i = 0; i < 2; i++) {
         __half* p16 = a.take<__half>((size_t)B * h->max_act);
         if (run) run->h16[i] = p16;
@@ -326,15 +256,6 @@ static size_t vae_layout(const rqb200_vae* h, int B, void* base, size_t cap, Vae
             if (run) run->l16[i] = p16;
         }
     return a.off + 256;
-}
-
-static float* vae_zq_buffer(const rqb200_vae* h, int B, void* base, size_t cap) {
-    Arena a(base, cap);
-    for (int i = 0; i < 4; i++) a.take<float>((size_t)B * h->max_act);
-    a.take<double>(groupnorm_ws_doubles(B, (int)h->max_gn_hw));
-    const rqb200_vae_config& c = h->cfg;
-    int r = c.resolution >> (c.n_levels - 1);
-    return a.take<float>((size_t)B * r * r * c.embed_dim);
 }
 
 }  // namespace rqb
@@ -374,9 +295,7 @@ int rqb200_vae_finalize(rqb200_vae* h) {
         auto it = h->t.find("encoder.conv_out.weight");
         h->enc_fast = h->fast_ok && it != h->t.end() && it->second.dtype == RQB200_F16;
     }
-    run.fast = h->fast_ok;
     run.decode(nullptr, nullptr);
-    run.fast = h->fast_ok && h->enc_fast;
     run.encode(nullptr, nullptr);
     if (!run.missing.empty()) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor " + run.missing);
     {
@@ -414,7 +333,6 @@ static int vae_prepare(rqb200_vae* h, int B, void* ws, size_t ws_bytes, void* st
     if (B <= 0) return rqb::fail(RQB200_EINVAL, "vae: B must be > 0");
     if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "vae: no CUDA device");
     *run = rqb::VaeRun{h, (cudaStream_t)stream, B, false, {nullptr, nullptr, nullptr, nullptr}, nullptr, ""};
-    run->fast = h->fast_ok;
     size_t need = rqb::vae_layout(h, B, ws, ws_bytes, run);
     if (need > ws_bytes) return rqb::fail(RQB200_EWORKSPACE, "vae: workspace too small");
     rqb::g_launches = 0;
@@ -436,9 +354,8 @@ int rqb200_vae_decode_code(rqb200_vae* h, const int64_t* codes, int B, float* ou
     RQB_TRY(vae_prepare(h, B, workspace, workspace_bytes, stream, &run));
     const rqb200_vae_config& c = h->cfg;
     int r = c.resolution >> (c.n_levels - 1);
-    float* zq = rqb::vae_zq_buffer(h, B, workspace, workspace_bytes);
-    RQB_TRY(rqb::launch_rq_embed(codes, h->codebooks, (int64_t)B * r * r, c.depth, c.embed_dim, zq, true, (cudaStream_t)stream));
-    int rc = run.decode(zq, out);
+    RQB_TRY(rqb::launch_rq_embed(codes, h->codebooks, (int64_t)B * r * r, c.depth, c.embed_dim, run.zq, true, (cudaStream_t)stream));
+    int rc = run.decode(run.zq, out);
     h->last_launches = rqb::g_launches;
     return rc;
 }
@@ -447,7 +364,6 @@ int rqb200_vae_encode(rqb200_vae* h, const float* x, int B, float* z_e, void* wo
                       void* stream) {
     rqb::VaeRun run;
     RQB_TRY(vae_prepare(h, B, workspace, workspace_bytes, stream, &run));
-    run.fast = h->fast_ok && h->enc_fast;   // default: exact-tier kernels for the whole encoder; see encode_fast
     int rc = run.encode(x, z_e);
     h->last_launches = rqb::g_launches;
     return rc;

@@ -42,7 +42,7 @@ def gpu_identity():
 
 
 def conv_plan(dd=DD, embed_dim=EMBED_DIM):
-    """(ks, H, W, Cin, Cout) of every conv decode_code launches, in launch order (csrc/vae_engine.cu decode_fast)"""
+    """(ks, H, W, Cin, Cout) of every conv decode_code launches, in launch order (csrc/vae_engine.cu decode)"""
     nl, nb = len(dd["ch_mult"]), dd["num_res_blocks"]
     res = dd["resolution"] >> (nl - 1)
     ch = dd["ch"] * dd["ch_mult"][-1]
