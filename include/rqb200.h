@@ -199,6 +199,17 @@ int rqb200_ar_step(rqb200_ar* h, const int64_t* xs, int64_t xs_batch_stride, con
 size_t rqb200_ar_forward_workspace_bytes(const rqb200_ar* h, int B);
 int rqb200_ar_forward(rqb200_ar* h, const int64_t* codes, const int64_t* cond, int B, float* logits_out, float* cond_logits_out,
                       void* workspace, size_t workspace_bytes, void* stream);
+/* Teacher-forced log-likelihoods of complete code maps (RQTransformer.forward's logits, log-softmaxed and gathered at the codes), without
+ * materialising the logits.  Arguments as rqb200_ar_forward.  logp_out [D][H*W][B] f32 (token-major like rqb200_ar_forward's logits):
+ * log p(code (b, pos, d) | its prefix) at (d*H*W + pos)*B + b; cond_logp_out (nullable; fast tier, cond_len > 1, cond and w_ccls given)
+ * [cond_len-1][B] f32: log p(cond[b][s+1]) under the cond classifier's logits of body token s, over the vocab_cond real classes.
+ * Fast tier: the forward's passes, then the classifier in fixed chunks of rows, each chunk's logits (the forward's GEMM for those rows:
+ * the forward's values) reduced in a bounded fp32 buffer of the workspace.  Exact tier: the teacher-forced replay of rqb200_ar_sample in
+ * spans of positions whose logits fit a bounded buffer.  A code outside [0, vocab) gives NaN for its entry; each entry depends on its
+ * own row's logits only, deterministically. */
+size_t rqb200_ar_log_prob_workspace_bytes(const rqb200_ar* h, int B);
+int rqb200_ar_log_prob(rqb200_ar* h, const int64_t* codes, const int64_t* cond, int B, float* logp_out, float* cond_logp_out,
+                       void* workspace, size_t workspace_bytes, void* stream);
 /* fast tier with RQB200_AR_TRACE: copies 4 globaltimer stamps (ns: entry, dependency resolved, accumulator ready / mid, done) per
  * launch slot of the last graph replays to out_host[cap_launches][4] and the slot names ('\n'-separated) to names; returns the
  * number of slots (0 when tracing is off).  Synchronises the device. */
@@ -291,6 +302,11 @@ int rqb200_dbg_conv_tc_gn(const void* X16, const void* W16, const void* X16lo, c
  * W [N_out,K] 16-bit (fmt 0 fp16 / 1 bf16); exactly one of out_f32 / out_16; gelu applies to out_16 only. */
 int rqb200_dbg_rows_gemm(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                          int gelu, int fmt, int64_t M, int N_out, int K, void* stream);
+
+/* rqb200_dbg_log_prob_rows: one launch of the reduction behind rqb200_ar_log_prob (csrc/logprob.cu): for each of `rows` rows of
+ * logits [rows, ld] f32 (V <= ld valid columns), out[r] = logits[r, t] - logsumexp(logits[r, 0..V)) with t = targets[r] (int64); NaN
+ * when t is outside [0, V).  Nothing outside a row's V columns is read. */
+int rqb200_dbg_log_prob_rows(const float* logits, int64_t ld, int V, int64_t rows, const int64_t* targets, float* out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -217,6 +217,59 @@ static int ar_step_impl(rqb200_ar* h, const int64_t* xs, int64_t xs_stride, cons
     return head_depth(h, ws.CODES, B, idx, d, ws, logits_out, st);
 }
 
+// rqb200_ar_log_prob on the exact tier: the teacher-forced replay of ar_sample_impl over spans of positions whose logits fit one
+// bounded span buffer (each span resumes on the state the previous one left).  Per span: the targets gathered in the logits' row
+// order (token step, b), one reduction over all its rows into a [steps][B] buffer, and one strided copy per depth into logp_out.
+constexpr int64_t EXACT_LOGPROB_SPAN_BYTES = (int64_t)64 << 20;
+
+static int64_t lp_span_positions(const rqb200_ar_config& c, int B) {
+    const int64_t per_pos = (int64_t)c.D * B * c.vocab * (int64_t)sizeof(float);
+    return std::max<int64_t>(1, std::min<int64_t>((int64_t)c.H * c.W, EXACT_LOGPROB_SPAN_BYTES / per_pos));
+}
+struct LpSpan {
+    float* logits;               // [P*D][B][V] the span's logits, token-major in raster order
+    int64_t* tgt;                // [P*D][B] their targets
+    float* lp;                   // [P*D][B] their log-probs
+};
+static size_t lp_layout(const rqb200_ar_config& c, int B, void* base, size_t cap, ArWs* ws, LpSpan* sp) {
+    Arena a(base, cap);
+    a.off = ar_layout(c, B, base, cap, ws);
+    const int64_t rows = lp_span_positions(c, B) * c.D * B;
+    LpSpan s;
+    s.logits = a.take<float>(rows * c.vocab);
+    s.tgt = a.take<int64_t>(rows);
+    s.lp = a.take<float>(rows);
+    if (sp) *sp = s;
+    return a.off + 256;
+}
+
+static int ar_log_prob_impl(rqb200_ar* h, const int64_t* codes, const int64_t* cond, int B, float* logp_out, void* wsp, size_t ws_bytes,
+                            cudaStream_t st) {
+    const rqb200_ar_config& c = h->cfg;
+    const int D = c.D, HW = c.H * c.W, V = c.vocab;
+    if (B <= 0) return fail(RQB200_EINVAL, "ar_log_prob: B must be > 0");
+    ArWs ws;
+    LpSpan sp;
+    if (lp_layout(c, B, wsp, ws_bytes, &ws, &sp) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_log_prob: workspace too small");
+    const std::vector<int32_t> top_k(D, V);          // (the sampler writes the forced code; its settings are moot)
+    const std::vector<float> top_p(D, 1.f);
+    const int64_t P = lp_span_positions(c, B), HWD = (int64_t)HW * D;
+    for (int p0 = 0; p0 < HW; p0 += (int)P) {
+        const int p1 = (int)std::min<int64_t>(p0 + P, HW), n_pos = p1 - p0, steps = n_pos * D;
+        RQB_TRY(ar_sample_impl(h, codes, cond, B, p0, p1, p0 > 0, 1.f, top_k.data(), top_p.data(), nullptr, 0, sp.logits, codes, ws.CODES,
+                               wsp, ws_bytes, st));
+        // row (step, b), step = (idx - p0)*D + d  <-  codes[b][p0*D + step]
+        RQB_TRY(launch_gather_targets(codes, 1, steps, B, 0, 1, HWD, (int64_t)p0 * D, sp.tgt, st));
+        RQB_TRY(launch_logprob_rows(sp.logits, V, V, (int64_t)steps * B, sp.tgt, 1, sp.lp, st));
+        // depth d: rows (idx, d) of the span, D*B floats apart  ->  logp_out[d][p0 .. p1)[B]
+        for (int d = 0; d < D; d++)
+            RQB_CUDA(cudaMemcpy2DAsync(logp_out + ((int64_t)d * HW + p0) * B, (size_t)B * sizeof(float), sp.lp + (int64_t)d * B,
+                                       (size_t)D * B * sizeof(float), (size_t)B * sizeof(float), (size_t)n_pos, cudaMemcpyDeviceToDevice,
+                                       st));
+    }
+    return 0;
+}
+
 }  // namespace rqb
 
 extern "C" {
@@ -354,6 +407,28 @@ int rqb200_ar_forward(rqb200_ar* h, const int64_t* codes, const int64_t* cond, i
     if (!h->fast) return rqb::fail(RQB200_EINVAL, "ar_forward: the batched forward is a fast-tier path (exact tier: teacher-forced rqb200_ar_sample)");
     rqb::g_launches = 0;
     int rc = rqb::ar_fast_forward(h->fast, codes, cond, B, logits_out, cond_logits_out, workspace, workspace_bytes, (cudaStream_t)stream);
+    h->last_launches = rqb::g_launches;
+    return rc;
+}
+size_t rqb200_ar_log_prob_workspace_bytes(const rqb200_ar* h, int B) {
+    if (!h || B <= 0) return 0;
+    if (h->fast) return rqb::ar_fast_log_prob_workspace_bytes(h->fast, B);
+    return rqb::lp_layout(h->cfg, B, nullptr, 0, nullptr, nullptr);
+}
+int rqb200_ar_log_prob(rqb200_ar* h, const int64_t* codes, const int64_t* cond, int B, float* logp_out, float* cond_logp_out,
+                       void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h || !codes || !logp_out || !workspace) return rqb::fail(RQB200_EINVAL, "ar_log_prob: null argument");
+    if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "ar_log_prob: no CUDA device");
+    if (!h->fast && cond_logp_out) return rqb::fail(RQB200_EINVAL, "ar_log_prob: cond log-probs come from the fast tier's cond classifier");
+    if (h->cfg.weight_dtype != RQB200_F32 && !h->fast) return rqb::fail(RQB200_EINVAL, "ar_log_prob: 16-bit weights need the fast tier");
+    rqb::g_launches = 0;
+    int rc;
+    if (h->fast) {
+        rc = rqb::ar_fast_log_prob(h->fast, codes, cond, B, logp_out, cond_logp_out, workspace, workspace_bytes, (cudaStream_t)stream);
+    } else {
+        h->step_next = -1;               // the replay runs on the kind of workspace a stepped sequence keeps its caches in: that sequence ends
+        rc = rqb::ar_log_prob_impl(h, codes, cond, B, logp_out, workspace, workspace_bytes, (cudaStream_t)stream);
+    }
     h->last_launches = rqb::g_launches;
     return rc;
 }

@@ -1395,15 +1395,31 @@ static size_t forward_layout(const ArFast& f, int B, void* base, size_t cap, Fwd
 }
 size_t ar_fast_forward_workspace_bytes(const ArFast* f, int B) { return forward_layout(*f, B, nullptr, 0, nullptr); }
 
-int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B, float* logits_out, float* cond_logits_out, void* wsp,
-                    size_t ws_bytes, cudaStream_t st) {
+// A classifier GEMM over the activation rows [r0, r0 + n) of a launch the forward makes over Ms rows at xn, into out [n, N_out] f32
+// (r0 = 0, n = Ms: that launch itself).  The GEMM is the one the forward picks for the Ms rows -- the rows GEMM for 16-bit weights
+// when rows_ok and Ms > 256, else the weight streamer -- and both compute each output row from its own activation row alone, so a
+// chunk's logits are the forward's logits of those rows bit for bit.
+static int cls_gemm(const ArFast& f, const FastW& fw, const void* w16, const float* bias, int N_out, const h16* xn, int64_t Ms, int64_t r0,
+                    int64_t n, bool rows_ok, float* out, cudaStream_t st) {
+    const int E = f.cfg.embed_dim;
+    xn += r0 * E;
+    if (rows_ok && !f.fp8 && Ms > 256) return launch_rows_gemm_tc(xn, w16, bias, nullptr, out, nullptr, 0, f.bf, n, N_out, E, st);
+    CUtensorMap tx;
+    RQB_TRY(make_tmap_2d(&tx, xn, 1, E, n, (uint64_t)E * 2, 64, act_box(f, n)));
+    GemmTcParams p = gemm_base(f, N_out, E, (int)n, 1, GT_F32);
+    p.bias = bias; p.out = out;
+    return gemm_w(f, fw, tx, p, false, st);
+}
+
+// The passes the forward and the log-likelihood share: body tokens and body stack (ws.BX); with_cond: the cond classifier's LayerNorm
+// of the first (cond_len-1)*B body rows into ws.XN, then cond_cls(Mc) runs its GEMMs on them (before the head reuses ws.XN); head
+// tokens, head stack and the classifier's LayerNorm: ws.XN [D*H*W*B, E], row (d*H*W + pos)*B + b.
+template <class CondCls>
+static int forward_passes(ArFast* f, const FwdWs& ws, const int64_t* codes, const int64_t* cond, int B, bool with_cond, CondCls&& cond_cls,
+                          cudaStream_t st) {
     const rqb200_ar_config& c = f->cfg;
     const rqb200_ar_weights& w = f->w;
     const int E = c.embed_dim, D = c.D, HW = c.H * c.W, cl = c.cond_len, V = c.vocab, Tb = cl + HW - 1;
-    if (B < 1) return fail(RQB200_EINVAL, "ar_forward: B must be > 0");
-    if (cond_logits_out && (cl < 2 || !w.w_ccls)) return fail(RQB200_EINVAL, "ar_forward: cond logits need cond_len > 1 and a cond classifier");
-    FwdWs ws;
-    if (forward_layout(*f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_forward: workspace too small");
     StepState h = {};
     h.cond = cond; h.codes = const_cast<int64_t*>(codes);
     RQB_TRY(launch_pdl(init_state_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, h, 0));
@@ -1418,14 +1434,10 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
         RQB_TRY(body_tokens_batched(*f, ws.state, ws.BX, ws.S, B, Tb, st));
         BatchBufs bb = {ws.BX, ws.XN, ws.QKV, ws.ATT, ws.H};
         RQB_TRY(stack_batched(*f, f->body, f->lbody, bb, B, Tb, nullptr, nullptr, 0, Tb, st));
-        if (cond_logits_out) {                                  // cond_classifier(latents[:, :cond_len-1])        (:153-156)
+        if (with_cond) {                                        // cond_classifier(latents[:, :cond_len-1])        (:153-156)
             const int64_t Mc = (int64_t)(cl - 1) * B;
-            CUtensorMap tx;
-            RQB_TRY(make_tmap_2d(&tx, ws.XN, 1, E, Mc, (uint64_t)E * 2, 64, act_box(*f, Mc)));
             RQB_TRY(ln(*f, "", (int)Mc, ws.BX, nof, 0, nof, nof, nullptr, w.ccls_ln_w, w.ccls_ln_b, ws.XN, st));
-            GemmTcParams p = gemm_base(*f, (c.vocab_cond + 127) / 128 * 128, E, (int)Mc, 1, GT_F32);
-            p.bias = w.b_ccls; p.out = cond_logits_out;
-            RQB_TRY(gemm_w(*f, f->w_ccls, tx, p, false, st));
+            RQB_TRY(cond_cls(Mc));
         }
         // head tokens: d = 0 rows = spatial ctx (body rows of tokens cond_len-1 ..) + pos_emb_d[0]; d >= 1 rows = head_mlp(cumsum)
         RQB_TRY(ln(*f, "", G, ws.BX + (int64_t)(cl - 1) * B * E, nof, 0, nof, w.pos_emb_d, ws.HX, nof, nof, nullptr, st));
@@ -1447,36 +1459,103 @@ int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B,
         }
         BatchBufs hb = {ws.HX, ws.XN, ws.QKV, ws.ATT, ws.H};
         RQB_TRY(stack_batched(*f, f->head, f->lhead, hb, G, D, nullptr, nullptr, 0, D, st));
-        // classifier                                                                                   (:181-183)
-        RQB_TRY(ln(*f, "", (int)Mh, ws.HX, nof, 0, nof, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, st));
-        // one launch over all Mh rows, or (per-depth classifiers) one per depth over that depth's G rows d*G .. (d+1)*G-1, the rows
-        // GEMM or the weight streamer picked by the rows each launch covers (E4M3 weights: always the streamer).  (The rows GEMM reads
-        // whole 128-row tiles -- past a slice into the next depth's rows, past the last one into forward_layout's +128 -- and stores
-        // only the slice's rows.)
-        const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
-        const int n_cls = pd ? D : 1;
-        const int64_t Mc = pd ? G : Mh;
-        const size_t wsz = 2;
-        for (int d = 0; d < n_cls; d++) {
-            const h16* xn = ws.XN + (int64_t)d * Mc * E;
-            const void* wc = (const char*)w.w_cls + (size_t)d * V * E * wsz;
-            const float* bc = w.b_cls + (int64_t)d * V;
-            float* lo = logits_out + (int64_t)d * Mc * V;
-            if (!f->fp8 && Mc > 256) {
-                RQB_TRY(launch_rows_gemm_tc(xn, wc, bc, nullptr, lo, nullptr, 0, f->bf, Mc, V, E, st));
-            } else {
-                CUtensorMap tx;
-                RQB_TRY(make_tmap_2d(&tx, xn, 1, E, Mc, (uint64_t)E * 2, 64, act_box(*f, Mc)));
-                GemmTcParams p = gemm_base(*f, V, E, (int)Mc, 1, GT_F32);
-                p.bias = bc; p.out = lo;
-                RQB_TRY(gemm_w(*f, pd ? f->w_cls_d[d] : f->w_cls, tx, p, false, st));
-            }
-        }
-        return 0;
+        // classifier LayerNorm                                                                         (:181-183)
+        return ln(*f, "", (int)Mh, ws.HX, nof, 0, nof, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, st);
     }();
     f->use_pdl = save_pdl;
     f->trace = save_tr;
     return rc;
+}
+
+// The classifier launches of the forward: one over all D*H*W*B rows of ws.XN, or (per-depth classifiers) one per depth over that
+// depth's slice of H*W*B rows.  cls(fw, w16, bias, slice, rows) runs one of them.  (The rows GEMM reads whole 128-row tiles -- past a
+// slice into the next depth's rows, past the last one into forward_layout's +128 -- and stores only the slice's rows.)
+template <class Cls>
+static int for_each_cls_slice(const ArFast& f, int B, Cls&& cls) {
+    const rqb200_ar_config& c = f.cfg;
+    const rqb200_ar_weights& w = f.w;
+    const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
+    const int64_t Ms = (int64_t)(pd ? 1 : c.D) * c.H * c.W * B;
+    const size_t wsz = 2;            // (the rows GEMM's 16-bit weights; E4M3 weights always go through the streamer's FastW)
+    for (int d = 0; d < (pd ? c.D : 1); d++)
+        RQB_TRY(cls(pd ? f.w_cls_d[d] : f.w_cls, (const char*)w.w_cls + (size_t)d * c.vocab * c.embed_dim * wsz, w.b_cls + (int64_t)d * c.vocab,
+                    d, Ms));
+    return 0;
+}
+
+int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B, float* logits_out, float* cond_logits_out, void* wsp,
+                    size_t ws_bytes, cudaStream_t st) {
+    const rqb200_ar_config& c = f->cfg;
+    const rqb200_ar_weights& w = f->w;
+    const int V = c.vocab;
+    if (B < 1) return fail(RQB200_EINVAL, "ar_forward: B must be > 0");
+    if (cond_logits_out && (c.cond_len < 2 || !w.w_ccls)) return fail(RQB200_EINVAL, "ar_forward: cond logits need cond_len > 1 and a cond classifier");
+    FwdWs ws;
+    if (forward_layout(*f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_forward: workspace too small");
+    const int vcp = (c.vocab_cond + 127) / 128 * 128;
+    RQB_TRY(forward_passes(f, ws, codes, cond, B, cond_logits_out != nullptr, [&](int64_t Mc) {
+        return cls_gemm(*f, f->w_ccls, w.w_ccls, w.b_ccls, vcp, ws.XN, Mc, 0, Mc, false, cond_logits_out, st);
+    }, st));
+    return for_each_cls_slice(*f, B, [&](const FastW& fw, const void* w16, const float* bias, int d, int64_t Ms) {
+        return cls_gemm(*f, fw, w16, bias, V, ws.XN + (int64_t)d * Ms * c.embed_dim, Ms, 0, Ms, true, logits_out + (int64_t)d * Ms * V, st);
+    });
+}
+
+// ---- teacher-forced log-likelihood: the forward's passes, then the classifier in chunks of LOGPROB_CHUNK rows into one fp32 chunk
+// buffer, each chunk reduced to log p(target) by logprob_rows_kernel -- the [D*H*W*B, V] logits never exist.  Chunks never straddle
+// two depths' slices of per-depth classifiers, and each uses the GEMM the forward uses for its slice (cls_gemm), so the log-probs are
+// those of the forward's logits.  512 rows: at V = 16384 a 32 MB chunk that stays in the H100's 50 MB L2 between the GEMM's stores
+// and the reduction's loads (the chunk sweep is in DESIGN.md section 4).
+constexpr int64_t LOGPROB_CHUNK = 512;
+
+struct LpWs {
+    FwdWs fwd;
+    float* CHUNK;                // [LOGPROB_CHUNK, max(V, cond classifier rows)] f32
+    int64_t* TGT;                // [D*H*W*B] targets in the logits' row order, then [(cond_len-1)*B] cond targets
+};
+static size_t log_prob_layout(const ArFast& f, int B, void* base, size_t cap, LpWs* out) {
+    const rqb200_ar_config& c = f.cfg;
+    Arena a(base, cap);
+    a.off = forward_layout(f, B, base, cap, out ? &out->fwd : nullptr);
+    const int64_t vcp = (c.vocab_cond + 127) / 128 * 128, Mh = (int64_t)c.D * c.H * c.W * B, Mc = (int64_t)(c.cond_len - 1) * B;
+    float* chunk = a.take<float>(LOGPROB_CHUNK * std::max<int64_t>(c.vocab, f.w.w_ccls ? vcp : 0));
+    int64_t* tgt = a.take<int64_t>(Mh + Mc);
+    if (out) { out->CHUNK = chunk; out->TGT = tgt; }
+    return a.off + 256;
+}
+size_t ar_fast_log_prob_workspace_bytes(const ArFast* f, int B) { return log_prob_layout(*f, B, nullptr, 0, nullptr); }
+
+int ar_fast_log_prob(ArFast* f, const int64_t* codes, const int64_t* cond, int B, float* logp_out, float* cond_logp_out, void* wsp,
+                     size_t ws_bytes, cudaStream_t st) {
+    const rqb200_ar_config& c = f->cfg;
+    const rqb200_ar_weights& w = f->w;
+    const int E = c.embed_dim, D = c.D, HW = c.H * c.W, V = c.vocab, cl = c.cond_len;
+    if (B < 1) return fail(RQB200_EINVAL, "ar_log_prob: B must be > 0");
+    if (cond_logp_out && (cl < 2 || !w.w_ccls || !cond)) return fail(RQB200_EINVAL, "ar_log_prob: cond log-probs need cond_len > 1, cond and a cond classifier");
+    LpWs ws;
+    if (log_prob_layout(*f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_log_prob: workspace too small");
+    const int64_t Mh = (int64_t)D * HW * B;
+    // targets in the logits' row order: row (d*HW + pos)*B + b <- codes[b][pos][d]; cond row s*B + b <- cond[b][s+1]
+    RQB_TRY(launch_gather_targets(codes, D, HW, B, 1, D, (int64_t)HW * D, 0, ws.TGT, st));
+    if (cond_logp_out) RQB_TRY(launch_gather_targets(cond, 1, cl - 1, B, 0, 1, cl, 1, ws.TGT + Mh, st));
+    const int vcp = (c.vocab_cond + 127) / 128 * 128;
+    RQB_TRY(forward_passes(f, ws.fwd, codes, cond, B, cond_logp_out != nullptr, [&](int64_t Mc) {
+        for (int64_t r0 = 0; r0 < Mc; r0 += LOGPROB_CHUNK) {
+            const int64_t n = std::min(LOGPROB_CHUNK, Mc - r0);
+            RQB_TRY(cls_gemm(*f, f->w_ccls, w.w_ccls, w.b_ccls, vcp, ws.fwd.XN, Mc, r0, n, false, ws.CHUNK, st));
+            // over the vocab_cond real columns: the zero padding rows' logits (0) are no class
+            RQB_TRY(launch_logprob_rows(ws.CHUNK, vcp, c.vocab_cond, n, ws.TGT + Mh + r0, 1, cond_logp_out + r0, st));
+        }
+        return 0;
+    }, st));
+    return for_each_cls_slice(*f, B, [&](const FastW& fw, const void* w16, const float* bias, int d, int64_t Ms) {
+        for (int64_t r0 = 0; r0 < Ms; r0 += LOGPROB_CHUNK) {
+            const int64_t n = std::min(LOGPROB_CHUNK, Ms - r0), row = (int64_t)d * Ms + r0;
+            RQB_TRY(cls_gemm(*f, fw, w16, bias, V, ws.fwd.XN + (int64_t)d * Ms * E, Ms, r0, n, true, ws.CHUNK, st));
+            RQB_TRY(launch_logprob_rows(ws.CHUNK, V, V, n, ws.TGT + row, 1, logp_out + row, st));
+        }
+        return 0;
+    });
 }
 
 // (re)binds the activation tensor maps + graphs to the workspace wsp at batch B

@@ -28,6 +28,12 @@ int launch_rq_embed(const int64_t* codes, const RqTables& tabs, int64_t N, int D
 // sampler.cu
 int launch_sample(const float* logits, const float* q, int B, int V, float temperature, int top_k, float top_p,
                   int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo = 1);
+// logprob.cu -- out[r] = lg[r*ld + t] - logsumexp(lg[r*ld .. r*ld + V)), t = tgt[r*tgt_stride]; NaN when t is outside [0, V)
+int launch_logprob_rows(const float* lg, int64_t ld, int V, int64_t rows, const int64_t* tgt, int64_t tgt_stride, float* out,
+                        cudaStream_t st);
+// dst[(a*A2 + c)*G + g] = src[off + a*sa + c*sc + g*sg] for a < A1, c < A2, g < G
+int launch_gather_targets(const int64_t* src, int A1, int A2, int G, int64_t sa, int64_t sc, int64_t sg, int64_t off, int64_t* dst,
+                          cudaStream_t st);
 // ar_kernels.cu
 int launch_linear(const float* X, int64_t ldx, const void* W, int wdtype, const float* bias, const float* R, float* Y,
                   int64_t ldy, int M, int N, int K, int act, cudaStream_t st);
@@ -141,6 +147,9 @@ int ar_fast_step(ArFast* f, const int64_t* xs, int64_t xs_stride, const int64_t*
 size_t ar_fast_forward_workspace_bytes(const ArFast* f, int B);
 int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B, float* logits_out, float* cond_logits_out, void* wsp,
                     size_t ws_bytes, cudaStream_t st);
+size_t ar_fast_log_prob_workspace_bytes(const ArFast* f, int B);
+int ar_fast_log_prob(ArFast* f, const int64_t* codes, const int64_t* cond, int B, float* logp_out, float* cond_logp_out, void* wsp,
+                     size_t ws_bytes, cudaStream_t st);
 // diagnostics: copies the stage trace of the last replays to the host (RQB200 ar_config.trace); returns the number of launches traced
 int ar_fast_trace(ArFast* f, long long* out_host, int cap_launches, char* names, int names_cap);
 }  // namespace rqb

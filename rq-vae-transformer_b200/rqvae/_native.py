@@ -101,6 +101,10 @@ def lib():
     L.rqb200_ar_forward_workspace_bytes.argtypes = [C.c_void_p, C.c_int]
     L.rqb200_ar_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                     C.c_void_p]
+    L.rqb200_ar_log_prob_workspace_bytes.restype = C.c_size_t
+    L.rqb200_ar_log_prob_workspace_bytes.argtypes = [C.c_void_p, C.c_int]
+    L.rqb200_ar_log_prob.argtypes = L.rqb200_ar_forward.argtypes
+    L.rqb200_dbg_log_prob_rows.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     L.rqb200_ar_trace.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_char_p, C.c_int]
     L.rqb200_ar_last_launches.restype = C.c_int64
     L.rqb200_ar_last_launches.argtypes = [C.c_void_p]
@@ -134,7 +138,8 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_vae_decode", "rqb200_vae_decode_code", "rqb200_vae_encode", "rqb200_vae_last_launches",
            "rqb200_dbg_gemm_tc", "rqb200_dbg_gemm_tc_fp8", "rqb200_dbg_conv_tc", "rqb200_dbg_conv_tc_gn", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
            "rqb200_dbg_rows_gemm", "rqb200_rq_quantize_depthwise", "rqb200_rq_embed_sum_depthwise",
-           "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise"]
+           "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise", "rqb200_ar_log_prob",
+           "rqb200_ar_log_prob_workspace_bytes", "rqb200_dbg_log_prob_rows"]
 
 
 def check(rc, what=""):

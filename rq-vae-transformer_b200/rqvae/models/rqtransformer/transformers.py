@@ -3,7 +3,8 @@
 Boundary kept (SURVEY.md section 8b): constructor from an ``RQTransformerConfig``-shaped object, parameter names
 (state_dict layout A.3), ``sample`` :294-307 (same signature; ``fast``/``cached``/``is_tqdm``/``desc`` accepted),
 ``cached_forward`` :191 (stateful after ``init_cache``: one native token step per call, ``rqb200_ar_step``), ``init_cache`` :289, ``get_block_size``, attributes ``block_size`` / ``block_size_cond`` /
-``vocab_size``.  The (h,w,d) loop, KV caches, embedding glue, classifier and ``sample_from_logits`` all run inside
+``vocab_size``, the losses ``compute_loss`` / ``compute_cond_loss`` / ``compute_codebook_loss`` :371-410, and ``log_prob`` (teacher-forced
+log-likelihoods without the logits, ``rqb200_ar_log_prob``).  The (h,w,d) loop, KV caches, embedding glue, classifier and ``sample_from_logits`` all run inside
 ``rqb200_ar_sample`` (csrc/ar_engine.cu): one native call per ``sample``, no per-token host work.
 
 Arithmetic tiers: ``amp=False`` -> 'exact' (fp32 weights/activations, FFMA -- the tier the bit-exact-indices gate is
@@ -619,5 +620,83 @@ class RQTransformer(Stage2Model):
             return out, cond_logits[..., :self.vocab_size_cond].permute(1, 0, 2).contiguous()
         return out
 
+    @torch.no_grad()
+    def log_prob(self, xs, model_aux=None, cond=None, amp=False):
+        """teacher-forced log-likelihoods log p(x_{h,w,d} | x before it, cond) [B,H,W,D] fp32: forward's logits log-softmaxed and gathered
+        at xs, computed without the [B,H,W,D,V] logits (rqb200_ar_log_prob: fast tier, the classifier in bounded row chunks; exact tier,
+        the teacher-forced replay in bounded spans).  Tiers and return convention as forward: with cond_len > 1 and a cond classifier
+        (fast tier) also the cond log-likelihoods [B,cond_len-1] of cond[:, 1:].  Codes outside [0, V) (and cond entries outside
+        [0, vocab_size_cond)) raise ValueError before any kernel runs."""
+        H, W, D = self.block_size
+        if xs.dim() != 4 or tuple(xs.shape[1:]) != (H, W, D):
+            raise ValueError("rqb200: log_prob expects codes [B,%d,%d,%d], got %s" % (H, W, D, tuple(xs.shape)))
+        B = xs.shape[0]
+        self._check_computable()
+        mode = self._mode(amp)
+        cl, V = self.block_size_cond, self.vocab_size[0]
+        want_cond = cl > 1 and hasattr(self, "cond_classifier")
+        if mode == N.MODE_EXACT and want_cond:
+            raise NotImplementedError("rqb200: cond log-likelihoods (cond_len > 1) are produced by the fast tier only (amp=True)")
+        N.require_cuda(xs, cond, self.pos_emb_hw)
+        dev = self.pos_emb_hw.device
+        xs = xs.to(torch.int64).contiguous()
+        cond_t = None if cond is None else cond.reshape(B, cl).to(torch.int64).contiguous()
+        if want_cond and cond_t is None:
+            cond_t = torch.zeros(B, cl, dtype=torch.int64, device=dev)        # (forward's cond = None: zeros)
+        bad = ((xs < 0) | (xs >= V)).any()
+        if cond_t is not None:
+            bad = bad | ((cond_t < 0) | (cond_t >= self.vocab_size_cond)).any()
+        if bool(bad):                                                       # one reduction, one host read per call
+            raise ValueError("rqb200: log_prob: codes must lie in [0, %d) and cond in [0, %d)" % (V, self.vocab_size_cond))
+        codebook = self._codebook_of(model_aux, D)
+        eng = self._engine(codebook, mode)
+        L = N.lib()
+        with torch.cuda.device(dev):
+            need = L.rqb200_ar_log_prob_workspace_bytes(eng["handle"], B)
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            logp = torch.empty(D, H * W, B, dtype=torch.float32, device=dev)
+            cond_logp = torch.empty(cl - 1, B, dtype=torch.float32, device=dev) if want_cond else None
+            N.check(L.rqb200_ar_log_prob(eng["handle"], N.ptr(xs), N.ptr(cond_t), B, N.ptr(logp), N.ptr(cond_logp), N.ptr(ws), ws.numel(),
+                                         N.stream_ptr(dev)), "ar_log_prob")
+            self.last_launches = L.rqb200_ar_last_launches(eng["handle"])
+            N.launch_count["total"] += self.last_launches
+        out = logp.permute(2, 1, 0).reshape(B, H, W, D)
+        if want_cond:
+            return out, cond_logp.t().contiguous()
+        return out
+
+    # ------------------------------------------------------------------ stage-2 losses (transformers.py:371-410), torch over given logits
     def compute_loss(self, logits, targets, use_soft_target=False):
+        if use_soft_target:
+            return _soft_target_cross_entropy(logits.reshape(-1, logits.shape[-1]), targets.reshape(-1, targets.shape[-1]))
         return torch.nn.functional.cross_entropy(logits.reshape(-1, logits.shape[-1]), targets.reshape(-1))
+
+    def compute_cond_loss(self, cond_logits, conds):
+        assert cond_logits.shape[1] == (conds.shape[1] - 1)
+        targets = conds[:, 1:].contiguous()
+        return torch.nn.functional.cross_entropy(cond_logits.reshape(-1, cond_logits.shape[-1]), targets.reshape(-1))
+
+    @torch.no_grad()
+    def compute_codebook_loss(self, logits, targets, use_soft_target=False):
+        """the cross-entropy of each depth's codes [D] (the reference logs it)"""
+        B, H, W, D, _ = logits.shape
+        logits = logits.reshape(-1, logits.shape[-1])
+        if use_soft_target:
+            tokenwise = _soft_target_cross_entropy(logits, targets.reshape(-1, targets.shape[-1]), reduction="none")
+        else:
+            tokenwise = torch.nn.functional.cross_entropy(logits, targets.reshape(-1), reduction="none")
+        return tokenwise.reshape(-1, D).mean(dim=0)
+
+
+_REDUCE = {"mean": torch.mean, "sum": torch.sum, "none": lambda t: t}
+
+
+def _soft_target_cross_entropy(logits, target, reduction="mean"):
+    """cross-entropy of each row of `logits` [N,V] against a distribution `target` [N,V]: -(target * log p).sum(-1), reduced by
+    `reduction`.  log p is the log-softmax the reference's soft-target loss uses (rqvae/optimizer/loss.py:68-84): logits shifted by
+    their row maximum, with 1e-7 added to the sum of exponentials before the log."""
+    if reduction not in _REDUCE:
+        raise ValueError(reduction)
+    shifted = logits - logits.amax(dim=-1, keepdim=True)
+    log_p = shifted - (shifted.exp().sum(dim=-1, keepdim=True) + 1e-7).log()
+    return _REDUCE[reduction]((target * log_p).sum(dim=-1).neg())
