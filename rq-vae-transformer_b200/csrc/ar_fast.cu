@@ -814,9 +814,11 @@ step_ingest_kernel(StepState* stt, StepState v, int restart, const int64_t* __re
 }
 
 // ------------------------------------------------------------------------------------------------ engine
-// One streamed weight in the engine's format: a TMA tensor map of the [N,K] 16-bit matrix, or (RQB200_E4M3) the packed E4M3 tiles and
-// their fp32 row scales.  gemm_w() is the only place that tells the two apart.
+// One streamed weight [N_out, K] in the engine's format: the 16-bit matrix and its TMA tensor map, or (RQB200_E4M3; w16 null) the
+// packed E4M3 tiles and their fp32 row scales.  make_w() fills it; gemm_w() and linear_rows() are the only places that tell the two apart.
 struct FastW {
+    int N_out = 0, K = 0;
+    const void* w16 = nullptr;
     CUtensorMap tm;
     const void* q8 = nullptr;
     const float* s8 = nullptr;
@@ -845,11 +847,12 @@ struct ArFast {
     cudaGraphExec_t graphs[G_COUNT] = {};
     int64_t n_nodes[G_COUNT] = {};       // kernels recorded in each graph (for the launch counter)
     cudaStream_t cap_stream = nullptr;   // capture never happens on the caller's stream (it may be the legacy default stream)
+    // launch options (cfg.flags), set by ar_fast_create and never changed afterwards.  use_pdl and trace are the single-token chain's;
+    // a batched pass states each launch's PDL attribute at the launch and is never traced.
     bool use_graph = true, use_pdl = true, batched_prefill = true;
+    bool trace = false;                  // diagnostic stage trace (RQB200_AR_TRACE)
     int split_qkv = 4, split_proj = 12, split_fc1 = 1, split_fc2 = 12;
-    int n_sm = 148;
-    // diagnostic stage trace (cfg.flags & RQB200_AR_TRACE)
-    bool trace = false;
+    int n_sm = 0;
     mutable long long* tr_base = nullptr;
     mutable int tr_next = 0;
     mutable std::vector<std::string> tr_names;
@@ -922,37 +925,39 @@ static size_t fast_layout(const ArFast& f, int B, void* base, size_t cap, FastWs
     return a.off + 256;
 }
 
-static GemmTcParams gemm_base(const ArFast& f, int N_out, int K, int rows, int splits, int mode) {
-    GemmTcParams p = {};
-    p.N_out = N_out; p.K = K; p.B = rows; p.splits = splits; p.mode = mode;
-    p.fmt = f.bf; p.bias_scale = 1.f; p.ld_out = N_out;
-    return p;
-}
-
 // rows per box of an activation tensor map: the row chunk of the weight streamer that reads it (at most 128 rows for E4M3 weights)
 static uint32_t act_box(const ArFast& f, int64_t rows) {
     const int r = (int)std::min<int64_t>(rows, 256);
     return (uint32_t)(f.fp8 ? gemm_tc_fp8_bn(r) : gemm_tc_bn(r));
 }
 
-// the weight streamer on one engine weight, in the engine's format
-static int gemm_w(const ArFast& f, const FastW& w, const CUtensorMap& tx, const GemmTcParams& p, bool pdl, cudaStream_t st) {
+static int make_w(const ArFast& f, FastW* out, const void* w, const float* s, int N_out, int K) {
+    out->N_out = N_out;
+    out->K = K;
+    if (f.fp8) {
+        out->q8 = w;
+        out->s8 = s;
+        return 0;
+    }
+    out->w16 = w;
+    return make_tmap_weight(&out->tm, w, N_out, K);
+}
+
+// the weight streamer on one engine weight, in the engine's format, over the p.B activation rows behind tx; p carries the split, the
+// mode and the epilogue, the weight and the engine give the rest
+static int gemm_w(const ArFast& f, const FastW& w, const CUtensorMap& tx, GemmTcParams p, bool pdl, cudaStream_t st) {
+    p.N_out = w.N_out; p.K = w.K; p.fmt = f.bf; p.ld_out = w.N_out;
     if (!f.fp8) return launch_gemm_tc(w.tm, tx, p, pdl, st);
     if (ceil_div(p.B, gemm_tc_fp8_bn(p.B)) > 65535) return fail(RQB200_EINVAL, "ar fast tier: too many activation rows for one E4M3 GEMM");
     return launch_gemm_tc_fp8(w.q8, w.s8, tx, p, pdl, st);
 }
 
-static int make_w(const ArFast& f, FastW* out, const void* w, const float* s, int N_out, int K) {
-    if (!f.fp8) return make_tmap_weight(&out->tm, w, N_out, K);
-    out->q8 = w;
-    out->s8 = s;
-    return 0;
-}
-
-static int gemm(const ArFast& f, const char* name, const FastW& w, const CUtensorMap& tx, int N_out, int K, int B, int splits,
-                int mode, const float* bias, float bias_scale, void* out, float* partial, const float* residual, int64_t ld_res,
-                const int* res_row_ptr, int64_t res_row_stride, cudaStream_t st) {
-    GemmTcParams p = gemm_base(f, N_out, K, B, splits, mode);
+// ---- the single-token chain's launchers: PDL attribute from f.use_pdl, one trace slot each
+static int gemm(const ArFast& f, const char* name, const FastW& w, const CUtensorMap& tx, int B, int splits, int mode, const float* bias,
+                float bias_scale, void* out, float* partial, const float* residual, int64_t ld_res, const int* res_row_ptr,
+                int64_t res_row_stride, cudaStream_t st) {
+    GemmTcParams p = {};
+    p.B = B; p.splits = splits; p.mode = mode;
     p.bias = bias; p.bias_scale = bias_scale; p.out = out; p.partial = partial;
     p.residual = residual; p.ld_res = ld_res; p.res_row_ptr = res_row_ptr; p.res_row_stride = res_row_stride;
     p.trace = tr_slot(f, name);
@@ -962,20 +967,9 @@ static int gemm(const ArFast& f, const char* name, const FastW& w, const CUtenso
 static int ln(const ArFast& f, const char* name, int rows, const float* x_in, const float* partial, int S, const float* bias,
               const float* extra, float* x_out, const float* g, const float* be, h16* xn, cudaStream_t st,
               const PrefetchList* pf = nullptr) {
-    const int E = f.cfg.embed_dim;
-    if (rows >= 512 && S == 0 && bias == nullptr && x_in != nullptr) {        // batched passes: warp per row
-        const dim3 grid((unsigned)std::min<int64_t>(ceil_div(rows, 8), (int64_t)f.n_sm * 8));
-        const int nv = ceil_div(E, 128);
-#define RQB_LN_ROWS(NV) launch_pdl(ln_rows_kernel<NV>, grid, dim3(256), (size_t)0, st, true, x_in, extra, x_out, g, be, xn, (int64_t)rows, E, f.bf)
-        if (nv <= 8) return RQB_LN_ROWS(8);
-        if (nv <= 12) return RQB_LN_ROWS(12);
-        if (nv <= 20) return RQB_LN_ROWS(20);
-        return RQB_LN_ROWS(36);
-#undef RQB_LN_ROWS
-    }
     PrefetchList none = {};
     return launch_pdl(ln_reduce_kernel<384, 3>, dim3((unsigned)rows), dim3(384), (size_t)0, st, f.use_pdl, x_in, partial, S, bias, extra, x_out,
-                      g, be, xn, rows, E, f.bf, tr_slot(f, name), pf ? *pf : none);
+                      g, be, xn, rows, f.cfg.embed_dim, f.bf, tr_slot(f, name), pf ? *pf : none);
 }
 
 static int attn(const ArFast& f, FastWs& ws, const float* bqkv, h16* kc, h16* vc, int Tmax, const int* t_ptr, int t_host,
@@ -1030,23 +1024,19 @@ static int fast_stack(const ArFast& f, const std::vector<rqb200_block_weights>& 
         }
         RQB_TRY(ln(f, "ln1", B, first ? x_src : x, pend ? ws.P : nof, pend ? f.split_fc2 : 0, pend ? blocks[l - 1].b2 : nof,
                    first ? pending_extra : nof, x, bw.ln1_w, bw.ln1_b, ws.XN, st, &pf));
-        RQB_TRY(gemm(f, "qkv", maps[l].qkv, f.tx_xn, 3 * E, E, B, f.split_qkv, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0,
-                     st));
+        RQB_TRY(gemm(f, "qkv", maps[l].qkv, f.tx_xn, B, f.split_qkv, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0, st));
         RQB_TRY(attn(f, ws, bw.bqkv, kc + per * l, vc + per * l, Tmax, t_ptr, t_host, st));
-        RQB_TRY(gemm(f, "proj", maps[l].proj, f.tx_att, E, E, B, f.split_proj, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr,
-                     0, st));
+        RQB_TRY(gemm(f, "proj", maps[l].proj, f.tx_att, B, f.split_proj, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0, st));
         RQB_TRY(ln(f, "ln2", B, x, ws.P, f.split_proj, bw.bproj, nof, x, bw.ln2_w, bw.ln2_b, ws.XN, st));
         if (f.split_fc1 == 1) {
-            RQB_TRY(gemm(f, "fc1", maps[l].fc1, f.tx_xn, 4 * E, E, B, 1, GT_H16_GELU, bw.b1, 1.f, ws.Hh, nullptr, nullptr, 0, nullptr, 0, st));
+            RQB_TRY(gemm(f, "fc1", maps[l].fc1, f.tx_xn, B, 1, GT_H16_GELU, bw.b1, 1.f, ws.Hh, nullptr, nullptr, 0, nullptr, 0, st));
         } else {
-            RQB_TRY(gemm(f, "fc1", maps[l].fc1, f.tx_xn, 4 * E, E, B, f.split_fc1, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0,
-                         nullptr, 0, st));
+            RQB_TRY(gemm(f, "fc1", maps[l].fc1, f.tx_xn, B, f.split_fc1, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0, st));
             RQB_TRY(launch_pdl(act_reduce_kernel, dim3((unsigned)std::min<int64_t>(ceil_div((int64_t)B * 4 * E / 4, 256), 1184)), dim3(256),
                                (size_t)0, st, f.use_pdl, (const float*)ws.P, f.split_fc1, bw.b1, ws.Hh, B, 4 * E, f.bf,
                                tr_slot(f, "act_reduce")));
         }
-        RQB_TRY(gemm(f, "fc2", maps[l].fc2, f.tx_h, E, 4 * E, B, f.split_fc2, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0,
-                     st));
+        RQB_TRY(gemm(f, "fc2", maps[l].fc2, f.tx_h, B, f.split_fc2, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0, st));
     }
     // fold the last block's pending fc2 reduction into x (x is final on return) -- and the caller's LayerNorm, if any.  An empty
     // stack (a head-less model) only forms its input token x = x_src + pending_extra.
@@ -1072,8 +1062,8 @@ static int record_body(ArFast& f, FastWs& ws, bool cond_token, cudaStream_t st) 
         RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
                            cb_dstride(c), HW, c.D, c.codebook_size, c.code_dim, 0, 0, ws.S, f.bf, 0));
         // x = W_in (sum_d e_d) + D b_in + pos_emb_hw[idx-1]       (bias counted D times, transformers.py:220,225)
-        RQB_TRY(gemm(f, "w_in", f.w_in, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_in, (float)c.D, ws.XB, nullptr,
-                     w.pos_emb_hw - E /* row idx-1 */, 0, &ws.state->idx, E, st));
+        RQB_TRY(gemm(f, "w_in", f.w_in, f.tx_s, B, 1, GT_F32, w.b_in, (float)c.D, ws.XB, nullptr, w.pos_emb_hw - E /* row idx-1 */, 0,
+                     &ws.state->idx, E, st));
     }
     RQB_TRY(fast_stack(f, f.body, f.lbody, ws, ws.XB, nullptr, ws.XB, ws.kc_body, ws.vc_body, Tb, &ws.state->s, 0, nullptr, nullptr, st));
     RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, f.use_pdl, ws.state, 1, 0, 0));
@@ -1101,7 +1091,7 @@ static int record_head_depth(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
             RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
                                cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf,
                                (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
-            RQB_TRY(gemm(f, "w_head", f.w_head, f.tx_s, E, c.code_dim, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
+            RQB_TRY(gemm(f, "w_head", f.w_head, f.tx_s, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
                          w.pos_emb_d + (int64_t)d * E, 0, nullptr, 0, st));
         }
         RQB_TRY(fast_stack(f, f.head, f.lhead, ws, ws.XH, nullptr, ws.XH, ws.kc_head, ws.vc_head, D, nullptr, d, w.cls_ln_w,
@@ -1110,7 +1100,7 @@ static int record_head_depth(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
     // classifier: LN(x) (fused into the stack's last launch) -> logits                       (transformers.py:278-285)
     // per-depth classifiers (BatchLinear): depth d's [V,E] slice and bias row
     const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
-    RQB_TRY(gemm(f, "cls", pd ? f.w_cls_d[d] : f.w_cls, f.tx_xn, V, E, B, 1, GT_F32, w.b_cls + (pd ? (int64_t)d * V : 0), 1.f,
+    RQB_TRY(gemm(f, "cls", pd ? f.w_cls_d[d] : f.w_cls, f.tx_xn, B, 1, GT_F32, w.b_cls + (pd ? (int64_t)d * V : 0), 1.f,
                  ws.LOGITS, nullptr, nullptr, 0, nullptr, 0, st));
     return 0;
 }
@@ -1194,10 +1184,12 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
     f->use_pdl = !(cfg.flags & RQB200_AR_NO_PDL);
     f->trace = (cfg.flags & RQB200_AR_TRACE) != 0;
     f->batched_prefill = !(cfg.flags & RQB200_AR_SEQUENTIAL_PREFILL);
-    {
-        int dev = 0, n = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) f->n_sm = n;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&f->n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        f->n_sm < 1) {
+        set_error("ar fast tier: cannot read the device's SM count (the split-K factors are planned for it)");
+        delete f;
+        return nullptr;
     }
     const int nkbE = E / 64;
     f->split_qkv = pick_split(3 * E / 128, nkbE, cfg.split_qkv, f->n_sm);
@@ -1244,6 +1236,59 @@ struct BatchBufs {
     h16 *XN, *QKV, *ATT, *H;     // [M,E], [M,3E], [M,E], [M,4E] scratch
 };
 
+// The epilogue of one linear layer of a batched pass, in the weight streamer's terms: out = acc + bias, to 16 bits (GT_H16, GT_H16_GELU) or,
+// after adding activation row b's residual row b * ld_res, to fp32 (GT_F32).
+static GemmTcParams epilogue(int mode, const float* bias, void* out, const float* residual = nullptr, int64_t ld_res = 0) {
+    GemmTcParams p = {};
+    p.splits = 1; p.mode = mode; p.bias = bias; p.bias_scale = 1.f; p.out = out; p.residual = residual; p.ld_res = ld_res;
+    return p;
+}
+
+// One linear layer of a batched pass: the weight w over the M activation rows x [M, w.K], with the epilogue p.  The one place that picks
+// the GEMM:
+//   16-bit weights, M_launch > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue,
+//   like the next tile); it has no PDL attribute;
+//   M_launch <= 256, and E4M3 weights at every M: the weight streamer (E4M3: 128-row chunks, faster than the fp16 rows GEMM at the
+//   forward's shapes) over a tensor map of x, with the PDL attribute `pdl`.
+// M_launch = M, except for a chunk of a launch the forward makes over M_launch rows (log_prob's classifier chunks): both GEMMs compute
+// each output row from its own activation row alone, so the GEMM the forward picks gives the chunk the forward's logits bit for bit.
+// streamer_only: never the rows GEMM.  For w_in / w_head, whose epilogues (bias_scale, a broadcast residual, res_div) the rows GEMM
+// does not have, and for the cond classifier, whose logits have always been the streamer's (the rows GEMM sums in another order).
+static int linear_rows(const ArFast& f, const FastW& w, const h16* x, int64_t M, int64_t M_launch, bool streamer_only, GemmTcParams p,
+                       bool pdl, cudaStream_t st) {
+    if (!streamer_only && !f.fp8 && M_launch > 256) {
+        const bool f32 = p.mode == GT_F32;
+        return launch_rows_gemm_tc(x, w.w16, p.bias, p.residual, f32 ? (float*)p.out : nullptr, f32 ? nullptr : p.out, p.mode == GT_H16_GELU,
+                                   f.bf, M, w.N_out, w.K, st);
+    }
+    CUtensorMap tx;
+    RQB_TRY(make_tmap_2d(&tx, x, 1, w.K, M, (uint64_t)w.K * 2, 64, act_box(f, M)));
+    p.B = (int)M;
+    return gemm_w(f, w, tx, p, pdl, st);
+}
+
+// LayerNorm over the rows of a batched pass: x_out (nullable) = x_in + extra (nullable), xn (nullable) = LN(x_out).  512 rows and more: a
+// warp per row, launched with the PDL attribute; fewer: ln_reduce_kernel with nothing to reduce, launched without.  The two kernels
+// sum in different orders, so the threshold is part of the results.
+static int ln_rows(const ArFast& f, int64_t rows, const float* x_in, const float* extra, float* x_out, const float* g, const float* be,
+                   h16* xn, cudaStream_t st) {
+    const int E = f.cfg.embed_dim;
+    if (rows < 512) {
+        const float* nof = nullptr;
+        long long* no_trace = nullptr;
+        return launch_pdl(ln_reduce_kernel<384, 3>, dim3((unsigned)rows), dim3(384), (size_t)0, st, false, x_in, nof, 0, nof, extra, x_out, g, be,
+                          xn, (int)rows, E, f.bf, no_trace, PrefetchList{});
+    }
+    const dim3 grid((unsigned)std::min<int64_t>(ceil_div(rows, 8), (int64_t)f.n_sm * 8));
+    const int nv = ceil_div(E, 128);
+#define RQB_LN_ROWS(NV) launch_pdl(ln_rows_kernel<NV>, grid, dim3(256), (size_t)0, st, true, x_in, extra, x_out, g, be, xn, rows, E, f.bf)
+    if (nv <= 8) return RQB_LN_ROWS(8);
+    if (nv <= 12) return RQB_LN_ROWS(12);
+    if (nv <= 20) return RQB_LN_ROWS(20);
+    return RQB_LN_ROWS(36);
+#undef RQB_LN_ROWS
+}
+
 static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights>& blocks, const std::vector<FastLayer>& maps,
                          const BatchBufs& bb, int G, int T, h16* kc, h16* vc, int64_t kv_per_layer, int Tmax, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
@@ -1251,26 +1296,11 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
     const int64_t M = (int64_t)G * T;
     if (M > (int64_t)1 << 30 || T > FAST_MAXT) return fail(RQB200_EINVAL, "ar fast tier: batched pass too large");
     const bool pdl = true;               // the pass is a PDL chain too: a launch's set-up overlaps its predecessor's tail
-    CUtensorMap tx_xn, tx_att, tx_h;
-    const uint32_t bn = act_box(f, M);
-    RQB_TRY(make_tmap_2d(&tx_xn, bb.XN, 1, E, M, (uint64_t)E * 2, 64, bn));
-    RQB_TRY(make_tmap_2d(&tx_att, bb.ATT, 1, E, M, (uint64_t)E * 2, 64, bn));
-    RQB_TRY(make_tmap_2d(&tx_h, bb.H, 1, 4 * E, M, (uint64_t)E * 8, 64, bn));
     const float* nof = nullptr;
-    // 16-bit weights, M > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue, like
-    // the next tile); M <= 256, and E4M3 weights at every M: the weight streamer (E4M3: 128-row chunks, faster than the fp16 rows GEMM
-    // at the forward's shapes)
-    const bool rows = !f.fp8 && M > 256;
     for (size_t l = 0; l < blocks.size(); l++) {
         const rqb200_block_weights& bw = blocks[l];
-        RQB_TRY(ln(f, "", (int)M, bb.X, nof, 0, nof, nof, nullptr, bw.ln1_w, bw.ln1_b, bb.XN, st));
-        if (rows) {
-            RQB_TRY(launch_rows_gemm_tc(bb.XN, bw.wqkv, bw.bqkv, nullptr, nullptr, bb.QKV, 0, f.bf, M, 3 * E, E, st));
-        } else {
-            GemmTcParams p = gemm_base(f, 3 * E, E, (int)M, 1, GT_H16);
-            p.bias = bw.bqkv; p.out = bb.QKV;
-            RQB_TRY(gemm_w(f, maps[l].qkv, tx_xn, p, pdl, st));
-        }
+        RQB_TRY(ln_rows(f, M, bb.X, nof, nullptr, bw.ln1_w, bw.ln1_b, bb.XN, st));
+        RQB_TRY(linear_rows(f, maps[l].qkv, bb.XN, M, M, false, epilogue(GT_H16, bw.bqkv, bb.QKV), pdl, st));
         h16* kcl = kc ? kc + kv_per_layer * l : nullptr;
         h16* vcl = vc ? vc + kv_per_layer * l : nullptr;
         if (T <= 4) {                                     // tiny groups (the forward's head stack): a warp per (group, head)
@@ -1289,36 +1319,17 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
                                    G, T, E, c.n_head, Tmax));
             }
         }
-        if (rows) {
-            RQB_TRY(launch_rows_gemm_tc(bb.ATT, bw.wproj, bw.bproj, bb.X, bb.X, nullptr, 0, f.bf, M, E, E, st));
-        } else {
-            GemmTcParams p = gemm_base(f, E, E, (int)M, 1, GT_F32);
-            p.bias = bw.bproj; p.out = bb.X; p.residual = bb.X; p.ld_res = E;
-            RQB_TRY(gemm_w(f, maps[l].proj, tx_att, p, pdl, st));
-        }
-        RQB_TRY(ln(f, "", (int)M, bb.X, nof, 0, nof, nof, nullptr, bw.ln2_w, bw.ln2_b, bb.XN, st));
-        if (rows) {
-            RQB_TRY(launch_rows_gemm_tc(bb.XN, bw.w1, bw.b1, nullptr, nullptr, bb.H, 1, f.bf, M, 4 * E, E, st));
-            RQB_TRY(launch_rows_gemm_tc(bb.H, bw.w2, bw.b2, bb.X, bb.X, nullptr, 0, f.bf, M, E, 4 * E, st));
-        } else {
-            {
-                GemmTcParams p = gemm_base(f, 4 * E, E, (int)M, 1, GT_H16_GELU);
-                p.bias = bw.b1; p.out = bb.H;
-                RQB_TRY(gemm_w(f, maps[l].fc1, tx_xn, p, pdl, st));
-            }
-            {
-                GemmTcParams p = gemm_base(f, E, 4 * E, (int)M, 1, GT_F32);
-                p.bias = bw.b2; p.out = bb.X; p.residual = bb.X; p.ld_res = E;
-                RQB_TRY(gemm_w(f, maps[l].fc2, tx_h, p, pdl, st));
-            }
-        }
+        RQB_TRY(linear_rows(f, maps[l].proj, bb.ATT, M, M, false, epilogue(GT_F32, bw.bproj, bb.X, bb.X, E), pdl, st));
+        RQB_TRY(ln_rows(f, M, bb.X, nof, nullptr, bw.ln2_w, bw.ln2_b, bb.XN, st));
+        RQB_TRY(linear_rows(f, maps[l].fc1, bb.XN, M, M, false, epilogue(GT_H16_GELU, bw.b1, bb.H), pdl, st));
+        RQB_TRY(linear_rows(f, maps[l].fc2, bb.H, M, M, false, epilogue(GT_F32, bw.b2, bb.X, bb.X, E), pdl, st));
     }
     return 0;
 }
 
 // body input tokens [0, T) of every batch row into X (token-major): token s < cond_len is a cond token (transformers.py:224),
 // token s >= cond_len carries the summed input embeddings of the codes of position s - cond_len (:219-225)
-static int body_tokens_batched(ArFast& f, const StepState* state, float* X, h16* S, int B, int T, cudaStream_t st) {
+static int body_tokens_batched(const ArFast& f, const StepState* state, float* X, h16* S, int B, int T, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const rqb200_ar_weights& w = f.w;
     const int E = c.embed_dim, HW = c.H * c.W, cl = c.cond_len;
@@ -1330,40 +1341,29 @@ static int body_tokens_batched(ArFast& f, const StepState* state, float* X, h16*
         RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, n_code), dim3(128), (size_t)0, st, false, state, w.tok_emb, tok_dstride(c), HW, c.D,
                            c.vocab, E, 0, c.D, 2, 0, w.pos_emb_hw, (int64_t)E, X + (int64_t)cl * B * E));
     } else if (n_code > 0) {
-        const int64_t Mc = (int64_t)B * n_code;
-        CUtensorMap tx_s;
-        RQB_TRY(make_tmap_2d(&tx_s, S, 1, c.code_dim, Mc, (uint64_t)c.code_dim * 2, 64, act_box(f, Mc)));
         RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, n_code), dim3(64), (size_t)0, st, false, state, w.codebook, cb_dstride(c), HW, c.D,
                            c.codebook_size, c.code_dim, -c.D, 0, S, f.bf, 0));
-        GemmTcParams p = gemm_base(f, E, c.code_dim, (int)Mc, 1, GT_F32);
-        p.bias = w.b_in; p.bias_scale = (float)c.D; p.out = X + (int64_t)cl * B * E;
-        p.residual = w.pos_emb_hw; p.ld_res = E; p.res_div = B;          // row (j, b) gets pos_emb_hw[j]
-        RQB_TRY(gemm_w(f, f.w_in, tx_s, p, false, st));
+        const int64_t Mc = (int64_t)B * n_code;
+        GemmTcParams e = epilogue(GT_F32, w.b_in, X + (int64_t)cl * B * E, w.pos_emb_hw, E);
+        e.bias_scale = (float)c.D;       // (the bias is counted D times, as in the single-token step)
+        e.res_div = B;                   // row (j, b) gets pos_emb_hw[j]
+        RQB_TRY(linear_rows(f, f.w_in, S, Mc, Mc, true, e, false, st));
     }
     return 0;
 }
 
 // ---- batched prefill: body tokens [0, T) of every batch row in one pass.  Leaves ws.XB = the last token's output rows, the KV
 // cache rows [0, T) written, state.s = T.
-static int prefill_batched(ArFast& f, FastWs& ws, int T, cudaStream_t st) {
+static int prefill_batched(const ArFast& f, FastWs& ws, int T, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const int E = c.embed_dim, B = f.B, HW = c.H * c.W, cl = c.cond_len, Tb = cl + HW;
     const int64_t M = (int64_t)B * T;
     if (M > ws.Mmax) return fail(RQB200_EINVAL, "ar fast tier: prefix too long for the batched prefill");
-    const bool save_pdl = f.use_pdl, save_tr = f.trace;
-    f.use_pdl = false;
-    f.trace = false;
-    int rc = [&]() -> int {
-        RQB_TRY(body_tokens_batched(f, ws.state, ws.PX, ws.PS, B, T, st));
-        BatchBufs bb = {ws.PX, ws.PXN, ws.PQKV, ws.PATT, ws.PH};
-        RQB_TRY(stack_batched(f, f.body, f.lbody, bb, B, T, ws.kc_body, ws.vc_body, (int64_t)B * c.n_head * Tb * 64, Tb, st));
-        RQB_CUDA(cudaMemcpyAsync(ws.XB, ws.PX + (int64_t)(T - 1) * B * E, (size_t)B * E * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, T, 0, 0));
-        return 0;
-    }();
-    f.use_pdl = save_pdl;
-    f.trace = save_tr;
-    return rc;
+    RQB_TRY(body_tokens_batched(f, ws.state, ws.PX, ws.PS, B, T, st));
+    BatchBufs bb = {ws.PX, ws.PXN, ws.PQKV, ws.PATT, ws.PH};
+    RQB_TRY(stack_batched(f, f.body, f.lbody, bb, B, T, ws.kc_body, ws.vc_body, (int64_t)B * c.n_head * Tb * 64, Tb, st));
+    RQB_CUDA(cudaMemcpyAsync(ws.XB, ws.PX + (int64_t)(T - 1) * B * E, (size_t)B * E * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, T, 0, 0);
 }
 
 // ---- teacher-forced forward (transformers.py:113-188): all H*W*D logits of given code maps in a handful of large-M GEMM passes.
@@ -1395,115 +1395,85 @@ static size_t forward_layout(const ArFast& f, int B, void* base, size_t cap, Fwd
 }
 size_t ar_fast_forward_workspace_bytes(const ArFast* f, int B) { return forward_layout(*f, B, nullptr, 0, nullptr); }
 
-// A classifier GEMM over the activation rows [r0, r0 + n) of a launch the forward makes over Ms rows at xn, into out [n, N_out] f32
-// (r0 = 0, n = Ms: that launch itself).  The GEMM is the one the forward picks for the Ms rows -- the rows GEMM for 16-bit weights
-// when rows_ok and Ms > 256, else the weight streamer -- and both compute each output row from its own activation row alone, so a
-// chunk's logits are the forward's logits of those rows bit for bit.
-static int cls_gemm(const ArFast& f, const FastW& fw, const void* w16, const float* bias, int N_out, const h16* xn, int64_t Ms, int64_t r0,
-                    int64_t n, bool rows_ok, float* out, cudaStream_t st) {
-    const int E = f.cfg.embed_dim;
-    xn += r0 * E;
-    if (rows_ok && !f.fp8 && Ms > 256) return launch_rows_gemm_tc(xn, w16, bias, nullptr, out, nullptr, 0, f.bf, n, N_out, E, st);
-    CUtensorMap tx;
-    RQB_TRY(make_tmap_2d(&tx, xn, 1, E, n, (uint64_t)E * 2, 64, act_box(f, n)));
-    GemmTcParams p = gemm_base(f, N_out, E, (int)n, 1, GT_F32);
-    p.bias = bias; p.out = out;
-    return gemm_w(f, fw, tx, p, false, st);
-}
-
 // The passes the forward and the log-likelihood share: body tokens and body stack (ws.BX); with_cond: the cond classifier's LayerNorm
 // of the first (cond_len-1)*B body rows into ws.XN, then cond_cls(Mc) runs its GEMMs on them (before the head reuses ws.XN); head
 // tokens, head stack and the classifier's LayerNorm: ws.XN [D*H*W*B, E], row (d*H*W + pos)*B + b.
 template <class CondCls>
-static int forward_passes(ArFast* f, const FwdWs& ws, const int64_t* codes, const int64_t* cond, int B, bool with_cond, CondCls&& cond_cls,
-                          cudaStream_t st) {
-    const rqb200_ar_config& c = f->cfg;
-    const rqb200_ar_weights& w = f->w;
+static int forward_passes(const ArFast& f, const FwdWs& ws, const int64_t* codes, const int64_t* cond, int B, bool with_cond,
+                          CondCls&& cond_cls, cudaStream_t st) {
+    const rqb200_ar_config& c = f.cfg;
+    const rqb200_ar_weights& w = f.w;
     const int E = c.embed_dim, D = c.D, HW = c.H * c.W, cl = c.cond_len, V = c.vocab, Tb = cl + HW - 1;
     StepState h = {};
     h.cond = cond; h.codes = const_cast<int64_t*>(codes);
     RQB_TRY(launch_pdl(init_state_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, h, 0));
-    const bool save_pdl = f->use_pdl, save_tr = f->trace;
-    f->use_pdl = false;
-    f->trace = false;
     const float* nof = nullptr;
-    int rc = [&]() -> int {
-        const int G = HW * B;                                  // head groups, g = pos * B + b
-        const int64_t Mh = (int64_t)D * G;
-        // body
-        RQB_TRY(body_tokens_batched(*f, ws.state, ws.BX, ws.S, B, Tb, st));
-        BatchBufs bb = {ws.BX, ws.XN, ws.QKV, ws.ATT, ws.H};
-        RQB_TRY(stack_batched(*f, f->body, f->lbody, bb, B, Tb, nullptr, nullptr, 0, Tb, st));
-        if (with_cond) {                                        // cond_classifier(latents[:, :cond_len-1])        (:153-156)
-            const int64_t Mc = (int64_t)(cl - 1) * B;
-            RQB_TRY(ln(*f, "", (int)Mc, ws.BX, nof, 0, nof, nof, nullptr, w.ccls_ln_w, w.ccls_ln_b, ws.XN, st));
-            RQB_TRY(cond_cls(Mc));
+    const int G = HW * B;                                  // head groups, g = pos * B + b
+    const int64_t Mh = (int64_t)D * G;
+    // body
+    RQB_TRY(body_tokens_batched(f, ws.state, ws.BX, ws.S, B, Tb, st));
+    BatchBufs bb = {ws.BX, ws.XN, ws.QKV, ws.ATT, ws.H};
+    RQB_TRY(stack_batched(f, f.body, f.lbody, bb, B, Tb, nullptr, nullptr, 0, Tb, st));
+    if (with_cond) {                                        // cond_classifier(latents[:, :cond_len-1])        (:153-156)
+        const int64_t Mc = (int64_t)(cl - 1) * B;
+        RQB_TRY(ln_rows(f, Mc, ws.BX, nof, nullptr, w.ccls_ln_w, w.ccls_ln_b, ws.XN, st));
+        RQB_TRY(cond_cls(Mc));
+    }
+    // head tokens: d = 0 rows = spatial ctx (body rows of tokens cond_len-1 ..) + pos_emb_d[0]; d >= 1 rows = head_mlp(cumsum)
+    RQB_TRY(ln_rows(f, G, ws.BX + (int64_t)(cl - 1) * B * E, w.pos_emb_d, ws.HX, nof, nof, nullptr, st));
+    for (int d = 1; d < D; d++) {
+        if (c.embed_variant & RQB200_EMB_TOK_HEAD) {        // tok_emb(code_{d-1}) + pos_emb_d[d]        (:164,177)
+            RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, HW), dim3(128), (size_t)0, st, false, (const StepState*)ws.state, w.tok_emb,
+                               tok_dstride(c), HW, D, V, E, d - 1, 1, 2, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
+                               ws.HX + (int64_t)d * G * E));
+            continue;
         }
-        // head tokens: d = 0 rows = spatial ctx (body rows of tokens cond_len-1 ..) + pos_emb_d[0]; d >= 1 rows = head_mlp(cumsum)
-        RQB_TRY(ln(*f, "", G, ws.BX + (int64_t)(cl - 1) * B * E, nof, 0, nof, w.pos_emb_d, ws.HX, nof, nof, nullptr, st));
-        CUtensorMap tx_s;
-        RQB_TRY(make_tmap_2d(&tx_s, ws.S, 1, c.code_dim, G, (uint64_t)c.code_dim * 2, 64, act_box(*f, G)));
-        for (int d = 1; d < D; d++) {
-            if (c.embed_variant & RQB200_EMB_TOK_HEAD) {        // tok_emb(code_{d-1}) + pos_emb_d[d]        (:164,177)
-                RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, HW), dim3(128), (size_t)0, st, false, (const StepState*)ws.state, w.tok_emb,
-                                   tok_dstride(c), HW, D, V, E, d - 1, 1, 2, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
-                                   ws.HX + (int64_t)d * G * E));
-                continue;
-            }
-            RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, HW), dim3(64), (size_t)0, st, false, (const StepState*)ws.state, w.codebook,
-                               cb_dstride(c), HW, D, c.codebook_size, c.code_dim, -d, 0, ws.S, f->bf,
-                               (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
-            GemmTcParams p = gemm_base(*f, E, c.code_dim, G, 1, GT_F32);
-            p.bias = w.b_head; p.out = ws.HX + (int64_t)d * G * E; p.residual = w.pos_emb_d + (int64_t)d * E; p.ld_res = 0;
-            RQB_TRY(gemm_w(*f, f->w_head, tx_s, p, false, st));
-        }
-        BatchBufs hb = {ws.HX, ws.XN, ws.QKV, ws.ATT, ws.H};
-        RQB_TRY(stack_batched(*f, f->head, f->lhead, hb, G, D, nullptr, nullptr, 0, D, st));
-        // classifier LayerNorm                                                                         (:181-183)
-        return ln(*f, "", (int)Mh, ws.HX, nof, 0, nof, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, st);
-    }();
-    f->use_pdl = save_pdl;
-    f->trace = save_tr;
-    return rc;
+        RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, HW), dim3(64), (size_t)0, st, false, (const StepState*)ws.state, w.codebook,
+                           cb_dstride(c), HW, D, c.codebook_size, c.code_dim, -d, 0, ws.S, f.bf,
+                           (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
+        RQB_TRY(linear_rows(f, f.w_head, ws.S, G, G, true,
+                            epilogue(GT_F32, w.b_head, ws.HX + (int64_t)d * G * E, w.pos_emb_d + (int64_t)d * E, 0 /* one row for all */), false, st));
+    }
+    BatchBufs hb = {ws.HX, ws.XN, ws.QKV, ws.ATT, ws.H};
+    RQB_TRY(stack_batched(f, f.head, f.lhead, hb, G, D, nullptr, nullptr, 0, D, st));
+    // classifier LayerNorm                                                                         (:181-183)
+    return ln_rows(f, Mh, ws.HX, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, st);
 }
 
 // The classifier launches of the forward: one over all D*H*W*B rows of ws.XN, or (per-depth classifiers) one per depth over that
-// depth's slice of H*W*B rows.  cls(fw, w16, bias, slice, rows) runs one of them.  (The rows GEMM reads whole 128-row tiles -- past a
+// depth's slice of H*W*B rows.  cls(weight, bias, slice, rows) runs one of them.  (The rows GEMM reads whole 128-row tiles -- past a
 // slice into the next depth's rows, past the last one into forward_layout's +128 -- and stores only the slice's rows.)
 template <class Cls>
 static int for_each_cls_slice(const ArFast& f, int B, Cls&& cls) {
     const rqb200_ar_config& c = f.cfg;
-    const rqb200_ar_weights& w = f.w;
     const bool pd = c.embed_variant & RQB200_EMB_CLS_PER_DEPTH;
     const int64_t Ms = (int64_t)(pd ? 1 : c.D) * c.H * c.W * B;
-    const size_t wsz = 2;            // (the rows GEMM's 16-bit weights; E4M3 weights always go through the streamer's FastW)
-    for (int d = 0; d < (pd ? c.D : 1); d++)
-        RQB_TRY(cls(pd ? f.w_cls_d[d] : f.w_cls, (const char*)w.w_cls + (size_t)d * c.vocab * c.embed_dim * wsz, w.b_cls + (int64_t)d * c.vocab,
-                    d, Ms));
+    for (int d = 0; d < (pd ? c.D : 1); d++) RQB_TRY(cls(pd ? f.w_cls_d[d] : f.w_cls, f.w.b_cls + (int64_t)d * c.vocab, d, Ms));
     return 0;
 }
 
-int ar_fast_forward(ArFast* f, const int64_t* codes, const int64_t* cond, int B, float* logits_out, float* cond_logits_out, void* wsp,
+int ar_fast_forward(ArFast* fp, const int64_t* codes, const int64_t* cond, int B, float* logits_out, float* cond_logits_out, void* wsp,
                     size_t ws_bytes, cudaStream_t st) {
-    const rqb200_ar_config& c = f->cfg;
-    const rqb200_ar_weights& w = f->w;
+    const ArFast& f = *fp;
+    const rqb200_ar_config& c = f.cfg;
+    const rqb200_ar_weights& w = f.w;
     const int V = c.vocab;
     if (B < 1) return fail(RQB200_EINVAL, "ar_forward: B must be > 0");
     if (cond_logits_out && (c.cond_len < 2 || !w.w_ccls)) return fail(RQB200_EINVAL, "ar_forward: cond logits need cond_len > 1 and a cond classifier");
     FwdWs ws;
-    if (forward_layout(*f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_forward: workspace too small");
-    const int vcp = (c.vocab_cond + 127) / 128 * 128;
+    if (forward_layout(f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_forward: workspace too small");
     RQB_TRY(forward_passes(f, ws, codes, cond, B, cond_logits_out != nullptr, [&](int64_t Mc) {
-        return cls_gemm(*f, f->w_ccls, w.w_ccls, w.b_ccls, vcp, ws.XN, Mc, 0, Mc, false, cond_logits_out, st);
+        return linear_rows(f, f.w_ccls, ws.XN, Mc, Mc, true, epilogue(GT_F32, w.b_ccls, cond_logits_out), false, st);
     }, st));
-    return for_each_cls_slice(*f, B, [&](const FastW& fw, const void* w16, const float* bias, int d, int64_t Ms) {
-        return cls_gemm(*f, fw, w16, bias, V, ws.XN + (int64_t)d * Ms * c.embed_dim, Ms, 0, Ms, true, logits_out + (int64_t)d * Ms * V, st);
+    return for_each_cls_slice(f, B, [&](const FastW& fw, const float* bias, int d, int64_t Ms) {
+        return linear_rows(f, fw, ws.XN + (int64_t)d * Ms * c.embed_dim, Ms, Ms, false, epilogue(GT_F32, bias, logits_out + (int64_t)d * Ms * V),
+                           false, st);
     });
 }
 
 // ---- teacher-forced log-likelihood: the forward's passes, then the classifier in chunks of LOGPROB_CHUNK rows into one fp32 chunk
 // buffer, each chunk reduced to log p(target) by logprob_rows_kernel -- the [D*H*W*B, V] logits never exist.  Chunks never straddle
-// two depths' slices of per-depth classifiers, and each uses the GEMM the forward uses for its slice (cls_gemm), so the log-probs are
+// two depths' slices of per-depth classifiers, and each uses the GEMM the forward uses for its slice (linear_rows), so the log-probs are
 // those of the forward's logits.  512 rows: at V = 16384 a 32 MB chunk that stays in the H100's 50 MB L2 between the GEMM's stores
 // and the reduction's loads (the chunk sweep is in DESIGN.md section 4).
 constexpr int64_t LOGPROB_CHUNK = 512;
@@ -1525,33 +1495,33 @@ static size_t log_prob_layout(const ArFast& f, int B, void* base, size_t cap, Lp
 }
 size_t ar_fast_log_prob_workspace_bytes(const ArFast* f, int B) { return log_prob_layout(*f, B, nullptr, 0, nullptr); }
 
-int ar_fast_log_prob(ArFast* f, const int64_t* codes, const int64_t* cond, int B, float* logp_out, float* cond_logp_out, void* wsp,
+int ar_fast_log_prob(ArFast* fp, const int64_t* codes, const int64_t* cond, int B, float* logp_out, float* cond_logp_out, void* wsp,
                      size_t ws_bytes, cudaStream_t st) {
-    const rqb200_ar_config& c = f->cfg;
-    const rqb200_ar_weights& w = f->w;
+    const ArFast& f = *fp;
+    const rqb200_ar_config& c = f.cfg;
+    const rqb200_ar_weights& w = f.w;
     const int E = c.embed_dim, D = c.D, HW = c.H * c.W, V = c.vocab, cl = c.cond_len;
     if (B < 1) return fail(RQB200_EINVAL, "ar_log_prob: B must be > 0");
     if (cond_logp_out && (cl < 2 || !w.w_ccls || !cond)) return fail(RQB200_EINVAL, "ar_log_prob: cond log-probs need cond_len > 1, cond and a cond classifier");
     LpWs ws;
-    if (log_prob_layout(*f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_log_prob: workspace too small");
+    if (log_prob_layout(f, B, wsp, ws_bytes, &ws) > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_log_prob: workspace too small");
     const int64_t Mh = (int64_t)D * HW * B;
     // targets in the logits' row order: row (d*HW + pos)*B + b <- codes[b][pos][d]; cond row s*B + b <- cond[b][s+1]
     RQB_TRY(launch_gather_targets(codes, D, HW, B, 1, D, (int64_t)HW * D, 0, ws.TGT, st));
     if (cond_logp_out) RQB_TRY(launch_gather_targets(cond, 1, cl - 1, B, 0, 1, cl, 1, ws.TGT + Mh, st));
-    const int vcp = (c.vocab_cond + 127) / 128 * 128;
     RQB_TRY(forward_passes(f, ws.fwd, codes, cond, B, cond_logp_out != nullptr, [&](int64_t Mc) {
         for (int64_t r0 = 0; r0 < Mc; r0 += LOGPROB_CHUNK) {
             const int64_t n = std::min(LOGPROB_CHUNK, Mc - r0);
-            RQB_TRY(cls_gemm(*f, f->w_ccls, w.w_ccls, w.b_ccls, vcp, ws.fwd.XN, Mc, r0, n, false, ws.CHUNK, st));
+            RQB_TRY(linear_rows(f, f.w_ccls, ws.fwd.XN + r0 * E, n, Mc, true, epilogue(GT_F32, w.b_ccls, ws.CHUNK), false, st));
             // over the vocab_cond real columns: the zero padding rows' logits (0) are no class
-            RQB_TRY(launch_logprob_rows(ws.CHUNK, vcp, c.vocab_cond, n, ws.TGT + Mh + r0, 1, cond_logp_out + r0, st));
+            RQB_TRY(launch_logprob_rows(ws.CHUNK, f.w_ccls.N_out, c.vocab_cond, n, ws.TGT + Mh + r0, 1, cond_logp_out + r0, st));
         }
         return 0;
     }, st));
-    return for_each_cls_slice(*f, B, [&](const FastW& fw, const void* w16, const float* bias, int d, int64_t Ms) {
+    return for_each_cls_slice(f, B, [&](const FastW& fw, const float* bias, int d, int64_t Ms) {
         for (int64_t r0 = 0; r0 < Ms; r0 += LOGPROB_CHUNK) {
             const int64_t n = std::min(LOGPROB_CHUNK, Ms - r0), row = (int64_t)d * Ms + r0;
-            RQB_TRY(cls_gemm(*f, fw, w16, bias, V, ws.fwd.XN + (int64_t)d * Ms * E, Ms, r0, n, true, ws.CHUNK, st));
+            RQB_TRY(linear_rows(f, fw, ws.fwd.XN + row * E, n, Ms, false, epilogue(GT_F32, bias, ws.CHUNK), false, st));
             RQB_TRY(launch_logprob_rows(ws.CHUNK, V, V, n, ws.TGT + row, 1, logp_out + row, st));
         }
         return 0;

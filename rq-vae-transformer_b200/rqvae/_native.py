@@ -249,15 +249,14 @@ def pack_fp8_weight(w):
 
 
 def ar_engine_options():
-    """engine-creation options of the fast AR tier, read ONCE per engine from the environment (diagnostics / experiments)"""
+    """rqb200_ar_config.flags of the fast AR tier, read ONCE per engine from the environment (diagnostics)"""
     env = os.environ.get
     flags = 0
     flags |= AR_NO_GRAPH if env("RQB200_NO_GRAPH", "0") == "1" else 0
     flags |= AR_NO_PDL if env("RQB200_NO_PDL", "0") == "1" else 0
     flags |= AR_TRACE if env("RQB200_TRACE", "0") == "1" else 0
     flags |= AR_SEQUENTIAL_PREFILL if env("RQB200_SEQ_PREFILL", "0") == "1" else 0
-    return {"flags": flags,
-            "splits": [int(env("RQB200_SPLIT_" + k, "0")) for k in ("QKV", "PROJ", "FC1", "FC2")]}
+    return flags
 
 
 def param_fingerprint(module):

@@ -222,7 +222,6 @@ class RQTransformer(Stage2Model):
         per_depth = isinstance(codebook, list)
         fmt = N.fast_weight_format() if mode == N.MODE_FAST else "fp32"
         wdt = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16, "fp8": None}[fmt]
-        opts = N.ar_engine_options() if mode == N.MODE_FAST else {"flags": 0, "splits": [0, 0, 0, 0]}
         keep, streamed = [], []
 
         def f32(t):
@@ -270,8 +269,7 @@ class RQTransformer(Stage2Model):
             cfg.code_dim, cfg.codebook_size = table0.shape[1], table0.shape[0]
         cfg.codebook_per_depth = int(per_depth)
         cfg.mode, cfg.weight_dtype = mode, N.E4M3 if fmt == "fp8" else N._DT[wdt]
-        cfg.flags = opts["flags"]
-        cfg.split_qkv, cfg.split_proj, cfg.split_fc1, cfg.split_fc2 = opts["splits"]
+        cfg.flags = N.ar_engine_options() if mode == N.MODE_FAST else 0      # (the split_* fields stay 0: the engine fills the SMs)
         cfg.embed_variant = self._embed_variant()
         if c.head.block.n_head != c.body.block.n_head:
             raise NotImplementedError("rqb200: body and head stacks must share n_head")
@@ -379,13 +377,9 @@ class RQTransformer(Stage2Model):
             kk = (C.c_int32 * D)(*[int(k) for k in ks])
             pp = (C.c_float * D)(*[float(p) for p in ps])
             fc = None if force_codes is None else force_codes.to(torch.int64).contiguous()
-            bounds = [(0, B)]
-            if mode == N.MODE_FAST and B > 256:
-                # the wgmma tier takes at most 256 batch rows per call (wgmma N <= 256): run equal chunks back to back
-                if return_logits:
-                    raise N.NativeError("rqb200: return_logits with B > 256 is not supported on the fast tier")
-                n_chunks = -(-B // 256)
-                bounds = [(i * B // n_chunks, (i + 1) * B // n_chunks) for i in range(n_chunks)]
+            bounds = _chunk_bounds(B, mode)
+            if len(bounds) > 1 and return_logits:
+                raise N.NativeError("rqb200: return_logits with B > 256 is not supported on the fast tier")
             # position spans: when the noise is drawn here it is drawn span by span into one bounded buffer (noise_budget_bytes)
             # instead of one [n_tok,B,V] tensor (1 GB at 8x8x4, B=64, V=16384); every batch chunk keeps its own engine slot
             # (workspace + KV state) so that all chunks can resume on the next span
@@ -399,9 +393,7 @@ class RQTransformer(Stage2Model):
             engines = []
             for slot, (lo, hi) in enumerate(bounds):
                 eng = self._engine(codebook, mode, slot)
-                need = N.lib().rqb200_ar_workspace_bytes(eng["handle"], hi - lo)
-                if eng["ws"] is None or eng["ws"].numel() < need:
-                    eng["ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+                _workspace(eng, N.lib().rqb200_ar_workspace_bytes(eng["handle"], hi - lo), dev)
                 engines.append(eng)
 
             def off(t, lo, row_elems, esize, extra=0):
@@ -535,10 +527,7 @@ class RQTransformer(Stage2Model):
         B, V, cl = xs.shape[0], self.vocab_size[0], self.block_size_cond
         dev = self.pos_emb_hw.device
         N.require_cuda(xs, cond, self.pos_emb_hw)
-        bounds = [(0, B)]
-        if mode == N.MODE_FAST and B > 256:
-            n_chunks = -(-B // 256)
-            bounds = [(i * B // n_chunks, (i + 1) * B // n_chunks) for i in range(n_chunks)]
+        bounds = _chunk_bounds(B, mode)
         st = self._step
         restart = route == "restart"
         try:
@@ -563,9 +552,7 @@ class RQTransformer(Stage2Model):
                 stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
                 for eng, (lo, hi) in zip(engines, bounds):
                     if restart:                      # (sized when a sequence begins; its batch stays until the next one)
-                        need = L.rqb200_ar_workspace_bytes(eng["handle"], hi - lo)
-                        if eng["ws"] is None or eng["ws"].numel() < need:
-                            eng["ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+                        _workspace(eng, L.rqb200_ar_workspace_bytes(eng["handle"], hi - lo), dev)
                     N.check(L.rqb200_ar_step(
                         eng["handle"], C.c_void_p(xs.data_ptr() + lo * stride * 8), stride,
                         C.c_void_p(cond_t.data_ptr() + lo * cl * 8) if cond_t is not None else C.c_void_p(0), hi - lo, h, w, d,
@@ -606,8 +593,7 @@ class RQTransformer(Stage2Model):
         cond_t = None if cond is None else cond.reshape(B, cl).to(torch.int64).contiguous()
         want_cond = cl > 1 and hasattr(self, "cond_classifier")
         with torch.cuda.device(dev):
-            need = N.lib().rqb200_ar_forward_workspace_bytes(eng["handle"], B)
-            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            ws = _workspace(None, N.lib().rqb200_ar_forward_workspace_bytes(eng["handle"], B), dev)
             logits = torch.empty(D, H * W, B, V, dtype=torch.float32, device=dev)
             vcp = -(-self.vocab_size_cond // 128) * 128
             cond_logits = torch.empty(cl - 1, B, vcp, dtype=torch.float32, device=dev) if want_cond else None
@@ -652,8 +638,7 @@ class RQTransformer(Stage2Model):
         eng = self._engine(codebook, mode)
         L = N.lib()
         with torch.cuda.device(dev):
-            need = L.rqb200_ar_log_prob_workspace_bytes(eng["handle"], B)
-            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            ws = _workspace(None, L.rqb200_ar_log_prob_workspace_bytes(eng["handle"], B), dev)
             logp = torch.empty(D, H * W, B, dtype=torch.float32, device=dev)
             cond_logp = torch.empty(cl - 1, B, dtype=torch.float32, device=dev) if want_cond else None
             N.check(L.rqb200_ar_log_prob(eng["handle"], N.ptr(xs), N.ptr(cond_t), B, N.ptr(logp), N.ptr(cond_logp), N.ptr(ws), ws.numel(),
@@ -686,6 +671,23 @@ class RQTransformer(Stage2Model):
         else:
             tokenwise = torch.nn.functional.cross_entropy(logits, targets.reshape(-1), reduction="none")
         return tokenwise.reshape(-1, D).mean(dim=0)
+
+
+def _chunk_bounds(B, mode):
+    """the batch chunks [(lo, hi)] of one native call each: the fast tier takes at most 256 batch rows per call (wgmma N <= 256), so
+    a larger batch runs as equal chunks back to back"""
+    n = max(1, -(-B // 256)) if mode == N.MODE_FAST else 1
+    return [(i * B // n, (i + 1) * B // n) for i in range(n)]
+
+
+def _workspace(eng, need, dev):
+    """a workspace of at least `need` bytes on dev: the engine slot's own (it holds the KV state between calls), replaced when too
+    small; eng = None: one for this call only (forward / log_prob, whose activation rows would otherwise stay allocated)"""
+    if eng is None:
+        return torch.empty(need, dtype=torch.uint8, device=dev)
+    if eng["ws"] is None or eng["ws"].numel() < need:
+        eng["ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+    return eng["ws"]
 
 
 _REDUCE = {"mean": torch.mean, "sum": torch.sum, "none": lambda t: t}
