@@ -3,8 +3,8 @@
 // Same semantics as ar_engine.cu's exact tier (reference: transformers.py:190-369, attentions.py:60-142), different
 // arithmetic class: 16-bit weights / activations / KV cache on wgmma (gemm_tc.cu) -- fp16 by default, the reference's own
 // autocast class (transformers.py:114,206; main_sampling_fid.py:216), bf16 on request -- fp32 accumulation, fp32 residual
-// stream, fp32 LayerNorm / softmax / sampler.  RQB200_E4M3: E4M3 weights with fp32 row scales on the fp8 weight streamer
-// (gemm_tc_fp8_kernel) in every GEMM, fp16 activations / KV cache; everything else as with fp16.
+// stream, fp32 LayerNorm / softmax / sampler.  RQB200_E4M3: E4M3 weights with fp32 row scales on the weight streamer's E4M3 form
+// (gemm_tc_kernel<BN, GT_E4M3>) in every GEMM, fp16 activations / KV cache; everything else as with fp16.
 //
 // One transformer block on the single new token of every batch row (M = batch rows):
 //
@@ -43,23 +43,6 @@ namespace rqb {
 #define TR_IN(tr)  do { if ((tr) != nullptr && blockIdx.x == 0 && threadIdx.x == 0) (tr)[0] = tc::gtimer(); } while (0)
 #define TR_DEP(tr) do { if ((tr) != nullptr && blockIdx.x == 0 && threadIdx.x == 0) (tr)[1] = tc::gtimer(); } while (0)
 #define TR_OUT(tr) do { if ((tr) != nullptr && blockIdx.x == 0 && threadIdx.x == 0) { (tr)[2] = tc::gtimer(); (tr)[3] = (tr)[2]; } } while (0)
-
-template <typename... KArgs, typename... Args>
-static int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    RQB_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
-    g_launches++;
-    return 0;
-}
 
 // ------------------------------------------------------------------------------------------------ kernels
 // The per-block small vectors (biases, LayerNorm parameters: ~80 KB per block, read once per token) are DRAM misses -- 2.8 GB of
@@ -223,7 +206,7 @@ act_reduce_kernel(const float* __restrict__ partial, int S, const float* __restr
         }
         float r[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-        for (int k = 0; k < 4; k++) r[k] = 0.5f * r[k] * (1.0f + erff(r[k] * 0.70710678118654752440f));
+        for (int k = 0; k < 4; k++) r[k] = gelu_erf(r[k]);
         uint2 pk;
         pk.x = pack_h16x2(r[0], r[1], bf);
         pk.y = pack_h16x2(r[2], r[3], bf);
@@ -814,18 +797,9 @@ step_ingest_kernel(StepState* stt, StepState v, int restart, const int64_t* __re
 }
 
 // ------------------------------------------------------------------------------------------------ engine
-// One streamed weight [N_out, K] in the engine's format: the 16-bit matrix and its TMA tensor map, or (RQB200_E4M3; w16 null) the
-// packed E4M3 tiles and their fp32 row scales.  make_w() fills it; gemm_w() and linear_rows() are the only places that tell the two apart.
-struct FastW {
-    int N_out = 0, K = 0;
-    const void* w16 = nullptr;
-    CUtensorMap tm;
-    const void* q8 = nullptr;
-    const float* s8 = nullptr;
-};
-
+// Every weight is a StreamedWeight in the engine's format (16-bit, or E4M3 with RQB200_E4M3); only linear_rows() tells the two apart.
 struct FastLayer {
-    FastW qkv, proj, fc1, fc2;
+    StreamedWeight qkv, proj, fc1, fc2;
 };
 
 // G_HEAD_STEP + d: head depth d alone with its logits copied out (rqb200_ar_step), d < 8
@@ -836,8 +810,8 @@ struct ArFast {
     rqb200_ar_weights w;
     std::vector<rqb200_block_weights> body, head;
     std::vector<FastLayer> lbody, lhead;
-    FastW w_in, w_head, w_cls, w_ccls;
-    FastW w_cls_d[8];                    // RQB200_EMB_CLS_PER_DEPTH: depth d's [V,E] slice of w_cls
+    StreamedWeight w_in, w_head, w_cls, w_ccls;
+    StreamedWeight w_cls_d[8];           // RQB200_EMB_CLS_PER_DEPTH: depth d's [V,E] slice of w_cls
     int bf = 0;                          // 16-bit activation format: 0 fp16, 1 bf16
     bool fp8 = false;                    // RQB200_E4M3 weights (fp16 activations)
     // per (workspace, B) state
@@ -925,35 +899,15 @@ static size_t fast_layout(const ArFast& f, int B, void* base, size_t cap, FastWs
     return a.off + 256;
 }
 
-// rows per box of an activation tensor map: the row chunk of the weight streamer that reads it (at most 128 rows for E4M3 weights)
-static uint32_t act_box(const ArFast& f, int64_t rows) {
-    const int r = (int)std::min<int64_t>(rows, 256);
-    return (uint32_t)(f.fp8 ? gemm_tc_fp8_bn(r) : gemm_tc_bn(r));
-}
-
-static int make_w(const ArFast& f, FastW* out, const void* w, const float* s, int N_out, int K) {
-    out->N_out = N_out;
-    out->K = K;
-    if (f.fp8) {
-        out->q8 = w;
-        out->s8 = s;
-        return 0;
-    }
-    out->w16 = w;
-    return make_tmap_weight(&out->tm, w, N_out, K);
-}
-
-// the weight streamer on one engine weight, in the engine's format, over the p.B activation rows behind tx; p carries the split, the
-// mode and the epilogue, the weight and the engine give the rest
-static int gemm_w(const ArFast& f, const FastW& w, const CUtensorMap& tx, GemmTcParams p, bool pdl, cudaStream_t st) {
-    p.N_out = w.N_out; p.K = w.K; p.fmt = f.bf; p.ld_out = w.N_out;
-    if (!f.fp8) return launch_gemm_tc(w.tm, tx, p, pdl, st);
-    if (ceil_div(p.B, gemm_tc_fp8_bn(p.B)) > 65535) return fail(RQB200_EINVAL, "ar fast tier: too many activation rows for one E4M3 GEMM");
-    return launch_gemm_tc_fp8(w.q8, w.s8, tx, p, pdl, st);
+// the weight streamer on one engine weight over the p.B activation rows behind tx; p carries the split, the mode and the epilogue, the
+// weight and the engine give the rest
+static int gemm_w(const ArFast& f, const StreamedWeight& w, const CUtensorMap& tx, GemmTcParams p, bool pdl, cudaStream_t st) {
+    p.fmt = f.bf; p.ld_out = w.N_out;
+    return launch_gemm_tc(w, tx, p, pdl, st);
 }
 
 // ---- the single-token chain's launchers: PDL attribute from f.use_pdl, one trace slot each
-static int gemm(const ArFast& f, const char* name, const FastW& w, const CUtensorMap& tx, int B, int splits, int mode, const float* bias,
+static int gemm(const ArFast& f, const char* name, const StreamedWeight& w, const CUtensorMap& tx, int B, int splits, int mode, const float* bias,
                 float bias_scale, void* out, float* partial, const float* residual, int64_t ld_res, const int* res_row_ptr,
                 int64_t res_row_stride, cudaStream_t st) {
     GemmTcParams p = {};
@@ -1196,26 +1150,29 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
     f->split_proj = pick_split(E / 128, nkbE, cfg.split_proj, f->n_sm);
     f->split_fc1 = pick_split(4 * E / 128, nkbE, cfg.split_fc1, f->n_sm);
     f->split_fc2 = pick_split(E / 128, 4 * nkbE, cfg.split_fc2, f->n_sm);
+    auto make_w = [&](StreamedWeight* out, const void* wt, const float* s, int N_out, int K) {
+        return make_streamed_weight(out, f->fp8, wt, s, N_out, K);
+    };
     auto mk = [&](const std::vector<rqb200_block_weights>& bl, std::vector<FastLayer>& out) -> int {
         out.resize(bl.size());
         for (size_t l = 0; l < bl.size(); l++) {
-            RQB_TRY(make_w(*f, &out[l].qkv, bl[l].wqkv, bl[l].sqkv, 3 * E, E));
-            RQB_TRY(make_w(*f, &out[l].proj, bl[l].wproj, bl[l].sproj, E, E));
-            RQB_TRY(make_w(*f, &out[l].fc1, bl[l].w1, bl[l].s1, 4 * E, E));
-            RQB_TRY(make_w(*f, &out[l].fc2, bl[l].w2, bl[l].s2, E, 4 * E));
+            RQB_TRY(make_w(&out[l].qkv, bl[l].wqkv, bl[l].sqkv, 3 * E, E));
+            RQB_TRY(make_w(&out[l].proj, bl[l].wproj, bl[l].sproj, E, E));
+            RQB_TRY(make_w(&out[l].fc1, bl[l].w1, bl[l].s1, 4 * E, E));
+            RQB_TRY(make_w(&out[l].fc2, bl[l].w2, bl[l].s2, E, 4 * E));
         }
         return 0;
     };
     int rc = mk(body, f->lbody);
     if (!rc) rc = mk(head, f->lhead);
-    if (!rc && w.w_in) rc = make_w(*f, &f->w_in, w.w_in, w.s_in, E, cfg.code_dim);
-    if (!rc && w.w_head) rc = make_w(*f, &f->w_head, w.w_head, w.s_head, E, cfg.code_dim);
-    if (!rc) rc = make_w(*f, &f->w_cls, w.w_cls, w.s_cls, cfg.vocab, E);
+    if (!rc && w.w_in) rc = make_w(&f->w_in, w.w_in, w.s_in, E, cfg.code_dim);
+    if (!rc && w.w_head) rc = make_w(&f->w_head, w.w_head, w.s_head, E, cfg.code_dim);
+    if (!rc) rc = make_w(&f->w_cls, w.w_cls, w.s_cls, cfg.vocab, E);
     if (cfg.embed_variant & RQB200_EMB_CLS_PER_DEPTH)       // depth d's [V,E] slice: V*E weight bytes per depth (2 per element in 16 bits)
         for (int d = 0; d < cfg.D && !rc; d++)
-            rc = make_w(*f, &f->w_cls_d[d], (const char*)w.w_cls + (size_t)d * cfg.vocab * E * (f->fp8 ? 1 : 2),
+            rc = make_w(&f->w_cls_d[d], (const char*)w.w_cls + (size_t)d * cfg.vocab * E * (f->fp8 ? 1 : 2),
                         f->fp8 ? w.s_cls + (size_t)d * cfg.vocab : nullptr, cfg.vocab, E);
-    if (!rc && w.w_ccls) rc = make_w(*f, &f->w_ccls, w.w_ccls, w.s_ccls, (cfg.vocab_cond + 127) / 128 * 128, E);
+    if (!rc && w.w_ccls) rc = make_w(&f->w_ccls, w.w_ccls, w.s_ccls, (cfg.vocab_cond + 127) / 128 * 128, E);
     if (rc) { delete f; return nullptr; }
     for (int i = 0; i <= G_COUNT; i++) f->tr_graph_base[i] = i * (TR_CAP / G_COUNT);
     return f;
@@ -1246,7 +1203,7 @@ static GemmTcParams epilogue(int mode, const float* bias, void* out, const float
 
 // One linear layer of a batched pass: the weight w over the M activation rows x [M, w.K], with the epilogue p.  The one place that picks
 // the GEMM:
-//   16-bit weights, M_launch > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue,
+//   weights with a 16-bit copy, M_launch > 256: the persistent rows GEMM (conv_tc.cu: 128 x 256 tiles, operand loads overlapped with the epilogue,
 //   like the next tile); it has no PDL attribute;
 //   M_launch <= 256, and E4M3 weights at every M: the weight streamer (E4M3: 128-row chunks, faster than the fp16 rows GEMM at the
 //   forward's shapes) over a tensor map of x, with the PDL attribute `pdl`.
@@ -1254,15 +1211,15 @@ static GemmTcParams epilogue(int mode, const float* bias, void* out, const float
 // each output row from its own activation row alone, so the GEMM the forward picks gives the chunk the forward's logits bit for bit.
 // streamer_only: never the rows GEMM.  For w_in / w_head, whose epilogues (bias_scale, a broadcast residual, res_div) the rows GEMM
 // does not have, and for the cond classifier, whose logits have always been the streamer's (the rows GEMM sums in another order).
-static int linear_rows(const ArFast& f, const FastW& w, const h16* x, int64_t M, int64_t M_launch, bool streamer_only, GemmTcParams p,
+static int linear_rows(const ArFast& f, const StreamedWeight& w, const h16* x, int64_t M, int64_t M_launch, bool streamer_only, GemmTcParams p,
                        bool pdl, cudaStream_t st) {
-    if (!streamer_only && !f.fp8 && M_launch > 256) {
+    if (!streamer_only && !w.e4m3() && M_launch > 256) {
         const bool f32 = p.mode == GT_F32;
         return launch_rows_gemm_tc(x, w.w16, p.bias, p.residual, f32 ? (float*)p.out : nullptr, f32 ? nullptr : p.out, p.mode == GT_H16_GELU,
                                    f.bf, M, w.N_out, w.K, st);
     }
     CUtensorMap tx;
-    RQB_TRY(make_tmap_2d(&tx, x, 1, w.K, M, (uint64_t)w.K * 2, 64, act_box(f, M)));
+    RQB_TRY(make_tmap_2d(&tx, x, 1, w.K, M, (uint64_t)w.K * 2, 64, gemm_tc_chunk_rows(w, M)));
     p.B = (int)M;
     return gemm_w(f, w, tx, p, pdl, st);
 }
@@ -1465,7 +1422,7 @@ int ar_fast_forward(ArFast* fp, const int64_t* codes, const int64_t* cond, int B
     RQB_TRY(forward_passes(f, ws, codes, cond, B, cond_logits_out != nullptr, [&](int64_t Mc) {
         return linear_rows(f, f.w_ccls, ws.XN, Mc, Mc, true, epilogue(GT_F32, w.b_ccls, cond_logits_out), false, st);
     }, st));
-    return for_each_cls_slice(f, B, [&](const FastW& fw, const float* bias, int d, int64_t Ms) {
+    return for_each_cls_slice(f, B, [&](const StreamedWeight& fw, const float* bias, int d, int64_t Ms) {
         return linear_rows(f, fw, ws.XN + (int64_t)d * Ms * c.embed_dim, Ms, Ms, false, epilogue(GT_F32, bias, logits_out + (int64_t)d * Ms * V),
                            false, st);
     });
@@ -1518,7 +1475,7 @@ int ar_fast_log_prob(ArFast* fp, const int64_t* codes, const int64_t* cond, int 
         }
         return 0;
     }, st));
-    return for_each_cls_slice(f, B, [&](const FastW& fw, const float* bias, int d, int64_t Ms) {
+    return for_each_cls_slice(f, B, [&](const StreamedWeight& fw, const float* bias, int d, int64_t Ms) {
         for (int64_t r0 = 0; r0 < Ms; r0 += LOGPROB_CHUNK) {
             const int64_t n = std::min(LOGPROB_CHUNK, Ms - r0), row = (int64_t)d * Ms + r0;
             RQB_TRY(linear_rows(f, fw, ws.fwd.XN + row * E, n, Ms, false, epilogue(GT_F32, bias, ws.CHUNK), false, st));
@@ -1534,7 +1491,7 @@ static int bind(ArFast& f, const FastWs& ws, void* wsp, int B) {
     const int E = c.embed_dim;
     drop_graphs(f);
     f.ws_base = nullptr;
-    const uint32_t bn = act_box(f, B);
+    const uint32_t bn = gemm_tc_chunk_rows(f.w_cls, B);      // (every weight of the engine has the classifier's format)
     RQB_TRY(make_tmap_2d(&f.tx_xn, ws.XN, 1, E, B, (uint64_t)E * 2, 64, bn));
     RQB_TRY(make_tmap_2d(&f.tx_att, ws.ATT, 1, E, B, (uint64_t)E * 2, 64, bn));
     RQB_TRY(make_tmap_2d(&f.tx_h, ws.Hh, 1, 4 * E, B, (uint64_t)E * 8, 64, bn));

@@ -29,8 +29,6 @@ __device__ __forceinline__ float4 load_w4<__nv_bfloat16>(const __nv_bfloat16* p)
     return make_float4(fa.x, fa.y, fb.x, fb.y);
 }
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
-
 // X [M,K] f32 (row stride ldx), W [N,K] WT, bias [N] f32 (nullable), R [M,N] f32 residual (nullable, ld = ldy),
 // Y [M,N] f32.  K % 4 == 0.  act: 0 none, 1 exact GELU.
 template <typename WT>

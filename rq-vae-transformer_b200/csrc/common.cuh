@@ -49,6 +49,25 @@ inline int check_launch(const char* what) {
         }                                                                                                         \
     } while (0)
 
+// cudaLaunchKernelEx with the programmatic-stream-serialization attribute `pdl`: the kernel may start before the previous kernel on
+// the stream has finished, so it must read upstream data only after griddepcontrol.wait.
+template <typename... KArgs, typename... Args>
+int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    RQB_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
+    g_launches++;
+    return 0;
+}
+
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 
@@ -128,6 +147,9 @@ __device__ __forceinline__ h16 pack_h16(float a, int bf) {
     __half h = __float2half_rn(a);
     return *reinterpret_cast<h16*>(&h);
 }
+
+// GELU in the exact erf form (F.gelu's default, the reference's gelu='v1')
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
 template <typename T>
 __device__ __forceinline__ float to_f32(T v);

@@ -53,7 +53,6 @@ struct ConvTcParams {
 };
 
 constexpr int CT_THREADS = 288;            // warps 0-7: two consumer warpgroups (64 tile rows each), warp 8: TMA producer
-constexpr int CT_CONSUMERS = 256;
 constexpr int CT_A_BYTES = 128 * 64 * 2;
 
 // PASSES == 1: single fp16 product.  PASSES == 3: split-fp16 ("fp16x3") -- both operands are carried as hi + lo fp16 pairs and
@@ -127,7 +126,7 @@ __device__ __forceinline__ void ct_epilogue16(const ConvTcParams& p, const float
         }
         if (p.gelu) {
 #pragma unroll
-            for (int i = 0; i < 16; i++) w[i] = 0.5f * w[i] * (1.0f + erff(w[i] * 0.70710678118654752440f));
+            for (int i = 0; i < 16; i++) w[i] = gelu_erf(w[i]);
         }
         uint4 pk[2];
         uint32_t* pw = reinterpret_cast<uint32_t*>(pk);
@@ -167,29 +166,6 @@ __device__ __forceinline__ void ct_epilogue16(const ConvTcParams& p, const float
             if (writer && bw < p.B)                                    // vidx < ngr: sum of group vidx; else sum of squares
                 p.gn_part[(((int64_t)bw * p.gn_chunks + chunk) * 32 + (n0 / cg + (vidx % ngr))) * 2 + (vidx / ngr)] = (double)tot;
         }
-    }
-}
-
-// accumulator columns [C0, BN) in chunks of CW through the staging buffer; thread t <-> tile row t % 128, columns 16 (t / 128) of the chunk
-template <int BN, int CW, int C0>
-__device__ __forceinline__ void ct_drain(const ConvTcParams& p, const float (&acc)[BN / 2], float* stage, int wg, int t, int nt, int tx,
-                                         int ty, int tb, int b, int y, int x, int64_t pix, bool valid) {
-    if constexpr (C0 < BN) {
-        tc::stage_acc<BN, CW, C0>(acc, stage, wg, t);
-        tc::bar_sync(1, CT_CONSUMERS);
-        const int r = t & 127, h = t >> 7;
-        if (h * 16 < CW) {
-            float v[16];
-            const float4* src = reinterpret_cast<const float4*>(stage + r * (CW + 4) + h * 16);
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const float4 z = src[i];
-                v[4 * i] = z.x; v[4 * i + 1] = z.y; v[4 * i + 2] = z.z; v[4 * i + 3] = z.w;
-            }
-            ct_epilogue16(p, v, nt * BN + C0 + h * 16, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
-        }
-        tc::bar_sync(1, CT_CONSUMERS);
-        ct_drain<BN, CW, C0 + CW>(p, acc, stage, wg, t, nt, tx, ty, tb, b, y, x, pix, valid);
     }
 }
 
@@ -298,7 +274,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int x = tx * p.TW + rx, y = ty * p.TH + ry, b = tb * p.NB + rb;
         const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
         const bool valid = (x < p.W) && (y < p.H) && (b < p.B) && (p.m_rows == 0 || pix < p.m_rows);
-        ct_drain<BN, CW, 0>(p, acc, stage, wg, t, nt, tx, ty, tb, b, y, x, pix, valid);
+        tc::drain_acc<BN, CW, 0>(acc, stage, wg, t, [&p, t, nt, tx, ty, tb, b, y, x, pix, valid](const float (&v)[16], int, int c) {
+            ct_epilogue16(p, v, nt * BN + c, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
+        });
     }
 }
 
@@ -456,7 +434,9 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int x = tx * 8 + rx, y = ty * p.TH + ry, b = tb * p.NB + rb;
         const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
         const bool valid = (x < p.W) && (y < p.H) && (b < p.B);
-        ct_drain<BN, CW, 0>(p, acc, stage, wg, t, nt, tx, ty, tb, b, y, x, pix, valid);
+        tc::drain_acc<BN, CW, 0>(acc, stage, wg, t, [&p, t, nt, tx, ty, tb, b, y, x, pix, valid](const float (&v)[16], int, int c) {
+            ct_epilogue16(p, v, nt * BN + c, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
+        });
     }
 }
 

@@ -103,14 +103,26 @@ struct GemmTcParams {
     float* partial;               // GT_PARTIAL: [splits][B][N_out] f32 (no bias)
     long long* trace;             // diagnostics, nullable: 4 globaltimer stamps of CTA 0 (entry, dependency resolved, accumulator ready, done)
 };
-inline int gemm_tc_bn(int B) { return B <= 16 ? 16 : B <= 32 ? 32 : B <= 64 ? 64 : B <= 128 ? 128 : 256; }
-int make_tmap_weight(CUtensorMap* out, const void* W, int N_out, int K);
-int launch_gemm_tc(const CUtensorMap& tmW, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl, cudaStream_t st);
-// E4M3 weights packed in 128 x 64 fragment-order tiles (16 B aligned), one fp32 scale per output row; p.fmt must be 0 (fp16 X).
-// Row chunks are at most 128 activation rows (BN = 256 would need both A fragment sets beside 128 accumulators per thread): the
-// activation tensor map's box is gemm_tc_fp8_bn(B) rows.
-inline int gemm_tc_fp8_bn(int B) { return B <= 64 ? gemm_tc_bn(B) : 128; }
-int launch_gemm_tc_fp8(const void* W8, const float* scale, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl, cudaStream_t st);
+// One weight [N_out, K] of the streamer: 16-bit (fp16 or bf16, the activations' GemmTcParams.fmt) behind its TMA tensor map, or E4M3
+// packed in 128 x 64 fragment-order tiles (rqvae._native.pack_fp8_tiles) with one fp32 scale per output row, which takes fp16
+// activations only.
+struct StreamedWeight {
+    int N_out = 0, K = 0;
+    const void* w16 = nullptr;          // 16-bit [N_out, K]; null for E4M3
+    CUtensorMap tm;                     // of w16
+    const uint8_t* q8 = nullptr;        // E4M3 tiles
+    const float* s8 = nullptr;          // E4M3 row scales [N_out]
+    bool e4m3() const { return w16 == nullptr; }
+};
+// e4m3: w = the packed tiles (16 B aligned) and scale their row scales (non-null); else w = the 16-bit matrix and scale unused
+int make_streamed_weight(StreamedWeight* out, bool e4m3, const void* w, const float* scale, int N_out, int K);
+// activation rows per row chunk (gridDim.y) of a launch over `rows` rows: the box height of the activation tensor map.  At most 256,
+// and 128 for E4M3 weights (BN = 256 would need both A fragment sets beside 128 accumulators per thread).
+inline int gemm_tc_chunk_rows(const StreamedWeight& w, int64_t rows) {
+    return rows <= 16 ? 16 : rows <= 32 ? 32 : rows <= 64 ? 64 : (rows <= 128 || w.e4m3()) ? 128 : 256;
+}
+// D = W X over the p.B activation rows behind tmX; p.N_out and p.K are the weight's
+int launch_gemm_tc(const StreamedWeight& w, const CUtensorMap& tmX, GemmTcParams p, bool pdl, cudaStream_t st);
 int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes_log2, uint64_t inner, uint64_t outer,
                  uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer);
 

@@ -413,20 +413,8 @@ int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, i
     while (vpad < V) vpad <<= 1;
     size_t smem = (size_t)V * sizeof(float) + (size_t)vpad * sizeof(SortItem);   // top_p is only known on the device
     RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(B);
-    cfg.blockDim = dim3(SMP_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    RQB_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel, logits, (const float*)nullptr, V, 1.0f, 0, 1.0f, (int64_t*)nullptr,
-                                (const int64_t*)nullptr, (int64_t)0, stt, d, HW, D, SAMPLER_ALGO_DEFAULT));
-    g_launches++;
-    return 0;
+    return launch_pdl(sample_kernel, dim3(B), dim3(SMP_THREADS), smem, st, pdl, logits, (const float*)nullptr, V, 1.0f, 0, 1.0f,
+                      (int64_t*)nullptr, (const int64_t*)nullptr, (int64_t)0, stt, d, HW, D, SAMPLER_ALGO_DEFAULT);
 }
 
 }  // namespace rqb

@@ -128,6 +128,30 @@ __device__ __forceinline__ void stage_acc(const float (&d)[N / 2], float* stage,
     }
 }
 
+// The epilogue of the two consumer warpgroups (256 threads, named barrier 1): accumulator columns [C0, N) in chunks of CW through the
+// staging buffer.  Per chunk, consumer thread t passes tile row t % 128, columns [c, c + 16) with c = C0 + 16 (t / 128) < C0 + CW, to
+// epi(v, row, c).
+template <int N, int CW, int C0, typename Epi>
+__device__ __forceinline__ void drain_acc(const float (&acc)[N / 2], float* stage, int wg, int t, const Epi& epi) {
+    if constexpr (C0 < N) {
+        stage_acc<N, CW, C0>(acc, stage, wg, t);
+        bar_sync(1, 256);
+        const int r = t & 127, h = t >> 7;
+        if (h * 16 < CW) {
+            float v[16];
+            const float4* src = reinterpret_cast<const float4*>(stage + r * (CW + 4) + h * 16);
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const float4 x = src[i];
+                v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
+            }
+            epi(v, r, C0 + h * 16);
+        }
+        bar_sync(1, 256);
+        drain_acc<N, CW, C0 + CW>(acc, stage, wg, t, epi);
+    }
+}
+
 }  // namespace tc
 
 // host: cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time libcuda dependency)
