@@ -308,6 +308,31 @@ int rqb200_dbg_rows_gemm(const void* X16, const void* W16, const float* bias, co
  * when t is outside [0, V).  Nothing outside a row's V columns is read. */
 int rqb200_dbg_log_prob_rows(const float* logits, int64_t ld, int V, int64_t rows, const int64_t* targets, float* out, void* stream);
 
+/* The fast AR tier's non-GEMM kernels (csrc/ar_fast.cu), one launch each through the launcher the engine calls (its form choice
+ * included).  16-bit tensors are fp16 (fmt 0) or bf16 (fmt 1); nh = E / 64 heads of 64 dims; a KV cache is [B or G][nh][Tmax][64].
+ * rqb200_dbg_attn_step: one step attention over B rows.  q, k, v [B, nh, 64] = fp32 (bqkv + part[0] + ... + part[S-1]) in that order,
+ *   rounded to 16 bits (bqkv [3E] f32; part [S, B, 3E] f32, rows query|key|value); k, v are written at cache row t of kc / vc; att [B, E]
+ *   = softmax(q k^T / 8) v over the cached rows [0, t) and the new token.  t is *t_dev (a device int32, the body graph's path) when
+ *   t_dev != NULL, else t_host.  form 1 = attn_fast_kernel, 2 = attn_fast2_kernel (RQB200_EINVAL unless Tmax <= 321), 0 = the form the
+ *   engine runs for this Tmax (2 for 16 <= Tmax <= 321, else 1).  Tmax <= 2048. */
+int rqb200_dbg_attn_step(int form, const float* part, int S, const float* bqkv, void* kc, void* vc, void* att, int B, int E, int Tmax,
+                         const int* t_dev, int t_host, int fmt, void* stream);
+/* rqb200_dbg_prefill_attn: the causal attention of a batched pass over G groups of T <= 2048 tokens: qkv [T*G, 3E] 16-bit, token-major
+ *   (row of token t of group g = t*G + g; query|key|value); att [T*G, E].  kc / vc (both or neither, T <= Tmax) receive the cache rows
+ *   [0, T) of every (group, head), nothing else.  The kernel is chosen by T as in the engine: a warp per (group, head) for T <= 4 and
+ *   T <= 8, 64 x 64 tiles with an online softmax above. */
+int rqb200_dbg_prefill_attn(const void* qkv, void* kc, void* vc, void* att, int G, int T, int E, int Tmax, int fmt, void* stream);
+/* rqb200_dbg_ln: LayerNorm (eps 1e-5) of `rows` rows of E <= 4608 (E % 128 == 0) f32: x_out (nullable) = x_in + bias + part[0] + ...
+ *   + part[S-1] + extra, summed in fp32 in that order (x_in / bias / extra nullable, bias / extra one [E] row for all rows; part [S, rows,
+ *   E]); xn (nullable; g, b [E]) = 16-bit LN(x).  x_in == x_out is allowed.  form 1: ln_reduce_kernel (the step's LN1 / LN2 form, one CTA
+ *   per row); form 2: ln_rows_kernel (the batched passes', a warp per row, rows grid-strided); form 0: the batched passes' choice by the
+ *   row count (form 1 below 512 rows, else form 2).  Forms 0 and 2 need x_in and take no part or bias. */
+int rqb200_dbg_ln(int form, const float* x_in, const float* part, int S, const float* bias, const float* extra, float* x_out, const float* g,
+                  const float* b, void* xn, int64_t rows, int E, int fmt, void* stream);
+/* rqb200_dbg_act_reduce: h [B, N] 16-bit = gelu_erf(fp32 (bias + part[0] + ... + part[S-1])) with bias [N], part [S, B, N] f32;
+ *   N % 4 == 0. */
+int rqb200_dbg_act_reduce(const float* part, int S, const float* bias, void* h, int B, int N, int fmt, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -918,18 +918,27 @@ static int gemm(const ArFast& f, const char* name, const StreamedWeight& w, cons
     return gemm_w(f, w, tx, p, f.use_pdl, st);
 }
 
-static int ln(const ArFast& f, const char* name, int rows, const float* x_in, const float* partial, int S, const float* bias,
-              const float* extra, float* x_out, const float* g, const float* be, h16* xn, cudaStream_t st,
-              const PrefetchList* pf = nullptr) {
-    PrefetchList none = {};
-    return launch_pdl(ln_reduce_kernel<384, 3>, dim3((unsigned)rows), dim3(384), (size_t)0, st, f.use_pdl, x_in, partial, S, bias, extra, x_out,
-                      g, be, xn, rows, f.cfg.embed_dim, f.bf, tr_slot(f, name), pf ? *pf : none);
+// ---- the single-token chain's non-GEMM launchers, functions of plain arguments: the engine and the rqb200_dbg_* entry points at the
+// end of this file call the same functions, so a kernel-level test runs the engine's own dispatch.  nh = E / 64 heads.
+
+// ln_reduce_kernel over `rows` rows (one CTA each): x_out = x_in + bias + sum_s partial[s] + extra ; xn = LN(x_out)
+static int ln(int rows, const float* x_in, const float* partial, int S, const float* bias, const float* extra, float* x_out, const float* g,
+              const float* be, h16* xn, int E, int bf, bool pdl, long long* tr, const PrefetchList& pf, cudaStream_t st) {
+    return launch_pdl(ln_reduce_kernel<384, 3>, dim3((unsigned)rows), dim3(384), (size_t)0, st, pdl, x_in, partial, S, bias, extra, x_out,
+                      g, be, xn, rows, E, bf, tr, pf);
 }
 
-static int attn(const ArFast& f, FastWs& ws, const float* bqkv, h16* kc, h16* vc, int Tmax, const int* t_ptr, int t_host,
-                cudaStream_t st) {
-    const rqb200_ar_config& c = f.cfg;
-    if (Tmax >= 16 && Tmax - 1 <= AF2_MAXROWS) {          // the body stack: four warps per (b, head)
+// the step attention form a cache of Tmax rows runs: 2 = attn_fast2_kernel (the body stack: four warps per (b, head), cached rows
+// staged in shared memory), 1 = attn_fast_kernel (head stacks, and body stacks past AF2_MAXROWS cached rows)
+static int attn_form(int Tmax) { return Tmax >= 16 && Tmax - 1 <= AF2_MAXROWS ? 2 : 1; }
+
+// one step attention over B rows: q/k/v = bqkv + sum of the S split-K partials part [S][B][3E], k/v appended at cache row t (t_ptr, a
+// device int, or t_host), att [B, E] = softmax(q k^T / 8) v.  form 0: attn_form(Tmax).
+static int attn(int form, const float* part, int S, const float* bqkv, h16* kc, h16* vc, h16* att, int B, int E, int Tmax, const int* t_ptr,
+                int t_host, int bf, bool pdl, long long* tr, cudaStream_t st) {
+    const int nh = E / 64;
+    if (form == 0) form = attn_form(Tmax);
+    if (form == 2) {
         const int rows = (Tmax - 1 + 7) & ~7;                        // cached rows a step can read (row t is the new token); 32 B-aligned float arrays behind them
         RQB_ENSURE_SMEM(attn2_smem(AF2_MAXROWS), attn_fast2_kernel);
         {   // 11 CTAs x 19.6 KB need the largest shared-memory carve-out (L1 is not used by this kernel)
@@ -941,14 +950,18 @@ static int attn(const ArFast& f, FastWs& ws, const float* bqkv, h16* kc, h16* vc
                 carve.fetch_or(1ull << (dev & 63), std::memory_order_release);
             }
         }
-        return launch_pdl(attn_fast2_kernel, dim3((unsigned)(f.B * c.n_head)), dim3(128), attn2_smem(rows), st, f.use_pdl,
-                          (const float*)ws.P, f.split_qkv, bqkv, kc, vc, ws.ATT, f.B, c.embed_dim, c.n_head, Tmax, rows, t_ptr, t_host,
-                          f.bf, tr_slot(f, "attn"));
+        return launch_pdl(attn_fast2_kernel, dim3((unsigned)(B * nh)), dim3(128), attn2_smem(rows), st, pdl, part, S, bqkv, kc, vc, att, B, E,
+                          nh, Tmax, rows, t_ptr, t_host, bf, tr);
     }
     const size_t smem = (size_t)(4 * ((Tmax + 31) & ~31)) * sizeof(float);
-    return launch_pdl(attn_fast_kernel, dim3((unsigned)ceil_div(f.B * c.n_head, 4)), dim3(128), smem, st, f.use_pdl,
-                      (const float*)ws.P, f.split_qkv, bqkv, kc, vc, ws.ATT, f.B, c.embed_dim, c.n_head, Tmax, t_ptr, t_host, f.bf,
-                      tr_slot(f, "attn"));
+    return launch_pdl(attn_fast_kernel, dim3((unsigned)ceil_div(B * nh, 4)), dim3(128), smem, st, pdl, part, S, bqkv, kc, vc, att, B, E, nh,
+                      Tmax, t_ptr, t_host, bf, tr);
+}
+
+// h [B, N] = 16-bit(gelu(bias + sum of the S split-K partials partial [S][B][N]))
+static int act_reduce(const float* partial, int S, const float* bias, h16* h, int B, int N, int bf, bool pdl, long long* tr, cudaStream_t st) {
+    return launch_pdl(act_reduce_kernel, dim3((unsigned)std::min<int64_t>(ceil_div((int64_t)B * N / 4, 256), 1184)), dim3(256), (size_t)0, st,
+                      pdl, partial, S, bias, h, B, N, bf, tr);
 }
 
 // one transformer stack on the single new token of every batch row; x lives in `x` (fp32); residual additions are deferred
@@ -976,28 +989,30 @@ static int fast_stack(const ArFast& f, const std::vector<rqb200_block_weights>& 
             for (int i = 0; i < 8; i++) { pf.p[i] = ptrs[i]; pf.bytes[i] = words[i] * 4u; }
             pf.n = 8;
         }
-        RQB_TRY(ln(f, "ln1", B, first ? x_src : x, pend ? ws.P : nof, pend ? f.split_fc2 : 0, pend ? blocks[l - 1].b2 : nof,
-                   first ? pending_extra : nof, x, bw.ln1_w, bw.ln1_b, ws.XN, st, &pf));
+        RQB_TRY(ln(B, first ? x_src : x, pend ? ws.P : nof, pend ? f.split_fc2 : 0, pend ? blocks[l - 1].b2 : nof, first ? pending_extra : nof,
+                   x, bw.ln1_w, bw.ln1_b, ws.XN, E, f.bf, f.use_pdl, tr_slot(f, "ln1"), pf, st));
         RQB_TRY(gemm(f, "qkv", maps[l].qkv, f.tx_xn, B, f.split_qkv, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0, st));
-        RQB_TRY(attn(f, ws, bw.bqkv, kc + per * l, vc + per * l, Tmax, t_ptr, t_host, st));
+        RQB_TRY(attn(0, ws.P, f.split_qkv, bw.bqkv, kc + per * l, vc + per * l, ws.ATT, B, E, Tmax, t_ptr, t_host, f.bf, f.use_pdl,
+                     tr_slot(f, "attn"), st));
         RQB_TRY(gemm(f, "proj", maps[l].proj, f.tx_att, B, f.split_proj, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0, st));
-        RQB_TRY(ln(f, "ln2", B, x, ws.P, f.split_proj, bw.bproj, nof, x, bw.ln2_w, bw.ln2_b, ws.XN, st));
+        RQB_TRY(ln(B, x, ws.P, f.split_proj, bw.bproj, nof, x, bw.ln2_w, bw.ln2_b, ws.XN, E, f.bf, f.use_pdl, tr_slot(f, "ln2"), PrefetchList{},
+                   st));
         if (f.split_fc1 == 1) {
             RQB_TRY(gemm(f, "fc1", maps[l].fc1, f.tx_xn, B, 1, GT_H16_GELU, bw.b1, 1.f, ws.Hh, nullptr, nullptr, 0, nullptr, 0, st));
         } else {
             RQB_TRY(gemm(f, "fc1", maps[l].fc1, f.tx_xn, B, f.split_fc1, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0, st));
-            RQB_TRY(launch_pdl(act_reduce_kernel, dim3((unsigned)std::min<int64_t>(ceil_div((int64_t)B * 4 * E / 4, 256), 1184)), dim3(256),
-                               (size_t)0, st, f.use_pdl, (const float*)ws.P, f.split_fc1, bw.b1, ws.Hh, B, 4 * E, f.bf,
-                               tr_slot(f, "act_reduce")));
+            RQB_TRY(act_reduce(ws.P, f.split_fc1, bw.b1, ws.Hh, B, 4 * E, f.bf, f.use_pdl, tr_slot(f, "act_reduce"), st));
         }
         RQB_TRY(gemm(f, "fc2", maps[l].fc2, f.tx_h, B, f.split_fc2, GT_PARTIAL, nullptr, 1.f, nullptr, ws.P, nullptr, 0, nullptr, 0, st));
     }
     // fold the last block's pending fc2 reduction into x (x is final on return) -- and the caller's LayerNorm, if any.  An empty
     // stack (a head-less model) only forms its input token x = x_src + pending_extra.
     if (blocks.empty())
-        RQB_TRY(ln(f, "finalize", B, x_src, nof, 0, nof, pending_extra, x, fin_g, fin_b, fin_g ? ws.XN : nullptr, st));
+        RQB_TRY(ln(B, x_src, nof, 0, nof, pending_extra, x, fin_g, fin_b, fin_g ? ws.XN : nullptr, E, f.bf, f.use_pdl, tr_slot(f, "finalize"),
+                   PrefetchList{}, st));
     else
-        RQB_TRY(ln(f, "finalize", B, x, ws.P, f.split_fc2, blocks.back().b2, nof, x, fin_g, fin_b, fin_g ? ws.XN : nullptr, st));
+        RQB_TRY(ln(B, x, ws.P, f.split_fc2, blocks.back().b2, nof, x, fin_g, fin_b, fin_g ? ws.XN : nullptr, E, f.bf, f.use_pdl,
+                   tr_slot(f, "finalize"), PrefetchList{}, st));
     return 0;
 }
 
@@ -1227,23 +1242,40 @@ static int linear_rows(const ArFast& f, const StreamedWeight& w, const h16* x, i
 // LayerNorm over the rows of a batched pass: x_out (nullable) = x_in + extra (nullable), xn (nullable) = LN(x_out).  512 rows and more: a
 // warp per row, launched with the PDL attribute; fewer: ln_reduce_kernel with nothing to reduce, launched without.  The two kernels
 // sum in different orders, so the threshold is part of the results.
-static int ln_rows(const ArFast& f, int64_t rows, const float* x_in, const float* extra, float* x_out, const float* g, const float* be,
-                   h16* xn, cudaStream_t st) {
-    const int E = f.cfg.embed_dim;
-    if (rows < 512) {
-        const float* nof = nullptr;
-        long long* no_trace = nullptr;
-        return launch_pdl(ln_reduce_kernel<384, 3>, dim3((unsigned)rows), dim3(384), (size_t)0, st, false, x_in, nof, 0, nof, extra, x_out, g, be,
-                          xn, (int)rows, E, f.bf, no_trace, PrefetchList{});
-    }
-    const dim3 grid((unsigned)std::min<int64_t>(ceil_div(rows, 8), (int64_t)f.n_sm * 8));
+// The warp-per-row form alone (ln_rows_kernel<NV>, the smallest NV with E <= 128 * NV), rows grid-strided over at most 8 CTAs per SM.
+static int ln_rows_warp(int64_t rows, const float* x_in, const float* extra, float* x_out, const float* g, const float* be, h16* xn, int E,
+                        int bf, int n_sm, cudaStream_t st) {
+    const dim3 grid((unsigned)std::min<int64_t>(ceil_div(rows, 8), (int64_t)n_sm * 8));
     const int nv = ceil_div(E, 128);
-#define RQB_LN_ROWS(NV) launch_pdl(ln_rows_kernel<NV>, grid, dim3(256), (size_t)0, st, true, x_in, extra, x_out, g, be, xn, rows, E, f.bf)
+#define RQB_LN_ROWS(NV) launch_pdl(ln_rows_kernel<NV>, grid, dim3(256), (size_t)0, st, true, x_in, extra, x_out, g, be, xn, rows, E, bf)
     if (nv <= 8) return RQB_LN_ROWS(8);
     if (nv <= 12) return RQB_LN_ROWS(12);
     if (nv <= 20) return RQB_LN_ROWS(20);
     return RQB_LN_ROWS(36);
 #undef RQB_LN_ROWS
+}
+static int ln_rows(int64_t rows, const float* x_in, const float* extra, float* x_out, const float* g, const float* be, h16* xn, int E, int bf,
+                   int n_sm, cudaStream_t st) {
+    if (rows < 512) {
+        const float* nof = nullptr;
+        return ln((int)rows, x_in, nof, 0, nof, extra, x_out, g, be, xn, E, bf, false, nullptr, PrefetchList{}, st);
+    }
+    return ln_rows_warp(rows, x_in, extra, x_out, g, be, xn, E, bf, n_sm, st);
+}
+
+// Causal attention of a batched pass over G groups of T tokens (qkv token-major [T*G, 3E], bias added), the cache rows [0, T) of every
+// (group, head) written when kc != NULL: a warp per (group, head) for T <= 8, 64-query tiles over 64-key tiles above.
+static int prefill_attn(const h16* qkv, h16* kc, h16* vc, h16* att, int G, int T, int E, int Tmax, int bf, bool pdl, cudaStream_t st) {
+    const int nh = E / 64;
+    if (T <= 4)                                       // tiny groups (the forward's head stack): a warp per (group, head)
+        return launch_pdl(prefill_attn_small_kernel<4>, dim3((unsigned)ceil_div((int64_t)G * nh, 4)), dim3(128), (size_t)0, st, pdl, qkv, kc,
+                          vc, att, G, T, E, nh, Tmax, bf);
+    if (T <= 8)
+        return launch_pdl(prefill_attn_small_kernel<8>, dim3((unsigned)ceil_div((int64_t)G * nh, 4)), dim3(128), (size_t)0, st, pdl, qkv, kc,
+                          vc, att, G, T, E, nh, Tmax, bf);
+    const dim3 grid((unsigned)((int64_t)ceil_div(T, 64) * G * nh));     // 64-query tiles over 64-key tiles, online softmax
+    if (bf) return launch_pdl(prefill_attn_flash_kernel<true>, grid, dim3(128), (size_t)0, st, pdl, qkv, kc, vc, att, G, T, E, nh, Tmax);
+    return launch_pdl(prefill_attn_flash_kernel<false>, grid, dim3(128), (size_t)0, st, pdl, qkv, kc, vc, att, G, T, E, nh, Tmax);
 }
 
 static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights>& blocks, const std::vector<FastLayer>& maps,
@@ -1256,28 +1288,13 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
     const float* nof = nullptr;
     for (size_t l = 0; l < blocks.size(); l++) {
         const rqb200_block_weights& bw = blocks[l];
-        RQB_TRY(ln_rows(f, M, bb.X, nof, nullptr, bw.ln1_w, bw.ln1_b, bb.XN, st));
+        RQB_TRY(ln_rows(M, bb.X, nof, nullptr, bw.ln1_w, bw.ln1_b, bb.XN, E, f.bf, f.n_sm, st));
         RQB_TRY(linear_rows(f, maps[l].qkv, bb.XN, M, M, false, epilogue(GT_H16, bw.bqkv, bb.QKV), pdl, st));
         h16* kcl = kc ? kc + kv_per_layer * l : nullptr;
         h16* vcl = vc ? vc + kv_per_layer * l : nullptr;
-        if (T <= 4) {                                     // tiny groups (the forward's head stack): a warp per (group, head)
-            RQB_TRY(launch_pdl(prefill_attn_small_kernel<4>, dim3((unsigned)ceil_div((int64_t)G * c.n_head, 4)), dim3(128), (size_t)0, st, pdl,
-                               (const h16*)bb.QKV, kcl, vcl, bb.ATT, G, T, E, c.n_head, Tmax, f.bf));
-        } else if (T <= 8) {
-            RQB_TRY(launch_pdl(prefill_attn_small_kernel<8>, dim3((unsigned)ceil_div((int64_t)G * c.n_head, 4)), dim3(128), (size_t)0, st, pdl,
-                               (const h16*)bb.QKV, kcl, vcl, bb.ATT, G, T, E, c.n_head, Tmax, f.bf));
-        } else {                                          // 64-query tiles over 64-key tiles, online softmax
-            const dim3 grid((unsigned)((int64_t)ceil_div(T, 64) * G * c.n_head));
-            if (f.bf) {
-                RQB_TRY(launch_pdl(prefill_attn_flash_kernel<true>, grid, dim3(128), (size_t)0, st, pdl, (const h16*)bb.QKV, kcl, vcl, bb.ATT,
-                                   G, T, E, c.n_head, Tmax));
-            } else {
-                RQB_TRY(launch_pdl(prefill_attn_flash_kernel<false>, grid, dim3(128), (size_t)0, st, pdl, (const h16*)bb.QKV, kcl, vcl, bb.ATT,
-                                   G, T, E, c.n_head, Tmax));
-            }
-        }
+        RQB_TRY(prefill_attn(bb.QKV, kcl, vcl, bb.ATT, G, T, E, Tmax, f.bf, pdl, st));
         RQB_TRY(linear_rows(f, maps[l].proj, bb.ATT, M, M, false, epilogue(GT_F32, bw.bproj, bb.X, bb.X, E), pdl, st));
-        RQB_TRY(ln_rows(f, M, bb.X, nof, nullptr, bw.ln2_w, bw.ln2_b, bb.XN, st));
+        RQB_TRY(ln_rows(M, bb.X, nof, nullptr, bw.ln2_w, bw.ln2_b, bb.XN, E, f.bf, f.n_sm, st));
         RQB_TRY(linear_rows(f, maps[l].fc1, bb.XN, M, M, false, epilogue(GT_H16_GELU, bw.b1, bb.H), pdl, st));
         RQB_TRY(linear_rows(f, maps[l].fc2, bb.H, M, M, false, epilogue(GT_F32, bw.b2, bb.X, bb.X, E), pdl, st));
     }
@@ -1373,11 +1390,11 @@ static int forward_passes(const ArFast& f, const FwdWs& ws, const int64_t* codes
     RQB_TRY(stack_batched(f, f.body, f.lbody, bb, B, Tb, nullptr, nullptr, 0, Tb, st));
     if (with_cond) {                                        // cond_classifier(latents[:, :cond_len-1])        (:153-156)
         const int64_t Mc = (int64_t)(cl - 1) * B;
-        RQB_TRY(ln_rows(f, Mc, ws.BX, nof, nullptr, w.ccls_ln_w, w.ccls_ln_b, ws.XN, st));
+        RQB_TRY(ln_rows(Mc, ws.BX, nof, nullptr, w.ccls_ln_w, w.ccls_ln_b, ws.XN, E, f.bf, f.n_sm, st));
         RQB_TRY(cond_cls(Mc));
     }
     // head tokens: d = 0 rows = spatial ctx (body rows of tokens cond_len-1 ..) + pos_emb_d[0]; d >= 1 rows = head_mlp(cumsum)
-    RQB_TRY(ln_rows(f, G, ws.BX + (int64_t)(cl - 1) * B * E, w.pos_emb_d, ws.HX, nof, nof, nullptr, st));
+    RQB_TRY(ln_rows(G, ws.BX + (int64_t)(cl - 1) * B * E, w.pos_emb_d, ws.HX, nof, nof, nullptr, E, f.bf, f.n_sm, st));
     for (int d = 1; d < D; d++) {
         if (c.embed_variant & RQB200_EMB_TOK_HEAD) {        // tok_emb(code_{d-1}) + pos_emb_d[d]        (:164,177)
             RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, HW), dim3(128), (size_t)0, st, false, (const StepState*)ws.state, w.tok_emb,
@@ -1394,7 +1411,7 @@ static int forward_passes(const ArFast& f, const FwdWs& ws, const int64_t* codes
     BatchBufs hb = {ws.HX, ws.XN, ws.QKV, ws.ATT, ws.H};
     RQB_TRY(stack_batched(f, f.head, f.lhead, hb, G, D, nullptr, nullptr, 0, D, st));
     // classifier LayerNorm                                                                         (:181-183)
-    return ln_rows(f, Mh, ws.HX, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, st);
+    return ln_rows(Mh, ws.HX, nof, nullptr, w.cls_ln_w, w.cls_ln_b, ws.XN, E, f.bf, f.n_sm, st);
 }
 
 // The classifier launches of the forward: one over all D*H*W*B rows of ws.XN, or (per-depth classifiers) one per depth over that
@@ -1611,3 +1628,55 @@ int ar_fast_trace(ArFast* f, long long* out_host, int cap_launches, char* names,
 }
 
 }  // namespace rqb
+
+// ---- diagnostic entry points (tests/test_gpu_ar_kernels.py): one launch of a step or batched-pass kernel through the launcher the
+// engine calls, without the PDL attribute and the trace
+
+extern "C" int rqb200_dbg_attn_step(int form, const float* part, int S, const float* bqkv, void* kc, void* vc, void* att, int B, int E, int Tmax,
+                                    const int* t_dev, int t_host, int fmt, void* stream) {
+    using namespace rqb;
+    if (form < 0 || form > 2 || fmt < 0 || fmt > 1 || B < 1 || S < 0 || E < 64 || E % 64 || Tmax < 1 || Tmax > FAST_MAXT)
+        return fail(RQB200_EINVAL, "dbg_attn_step: need form 0..2, fmt 0..1, B >= 1, S >= 0, E % 64 == 0, 1 <= Tmax <= 2048");
+    if (!bqkv || !kc || !vc || !att || (S > 0 && !part)) return fail(RQB200_EINVAL, "dbg_attn_step: null argument");
+    if (!t_dev && (t_host < 0 || t_host >= Tmax)) return fail(RQB200_EINVAL, "dbg_attn_step: t outside [0, Tmax)");
+    if (form == 2 && Tmax - 1 > AF2_MAXROWS) return fail(RQB200_EINVAL, "dbg_attn_step: form 2 takes at most 320 cached rows (Tmax <= 321)");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_attn_step: no CUDA device");
+    return attn(form, part, S, bqkv, (h16*)kc, (h16*)vc, (h16*)att, B, E, Tmax, t_dev, t_host, fmt, false, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int rqb200_dbg_prefill_attn(const void* qkv, void* kc, void* vc, void* att, int G, int T, int E, int Tmax, int fmt, void* stream) {
+    using namespace rqb;
+    if (fmt < 0 || fmt > 1 || G < 1 || T < 1 || T > FAST_MAXT || E < 64 || E % 64 || (int64_t)ceil_div(T, 64) * G * (E / 64) > INT32_MAX)
+        return fail(RQB200_EINVAL, "dbg_prefill_attn: need fmt 0..1, G >= 1, 1 <= T <= 2048, E % 64 == 0");
+    if (!qkv || !att || !kc != !vc) return fail(RQB200_EINVAL, "dbg_prefill_attn: null qkv / att, or only one of kc / vc");
+    if (kc && T > Tmax) return fail(RQB200_EINVAL, "dbg_prefill_attn: T > Tmax");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_prefill_attn: no CUDA device");
+    return prefill_attn((const h16*)qkv, (h16*)kc, (h16*)vc, (h16*)att, G, T, E, Tmax, fmt, false, (cudaStream_t)stream);
+}
+
+extern "C" int rqb200_dbg_ln(int form, const float* x_in, const float* partial, int S, const float* bias, const float* extra, float* x_out,
+                             const float* g, const float* b, void* xn, int64_t rows, int E, int fmt, void* stream) {
+    using namespace rqb;
+    if (form < 0 || form > 2 || fmt < 0 || fmt > 1 || rows < 1 || rows > INT32_MAX || S < 0 || E < 128 || E % 128 || E > 4608)
+        return fail(RQB200_EINVAL, "dbg_ln: need form 0..2, fmt 0..1, 1 <= rows < 2^31, S >= 0, E % 128 == 0, E <= 4608");
+    if ((S > 0 && !partial) || (xn && (!g || !b))) return fail(RQB200_EINVAL, "dbg_ln: null partial, or xn without g / b");
+    if (form != 1 && (S > 0 || partial || bias || !x_in))
+        return fail(RQB200_EINVAL, "dbg_ln: forms 0 and 2 (the batched passes' LayerNorm) take x_in and no partials or bias");
+    int dev = 0, n_sm = 0;
+    if (rqb200_device_count() <= 0 || cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+        return fail(RQB200_ENODEV, "dbg_ln: no CUDA device");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (form == 1) return ln((int)rows, x_in, partial, S, bias, extra, x_out, g, b, (h16*)xn, E, fmt, false, nullptr, PrefetchList{}, st);
+    if (form == 2) return ln_rows_warp(rows, x_in, extra, x_out, g, b, (h16*)xn, E, fmt, n_sm, st);
+    return ln_rows(rows, x_in, extra, x_out, g, b, (h16*)xn, E, fmt, n_sm, st);
+}
+
+extern "C" int rqb200_dbg_act_reduce(const float* partial, int S, const float* bias, void* h, int B, int N, int fmt, void* stream) {
+    using namespace rqb;
+    if (fmt < 0 || fmt > 1 || S < 0 || B < 1 || N < 4 || N % 4)
+        return fail(RQB200_EINVAL, "dbg_act_reduce: need fmt 0..1, S >= 0, B >= 1, N % 4 == 0");
+    if (!bias || !h || (S > 0 && !partial)) return fail(RQB200_EINVAL, "dbg_act_reduce: null argument");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_act_reduce: no CUDA device");
+    return act_reduce(partial, S, bias, (h16*)h, B, N, fmt, false, nullptr, (cudaStream_t)stream);
+}
