@@ -333,6 +333,34 @@ int rqb200_dbg_ln(int form, const float* x_in, const float* part, int S, const f
  *   N % 4 == 0. */
 int rqb200_dbg_act_reduce(const float* part, int S, const float* bias, void* h, int B, int N, int fmt, void* stream);
 
+/* The VAE engine's kernels between the convs, and the exact tier's conv (csrc/conv_kernels.cu, csrc/conv_tc.cu), one launch each
+ * through the launcher the engine calls.  Activations are NHWC f32 unless stated.
+ * rqb200_dbg_vae_conv: the fp32 FFMA implicit-GEMM conv of the exact tier (and of the encoder's conv_in on both tiers), with the
+ *   engine's geometry rule: X [B, H, W, Cin] (NCHW [B, Cin, H, W] when in_nchw), Wt OHWI [Cout, ks, ks, Cin] in wdtype (RQB200_F32,
+ *   RQB200_F16 or RQB200_BF16), ks 1 or 3.  upsample: the conv reads the nearest x2 upsample of X; stride 2 (no upsample): the
+ *   Downsample's F.pad (0, 1, 0, 1) then a 3x3 stride-2 conv.  Output extent Ho = (upsample ? 2H : H) / stride (Wo alike), padding 1
+ *   for 3x3 stride 1, else 0.  out [B, Ho, Wo, Cout] (NCHW [B, Cout, Ho, Wo] when out_nchw) = conv + bias (nullable) + residual
+ *   (nullable, [B, Ho, Wo, Cout]; not with out_nchw). */
+int rqb200_dbg_vae_conv(const float* X, const void* Wt, int wdtype, const float* bias, const float* residual, float* out, int B, int H,
+                        int W, int Cin, int Cout, int ks, int stride, int upsample, int in_nchw, int out_nchw, void* stream);
+/* rqb200_dbg_groupnorm: GroupNorm(32, eps 1e-6) of X [B, HW, C] (C % 32 == 0), then SiLU when silu, with gamma / beta [C] f32.
+ *   form 0: the exact tier (gn_stats_kernel + gn_apply_kernel) into Y [B, HW, C] f32.
+ *   form 1: the fast tier with stand-alone statistics (gn_stats_kernel, gn_finalize_kernel, gn_apply_f16_kernel) into the fp16 conv
+ *   operand Y16 [B, HW, C] and, when Y16lo != NULL, its lo half (value - fp16(value), rounded to fp16).  C % 128 == 0.
+ *   form 2: as form 1 from the partial statistics a conv epilogue left in stats_ws (rqb200_dbg_conv_tc_gn on X with gn_part =
+ *   stats_ws): HW / 32 chunks per image, HW % 32 == 0.
+ *   stats_ws holds ws_doubles doubles, at least B * ceil(HW / 32) * 64 + B * 64 (RQB200_EWORKSPACE otherwise); its contents after
+ *   the call are unspecified. */
+int rqb200_dbg_groupnorm(int form, const float* X, const float* gamma, const float* beta, float* Y, void* Y16, void* Y16lo,
+                         double* stats_ws, int64_t ws_doubles, int B, int HW, int C, int silu, void* stream);
+/* rqb200_dbg_cast_f16: the fast tier's conv operand of X [B, H, W, C] (C % 4 == 0): Y16 = fp16(X) and, when Y16lo != NULL,
+ *   Y16lo = fp16(X - Y16); upsample: of the nearest x2 upsample of X, [B, 2H, 2W, C]. */
+int rqb200_dbg_cast_f16(const float* X, void* Y16, void* Y16lo, int B, int H, int W, int C, int upsample, void* stream);
+/* rqb200_dbg_vae_attn: the core of the VAE's AttnBlock: qkv [B, HW, 3C] (q | k | v per pixel) -> out [B, HW, C] = softmax over the HW
+ *   keys of (q k^T * float(1 / sqrt(C))) v, single head.  RQB200_EINVAL, with nothing launched, when the C + HW floats of the query
+ *   and its scores do not fit in shared memory beside the kernel's static shared memory within 48 KB (C + HW > about 12000). */
+int rqb200_dbg_vae_attn(const float* qkv, float* out, int B, int HW, int C, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,6 +7,8 @@
 // is never materialised), Downsample :50-54 (F.pad (0,1,0,1) then 3x3 s2 p0 -- here implicit zero row/column),
 // AttnBlock.forward :158-182 (1x1 q/k/v convs, bmm, * c^-0.5, softmax over keys, bmm, 1x1 proj_out, x + h).
 // Layout: activations NHWC fp32 (channels contiguous -> the GEMM K axis is contiguous per tap), weights OHWI.
+#include <algorithm>
+
 #include "kernels.h"
 
 namespace rqb {
@@ -107,6 +109,16 @@ conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const f
             else Y[mm * N + n] = v;
         }
     }
+}
+
+ConvGeom vae_conv_geom(int B, int H, int W, int Cin, int Cout, int ks, int stride, int upsample, int in_nchw, int out_nchw) {
+    ConvGeom g;
+    g.B = B; g.Hi = H; g.Wi = W; g.Cin = Cin; g.Cout = Cout; g.KH = g.KW = ks; g.stride = stride;
+    g.upsample = upsample; g.in_nchw = in_nchw; g.out_nchw = out_nchw;
+    g.pad = (ks == 3 && stride == 1) ? 1 : 0;
+    g.Ho = (upsample ? 2 * H : H) / stride;
+    g.Wo = (upsample ? 2 * W : W) / stride;
+    return g;
 }
 
 int launch_conv(const float* X, const void* W, int wdtype, const float* bias, const float* R, float* Y, const ConvGeom& g,
@@ -254,8 +266,14 @@ __global__ void __launch_bounds__(256) vae_attn_kernel(const float* __restrict__
 }
 
 int launch_vae_attn(const float* qkv, float* out, int B, int HW, int C, cudaStream_t st) {
+    // the dynamic [C + HW] floats must fit beside the kernel's static shared memory in the 48 KB a launch takes without an opt-in
+    static const size_t max_dyn = [] {
+        cudaFuncAttributes a{};
+        if (cudaFuncGetAttributes(&a, vae_attn_kernel) != cudaSuccess) { cudaGetLastError(); return (size_t)0; }
+        return std::min((size_t)a.maxDynamicSharedSizeBytes, 48 * 1024 - a.sharedSizeBytes);
+    }();
     size_t smem = (size_t)(C + HW) * sizeof(float);
-    if (smem > 48 * 1024) return fail(RQB200_EINVAL, "vae_attn: C + HW too large");
+    if (smem > max_dyn) return fail(RQB200_EINVAL, "vae_attn: C + HW too large");
     float scale = (float)(1.0 / sqrt((double)C));                  // int(c) ** (-0.5) evaluated in double, then cast
     vae_attn_kernel<<<dim3(HW, B), 256, smem, st>>>(qkv, out, HW, C, scale);
     return check_launch("vae_attn");

@@ -64,6 +64,9 @@ struct ConvGeom {
     int out_nchw;            // 1: write [B,Cout,Ho,Wo] (final conv_out)
     int in_nchw;             // 1: read [B,Cin,Hi,Wi] (encoder conv_in)
 };
+// the geometry of one conv of the VAE layer plan (vae_engine.cu): H, W the input extent before the optional nearest x2 upsample;
+// Ho, Wo = the (upsampled) extent / stride; pad 1 for a 3x3 stride-1 conv, else 0 (stride 2: the Downsample's implicit (0,1,0,1))
+ConvGeom vae_conv_geom(int B, int H, int W, int Cin, int Cout, int ks, int stride, int upsample, int in_nchw, int out_nchw);
 int launch_conv(const float* X, const void* W, int wdtype, const float* bias, const float* R, float* Y, const ConvGeom& g,
                 cudaStream_t st);
 int launch_groupnorm_silu(const float* X, const float* gamma, const float* beta, float* Y, double* stats_ws, int B, int HW,

@@ -98,20 +98,13 @@ struct VaeRun {
     // goes to a GroupNorm next, so the wgmma epilogue emits its partial statistics.
     int conv(const std::string& name, const Operand& in, float* out, const float* resid, int H, int W, int Cin, int Cout, int ks,
              int stride, bool feeds_gn, int out_nchw) {
-        const int Ho = (in.upsample ? 2 * H : H) / stride, Wo = (in.upsample ? 2 * W : W) / stride;
+        const ConvGeom g = vae_conv_geom(B, H, W, Cin, Cout, ks, stride, in.upsample, in.nchw, out_nchw);
+        const int Ho = g.Ho, Wo = g.Wo;
         const VTensor* w = get(name + ".weight", (int64_t)Cout * ks * ks * Cin);
         const VTensor* b = get(name + ".bias", Cout);
         note_act((int64_t)Ho * Wo, Cout);
         if (dry || !w || !b) return 0;
-        if (in.slot < 0) {
-            ConvGeom g;
-            g.B = B; g.Hi = H; g.Wi = W; g.Cin = Cin; g.Cout = Cout; g.KH = g.KW = ks; g.stride = stride;
-            g.upsample = in.upsample; g.in_nchw = in.nchw; g.out_nchw = out_nchw;
-            g.pad = (ks == 3 && stride == 1) ? 1 : 0;
-            g.Ho = Ho;
-            g.Wo = Wo;
-            return launch_conv(in.x, w->ptr, w->dtype, (const float*)b->ptr, resid, out, g, st);
-        }
+        if (in.slot < 0) return launch_conv(in.x, w->ptr, w->dtype, (const float*)b->ptr, resid, out, g, st);
         if (w->dtype != RQB200_F16) return fail(RQB200_ESTATE, "vae fast tier: conv weights must be fp16: " + name);
         const __half* in_lo = nullptr;
         const void* w_lo = nullptr;
@@ -369,4 +362,49 @@ int rqb200_vae_encode(rqb200_vae* h, const float* x, int B, float* z_e, void* wo
     return rc;
 }
 int64_t rqb200_vae_last_launches(const rqb200_vae* h) { return h ? h->last_launches : 0; }
+
+// ---- diagnostic entry points (tests/test_gpu_vae_kernels.py): one launch of a kernel between the VAE's convs, or of the exact tier's
+// conv, through the launcher the engine calls
+
+int rqb200_dbg_vae_conv(const float* X, const void* Wt, int wdtype, const float* bias, const float* residual, float* out, int B, int H,
+                        int W, int Cin, int Cout, int ks, int stride, int upsample, int in_nchw, int out_nchw, void* stream) {
+    using namespace rqb;
+    if (B < 1 || H < 1 || W < 1 || Cin < 1 || Cout < 1 || (ks != 1 && ks != 3) || (stride != 1 && stride != 2) || (upsample && stride != 1))
+        return fail(RQB200_EINVAL, "dbg_vae_conv: need B, H, W, Cin, Cout >= 1, ks 1 | 3, stride 1 | 2, no upsample with stride 2");
+    if (!X || !Wt || !out || (residual && out_nchw)) return fail(RQB200_EINVAL, "dbg_vae_conv: null argument, or a residual with NCHW output");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_vae_conv: no CUDA device");
+    const ConvGeom g = vae_conv_geom(B, H, W, Cin, Cout, ks, stride, upsample != 0, in_nchw != 0, out_nchw != 0);
+    return launch_conv(X, Wt, wdtype, bias, residual, out, g, (cudaStream_t)stream);
+}
+
+int rqb200_dbg_groupnorm(int form, const float* X, const float* gamma, const float* beta, float* Y, void* Y16, void* Y16lo,
+                         double* stats_ws, int64_t ws_doubles, int B, int HW, int C, int silu, void* stream) {
+    using namespace rqb;
+    if (form < 0 || form > 2 || B < 1 || HW < 1 || C < 32 || C % 32 || (form > 0 && C % 128) || (form == 2 && HW % 32))
+        return fail(RQB200_EINVAL, "dbg_groupnorm: need form 0..2, B, HW >= 1, C % 32 == 0 (forms 1, 2: C % 128 == 0; form 2: HW % 32 == 0)");
+    if (!X || !gamma || !beta || !stats_ws || (form == 0 ? !Y : !Y16))
+        return fail(RQB200_EINVAL, "dbg_groupnorm: null argument");
+    if (ws_doubles < 0 || (size_t)ws_doubles < groupnorm_ws_doubles(B, HW))
+        return fail(RQB200_EWORKSPACE, "dbg_groupnorm: statistics workspace smaller than groupnorm_ws_doubles(B, HW)");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_groupnorm: no CUDA device");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (form == 0) return launch_groupnorm_silu(X, gamma, beta, Y, stats_ws, B, HW, C, silu != 0, st);
+    return launch_groupnorm_f16(X, gamma, beta, Y16, Y16lo, stats_ws, B, HW, C, silu != 0, st, form == 2 ? HW / 32 : 0);
+}
+
+int rqb200_dbg_cast_f16(const float* X, void* Y16, void* Y16lo, int B, int H, int W, int C, int upsample, void* stream) {
+    using namespace rqb;
+    if (B < 1 || H < 1 || W < 1 || C < 4) return fail(RQB200_EINVAL, "dbg_cast_f16: need B, H, W >= 1, C >= 4");
+    if (!X || !Y16) return fail(RQB200_EINVAL, "dbg_cast_f16: null argument");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_cast_f16: no CUDA device");
+    return launch_cast_f16(X, Y16, Y16lo, B, H, W, C, upsample != 0, (cudaStream_t)stream);
+}
+
+int rqb200_dbg_vae_attn(const float* qkv, float* out, int B, int HW, int C, void* stream) {
+    using namespace rqb;
+    if (B < 1 || HW < 1 || C < 1) return fail(RQB200_EINVAL, "dbg_vae_attn: need B, HW, C >= 1");
+    if (!qkv || !out) return fail(RQB200_EINVAL, "dbg_vae_attn: null argument");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_vae_attn: no CUDA device");
+    return launch_vae_attn(qkv, out, B, HW, C, (cudaStream_t)stream);
+}
 }

@@ -131,6 +131,10 @@ def lib():
     L.rqb200_dbg_prefill_attn.argtypes = [C.c_void_p] * 4 + [C.c_int] * 5 + [C.c_void_p]
     L.rqb200_dbg_ln.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 6 + [C.c_int64, C.c_int, C.c_int, C.c_void_p]
     L.rqb200_dbg_act_reduce.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p] + [C.c_int] * 3 + [C.c_void_p]
+    L.rqb200_dbg_vae_conv.argtypes = [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int] * 10 + [C.c_void_p]
+    L.rqb200_dbg_groupnorm.argtypes = [C.c_int] + [C.c_void_p] * 7 + [C.c_int64] + [C.c_int] * 4 + [C.c_void_p]
+    L.rqb200_dbg_cast_f16.argtypes = [C.c_void_p] * 3 + [C.c_int] * 5 + [C.c_void_p]
+    L.rqb200_dbg_vae_attn.argtypes = [C.c_void_p] * 2 + [C.c_int] * 3 + [C.c_void_p]
     _lib = L
     return L
 
@@ -145,7 +149,8 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_dbg_rows_gemm", "rqb200_rq_quantize_depthwise", "rqb200_rq_embed_sum_depthwise",
            "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise", "rqb200_ar_log_prob",
            "rqb200_ar_log_prob_workspace_bytes", "rqb200_dbg_log_prob_rows", "rqb200_dbg_attn_step", "rqb200_dbg_prefill_attn",
-           "rqb200_dbg_ln", "rqb200_dbg_act_reduce"]
+           "rqb200_dbg_ln", "rqb200_dbg_act_reduce", "rqb200_dbg_vae_conv", "rqb200_dbg_groupnorm", "rqb200_dbg_cast_f16",
+           "rqb200_dbg_vae_attn"]
 
 
 def check(rc, what=""):
