@@ -178,6 +178,16 @@ int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* c
                           float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
                           void* workspace, size_t workspace_bytes, void* stream);
+/* rqb200_ar_sample_span with classifier-free guidance: B = 2n rows, n >= 1.  partial, cond, out_codes, force_codes and logits_out
+ * are laid out [n conditional rows | n unconditional rows]; noise is per image, [n_tok][n][V] (noise_stride apart per token).  At
+ * every token both branches produce logits c and u, and the sampler draws image b's code from l = u + cfg_scale * (c - u) in fp32
+ * (three rounded operations, no FMA), then temperature, top-k and top-p as unguided, with noise row b; the code is written to
+ * rows b and n + b, and both branches consume it from the next token on.  Teacher forcing copies every row's own forced code.
+ * logits_out receives the raw logits of all 2n rows.  Fast tier: 2n <= 256. */
+int rqb200_ar_sample_span_cfg(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
+                              float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
+                              int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
+                              void* workspace, size_t workspace_bytes, void* stream, float cfg_scale);
 /* RQTransformer.cached_forward (transformers.py:190-287): the logits of ONE token (h, w, d) into logits_out [B,V] f32.
  *   xs: the caller's code map, int64, batch row b at xs + b*xs_batch_stride, positions in raster order, D codes each
  *       (only the codes this step consumes are read: position idx-1 when d == 0, codes 0..d-1 of position idx when d > 0;

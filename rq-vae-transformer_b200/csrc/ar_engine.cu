@@ -163,11 +163,12 @@ static int head_depth(const rqb200_ar* h, const int64_t* codes, int B, int idx, 
     return launch_linear(ws.XN, E, (const char*)w.w_cls + cd * V * E * wsz, wd, w.b_cls + cd * V, nullptr, lg, V, B, V, E, 0, st);
 }
 
-// positions [idx0, idx_end) of the raster; resume != 0: no prefill, continue on the caches / context left in this workspace
+// positions [idx0, idx_end) of the raster; resume != 0: no prefill, continue on the caches / context left in this workspace.
+// cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s (the sampler forms the guided logits)
 static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx0, int idx_end, int resume,
                           float temperature, const int32_t* top_k, const float* top_p, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force, int64_t* out, void* wsp,
-                          size_t ws_bytes, cudaStream_t st) {
+                          size_t ws_bytes, cudaStream_t st, int cfg_n = 0, float cfg_s = 0.f) {
     const rqb200_ar_config& c = h->cfg;
     const int D = c.D, HW = c.H * c.W, V = c.vocab;
     if (B <= 0) return fail(RQB200_EINVAL, "ar_sample: B must be > 0");
@@ -189,7 +190,7 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
             const float* q = noise ? noise + step * noise_stride : nullptr;
             const int64_t off = (int64_t)idx * D + d;
             RQB_TRY(launch_sample(lg, q, B, V, temperature, top_k[d], top_p[d], out + off, force ? force + off : nullptr,
-                                  (int64_t)HW * D, st));
+                                  (int64_t)HW * D, st, 1, cfg_n, cfg_s));
             step++;
         }
     }
@@ -333,10 +334,13 @@ size_t rqb200_ar_workspace_bytes(const rqb200_ar* h, int B) {
     if (h->fast) return rqb::ar_fast_workspace_bytes(h->fast, B);
     return rqb::ar_layout(h->cfg, B, nullptr, 0, nullptr);
 }
-int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
+}  // extern "C"
+
+// rqb200_ar_sample_span and rqb200_ar_sample_span_cfg: cfg_n = 0 unguided, else guided over B = 2 cfg_n rows
+static int ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                           float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                          void* workspace, size_t workspace_bytes, void* stream) {
+                          void* workspace, size_t workspace_bytes, void* stream, int cfg_n, float cfg_s) {
     if (!h || (!partial && !resume) || !out_codes || !top_k_host || !top_p_host || !workspace)
         return rqb::fail(RQB200_EINVAL, "ar_sample: null argument");
     if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "ar_sample: no CUDA device");
@@ -346,12 +350,31 @@ int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* c
     int rc;
     if (h->fast)
         rc = rqb::ar_fast_sample(h->fast, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
-                                 noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream);
+                                 noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream,
+                                 cfg_n, cfg_s);
     else
         rc = rqb::ar_sample_impl(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
-                                 noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream);
+                                 noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream,
+                                 cfg_n, cfg_s);
     h->last_launches = rqb::g_launches;
     return rc;
+}
+
+extern "C" {
+int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
+                          float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
+                          int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+    return ar_sample_span(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise, noise_stride,
+                          logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, 0, 0.f);
+}
+int rqb200_ar_sample_span_cfg(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
+                              float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
+                              int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
+                              void* workspace, size_t workspace_bytes, void* stream, float cfg_scale) {
+    if (B < 2 || B % 2) return rqb::fail(RQB200_EINVAL, "ar_sample_cfg: B must be 2n rows (n conditional, then n unconditional), n >= 1");
+    return ar_sample_span(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise, noise_stride,
+                          logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, B / 2, cfg_scale);
 }
 int rqb200_ar_sample(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int start_h, int start_w,
                      float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,

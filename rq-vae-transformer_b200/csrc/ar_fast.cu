@@ -1549,10 +1549,12 @@ static int prefill_prefix(ArFast& f, FastWs& ws, int idx_begin, cudaStream_t st)
 
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
-                   float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st) {
+                   float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st, int cfg_n,
+                   float cfg_s) {
     const rqb200_ar_config& c = f->cfg;
     const int D = c.D, HW = c.H * c.W;
     if (B < 1 || B > 256) return fail(RQB200_EINVAL, "ar fast tier: batch must be in [1,256] per call");
+    if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n)) return fail(RQB200_EINVAL, "ar_sample: a guided call takes B = 2 cfg_n rows");
     if (idx_begin < 0 || idx_end > HW || idx_begin > idx_end) return fail(RQB200_EINVAL, "ar_sample: bad position span");
     FastWs ws;
     size_t need = fast_layout(*f, B, wsp, ws_bytes, &ws);
@@ -1568,6 +1570,7 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
     h.s = 0; h.idx = 0; h.step = 0;
     h.cond = cond; h.codes = out; h.force = force; h.noise = noise; h.logits_out = logits_out; h.noise_stride = noise_stride;
     h.temperature = temperature;
+    h.cfg_n = cfg_n; h.cfg_scale = cfg_s;        // (the head graphs' samplers read them: no recapture between guided and unguided calls)
     for (int d = 0; d < D; d++) { h.top_k[d] = top_k[d]; h.top_p[d] = top_p[d]; }
     RQB_TRY(launch_pdl(init_state_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, h, resume ? 1 : 0));
     if (f->trace && !resume) RQB_CUDA(cudaMemsetAsync(ws.trace, 0, (size_t)4 * TR_CAP * sizeof(long long), st));

@@ -27,7 +27,8 @@ int launch_rq_quantize2(const float* x, const RqTables& tabs, int64_t N, int C, 
 int launch_rq_embed(const int64_t* codes, const RqTables& tabs, int64_t N, int D, int C, float* out, bool sum, cudaStream_t st);
 // sampler.cu
 int launch_sample(const float* logits, const float* q, int B, int V, float temperature, int top_k, float top_p,
-                  int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo = 1);
+                  int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo = 1, int cfg_n = 0,
+                  float cfg_s = 0.f);
 // logprob.cu -- out[r] = lg[r*ld + t] - logsumexp(lg[r*ld .. r*ld + V)), t = tgt[r*tgt_stride]; NaN when t is outside [0, V)
 int launch_logprob_rows(const float* lg, int64_t ld, int V, int64_t rows, const int64_t* tgt, int64_t tgt_stride, float* out,
                         cudaStream_t st);
@@ -134,7 +135,7 @@ struct StepState {
     int s;          // body sequence index of the token being processed (= cached body keys before it)
     int idx;        // spatial position whose codes are being sampled
     int step;       // tokens sampled so far in this call (indexes noise / logits_out); 0 in a single-token step
-    int pad;
+    int cfg_n;      // classifier-free guidance: images n of a guided call over 2n rows [cond | uncond]; 0 unguided
     const int64_t* cond;      // [B, cond_len] or null
     int64_t* codes;           // [B, HW, D] working copy (xs)
     const int64_t* force;     // teacher forcing or null
@@ -142,6 +143,7 @@ struct StepState {
     float* logits_out;        // [n_tok][B][V] or null
     int64_t noise_stride;
     float temperature;
+    float cfg_scale;          // guidance scale s (cfg_n > 0)
     int top_k[8];
     float top_p[8];
 };
@@ -152,10 +154,12 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
                        const rqb200_block_weights* head);
 void ar_fast_destroy(ArFast* f);
 size_t ar_fast_workspace_bytes(const ArFast* f, int B);
-// positions [idx_begin, idx_end) of the raster; resume != 0: continue on the KV state the previous call left in this workspace
+// positions [idx_begin, idx_end) of the raster; resume != 0: continue on the KV state the previous call left in this workspace.
+// cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
-                   float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st);
+                   float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st, int cfg_n = 0,
+                   float cfg_s = 0.f);
 // the logits of ONE token (idx, d) into logits_out [B,V] (rqb200_ar_step; arguments already checked by the caller)
 int ar_fast_step(ArFast* f, const int64_t* xs, int64_t xs_stride, const int64_t* cond, int B, int idx, int d, int restart,
                  float* logits_out, void* wsp, size_t ws_bytes, cudaStream_t st);

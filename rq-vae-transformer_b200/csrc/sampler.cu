@@ -16,6 +16,11 @@
 //      double accumulator for float), cut after the first position whose cumulative mass >= p, renormalise by the
 //      kept mass.
 //   5. out = argmax_i p_i / q_i, first index on ties.
+//
+// Classifier-free guidance (cfg_n > 0): the logits hold 2n rows, conditional rows [0, n) then unconditional rows [n, 2n).  CTA r < n
+// reads rows r and r + n in step 1 and samples l = u + s (c - u), formed in fp32 as three rounded operations (no FMA contraction,
+// so torch's `u + s * (c - u)` gives the same bits), with noise row r; it writes the code to rows r and r + n of the output.  CTAs
+// r >= n (the fast tier's captured grid covers all 2n rows) leave at once.  Teacher forcing still copies every row's own code.
 #include <cstdlib>
 
 #include "kernels.h"
@@ -48,7 +53,7 @@ __device__ __forceinline__ bool item_before(const SortItem& a, const SortItem& b
 __global__ void __launch_bounds__(SMP_THREADS, 1)
 sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise, int V, float temperature, int top_k,
               float top_p, int64_t* __restrict__ out_idx, const int64_t* __restrict__ force, int64_t out_stride,
-              const StepState* __restrict__ stt, int dyn_d, int dyn_HW, int dyn_D, int algo) {
+              const StepState* __restrict__ stt, int dyn_d, int dyn_HW, int dyn_D, int algo, int cfg_n, float cfg_s) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* xs = reinterpret_cast<float*>(smem_raw);                       // [V]   scaled logits, later probabilities
     SortItem* items = reinterpret_cast<SortItem*>(xs + V);                // [Vpad] only touched when top_p < 1
@@ -63,10 +68,14 @@ sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise
     __shared__ double scan_carry[33];
     __shared__ int cut_pos;
     __shared__ float kept_mass;
+    __shared__ int guided_n;                                // cfg_n for step 5's write (kept out of registers through 2-4)
 
     const int row = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
     const float* lg = logits + (int64_t)row * V;
     tc::pdl_launch_dependents();
+    // guided fast tier: an unconditional row's CTA has nothing to do.  (cfg_n and force are written by init_state_kernel before the
+    // graph launch, not by a kernel of the chain, so they may be read before the dependency wait.)
+    if (stt != nullptr && stt->cfg_n > 0 && row >= stt->cfg_n && stt->force == nullptr) return;
     tc::pdl_wait();
     if (stt != nullptr) {   // fast AR tier: per-token pointers and settings come from the device-resident StepState
         const int64_t off = (int64_t)stt->idx * dyn_D + dyn_d;
@@ -77,6 +86,8 @@ sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise
         temperature = stt->temperature;
         top_k = stt->top_k[dyn_d];
         top_p = stt->top_p[dyn_d];
+        cfg_n = stt->cfg_n;
+        cfg_s = stt->cfg_scale;
     }
 
     if (force != nullptr) {   // teacher forcing: emit the forced code, skip the work
@@ -84,7 +95,16 @@ sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise
         return;
     }
 
-    for (int i = t; i < V; i += SMP_THREADS) xs[i] = lg[i] / temperature;
+    if (t == 0) guided_n = cfg_n;
+    if (cfg_n > 0) {
+        const float* lu = lg + (int64_t)cfg_n * V;
+        for (int i = t; i < V; i += SMP_THREADS) {
+            const float c = lg[i], u = lu[i];
+            xs[i] = __fadd_rn(u, __fmul_rn(cfg_s, __fsub_rn(c, u))) / temperature;
+        }
+    } else {
+        for (int i = t; i < V; i += SMP_THREADS) xs[i] = lg[i] / temperature;
+    }
     __syncthreads();
 
     // ---- 2. top-k threshold: exact k-th largest by an 8-pass, 4-bit radix select.  No shared-memory atomics and no
@@ -383,7 +403,12 @@ sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise
             int oi = __shfl_xor_sync(0xffffffffu, besti, o);
             if (ob > best || (ob == best && oi < besti)) { best = ob; besti = oi; }
         }
-        if (lane == 0) out_idx[(int64_t)row * out_stride] = (besti == 0x7fffffff) ? 0 : besti;
+        if (lane == 0) {
+            const int code = (besti == 0x7fffffff) ? 0 : besti;
+            out_idx[(int64_t)row * out_stride] = code;
+            const int gn = guided_n;
+            if (gn > 0) out_idx[(int64_t)(row + gn) * out_stride] = code;
+        }
     }
 }
 
@@ -392,18 +417,21 @@ sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise
 constexpr int SAMPLER_ALGO_DEFAULT = 1;
 
 // out_stride: distance (in int64 elements) between consecutive rows' outputs -- lets the AR loop write straight into
-// codes[b, h, w, d] (stride H*W*D).  force (nullable) uses the same addressing.
+// codes[b, h, w, d] (stride H*W*D).  force (nullable) uses the same addressing.  cfg_n > 0: guided over B = 2 cfg_n rows, one CTA per
+// image (one per row when teacher forcing).
 int launch_sample(const float* logits, const float* q, int B, int V, float temperature, int top_k, float top_p,
-                  int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo) {
+                  int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo, int cfg_n, float cfg_s) {
     if (B <= 0) return B == 0 ? 0 : fail(RQB200_EINVAL, "sample: B < 0");
+    if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n)) return fail(RQB200_EINVAL, "sample: a guided call takes B = 2 cfg_n rows");
     if (V <= 0 || V > SMP_MAXV) return fail(RQB200_EINVAL, "sample: V must be in [1,16384]");
     if (!(temperature > 0.f)) return fail(RQB200_EINVAL, "sample: temperature must be > 0");
     int vpad = 1;
     while (vpad < V) vpad <<= 1;
     size_t smem = (size_t)V * sizeof(float) + (top_p < 1.0f ? (size_t)vpad * sizeof(SortItem) : 0);
     RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel);
-    sample_kernel<<<B, SMP_THREADS, smem, st>>>(logits, q, V, temperature, top_k, top_p, out_idx, force, out_stride, nullptr, 0, 0,
-                                                0, algo);
+    const int grid = (cfg_n > 0 && force == nullptr) ? cfg_n : B;
+    sample_kernel<<<grid, SMP_THREADS, smem, st>>>(logits, q, V, temperature, top_k, top_p, out_idx, force, out_stride, nullptr, 0, 0,
+                                                   0, algo, cfg_n, cfg_s);
     return check_launch("sample_logits");
 }
 
@@ -414,7 +442,7 @@ int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, i
     size_t smem = (size_t)V * sizeof(float) + (size_t)vpad * sizeof(SortItem);   // top_p is only known on the device
     RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel);
     return launch_pdl(sample_kernel, dim3(B), dim3(SMP_THREADS), smem, st, pdl, logits, (const float*)nullptr, V, 1.0f, 0, 1.0f,
-                      (int64_t*)nullptr, (const int64_t*)nullptr, (int64_t)0, stt, d, HW, D, SAMPLER_ALGO_DEFAULT);
+                      (int64_t*)nullptr, (const int64_t*)nullptr, (int64_t)0, stt, d, HW, D, SAMPLER_ALGO_DEFAULT, 0, 0.0f);
 }
 
 }  // namespace rqb
@@ -422,9 +450,9 @@ int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, i
 extern "C" int rqb200_sample_logits(const float* logits, const float* q, int B, int V, float temperature, int top_k,
                                     float top_p, int64_t* out_idx, void* stream) {
     return rqb::launch_sample(logits, q, B, V, temperature, top_k, top_p, out_idx, nullptr, 1, (cudaStream_t)stream,
-                              rqb::SAMPLER_ALGO_DEFAULT);
+                              rqb::SAMPLER_ALGO_DEFAULT, 0, 0.f);
 }
 extern "C" int rqb200_dbg_sample_logits(int algo, const float* logits, const float* q, int B, int V, float temperature, int top_k,
                                         float top_p, int64_t* out_idx, void* stream) {
-    return rqb::launch_sample(logits, q, B, V, temperature, top_k, top_p, out_idx, nullptr, 1, (cudaStream_t)stream, algo);
+    return rqb::launch_sample(logits, q, B, V, temperature, top_k, top_p, out_idx, nullptr, 1, (cudaStream_t)stream, algo, 0, 0.f);
 }

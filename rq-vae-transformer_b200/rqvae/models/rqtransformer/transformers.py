@@ -351,35 +351,73 @@ class RQTransformer(Stage2Model):
             ps = [min(top_p[i], 1.0) for i in range(D)]
         return ks, ps
 
+    def _guidance(self, B, cfg_scale, uncond):
+        """sample()'s classifier-free guidance arguments checked before any kernel runs: None (unguided) or (s, uncond [B, cond_len]
+        int64).  Raises ValueError for a scale without uncond or the reverse, an unconditional model, an uncond that does not reshape
+        to [B, cond_len] or is not integer, and entries outside [0, vocab_size_cond) (one host read)."""
+        if cfg_scale is None and uncond is None:
+            return None
+        if cfg_scale is None or uncond is None:
+            raise ValueError("rqb200: classifier-free guidance needs both cfg_scale and uncond")
+        if self.vocab_size_cond == 1:
+            raise ValueError("rqb200: classifier-free guidance needs a conditional model (vocab_size_cond > 1)")
+        if isinstance(cfg_scale, bool) or not isinstance(cfg_scale, (int, float)):
+            raise ValueError("rqb200: cfg_scale must be a float, got %r" % (cfg_scale,))
+        cl = self.block_size_cond
+        if not isinstance(uncond, torch.Tensor) or uncond.dtype.is_floating_point or uncond.dtype.is_complex or \
+                uncond.dtype == torch.bool or uncond.numel() != B * cl:
+            raise ValueError("rqb200: uncond must be an integer tensor that reshapes to cond's [%d, %d], got %s %s"
+                             % (B, cl, getattr(uncond, "dtype", type(uncond)), tuple(getattr(uncond, "shape", ()))))
+        u = uncond.reshape(B, cl).to(torch.int64)
+        if bool(((u < 0) | (u >= self.vocab_size_cond)).any()):
+            raise ValueError("rqb200: uncond entries must lie in [0, %d)" % self.vocab_size_cond)
+        return float(cfg_scale), u
+
     @torch.no_grad()
     def _native_sample(self, partial, model_aux, cond, start_loc, temperature, top_k, top_p, amp, noise=None,
-                       return_logits=False, force_codes=None):
+                       return_logits=False, force_codes=None, guidance=None):
+        """guidance: None, or (s, uncond [B, cond_len] int64) from _guidance -- classifier-free guidance: every image runs a cond and an
+        uncond branch as rows [cond | uncond] of one native call (rqb200_ar_sample_span_cfg), noise stays per image [n_tok, B, V],
+        logits (return_logits) and force_codes hold both branches' rows [2B]: [cond rows | uncond rows]"""
         H, W, D = self.block_size
         B = partial.shape[0]
         dev = self.pos_emb_hw.device
         self._check_computable()
-        N.require_cuda(partial, cond, self.pos_emb_hw)
+        N.require_cuda(partial, cond, self.pos_emb_hw, None if guidance is None else guidance[1])
         ks, ps = self._lists(top_k, top_p)
         codebook = self._codebook_of(model_aux, D)
         mode = self._mode(amp)
         partial = partial.to(torch.int64).contiguous()
-        cond_t = None if cond is None else cond.reshape(B, self.block_size_cond).to(torch.int64).contiguous()
+        cl = self.block_size_cond
+        cond_t = None if cond is None else cond.reshape(B, cl).to(torch.int64).contiguous()
         idx0 = start_loc[0] * W + start_loc[1]
         n_tok = max(H * W - idx0, 0) * D
         V = self.vocab_size[0]
         HWD = H * W * D
+        R = B if guidance is None else 2 * B          # batch rows of the engine: one per image, or one per image and branch
         with torch.cuda.device(dev):
             draw = noise is None            # draw the Exp(1) noise here, exactly as torch.multinomial would (utils.py:114)
             if noise is False:
                 noise = None
-            logits = torch.empty(n_tok, B, V, dtype=torch.float32, device=dev) if return_logits else None
+            logits = torch.empty(n_tok, R, V, dtype=torch.float32, device=dev) if return_logits else None
             out = torch.empty_like(partial)
             kk = (C.c_int32 * D)(*[int(k) for k in ks])
             pp = (C.c_float * D)(*[float(p) for p in ps])
             fc = None if force_codes is None else force_codes.to(torch.int64).contiguous()
-            bounds = _chunk_bounds(B, mode)
+            # images per native call: the fast tier runs at most 256 rows, so a guided call takes at most 128 images
+            bounds = _chunk_bounds(B, mode, 256 if guidance is None else 128)
             if len(bounds) > 1 and return_logits:
-                raise N.NativeError("rqb200: return_logits with B > 256 is not supported on the fast tier")
+                raise N.NativeError("rqb200: return_logits with more than one batch chunk (B > %d) is not supported on the fast tier"
+                                    % (256 if guidance is None else 128))
+            # per chunk: (rows, partial, cond, force, out) as the native call reads them, each row 0 the chunk's first
+            if guidance is None:
+                calls = [(hi - lo, _rows(partial, lo), _rows(cond_t, lo), _rows(fc, lo), _rows(out, lo)) for lo, hi in bounds]
+            else:
+                u = guidance[1]
+                cu = torch.zeros(B, cl, dtype=torch.int64, device=dev) if cond_t is None else cond_t
+                calls = [(2 * (hi - lo), torch.cat([partial[lo:hi], partial[lo:hi]]), torch.cat([cu[lo:hi], u[lo:hi]]),
+                          None if fc is None else torch.cat([fc[lo:hi], fc[B + lo:B + hi]]),
+                          torch.empty(2 * (hi - lo), H, W, D, dtype=torch.int64, device=dev)) for lo, hi in bounds]
             # position spans: when the noise is drawn here it is drawn span by span into one bounded buffer (noise_budget_bytes)
             # instead of one [n_tok,B,V] tensor (1 GB at 8x8x4, B=64, V=16384); every batch chunk keeps its own engine slot
             # (workspace + KV state) so that all chunks can resume on the next span
@@ -391,9 +429,9 @@ class RQTransformer(Stage2Model):
             st = torch.cuda.current_stream(dev)
             launches = 0
             engines = []
-            for slot, (lo, hi) in enumerate(bounds):
+            for slot, call in enumerate(calls):
                 eng = self._engine(codebook, mode, slot)
-                _workspace(eng, N.lib().rqb200_ar_workspace_bytes(eng["handle"], hi - lo), dev)
+                _workspace(eng, N.lib().rqb200_ar_workspace_bytes(eng["handle"], call[0]), dev)
                 engines.append(eng)
 
             def off(t, lo, row_elems, esize, extra=0):
@@ -406,15 +444,21 @@ class RQTransformer(Stage2Model):
                     for t in range((p1 - p0) * D):
                         noise[t].exponential_(1)
                 tok0 = 0 if draw else (p0 - idx0) * D                  # first token of this span inside `noise`
-                for eng, (lo, hi) in zip(engines, bounds):
-                    N.check(N.lib().rqb200_ar_sample_span(
-                        eng["handle"], off(partial, lo, HWD, 8), off(cond_t, lo, self.block_size_cond, 8), hi - lo, p0, p1,
-                        int(p0 > idx0), float(temperature), kk, pp, off(noise, lo, V, 4, tok0 * B * V),
-                        0 if noise is None else B * V, off(logits, lo, V, 4, (p0 - idx0) * D * B * V), off(fc, lo, HWD, 8),
-                        off(out, lo, HWD, 8), N.ptr(eng["ws"]), eng["ws"].numel(), C.c_void_p(st.cuda_stream)), "ar_sample")
+                for eng, (lo, hi), (rows, part_c, cond_c, fc_c, out_c) in zip(engines, bounds, calls):
+                    args = (eng["handle"], off(part_c, 0, HWD, 8), off(cond_c, 0, cl, 8), rows, p0, p1, int(p0 > idx0),
+                            float(temperature), kk, pp, off(noise, lo, V, 4, tok0 * B * V), 0 if noise is None else B * V,
+                            off(logits, 0, V, 4, (p0 - idx0) * D * R * V), off(fc_c, 0, HWD, 8), off(out_c, 0, HWD, 8),
+                            N.ptr(eng["ws"]), eng["ws"].numel(), C.c_void_p(st.cuda_stream))
+                    if guidance is None:
+                        N.check(N.lib().rqb200_ar_sample_span(*args), "ar_sample")
+                    else:
+                        N.check(N.lib().rqb200_ar_sample_span_cfg(*args, C.c_float(guidance[0])), "ar_sample_cfg")
                     launches += N.lib().rqb200_ar_last_launches(eng["handle"])
             if n_tok == 0:
                 out.copy_(partial)
+            elif guidance is not None:
+                for (lo, hi), call in zip(bounds, calls):
+                    out[lo:hi] = call[4][:hi - lo]
         self.last_launches = launches
         N.launch_count["total"] += launches
         return (out, logits) if return_logits else out
@@ -436,11 +480,16 @@ class RQTransformer(Stage2Model):
 
     @torch.no_grad()
     def sample(self, partial_sample, model_aux=None, cond=None, start_loc=(0, 0), temperature=1.0, top_k=None, top_p=None,
-               amp=False, cached=True, is_tqdm=False, desc="Sampling", fast=True):
-        """transformers.py:294-369.  Returns LongTensor [B,H,W,D]; ``partial_sample`` is not modified."""
+               amp=False, cached=True, is_tqdm=False, desc="Sampling", fast=True, cfg_scale=None, uncond=None):
+        """transformers.py:294-369.  Returns LongTensor [B,H,W,D]; ``partial_sample`` is not modified.
+        Classifier-free guidance: with a float ``cfg_scale`` s and ``uncond`` (cond's shape: an unconditional or negative condition
+        per image), every token is drawn from l = u + s * (c - u) -- c the logits under ``cond``, u under ``uncond`` -- then
+        temperature, top-k and top-p as unguided, with one Exp(1) draw per image and token.  Both branches share the
+        partial_sample / start_loc prefix and every drawn code.  The default ``cfg_scale=None`` samples unguided."""
         assert self.block_size == partial_sample.shape[1:]
+        guidance = self._guidance(partial_sample.shape[0], cfg_scale, uncond)
         self.init_cache()
-        out = self._native_sample(partial_sample, model_aux, cond, start_loc, temperature, top_k, top_p, amp)
+        out = self._native_sample(partial_sample, model_aux, cond, start_loc, temperature, top_k, top_p, amp, guidance=guidance)
         self.init_cache()
         return out
 
@@ -673,11 +722,16 @@ class RQTransformer(Stage2Model):
         return tokenwise.reshape(-1, D).mean(dim=0)
 
 
-def _chunk_bounds(B, mode):
+def _chunk_bounds(B, mode, limit=256):
     """the batch chunks [(lo, hi)] of one native call each: the fast tier takes at most 256 batch rows per call (wgmma N <= 256), so
-    a larger batch runs as equal chunks back to back"""
-    n = max(1, -(-B // 256)) if mode == N.MODE_FAST else 1
+    a larger batch runs as equal chunks back to back.  limit: images per call (128 when each image takes two rows)"""
+    n = max(1, -(-B // limit)) if mode == N.MODE_FAST else 1
     return [(i * B // n, (i + 1) * B // n) for i in range(n)]
+
+
+def _rows(t, lo):
+    """the rows of t from row lo on (a view), or None"""
+    return None if t is None else t[lo:]
 
 
 def _workspace(eng, need, dev):
