@@ -188,6 +188,24 @@ int rqb200_ar_sample_span_cfg(rqb200_ar* h, const int64_t* partial, const int64_
                               float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                               int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
                               void* workspace, size_t workspace_bytes, void* stream, float cfg_scale);
+/* Masked completion: rqb200_ar_sample_span (cfg_n = 0) or rqb200_ar_sample_span_cfg (cfg_n = B / 2 images, cfg_scale) that samples only
+ * the tokens the caller does not keep.
+ *   keep (nullable, device) uint8 [B, H*W, D], rows laid out like out_codes (guided: the image's mask in both branch rows): nonzero keeps
+ *     the token -- out_codes holds partial's code there (it was initialised from partial) and the sampler writes nothing, teacher
+ *     forcing included.
+ *   sampled_host (nullable, host) uint8 [H*W], the same array for every span of a call: nonzero where some row samples some depth of
+ *     the position.  Only those positions run the head stack, classifier and sampler; a position marked 0 is kept whole, whatever keep
+ *     says.  It must be 0 before the call's first position (start_loc).  NULL marks every position.
+ * Every token of a span still takes its noise row and logits_out slot (indexed from the span's first token, as above); the logits_out
+ * rows of skipped positions are left untouched.  The body consumes the code tokens of the positions between two sampled positions a < b
+ * right before b's head: on the fast tier in one batched pass at sequence offset cond_len + a when b - a is at least a few tokens
+ * (token by token with RQB200_AR_SEQUENTIAL_PREFILL), on the exact tier token by token.  That grouping depends on sampled_host alone, so
+ * a call split into spans gives the codes of one span bit for bit.  keep == sampled_host == NULL is rqb200_ar_sample_span(_cfg). */
+int rqb200_ar_sample_span_keep(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
+                               float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
+                               int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
+                               void* workspace, size_t workspace_bytes, void* stream, const uint8_t* keep, const uint8_t* sampled_host,
+                               int cfg_n, float cfg_scale);
 /* RQTransformer.cached_forward (transformers.py:190-287): the logits of ONE token (h, w, d) into logits_out [B,V] f32.
  *   xs: the caller's code map, int64, batch row b at xs + b*xs_batch_stride, positions in raster order, D codes each
  *       (only the codes this step consumes are read: position idx-1 when d == 0, codes 0..d-1 of position idx when d > 0;
@@ -332,6 +350,12 @@ int rqb200_dbg_attn_step(int form, const float* part, int S, const float* bqkv, 
  *   [0, T) of every (group, head), nothing else.  The kernel is chosen by T as in the engine: a warp per (group, head) for T <= 4 and
  *   T <= 8, 64 x 64 tiles with an online softmax above. */
 int rqb200_dbg_prefill_attn(const void* qkv, void* kc, void* vc, void* att, int G, int T, int E, int Tmax, int fmt, void* stream);
+/* rqb200_dbg_append_attn: the same attention for T new tokens at sequence offset T0 (the fast tier's append of a run of kept positions
+ *   to the body cache): qkv / att as above for the new tokens; new token t (sequence token T0 + t) sees the cache rows [0, T0) of kc / vc
+ *   and the new tokens 0 .. t, and its k / v are written at cache row T0 + t.  Cache rows outside [T0, T0 + T) are read (below T0) or
+ *   untouched.  kc, vc required; T0 + T <= Tmax <= 2048.  T0 > 0: the 64 x 64 tiled kernel for every T; T0 = 0 is
+ *   rqb200_dbg_prefill_attn's launch. */
+int rqb200_dbg_append_attn(const void* qkv, void* kc, void* vc, void* att, int G, int T0, int T, int E, int Tmax, int fmt, void* stream);
 /* rqb200_dbg_ln: LayerNorm (eps 1e-5) of `rows` rows of E <= 4608 (E % 128 == 0) f32: x_out (nullable) = x_in + bias + part[0] + ...
  *   + part[S-1] + extra, summed in fp32 in that order (x_in / bias / extra nullable, bias / extra one [E] row for all rows; part [S, rows,
  *   E]); xn (nullable; g, b [E]) = 16-bit LN(x).  x_in == x_out is allowed.  form 1: ln_reduce_kernel (the step's LN1 / LN2 form, one CTA

@@ -164,11 +164,12 @@ static int head_depth(const rqb200_ar* h, const int64_t* codes, int B, int idx, 
 }
 
 // positions [idx0, idx_end) of the raster; resume != 0: no prefill, continue on the caches / context left in this workspace.
-// cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s (the sampler forms the guided logits)
+// cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s (the sampler forms the guided logits).
+// keep / sampled: the masked-sample plan of the fast tier (kernels.h), with one body step per appended code token.
 static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx0, int idx_end, int resume,
                           float temperature, const int32_t* top_k, const float* top_p, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force, int64_t* out, void* wsp,
-                          size_t ws_bytes, cudaStream_t st, int cfg_n = 0, float cfg_s = 0.f) {
+                          size_t ws_bytes, cudaStream_t st, int cfg_n, float cfg_s, const uint8_t* keep, const uint8_t* sampled) {
     const rqb200_ar_config& c = h->cfg;
     const int D = c.D, HW = c.H * c.W, V = c.vocab;
     if (B <= 0) return fail(RQB200_EINVAL, "ar_sample: B must be > 0");
@@ -180,19 +181,23 @@ static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* c
     if (!resume && out != partial) RQB_CUDA(cudaMemcpyAsync(out, partial, code_bytes, cudaMemcpyDeviceToDevice, st));   // xs = partial_sample.clone()
     if (idx0 >= idx_end) return 0;
 
-    if (!resume) RQB_TRY(prefill_prefix(h, out, cond, B, idx0, ws, st));
-    int64_t step = 0;
+    int prev = resume ? plan_prev(sampled, idx0) : -1;     // the last sampled position before this span; none: prefill at the first
     for (int idx = idx0; idx < idx_end; idx++) {
-        if (idx > idx0 || resume) RQB_TRY(body_step(h, out, B, idx, ws, st));   // decode step on the token of position idx-1
+        if (!plan_sampled(sampled, idx)) continue;
+        if (prev < 0)
+            RQB_TRY(prefill_prefix(h, out, cond, B, idx, ws, st));
+        else
+            for (int j = prev + 1; j <= idx; j++) RQB_TRY(body_step(h, out, B, j, ws, st));   // decode steps on positions prev .. idx-1
         for (int d = 0; d < D; d++) {
+            const int64_t step = (int64_t)(idx - idx0) * D + d;
             float* lg = logits_out ? logits_out + step * (int64_t)B * V : ws.LOGITS;
             RQB_TRY(head_depth(h, out, B, idx, d, ws, lg, st));
             const float* q = noise ? noise + step * noise_stride : nullptr;
             const int64_t off = (int64_t)idx * D + d;
             RQB_TRY(launch_sample(lg, q, B, V, temperature, top_k[d], top_p[d], out + off, force ? force + off : nullptr,
-                                  (int64_t)HW * D, st, 1, cfg_n, cfg_s));
-            step++;
+                                  (int64_t)HW * D, st, 1, cfg_n, cfg_s, keep ? keep + off : nullptr));
         }
+        prev = idx;
     }
     return 0;
 }
@@ -258,7 +263,7 @@ static int ar_log_prob_impl(rqb200_ar* h, const int64_t* codes, const int64_t* c
     for (int p0 = 0; p0 < HW; p0 += (int)P) {
         const int p1 = (int)std::min<int64_t>(p0 + P, HW), n_pos = p1 - p0, steps = n_pos * D;
         RQB_TRY(ar_sample_impl(h, codes, cond, B, p0, p1, p0 > 0, 1.f, top_k.data(), top_p.data(), nullptr, 0, sp.logits, codes, ws.CODES,
-                               wsp, ws_bytes, st));
+                               wsp, ws_bytes, st, 0, 0.f, nullptr, nullptr));
         // row (step, b), step = (idx - p0)*D + d  <-  codes[b][p0*D + step]
         RQB_TRY(launch_gather_targets(codes, 1, steps, B, 0, 1, HWD, (int64_t)p0 * D, sp.tgt, st));
         RQB_TRY(launch_logprob_rows(sp.logits, V, V, (int64_t)steps * B, sp.tgt, 1, sp.lp, st));
@@ -336,26 +341,30 @@ size_t rqb200_ar_workspace_bytes(const rqb200_ar* h, int B) {
 }
 }  // extern "C"
 
-// rqb200_ar_sample_span and rqb200_ar_sample_span_cfg: cfg_n = 0 unguided, else guided over B = 2 cfg_n rows
+// rqb200_ar_sample_span, _cfg and _keep: cfg_n = 0 unguided, else guided over B = 2 cfg_n rows; keep / sampled null: every token sampled
 static int ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                           float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                          void* workspace, size_t workspace_bytes, void* stream, int cfg_n, float cfg_s) {
+                          void* workspace, size_t workspace_bytes, void* stream, int cfg_n, float cfg_s, const uint8_t* keep,
+                          const uint8_t* sampled) {
     if (!h || (!partial && !resume) || !out_codes || !top_k_host || !top_p_host || !workspace)
         return rqb::fail(RQB200_EINVAL, "ar_sample: null argument");
     if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "ar_sample: no CUDA device");
     if (h->cfg.weight_dtype != RQB200_F32 && !h->fast) return rqb::fail(RQB200_EINVAL, "ar_sample: 16-bit weights need the fast tier");
+    if (sampled && !resume && idx_begin > 0 && idx_begin <= h->cfg.H * h->cfg.W)
+        for (int p = 0; p < idx_begin; p++)
+            if (sampled[p]) return rqb::fail(RQB200_EINVAL, "ar_sample_keep: sampled_host must be 0 before the call's first position");
     h->step_next = -1;                   // sampling reuses the caches a stepped sequence keeps: that sequence ends here
     rqb::g_launches = 0;
     int rc;
     if (h->fast)
         rc = rqb::ar_fast_sample(h->fast, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
                                  noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream,
-                                 cfg_n, cfg_s);
+                                 cfg_n, cfg_s, keep, sampled);
     else
         rc = rqb::ar_sample_impl(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
                                  noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream,
-                                 cfg_n, cfg_s);
+                                 cfg_n, cfg_s, keep, sampled);
     h->last_launches = rqb::g_launches;
     return rc;
 }
@@ -366,15 +375,27 @@ int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* c
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
                           void* workspace, size_t workspace_bytes, void* stream) {
     return ar_sample_span(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise, noise_stride,
-                          logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, 0, 0.f);
+                          logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, 0, 0.f, nullptr, nullptr);
 }
 int rqb200_ar_sample_span_cfg(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                               float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                               int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
                               void* workspace, size_t workspace_bytes, void* stream, float cfg_scale) {
     if (B < 2 || B % 2) return rqb::fail(RQB200_EINVAL, "ar_sample_cfg: B must be 2n rows (n conditional, then n unconditional), n >= 1");
+    return rqb200_ar_sample_span_keep(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
+                                      noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, nullptr,
+                                      nullptr, B / 2, cfg_scale);
+}
+int rqb200_ar_sample_span_keep(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
+                               float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
+                               int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
+                               void* workspace, size_t workspace_bytes, void* stream, const uint8_t* keep, const uint8_t* sampled_host,
+                               int cfg_n, float cfg_scale) {
+    if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n))
+        return rqb::fail(RQB200_EINVAL, "ar_sample_cfg: B must be 2n rows (n conditional, then n unconditional), n >= 1");
     return ar_sample_span(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise, noise_stride,
-                          logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, B / 2, cfg_scale);
+                          logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, cfg_n, cfg_n > 0 ? cfg_scale : 0.f, keep,
+                          sampled_host);
 }
 int rqb200_ar_sample(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int start_h, int start_w,
                      float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,

@@ -28,7 +28,9 @@
 //
 // The prefix (cond tokens, and on a start_loc resume the code tokens before it) is prefilled in ONE pass of M = B*T row
 // GEMMs + a causal attention kernel that writes the KV cache (reference: transformers.py:237-239, attentions.py:60-104 with
-// Tnew > 1); the token-by-token replay of the single-step graph remains available (flag) and is the prefill's oracle.
+// Tnew > 1); the token-by-token replay of the single-step graph remains available (flag) and is the prefill's oracle.  A masked
+// sample (keep / sampled) runs the head graph at sampled positions only and appends each run of kept positions' code tokens to the
+// body cache with the same batched pass at the run's sequence offset.
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -484,19 +486,23 @@ __device__ __forceinline__ void pa_ldsm4_t(uint32_t (&r)[4], uint32_t addr) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
 constexpr int PM_ROW = 144;                           // bytes per staged row (64 x 16-bit + 16 B pad)
-// Causal attention over a whole prefix in one launch (batched prefill / teacher-forced forward) for groups of more than 8 tokens.
-// qkv [M, 3E] 16-bit (bias already added by the GEMM epilogue), row of (group g, token t) = t * G + g (token-major: the rows of one
-// token are contiguous, like the single-step buffers).  One CTA per (query tile of 64 rows, group, head), query tiles launched
-// heaviest (last) first; each of the four warps owns 16 query rows.  K / V are read in 64-key tiles double-buffered through cp.async
-// (144 B rows: conflict-free ldmatrix); per tile S = Q K^T on mma.sync (fp32 accumulate), the causal mask on the diagonal tile only,
-// an online softmax (running row max and sum in fp32, O rescaled between tiles), the probabilities repacked as 16-bit A fragments
-// (the m16n8 accumulator pair of two adjacent key tiles IS the m16k16 A fragment) and O += P V with V through ldmatrix.trans.  Key
-// tiles are visited in a fixed order: run-to-run deterministic.  When kc != NULL the CTA of query tile i writes the cache rows
-// [g][head][t][64] of tile i (every row exactly once).
+// Causal attention of T new tokens at sequence offset T0 in one launch (batched prefill, T0 = 0; an append to the KV cache, T0 > 0;
+// teacher-forced forward, T0 = 0 and no cache) for groups of more than 8 tokens.
+// qkv [M, 3E] 16-bit (bias already added by the GEMM epilogue), row of (group g, new token t) = t * G + g (token-major: the rows of one
+// token are contiguous, like the single-step buffers).  New token t is sequence token T0 + t and sees keys [0, T0 + t]: keys < T0 are
+// the cache rows [g][head][key][64] of kc / vc (written by earlier launches; no CTA of this one writes them), keys >= T0 are qkv's rows.
+// One CTA per (query tile of 64 new tokens, group, head), query tiles launched heaviest (last) first; each of the four warps owns 16
+// query rows.  K / V are read in 64-key tiles of the whole sequence (a tile may straddle T0) double-buffered through cp.async (144 B
+// rows: conflict-free ldmatrix); per tile S = Q K^T on mma.sync (fp32 accumulate), the causal mask on the tiles that hold keys past
+// some query row, an online softmax (running row max and sum in fp32, O rescaled between tiles), the probabilities repacked as 16-bit
+// A fragments (the m16n8 accumulator pair of two adjacent key tiles IS the m16k16 A fragment) and O += P V with V through
+// ldmatrix.trans.  Key tiles are visited in a fixed order: run-to-run deterministic.  When kc != NULL the CTA of query tile i writes
+// the cache rows T0 + t of its tile's new tokens t (every new row exactly once).  At T0 = 0 every tile but the diagonal one is
+// unmasked, as in the plain prefill.
 template <bool BF>
 __global__ void __launch_bounds__(128)
 prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* __restrict__ vc, h16* __restrict__ att, int G, int T, int E,
-                          int nh, int Tmax) {
+                          int nh, int Tmax, int T0) {
     __shared__ __align__(16) uint8_t sm[5 * 64 * PM_ROW];         // Q | K[2] | V[2]
     uint8_t* Qs = sm;
     tc::pdl_launch_dependents();
@@ -506,12 +512,17 @@ prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16
     const int pair = (int)(blockIdx.x % n_pairs);
     const int g = pair / nh, h = pair % nh;
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    // tile `kt` of matrix `mat` (0 Q, 1 K, 2 V) -> dst; rows beyond T are zeros (their scores are masked, but P V must not see NaN)
+    const int64_t crow0 = ((int64_t)g * nh + h) * Tmax;        // this (group, head)'s cache rows
+    // tile `kt` of matrix `mat` (0 Q: new tokens; 1 K, 2 V: sequence keys, < T0 from the cache) -> dst; rows beyond the last token are
+    // zeros (their scores are masked, but P V must not see NaN)
     auto load_tile = [&](int mat, int kt, uint8_t* dst) {
+        const int base = mat == 0 ? 0 : T0;               // sequence index of qkv row 0 in this tile's coordinates
         for (int i = threadIdx.x; i < 64 * 8; i += 128) {
-            const int r = i >> 3, c = i & 7, t = kt * 64 + r;
+            const int r = i >> 3, c = i & 7, t = kt * 64 + r - base;
             uint8_t* d = dst + r * PM_ROW + c * 16;
-            if (t < T)
+            if (t < 0)
+                cp_async16(tc::smem_u32(d), (mat == 1 ? kc : vc) + (crow0 + kt * 64 + r) * 64 + c * 8);
+            else if (t < T)
                 cp_async16(tc::smem_u32(d), qkv + ((int64_t)t * G + g) * 3 * E + mat * E + h * 64 + c * 8);
             else
                 *reinterpret_cast<uint4*>(d) = make_uint4(0u, 0u, 0u, 0u);
@@ -525,18 +536,21 @@ prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16
         for (int i = threadIdx.x; i < 2 * 64 * 8; i += 128) {
             const int mat = 1 + (i >> 9), r = (i >> 3) & 63, c = i & 7, t = qt * 64 + r;
             if (t < T)
-                *reinterpret_cast<uint4*>((mat == 1 ? kc : vc) + (((int64_t)g * nh + h) * Tmax + t) * 64 + c * 8) =
+                *reinterpret_cast<uint4*>((mat == 1 ? kc : vc) + (crow0 + T0 + t) * 64 + c * 8) =
                     *reinterpret_cast<const uint4*>(qkv + ((int64_t)t * G + g) * 3 * E + mat * E + h * 64 + c * 8);
         }
     }
-    const int r0 = qt * 64 + 16 * w + (lane >> 2), r1 = r0 + 8;
+    const int r0 = qt * 64 + 16 * w + (lane >> 2), r1 = r0 + 8;          // new-token rows; sequence rows T0 + r0, T0 + r1
+    const int q0 = T0 + r0, q1 = T0 + r1;
+    // the last key tile of this query tile: the one holding its last real query's key (rows past T see keys up to it, never beyond)
+    const int kt_last = (T0 + min(qt * 64 + 63, T - 1)) >> 6;
     uint32_t qa[4][4];
     float oacc[8][4];
 #pragma unroll
     for (int j = 0; j < 8; j++) { oacc[j][0] = oacc[j][1] = oacc[j][2] = oacc[j][3] = 0.f; }
     float m0 = -INFINITY, m1 = -INFINITY, s0 = 0.f, s1 = 0.f;      // running max; this lane's share of the running sum
-    for (int kt = 0; kt <= qt; kt++) {
-        if (kt < qt) {                                    // prefetch the next key tile into the other buffer
+    for (int kt = 0; kt <= kt_last; kt++) {
+        if (kt < kt_last) {                               // prefetch the next key tile into the other buffer
             load_tile(1, kt + 1, sm + (1 + ((kt + 1) & 1)) * 64 * PM_ROW);
             load_tile(2, kt + 1, sm + (3 + ((kt + 1) & 1)) * 64 * PM_ROW);
             asm volatile("cp.async.commit_group;" ::: "memory");
@@ -565,22 +579,24 @@ prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16
                 pa_mma<BF>(sacc[2 * jp + 1], qa[kk], b[2], b[3]);
             }
         }
-        // ---- scale (+ causal mask on the diagonal tile), new row maxima
-        const bool diag = kt == qt;
+        // ---- scale (+ causal mask where the tile holds keys past this tile's first query row), new row maxima
+        const bool masked = kt * 64 + 63 > T0 + qt * 64;
         float t0 = m0, t1 = m1;
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             const int c0 = kt * 64 + 8 * j + (lane & 3) * 2;
-            sacc[j][0] = (!diag || c0 <= r0) ? sacc[j][0] * 0.125f : -INFINITY;
-            sacc[j][1] = (!diag || c0 + 1 <= r0) ? sacc[j][1] * 0.125f : -INFINITY;
-            sacc[j][2] = (!diag || c0 <= r1) ? sacc[j][2] * 0.125f : -INFINITY;
-            sacc[j][3] = (!diag || c0 + 1 <= r1) ? sacc[j][3] * 0.125f : -INFINITY;
+            sacc[j][0] = (!masked || c0 <= q0) ? sacc[j][0] * 0.125f : -INFINITY;
+            sacc[j][1] = (!masked || c0 + 1 <= q0) ? sacc[j][1] * 0.125f : -INFINITY;
+            sacc[j][2] = (!masked || c0 <= q1) ? sacc[j][2] * 0.125f : -INFINITY;
+            sacc[j][3] = (!masked || c0 + 1 <= q1) ? sacc[j][3] * 0.125f : -INFINITY;
             t0 = fmaxf(t0, fmaxf(sacc[j][0], sacc[j][1]));
             t1 = fmaxf(t1, fmaxf(sacc[j][2], sacc[j][3]));
         }
         t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 1)); t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, 2));
         t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 1)); t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, 2));
-        // (every row sees at least one unmasked key in every tile it visits: t0 / t1 are finite, alpha of the first tile is 0)
+        // Key 0 is in tile 0 and every row sees it, so t0 / t1 are finite from the first tile on (alpha of the first tile is 0).  A
+        // later tile may be fully masked for some rows (an append's query tile straddles two key tiles): their max stays, alpha is 1
+        // and every exp(-inf - m) is 0 -- zero weight, no NaN.
         const float a0 = __expf(m0 - t0), a1 = __expf(m1 - t1);
         m0 = t0;
         m1 = t1;
@@ -1263,23 +1279,26 @@ static int ln_rows(int64_t rows, const float* x_in, const float* extra, float* x
     return ln_rows_warp(rows, x_in, extra, x_out, g, be, xn, E, bf, n_sm, st);
 }
 
-// Causal attention of a batched pass over G groups of T tokens (qkv token-major [T*G, 3E], bias added), the cache rows [0, T) of every
-// (group, head) written when kc != NULL: a warp per (group, head) for T <= 8, 64-query tiles over 64-key tiles above.
-static int prefill_attn(const h16* qkv, h16* kc, h16* vc, h16* att, int G, int T, int E, int Tmax, int bf, bool pdl, cudaStream_t st) {
+// Causal attention of a batched pass over G groups of T new tokens at sequence offset T0 (qkv token-major [T*G, 3E], bias added; keys
+// before T0 from the cache), the cache rows [T0, T0 + T) of every (group, head) written when kc != NULL: at T0 = 0 a warp per (group,
+// head) for T <= 8, 64-query tiles over 64-key tiles otherwise.
+static int prefill_attn(const h16* qkv, h16* kc, h16* vc, h16* att, int G, int T, int E, int Tmax, int bf, bool pdl, cudaStream_t st,
+                        int T0 = 0) {
     const int nh = E / 64;
-    if (T <= 4)                                       // tiny groups (the forward's head stack): a warp per (group, head)
+    if (T0 == 0 && T <= 4)                                       // tiny groups (the forward's head stack): a warp per (group, head)
         return launch_pdl(prefill_attn_small_kernel<4>, dim3((unsigned)ceil_div((int64_t)G * nh, 4)), dim3(128), (size_t)0, st, pdl, qkv, kc,
                           vc, att, G, T, E, nh, Tmax, bf);
-    if (T <= 8)
+    if (T0 == 0 && T <= 8)
         return launch_pdl(prefill_attn_small_kernel<8>, dim3((unsigned)ceil_div((int64_t)G * nh, 4)), dim3(128), (size_t)0, st, pdl, qkv, kc,
                           vc, att, G, T, E, nh, Tmax, bf);
     const dim3 grid((unsigned)((int64_t)ceil_div(T, 64) * G * nh));     // 64-query tiles over 64-key tiles, online softmax
-    if (bf) return launch_pdl(prefill_attn_flash_kernel<true>, grid, dim3(128), (size_t)0, st, pdl, qkv, kc, vc, att, G, T, E, nh, Tmax);
-    return launch_pdl(prefill_attn_flash_kernel<false>, grid, dim3(128), (size_t)0, st, pdl, qkv, kc, vc, att, G, T, E, nh, Tmax);
+    if (bf) return launch_pdl(prefill_attn_flash_kernel<true>, grid, dim3(128), (size_t)0, st, pdl, qkv, kc, vc, att, G, T, E, nh, Tmax, T0);
+    return launch_pdl(prefill_attn_flash_kernel<false>, grid, dim3(128), (size_t)0, st, pdl, qkv, kc, vc, att, G, T, E, nh, Tmax, T0);
 }
 
+// T new tokens of G groups at sequence offset T0 through one stack; cache rows [T0, T0 + T) written when kc != NULL (T0 > 0 needs kc)
 static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights>& blocks, const std::vector<FastLayer>& maps,
-                         const BatchBufs& bb, int G, int T, h16* kc, h16* vc, int64_t kv_per_layer, int Tmax, cudaStream_t st) {
+                         const BatchBufs& bb, int G, int T, h16* kc, h16* vc, int64_t kv_per_layer, int Tmax, cudaStream_t st, int T0 = 0) {
     const rqb200_ar_config& c = f.cfg;
     const int E = c.embed_dim;
     const int64_t M = (int64_t)G * T;
@@ -1292,7 +1311,7 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
         RQB_TRY(linear_rows(f, maps[l].qkv, bb.XN, M, M, false, epilogue(GT_H16, bw.bqkv, bb.QKV), pdl, st));
         h16* kcl = kc ? kc + kv_per_layer * l : nullptr;
         h16* vcl = vc ? vc + kv_per_layer * l : nullptr;
-        RQB_TRY(prefill_attn(bb.QKV, kcl, vcl, bb.ATT, G, T, E, Tmax, f.bf, pdl, st));
+        RQB_TRY(prefill_attn(bb.QKV, kcl, vcl, bb.ATT, G, T, E, Tmax, f.bf, pdl, st, T0));
         RQB_TRY(linear_rows(f, maps[l].proj, bb.ATT, M, M, false, epilogue(GT_F32, bw.bproj, bb.X, bb.X, E), pdl, st));
         RQB_TRY(ln_rows(M, bb.X, nof, nullptr, bw.ln2_w, bw.ln2_b, bb.XN, E, f.bf, f.n_sm, st));
         RQB_TRY(linear_rows(f, maps[l].fc1, bb.XN, M, M, false, epilogue(GT_H16_GELU, bw.b1, bb.H), pdl, st));
@@ -1301,24 +1320,28 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
     return 0;
 }
 
-// body input tokens [0, T) of every batch row into X (token-major): token s < cond_len is a cond token (transformers.py:224),
-// token s >= cond_len carries the summed input embeddings of the codes of position s - cond_len (:219-225)
-static int body_tokens_batched(const ArFast& f, const StepState* state, float* X, h16* S, int B, int T, cudaStream_t st) {
+// body input tokens [T0, T0 + T) of every batch row into X (token-major, token T0 + r in rows r * B ..): token s < cond_len is a cond
+// token (transformers.py:224), token s >= cond_len carries the summed input embeddings of the codes of position s - cond_len (:219-225).
+// The cond tokens' kernel reads their index from state->s, which must equal T0.
+static int body_tokens_batched(const ArFast& f, const StepState* state, float* X, h16* S, int B, int T, cudaStream_t st, int T0 = 0) {
     const rqb200_ar_config& c = f.cfg;
     const rqb200_ar_weights& w = f.w;
     const int E = c.embed_dim, HW = c.H * c.W, cl = c.cond_len;
-    RQB_TRY(launch_pdl(cond_tok_kernel, dim3(B, std::min(T, cl)), dim3(256), (size_t)0, st, false, state, w.cond_emb, w.pos_emb_cond, cl,
-                       c.vocab_cond, E, X));
-    const int n_code = T - cl;       // code tokens of positions 0 .. n_code-1
+    const int n_cond = std::max(0, std::min(T0 + T, cl) - T0);
+    if (n_cond > 0)
+        RQB_TRY(launch_pdl(cond_tok_kernel, dim3(B, n_cond), dim3(256), (size_t)0, st, false, state, w.cond_emb, w.pos_emb_cond, cl,
+                           c.vocab_cond, E, X));
+    const int n_code = T - n_cond, pos0 = T0 + n_cond - cl;     // code tokens of positions pos0 .. pos0 + n_code - 1
+    float* Xc = X + (int64_t)n_cond * B * E;
     if (n_code > 0 && (c.embed_variant & RQB200_EMB_TOK_INPUT)) {
         // row (j, b) = sum_d tok_emb(code_d of position j) + pos_emb_hw[j]                   (:222,225)
         RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, n_code), dim3(128), (size_t)0, st, false, state, w.tok_emb, tok_dstride(c), HW, c.D,
-                           c.vocab, E, 0, c.D, 2, 0, w.pos_emb_hw, (int64_t)E, X + (int64_t)cl * B * E));
+                           c.vocab, E, 0, c.D, 2, pos0, w.pos_emb_hw, (int64_t)E, Xc));
     } else if (n_code > 0) {
         RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, n_code), dim3(64), (size_t)0, st, false, state, w.codebook, cb_dstride(c), HW, c.D,
-                           c.codebook_size, c.code_dim, -c.D, 0, S, f.bf, 0));
+                           c.codebook_size, c.code_dim, -c.D, pos0, S, f.bf, 0));
         const int64_t Mc = (int64_t)B * n_code;
-        GemmTcParams e = epilogue(GT_F32, w.b_in, X + (int64_t)cl * B * E, w.pos_emb_hw, E);
+        GemmTcParams e = epilogue(GT_F32, w.b_in, Xc, w.pos_emb_hw + (int64_t)pos0 * E, E);
         e.bias_scale = (float)c.D;       // (the bias is counted D times, as in the single-token step)
         e.res_div = B;                   // row (j, b) gets pos_emb_hw[j]
         RQB_TRY(linear_rows(f, f.w_in, S, Mc, Mc, true, e, false, st));
@@ -1326,16 +1349,17 @@ static int body_tokens_batched(const ArFast& f, const StepState* state, float* X
     return 0;
 }
 
-// ---- batched prefill: body tokens [0, T) of every batch row in one pass.  Leaves ws.XB = the last token's output rows, the KV
-// cache rows [0, T) written, state.s = T.
-static int prefill_batched(const ArFast& f, FastWs& ws, int T, cudaStream_t st) {
+// ---- batched body pass: body tokens [T0, T0 + T) of every batch row in one pass, on the KV cache rows [0, T0) earlier passes or steps
+// left (state.s == T0).  Leaves ws.XB = the last token's output rows, the KV cache rows [T0, T0 + T) written, state.s = T0 + T.  The
+// prefill is T0 = 0; an append of a run of kept positions' code tokens to the cache is T0 > 0.
+static int body_batched(const ArFast& f, FastWs& ws, int T0, int T, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const int E = c.embed_dim, B = f.B, HW = c.H * c.W, cl = c.cond_len, Tb = cl + HW;
     const int64_t M = (int64_t)B * T;
-    if (M > ws.Mmax) return fail(RQB200_EINVAL, "ar fast tier: prefix too long for the batched prefill");
-    RQB_TRY(body_tokens_batched(f, ws.state, ws.PX, ws.PS, B, T, st));
+    if (M > ws.Mmax || T0 + T > Tb) return fail(RQB200_EINVAL, "ar fast tier: too many tokens for the batched body pass");
+    RQB_TRY(body_tokens_batched(f, ws.state, ws.PX, ws.PS, B, T, st, T0));
     BatchBufs bb = {ws.PX, ws.PXN, ws.PQKV, ws.PATT, ws.PH};
-    RQB_TRY(stack_batched(f, f.body, f.lbody, bb, B, T, ws.kc_body, ws.vc_body, (int64_t)B * c.n_head * Tb * 64, Tb, st));
+    RQB_TRY(stack_batched(f, f.body, f.lbody, bb, B, T, ws.kc_body, ws.vc_body, (int64_t)B * c.n_head * Tb * 64, Tb, st, T0));
     RQB_CUDA(cudaMemcpyAsync(ws.XB, ws.PX + (int64_t)(T - 1) * B * E, (size_t)B * E * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, T, 0, 0);
 }
@@ -1532,7 +1556,7 @@ static int run_graph(ArFast& f, FastWs& ws, int which, cudaStream_t st) {
 static int prefill_prefix(ArFast& f, FastWs& ws, int idx_begin, cudaStream_t st) {
     const int T0 = f.cfg.cond_len + idx_begin;
     if (f.batched_prefill && T0 >= 4 && (int64_t)f.B * T0 <= ws.Mmax) {
-        RQB_TRY(prefill_batched(f, ws, T0, st));
+        RQB_TRY(body_batched(f, ws, 0, T0, st));
         // state.idx must equal idx_begin for the first head graph
         if (idx_begin > 0) RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, idx_begin, 0));
     } else {
@@ -1547,12 +1571,17 @@ static int prefill_prefix(ArFast& f, FastWs& ws, int idx_begin, cudaStream_t st)
     return 0;
 }
 
+// Runs of kept positions shorter than this many code tokens are appended to the body cache by replaying the single-token body graph
+// once per token; longer runs take one batched body pass (body_batched at T0 > 0).  scripts/bench_keep.py --sweep, in1400m B = 64 on
+// an H100 80GB HBM3 at 700 W, runs of exactly k: batched / token by token = 1.03 at k = 5, 0.90 at k = 6, 0.68 at k = 8.
+constexpr int APPEND_BATCHED_MIN = 6;
+
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
                    float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st, int cfg_n,
-                   float cfg_s) {
+                   float cfg_s, const uint8_t* keep, const uint8_t* sampled) {
     const rqb200_ar_config& c = f->cfg;
-    const int D = c.D, HW = c.H * c.W;
+    const int D = c.D, HW = c.H * c.W, cl = c.cond_len;
     if (B < 1 || B > 256) return fail(RQB200_EINVAL, "ar fast tier: batch must be in [1,256] per call");
     if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n)) return fail(RQB200_EINVAL, "ar_sample: a guided call takes B = 2 cfg_n rows");
     if (idx_begin < 0 || idx_end > HW || idx_begin > idx_end) return fail(RQB200_EINVAL, "ar_sample: bad position span");
@@ -1561,9 +1590,14 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
     if (need > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_sample: workspace too small");
     if (!resume && out != partial)
         RQB_CUDA(cudaMemcpyAsync(out, partial, (size_t)B * HW * D * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
-    if (idx_begin >= idx_end) return 0;
+    int first = idx_begin;                            // the span's first sampled position
+    while (first < idx_end && !plan_sampled(sampled, first)) first++;
+    if (first >= idx_end) return 0;                   // nothing to sample: `out` holds partial
+    // prev: the last sampled position of the call before this span (its code tokens are the body's next input); none: the prefill runs
+    // at the first sampled position
+    int prev = resume ? plan_prev(sampled, idx_begin) : -1;
     if (f->ws_base != wsp || f->B != B) {
-        if (resume) return fail(RQB200_ESTATE, "ar_sample: resume on a workspace / batch the engine is not bound to");
+        if (prev >= 0) return fail(RQB200_ESTATE, "ar_sample: resume on a workspace / batch the engine is not bound to");
         RQB_TRY(bind(*f, ws, wsp, B));
     }
     StepState h = {};
@@ -1571,14 +1605,37 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
     h.cond = cond; h.codes = out; h.force = force; h.noise = noise; h.logits_out = logits_out; h.noise_stride = noise_stride;
     h.temperature = temperature;
     h.cfg_n = cfg_n; h.cfg_scale = cfg_s;        // (the head graphs' samplers read them: no recapture between guided and unguided calls)
+    h.keep = keep;
     for (int d = 0; d < D; d++) { h.top_k[d] = top_k[d]; h.top_p[d] = top_p[d]; }
-    RQB_TRY(launch_pdl(init_state_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, h, resume ? 1 : 0));
-    if (f->trace && !resume) RQB_CUDA(cudaMemsetAsync(ws.trace, 0, (size_t)4 * TR_CAP * sizeof(long long), st));
+    RQB_TRY(launch_pdl(init_state_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, h, prev >= 0 ? 1 : 0));
+    if (f->trace && prev < 0) RQB_CUDA(cudaMemsetAsync(ws.trace, 0, (size_t)4 * TR_CAP * sizeof(long long), st));
     const int head_graph = logits_out ? G_HEAD_LOGITS : G_HEAD;
-    if (!resume) RQB_TRY(prefill_prefix(*f, ws, idx_begin, st));
-    for (int idx = idx_begin; idx < idx_end; idx++) {
-        if (idx > idx_begin || resume) RQB_TRY(run_graph(*f, ws, G_CODE, st));   // body step on the token of position idx-1 (state.idx == idx)
-        RQB_TRY(run_graph(*f, ws, head_graph, st));                              // D head steps + sampling; advances idx, step
+    // the host's copy of state.idx / state.step: a head graph leaves idx one past its position; step counts the span's tokens, sampled
+    // or not, so that noise and logits_out stay indexed by token
+    int cur_idx = prev >= 0 ? prev + 1 : 0, cur_step = 0;
+    auto advance_to = [&](int idx, int step) -> int {
+        if (idx == cur_idx && step == cur_step) return 0;
+        RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, idx - cur_idx, step - cur_step));
+        cur_idx = idx; cur_step = step;
+        return 0;
+    };
+    for (int b = first; b < idx_end; b++) {
+        if (!plan_sampled(sampled, b)) continue;
+        if (prev < 0) {
+            RQB_TRY(prefill_prefix(*f, ws, b, st));                        // cond tokens and positions [0, b); state.idx = b
+            cur_idx = b;
+        } else if (f->batched_prefill && b - prev >= APPEND_BATCHED_MIN && (int64_t)B * (b - prev) <= ws.Mmax) {
+            RQB_TRY(body_batched(*f, ws, cl + prev, b - prev, st));       // the code tokens of positions [prev, b) in one pass
+        } else {
+            for (int j = prev; j < b; j++) {                               // one body step each (state.idx == j + 1: position j)
+                RQB_TRY(advance_to(j + 1, cur_step));
+                RQB_TRY(run_graph(*f, ws, G_CODE, st));
+            }
+        }
+        RQB_TRY(advance_to(b, (b - idx_begin) * D));
+        RQB_TRY(run_graph(*f, ws, head_graph, st));                        // D head steps + sampling; advances idx, step
+        cur_idx = b + 1; cur_step += D;
+        prev = b;
     }
     return 0;
 }
@@ -1655,6 +1712,17 @@ extern "C" int rqb200_dbg_prefill_attn(const void* qkv, void* kc, void* vc, void
     if (kc && T > Tmax) return fail(RQB200_EINVAL, "dbg_prefill_attn: T > Tmax");
     if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_prefill_attn: no CUDA device");
     return prefill_attn((const h16*)qkv, (h16*)kc, (h16*)vc, (h16*)att, G, T, E, Tmax, fmt, false, (cudaStream_t)stream);
+}
+
+extern "C" int rqb200_dbg_append_attn(const void* qkv, void* kc, void* vc, void* att, int G, int T0, int T, int E, int Tmax, int fmt,
+                                      void* stream) {
+    using namespace rqb;
+    if (fmt < 0 || fmt > 1 || G < 1 || T < 1 || T0 < 0 || E < 64 || E % 64 || Tmax > FAST_MAXT || T0 + T > Tmax ||
+        (int64_t)ceil_div(T, 64) * G * (E / 64) > INT32_MAX)
+        return fail(RQB200_EINVAL, "dbg_append_attn: need fmt 0..1, G >= 1, T >= 1, T0 >= 0, T0 + T <= Tmax <= 2048, E % 64 == 0");
+    if (!qkv || !att || !kc || !vc) return fail(RQB200_EINVAL, "dbg_append_attn: null argument");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_append_attn: no CUDA device");
+    return prefill_attn((const h16*)qkv, (h16*)kc, (h16*)vc, (h16*)att, G, T, E, Tmax, fmt, false, (cudaStream_t)stream, T0);
 }
 
 extern "C" int rqb200_dbg_ln(int form, const float* x_in, const float* partial, int S, const float* bias, const float* extra, float* x_out,

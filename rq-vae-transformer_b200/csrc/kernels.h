@@ -28,7 +28,7 @@ int launch_rq_embed(const int64_t* codes, const RqTables& tabs, int64_t N, int D
 // sampler.cu
 int launch_sample(const float* logits, const float* q, int B, int V, float temperature, int top_k, float top_p,
                   int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo = 1, int cfg_n = 0,
-                  float cfg_s = 0.f);
+                  float cfg_s = 0.f, const uint8_t* keep = nullptr);
 // logprob.cu -- out[r] = lg[r*ld + t] - logsumexp(lg[r*ld .. r*ld + V)), t = tgt[r*tgt_stride]; NaN when t is outside [0, V)
 int launch_logprob_rows(const float* lg, int64_t ld, int V, int64_t rows, const int64_t* tgt, int64_t tgt_stride, float* out,
                         cudaStream_t st);
@@ -144,9 +144,22 @@ struct StepState {
     int64_t noise_stride;
     float temperature;
     float cfg_scale;          // guidance scale s (cfg_n > 0)
+    const uint8_t* keep;      // [B, HW, D] nonzero: the token keeps the code `codes` was initialised with (the sampler writes nothing); or null
     int top_k[8];
     float top_p[8];
 };
+
+// The position plan of a masked sample (rqb200_ar_sample_span_keep): sampled[p] != 0 when some row samples some depth of position p;
+// sampled == NULL samples every position.  Only sampled positions run the head stack, classifier and sampler; the body consumes the
+// code tokens of the positions between two sampled ones right before the later one's head (positions after the last sampled one
+// are never consumed).
+inline bool plan_sampled(const uint8_t* sampled, int p) { return sampled == nullptr || sampled[p] != 0; }
+// the last sampled position before p, or -1
+inline int plan_prev(const uint8_t* sampled, int p) {
+    for (int i = p - 1; i >= 0; i--)
+        if (plan_sampled(sampled, i)) return i;
+    return -1;
+}
 int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, int V, int HW, int D, cudaStream_t st, bool pdl);
 
 struct ArFast;
@@ -155,11 +168,12 @@ ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, 
 void ar_fast_destroy(ArFast* f);
 size_t ar_fast_workspace_bytes(const ArFast* f, int B);
 // positions [idx_begin, idx_end) of the raster; resume != 0: continue on the KV state the previous call left in this workspace.
-// cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s
+// cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s.  keep / sampled: the masked-sample
+// plan (null: every token sampled)
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
-                   float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st, int cfg_n = 0,
-                   float cfg_s = 0.f);
+                   float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st, int cfg_n,
+                   float cfg_s, const uint8_t* keep, const uint8_t* sampled);
 // the logits of ONE token (idx, d) into logits_out [B,V] (rqb200_ar_step; arguments already checked by the caller)
 int ar_fast_step(ArFast* f, const int64_t* xs, int64_t xs_stride, const int64_t* cond, int B, int idx, int d, int restart,
                  float* logits_out, void* wsp, size_t ws_bytes, cudaStream_t st);

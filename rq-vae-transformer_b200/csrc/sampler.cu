@@ -17,6 +17,9 @@
 //      kept mass.
 //   5. out = argmax_i p_i / q_i, first index on ties.
 //
+// Masked sampling (keep != NULL, same addressing as force): a CTA whose row keeps its token returns without writing; that takes
+// precedence over teacher forcing.
+//
 // Classifier-free guidance (cfg_n > 0): the logits hold 2n rows, conditional rows [0, n) then unconditional rows [n, 2n).  CTA r < n
 // reads rows r and r + n in step 1 and samples l = u + s (c - u), formed in fp32 as three rounded operations (no FMA contraction,
 // so torch's `u + s * (c - u)` gives the same bits), with noise row r; it writes the code to rows r and r + n of the output.  CTAs
@@ -53,7 +56,8 @@ __device__ __forceinline__ bool item_before(const SortItem& a, const SortItem& b
 __global__ void __launch_bounds__(SMP_THREADS, 1)
 sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise, int V, float temperature, int top_k,
               float top_p, int64_t* __restrict__ out_idx, const int64_t* __restrict__ force, int64_t out_stride,
-              const StepState* __restrict__ stt, int dyn_d, int dyn_HW, int dyn_D, int algo, int cfg_n, float cfg_s) {
+              const StepState* __restrict__ stt, int dyn_d, int dyn_HW, int dyn_D, int algo, int cfg_n, float cfg_s,
+              const uint8_t* __restrict__ keep) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* xs = reinterpret_cast<float*>(smem_raw);                       // [V]   scaled logits, later probabilities
     SortItem* items = reinterpret_cast<SortItem*>(xs + V);                // [Vpad] only touched when top_p < 1
@@ -88,7 +92,11 @@ sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise
         top_p = stt->top_p[dyn_d];
         cfg_n = stt->cfg_n;
         cfg_s = stt->cfg_scale;
+        keep = stt->keep ? stt->keep + off : nullptr;
     }
+    // a kept token: `out` was initialised with its code (in both branch rows when guided).  The mask is constant during the call, but
+    // the fast tier's position stt->idx is advanced by launches of the chain, so the fast tier reads it only after the dependency wait.
+    if (keep != nullptr && keep[(int64_t)row * out_stride]) return;
 
     if (force != nullptr) {   // teacher forcing: emit the forced code, skip the work
         if (t == 0) out_idx[(int64_t)row * out_stride] = force[(int64_t)row * out_stride];
@@ -420,7 +428,8 @@ constexpr int SAMPLER_ALGO_DEFAULT = 1;
 // codes[b, h, w, d] (stride H*W*D).  force (nullable) uses the same addressing.  cfg_n > 0: guided over B = 2 cfg_n rows, one CTA per
 // image (one per row when teacher forcing).
 int launch_sample(const float* logits, const float* q, int B, int V, float temperature, int top_k, float top_p,
-                  int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo, int cfg_n, float cfg_s) {
+                  int64_t* out_idx, const int64_t* force, int64_t out_stride, cudaStream_t st, int algo, int cfg_n, float cfg_s,
+                  const uint8_t* keep) {
     if (B <= 0) return B == 0 ? 0 : fail(RQB200_EINVAL, "sample: B < 0");
     if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n)) return fail(RQB200_EINVAL, "sample: a guided call takes B = 2 cfg_n rows");
     if (V <= 0 || V > SMP_MAXV) return fail(RQB200_EINVAL, "sample: V must be in [1,16384]");
@@ -431,7 +440,7 @@ int launch_sample(const float* logits, const float* q, int B, int V, float tempe
     RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel);
     const int grid = (cfg_n > 0 && force == nullptr) ? cfg_n : B;
     sample_kernel<<<grid, SMP_THREADS, smem, st>>>(logits, q, V, temperature, top_k, top_p, out_idx, force, out_stride, nullptr, 0, 0,
-                                                   0, algo, cfg_n, cfg_s);
+                                                   0, algo, cfg_n, cfg_s, keep);
     return check_launch("sample_logits");
 }
 
@@ -442,7 +451,8 @@ int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, i
     size_t smem = (size_t)V * sizeof(float) + (size_t)vpad * sizeof(SortItem);   // top_p is only known on the device
     RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel);
     return launch_pdl(sample_kernel, dim3(B), dim3(SMP_THREADS), smem, st, pdl, logits, (const float*)nullptr, V, 1.0f, 0, 1.0f,
-                      (int64_t*)nullptr, (const int64_t*)nullptr, (int64_t)0, stt, d, HW, D, SAMPLER_ALGO_DEFAULT, 0, 0.0f);
+                      (int64_t*)nullptr, (const int64_t*)nullptr, (int64_t)0, stt, d, HW, D, SAMPLER_ALGO_DEFAULT, 0, 0.0f,
+                      (const uint8_t*)nullptr);
 }
 
 }  // namespace rqb

@@ -96,6 +96,7 @@ def lib():
                                         C.POINTER(C.c_int32), C.POINTER(C.c_float), C.c_void_p, C.c_int64, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.rqb200_ar_sample_span_cfg.argtypes = L.rqb200_ar_sample_span.argtypes + [C.c_float]
+    L.rqb200_ar_sample_span_keep.argtypes = L.rqb200_ar_sample_span.argtypes + [C.c_void_p, C.c_void_p, C.c_int, C.c_float]
     L.rqb200_ar_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.rqb200_ar_forward_workspace_bytes.restype = C.c_size_t
@@ -130,6 +131,7 @@ def lib():
     L.rqb200_dbg_attn_step.argtypes = [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 4 + [C.c_int] * 3 + [C.c_void_p] + [C.c_int] * 2 + \
                                       [C.c_void_p]
     L.rqb200_dbg_prefill_attn.argtypes = [C.c_void_p] * 4 + [C.c_int] * 5 + [C.c_void_p]
+    L.rqb200_dbg_append_attn.argtypes = [C.c_void_p] * 4 + [C.c_int] * 6 + [C.c_void_p]
     L.rqb200_dbg_ln.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 6 + [C.c_int64, C.c_int, C.c_int, C.c_void_p]
     L.rqb200_dbg_act_reduce.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p] + [C.c_int] * 3 + [C.c_void_p]
     L.rqb200_dbg_vae_conv.argtypes = [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int] * 10 + [C.c_void_p]
@@ -142,14 +144,14 @@ def lib():
 
 EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200_rq_quantize", "rqb200_rq_embed_sum",
            "rqb200_rq_embed_depth", "rqb200_rq_soft_codes", "rqb200_sample_logits", "rqb200_ar_create", "rqb200_ar_destroy",
-           "rqb200_ar_workspace_bytes", "rqb200_ar_sample", "rqb200_ar_sample_span", "rqb200_ar_sample_span_cfg", "rqb200_ar_step", "rqb200_ar_forward",
+           "rqb200_ar_workspace_bytes", "rqb200_ar_sample", "rqb200_ar_sample_span", "rqb200_ar_sample_span_cfg", "rqb200_ar_sample_span_keep", "rqb200_ar_step", "rqb200_ar_forward",
            "rqb200_ar_forward_workspace_bytes", "rqb200_ar_trace", "rqb200_ar_last_launches", "rqb200_vae_create",
            "rqb200_vae_destroy", "rqb200_vae_set_tensor", "rqb200_vae_finalize", "rqb200_vae_workspace_bytes",
            "rqb200_vae_decode", "rqb200_vae_decode_code", "rqb200_vae_encode", "rqb200_vae_last_launches",
            "rqb200_dbg_gemm_tc", "rqb200_dbg_gemm_tc_fp8", "rqb200_dbg_conv_tc", "rqb200_dbg_conv_tc_gn", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
            "rqb200_dbg_rows_gemm", "rqb200_rq_quantize_depthwise", "rqb200_rq_embed_sum_depthwise",
            "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise", "rqb200_ar_log_prob",
-           "rqb200_ar_log_prob_workspace_bytes", "rqb200_dbg_log_prob_rows", "rqb200_dbg_attn_step", "rqb200_dbg_prefill_attn",
+           "rqb200_ar_log_prob_workspace_bytes", "rqb200_dbg_log_prob_rows", "rqb200_dbg_attn_step", "rqb200_dbg_prefill_attn", "rqb200_dbg_append_attn",
            "rqb200_dbg_ln", "rqb200_dbg_act_reduce", "rqb200_dbg_vae_conv", "rqb200_dbg_groupnorm", "rqb200_dbg_cast_f16",
            "rqb200_dbg_vae_attn"]
 

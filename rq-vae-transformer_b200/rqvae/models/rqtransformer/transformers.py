@@ -373,12 +373,38 @@ class RQTransformer(Stage2Model):
             raise ValueError("rqb200: uncond entries must lie in [0, %d)" % self.vocab_size_cond)
         return float(cfg_scale), u
 
+    def _keep_mask(self, keep_mask, B, start_loc):
+        """sample()'s keep_mask checked before any kernel runs and laid out for the engine: None, or a contiguous uint8 [B, H, W, D] with
+        the start_loc prefix kept too.  Raises ValueError for a mask that is not a bool tensor, does not broadcast to [B, H, W, D] or lies
+        on another device than the model."""
+        if keep_mask is None:
+            return None
+        H, W, D = self.block_size
+        if not isinstance(keep_mask, torch.Tensor) or keep_mask.dtype != torch.bool:
+            raise ValueError("rqb200: keep_mask must be a torch.bool tensor, got %s" % getattr(keep_mask, "dtype", type(keep_mask)))
+        if keep_mask.device != self.pos_emb_hw.device:
+            raise ValueError("rqb200: keep_mask is on %s, the model on %s" % (keep_mask.device, self.pos_emb_hw.device))
+        want = (B, H, W, D)
+        try:
+            ok = tuple(torch.broadcast_shapes(tuple(keep_mask.shape), want)) == want
+        except RuntimeError:
+            ok = False
+        if not ok:
+            raise ValueError("rqb200: keep_mask of shape %s does not broadcast to [B, H, W, D] = %s" % (tuple(keep_mask.shape), want))
+        keep = keep_mask.expand(want).to(torch.uint8).contiguous()
+        idx0 = min(start_loc[0] * W + start_loc[1], H * W)
+        keep.view(B, H * W, D)[:, :idx0] = 1
+        return keep
+
     @torch.no_grad()
     def _native_sample(self, partial, model_aux, cond, start_loc, temperature, top_k, top_p, amp, noise=None,
-                       return_logits=False, force_codes=None, guidance=None):
+                       return_logits=False, force_codes=None, guidance=None, keep=None):
         """guidance: None, or (s, uncond [B, cond_len] int64) from _guidance -- classifier-free guidance: every image runs a cond and an
         uncond branch as rows [cond | uncond] of one native call (rqb200_ar_sample_span_cfg), noise stays per image [n_tok, B, V],
-        logits (return_logits) and force_codes hold both branches' rows [2B]: [cond rows | uncond rows]"""
+        logits (return_logits) and force_codes hold both branches' rows [2B]: [cond rows | uncond rows].
+        keep: None, or uint8 [B, H, W, D] from _keep_mask -- masked completion (rqb200_ar_sample_span_keep): each batch chunk passes its
+        rows of the mask (guided: in both branches' rows) and the positions where any of its rows samples any depth; those position
+        lists are formed on the device and read to the host once per call.  The logits of positions a chunk skips are not written."""
         H, W, D = self.block_size
         B = partial.shape[0]
         dev = self.pos_emb_hw.device
@@ -418,6 +444,13 @@ class RQTransformer(Stage2Model):
                 calls = [(2 * (hi - lo), torch.cat([partial[lo:hi], partial[lo:hi]]), torch.cat([cu[lo:hi], u[lo:hi]]),
                           None if fc is None else torch.cat([fc[lo:hi], fc[B + lo:B + hi]]),
                           torch.empty(2 * (hi - lo), H, W, D, dtype=torch.int64, device=dev)) for lo, hi in bounds]
+            if keep is not None:
+                HW = H * W
+                sampled = torch.stack([(keep[lo:hi] == 0).reshape(hi - lo, HW, D).any(2).any(0) for lo, hi in bounds])
+                sampled = sampled.to(torch.uint8).cpu()                 # the call's one host read
+                plans = [((C.c_uint8 * HW)(*sampled[i].tolist()),
+                          keep[lo:hi] if guidance is None else torch.cat([keep[lo:hi], keep[lo:hi]]).contiguous())
+                         for i, (lo, hi) in enumerate(bounds)]
             # position spans: when the noise is drawn here it is drawn span by span into one bounded buffer (noise_budget_bytes)
             # instead of one [n_tok,B,V] tensor (1 GB at 8x8x4, B=64, V=16384); every batch chunk keeps its own engine slot
             # (workspace + KV state) so that all chunks can resume on the next span
@@ -444,12 +477,17 @@ class RQTransformer(Stage2Model):
                     for t in range((p1 - p0) * D):
                         noise[t].exponential_(1)
                 tok0 = 0 if draw else (p0 - idx0) * D                  # first token of this span inside `noise`
-                for eng, (lo, hi), (rows, part_c, cond_c, fc_c, out_c) in zip(engines, bounds, calls):
+                for i, (eng, (lo, hi), (rows, part_c, cond_c, fc_c, out_c)) in enumerate(zip(engines, bounds, calls)):
                     args = (eng["handle"], off(part_c, 0, HWD, 8), off(cond_c, 0, cl, 8), rows, p0, p1, int(p0 > idx0),
                             float(temperature), kk, pp, off(noise, lo, V, 4, tok0 * B * V), 0 if noise is None else B * V,
                             off(logits, 0, V, 4, (p0 - idx0) * D * R * V), off(fc_c, 0, HWD, 8), off(out_c, 0, HWD, 8),
                             N.ptr(eng["ws"]), eng["ws"].numel(), C.c_void_p(st.cuda_stream))
-                    if guidance is None:
+                    if keep is not None:
+                        N.check(N.lib().rqb200_ar_sample_span_keep(*args, N.ptr(plans[i][1]), plans[i][0],
+                                                                   0 if guidance is None else rows // 2,
+                                                                   C.c_float(0.0 if guidance is None else guidance[0])),
+                                "ar_sample_keep")
+                    elif guidance is None:
                         N.check(N.lib().rqb200_ar_sample_span(*args), "ar_sample")
                     else:
                         N.check(N.lib().rqb200_ar_sample_span_cfg(*args, C.c_float(guidance[0])), "ar_sample_cfg")
@@ -480,16 +518,24 @@ class RQTransformer(Stage2Model):
 
     @torch.no_grad()
     def sample(self, partial_sample, model_aux=None, cond=None, start_loc=(0, 0), temperature=1.0, top_k=None, top_p=None,
-               amp=False, cached=True, is_tqdm=False, desc="Sampling", fast=True, cfg_scale=None, uncond=None):
+               amp=False, cached=True, is_tqdm=False, desc="Sampling", fast=True, cfg_scale=None, uncond=None, keep_mask=None):
         """transformers.py:294-369.  Returns LongTensor [B,H,W,D]; ``partial_sample`` is not modified.
         Classifier-free guidance: with a float ``cfg_scale`` s and ``uncond`` (cond's shape: an unconditional or negative condition
         per image), every token is drawn from l = u + s * (c - u) -- c the logits under ``cond``, u under ``uncond`` -- then
         temperature, top-k and top-p as unguided, with one Exp(1) draw per image and token.  Both branches share the
-        partial_sample / start_loc prefix and every drawn code.  The default ``cfg_scale=None`` samples unguided."""
+        partial_sample / start_loc prefix and every drawn code.  The default ``cfg_scale=None`` samples unguided.
+        Masked completion (editing): ``keep_mask``, a torch.bool tensor on the model's device that broadcasts to [B, H, W, D] (e.g.
+        [H, W, 1] for a region of every image, [1, 1, 1, D] for depths), keeps partial_sample's code wherever it is True; the positions
+        before start_loc are kept as always.  Every other token is sampled as sample() would, seeing the kept codes before it in raster
+        order (and none after it), and every token still takes its Exp(1) draw.  Positions where nothing is sampled skip the head stack;
+        their codes reach the body in one batched pass per run on the fast tier.  Which positions those are is read to the host once
+        per call.  Composes with guidance, both tiers and every fast weight format."""
         assert self.block_size == partial_sample.shape[1:]
         guidance = self._guidance(partial_sample.shape[0], cfg_scale, uncond)
+        keep = self._keep_mask(keep_mask, partial_sample.shape[0], start_loc)
         self.init_cache()
-        out = self._native_sample(partial_sample, model_aux, cond, start_loc, temperature, top_k, top_p, amp, guidance=guidance)
+        out = self._native_sample(partial_sample, model_aux, cond, start_loc, temperature, top_k, top_p, amp, guidance=guidance,
+                                  keep=keep)
         self.init_cache()
         return out
 
