@@ -156,40 +156,27 @@ rqb200_ar* rqb200_ar_create(const rqb200_ar_config* cfg, const rqb200_ar_weights
 void rqb200_ar_destroy(rqb200_ar* h);
 size_t rqb200_ar_workspace_bytes(const rqb200_ar* h, int B);
 
-/* RQTransformer.sample (transformers.py:294-369) with cached_forward (:190-287) and sample_from_logits fused
- * into one device-side loop (no host sync per token).
- *   partial [B,H,W,D] int64 (prefix used when start_h/start_w > 0), cond [B,cond_len] int64 or NULL (zeros),
+/* RQTransformer.sample (transformers.py:294-369) with cached_forward (:190-287) and sample_from_logits fused into one device-side
+ * loop (no host sync per token), over the positions [idx_begin, idx_end) of the raster.
+ *   partial [B,H,W,D] int64 (the prefix before idx_begin is used), cond [B,cond_len] int64 or NULL (zeros),
  *   top_k_host[D] / top_p_host[D]: per-depth settings (HOST arrays, already clamped like :314-330),
- *   noise (nullable): per-token Exp(1) draws, token t (= the t-th *sampled* (h,w,d) in raster order) at
+ *   noise (nullable): per-token Exp(1) draws, token t (= the t-th (h,w,d) of this span in raster order) at
  *   noise + t*noise_stride, each [B,V] f32; NULL -> q = 1,
  *   logits_out (nullable) [n_tokens,B,V] f32 receives every step's logits (teacher-forcing / parity tests),
  *   force_codes (nullable) [B,H,W,D] int64: teacher forcing -- logits are computed and (optionally) dumped but
  *   the code written back is force_codes' (so the step-parity protocol of SURVEY.md 8c can be run),
- *   out_codes [B,H,W,D] int64. */
-int rqb200_ar_sample(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int start_h, int start_w,
-                     float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
-                     int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                     void* workspace, size_t workspace_bytes, void* stream);
-/* The same loop over the positions [idx_begin, idx_end) of the raster only.  resume == 0: starts like rqb200_ar_sample with
- * start_loc = idx_begin (prefix prefill from `partial`); resume != 0: continues on the KV / context state the previous call left
- * in the SAME workspace (no prefill; `partial` is ignored, out_codes must be the buffer of the previous call).  noise /
- * logits_out are indexed from the first token of THIS span.  Lets a caller draw the per-token noise in bounded chunks. */
-int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
-                          float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
-                          int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                          void* workspace, size_t workspace_bytes, void* stream);
-/* rqb200_ar_sample_span with classifier-free guidance: B = 2n rows, n >= 1.  partial, cond, out_codes, force_codes and logits_out
- * are laid out [n conditional rows | n unconditional rows]; noise is per image, [n_tok][n][V] (noise_stride apart per token).  At
- * every token both branches produce logits c and u, and the sampler draws image b's code from l = u + cfg_scale * (c - u) in fp32
- * (three rounded operations, no FMA), then temperature, top-k and top-p as unguided, with noise row b; the code is written to
- * rows b and n + b, and both branches consume it from the next token on.  Teacher forcing copies every row's own forced code.
- * logits_out receives the raw logits of all 2n rows.  Fast tier: 2n <= 256. */
-int rqb200_ar_sample_span_cfg(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
-                              float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
-                              int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                              void* workspace, size_t workspace_bytes, void* stream, float cfg_scale);
-/* Masked completion: rqb200_ar_sample_span (cfg_n = 0) or rqb200_ar_sample_span_cfg (cfg_n = B / 2 images, cfg_scale) that samples only
- * the tokens the caller does not keep.
+ *   out_codes [B,H,W,D] int64.
+ * resume == 0: a new call; sample(start_loc=(h, w)) is idx_begin = h*W + w, idx_end = H*W (prefix prefill from `partial`).
+ * resume != 0: continues on the KV / context state the previous call left in the SAME workspace (no prefill; `partial` is
+ * ignored, out_codes must be the buffer of the previous call).  noise / logits_out are indexed from the first token of THIS
+ * span.  Lets a caller draw the per-token noise in bounded chunks.
+ * Classifier-free guidance: cfg_n = 0 is unguided (cfg_scale ignored); cfg_n = n >= 1 needs B = 2n rows.  partial, cond,
+ * out_codes, force_codes and logits_out are then laid out [n conditional rows | n unconditional rows]; noise is per image,
+ * [n_tok][n][V] (noise_stride apart per token).  At every token both branches produce logits c and u, and the sampler draws
+ * image b's code from l = u + cfg_scale * (c - u) in fp32 (three rounded operations, no FMA), then temperature, top-k and top-p
+ * as unguided, with noise row b; the code is written to rows b and n + b, and both branches consume it from the next token on.
+ * Teacher forcing copies every row's own forced code.  logits_out receives the raw logits of all 2n rows.
+ * Masked completion samples only the tokens the caller does not keep (keep == sampled_host == NULL: every token sampled):
  *   keep (nullable, device) uint8 [B, H*W, D], rows laid out like out_codes (guided: the image's mask in both branch rows): nonzero keeps
  *     the token -- out_codes holds partial's code there (it was initialised from partial) and the sampler writes nothing, teacher
  *     forcing included.
@@ -200,27 +187,29 @@ int rqb200_ar_sample_span_cfg(rqb200_ar* h, const int64_t* partial, const int64_
  * rows of skipped positions are left untouched.  The body consumes the code tokens of the positions between two sampled positions a < b
  * right before b's head: on the fast tier in one batched pass at sequence offset cond_len + a when b - a is at least a few tokens
  * (token by token with RQB200_AR_SEQUENTIAL_PREFILL), on the exact tier token by token.  That grouping depends on sampled_host alone, so
- * a call split into spans gives the codes of one span bit for bit.  keep == sampled_host == NULL is rqb200_ar_sample_span(_cfg). */
-int rqb200_ar_sample_span_keep(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
-                               float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
-                               int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                               void* workspace, size_t workspace_bytes, void* stream, const uint8_t* keep, const uint8_t* sampled_host,
-                               int cfg_n, float cfg_scale);
+ * a call split into spans gives the codes of one span bit for bit.
+ * Fast tier: B <= 256 rows per call (a guided call: n <= 128 images).  The null pointers, B, cfg_n, the span and sampled_host are
+ * checked before any CUDA call.  ABI 113 appended the last four arguments: a caller built against an older header must pass them. */
+int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
+                          float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
+                          int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
+                          void* workspace, size_t workspace_bytes, void* stream, const uint8_t* keep, const uint8_t* sampled_host,
+                          int cfg_n, float cfg_scale);
 /* RQTransformer.cached_forward (transformers.py:190-287): the logits of ONE token (h, w, d) into logits_out [B,V] f32.
  *   xs: the caller's code map, int64, batch row b at xs + b*xs_batch_stride, positions in raster order, D codes each
  *       (only the codes this step consumes are read: position idx-1 when d == 0, codes 0..d-1 of position idx when d > 0;
  *       idx = pos_h*W + pos_w);
  *   restart != 0: a new sequence -- d must be 0; prefill cond + positions [0, idx) from xs (batched prefill as in
- *       rqb200_ar_sample), then head depth 0;
+ *       rqb200_ar_sample_span), then head depth 0;
  *   restart == 0: continue on the KV / context state the previous step left in the SAME workspace; (h,w,d) must be the
- *       token after the previous step's, else RQB200_ESTATE.  A rqb200_ar_sample / _span call on the handle ends the sequence.
+ *       token after the previous step's, else RQB200_ESTATE.  A rqb200_ar_sample_span call on the handle ends the sequence.
  * The launches are those of the sampling loop (split-K factors included) minus the sampler: under teacher forcing the logits
- * equal rqb200_ar_sample's logits_out bit for bit.  Fast tier: B <= 256 per call.  Arguments are checked before any CUDA
+ * equal rqb200_ar_sample_span's logits_out bit for bit.  Fast tier: B <= 256 per call.  Arguments are checked before any CUDA
  * call. */
 int rqb200_ar_step(rqb200_ar* h, const int64_t* xs, int64_t xs_batch_stride, const int64_t* cond, int B, int pos_h, int pos_w,
                    int d, int restart, float* logits_out, void* workspace, size_t workspace_bytes, void* stream);
 /* RQTransformer.forward (transformers.py:113-188): teacher-forced logits of complete code maps, all positions at once (fast tier:
- * M = B*T row GEMMs on wgmma + causal attention; exact tier: returns RQB200_EINVAL -- use rqb200_ar_sample with force_codes and
+ * M = B*T row GEMMs on wgmma + causal attention; exact tier: returns RQB200_EINVAL -- use rqb200_ar_sample_span with force_codes and
  * logits_out, the sequential replay).  codes [B,H,W,D] int64, cond [B,cond_len] or NULL.
  * logits_out [D][H*W][B][V] f32 (token-major: logits of (b, pos, d) at ((d*H*W + pos)*B + b)*V); cond_logits_out (nullable,
  * cond_len > 1 and w_ccls given) [cond_len-1][B][Vc] f32 with Vc = vocab_cond rounded up to a multiple of 128. */
@@ -232,9 +221,9 @@ int rqb200_ar_forward(rqb200_ar* h, const int64_t* codes, const int64_t* cond, i
  * log p(code (b, pos, d) | its prefix) at (d*H*W + pos)*B + b; cond_logp_out (nullable; fast tier, cond_len > 1, cond and w_ccls given)
  * [cond_len-1][B] f32: log p(cond[b][s+1]) under the cond classifier's logits of body token s, over the vocab_cond real classes.
  * Fast tier: the forward's passes, then the classifier in fixed chunks of rows, each chunk's logits (the forward's GEMM for those rows:
- * the forward's values) reduced in a bounded fp32 buffer of the workspace.  Exact tier: the teacher-forced replay of rqb200_ar_sample in
- * spans of positions whose logits fit a bounded buffer.  A code outside [0, vocab) gives NaN for its entry; each entry depends on its
- * own row's logits only, deterministically. */
+ * the forward's values) reduced in a bounded fp32 buffer of the workspace.  Exact tier: the teacher-forced replay of
+ * rqb200_ar_sample_span in spans of positions whose logits fit a bounded buffer.  A code outside [0, vocab) gives NaN for its entry;
+ * each entry depends on its own row's logits only, deterministically. */
 size_t rqb200_ar_log_prob_workspace_bytes(const rqb200_ar* h, int B);
 int rqb200_ar_log_prob(rqb200_ar* h, const int64_t* codes, const int64_t* cond, int B, float* logp_out, float* cond_logp_out,
                        void* workspace, size_t workspace_bytes, void* stream);
@@ -242,7 +231,7 @@ int rqb200_ar_log_prob(rqb200_ar* h, const int64_t* codes, const int64_t* cond, 
  * launch slot of the last graph replays to out_host[cap_launches][4] and the slot names ('\n'-separated) to names; returns the
  * number of slots (0 when tracing is off).  Synchronises the device. */
 int rqb200_ar_trace(rqb200_ar* h, long long* out_host, int cap_launches, char* names, int names_cap);
-/* number of kernels the last rqb200_ar_sample / _step / _forward call launched (bench.py's gpu_launches) */
+/* number of kernels the last rqb200_ar_sample_span / _step / _forward call launched (bench.py's gpu_launches) */
 int64_t rqb200_ar_last_launches(const rqb200_ar* h);
 
 /* ------------------------------------------------------------------------------------------------ P2

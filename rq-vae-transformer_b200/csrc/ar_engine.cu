@@ -166,14 +166,13 @@ static int head_depth(const rqb200_ar* h, const int64_t* codes, int B, int idx, 
 // positions [idx0, idx_end) of the raster; resume != 0: no prefill, continue on the caches / context left in this workspace.
 // cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s (the sampler forms the guided logits).
 // keep / sampled: the masked-sample plan of the fast tier (kernels.h), with one body step per appended code token.
+// B >= 1 and a span within the raster: rqb200_ar_sample_span checks them, ar_log_prob_impl forms them.
 static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx0, int idx_end, int resume,
                           float temperature, const int32_t* top_k, const float* top_p, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force, int64_t* out, void* wsp,
                           size_t ws_bytes, cudaStream_t st, int cfg_n, float cfg_s, const uint8_t* keep, const uint8_t* sampled) {
     const rqb200_ar_config& c = h->cfg;
     const int D = c.D, HW = c.H * c.W, V = c.vocab;
-    if (B <= 0) return fail(RQB200_EINVAL, "ar_sample: B must be > 0");
-    if (idx0 < 0 || idx_end > HW || idx0 > idx_end) return fail(RQB200_EINVAL, "ar_sample: bad position span");
     ArWs ws;
     size_t need = ar_layout(c, B, wsp, ws_bytes, &ws);
     if (need > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_sample: workspace too small");
@@ -339,73 +338,39 @@ size_t rqb200_ar_workspace_bytes(const rqb200_ar* h, int B) {
     if (h->fast) return rqb::ar_fast_workspace_bytes(h->fast, B);
     return rqb::ar_layout(h->cfg, B, nullptr, 0, nullptr);
 }
-}  // extern "C"
-
-// rqb200_ar_sample_span, _cfg and _keep: cfg_n = 0 unguided, else guided over B = 2 cfg_n rows; keep / sampled null: every token sampled
-static int ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
+// The only way into the sampling loop and the one place its arguments are checked, before any CUDA call; the tiers check only their
+// own batch and workspace limits.  cfg_n = 0 unguided, else guided over B = 2 cfg_n rows; keep / sampled_host null: every token sampled
+int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                           float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                          void* workspace, size_t workspace_bytes, void* stream, int cfg_n, float cfg_s, const uint8_t* keep,
-                          const uint8_t* sampled) {
+                          void* workspace, size_t workspace_bytes, void* stream, const uint8_t* keep, const uint8_t* sampled_host,
+                          int cfg_n, float cfg_scale) {
     if (!h || (!partial && !resume) || !out_codes || !top_k_host || !top_p_host || !workspace)
         return rqb::fail(RQB200_EINVAL, "ar_sample: null argument");
+    if (B < 1) return rqb::fail(RQB200_EINVAL, "ar_sample: B must be > 0");
+    if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n))
+        return rqb::fail(RQB200_EINVAL, "ar_sample: cfg_n must be 0, or n >= 1 with B = 2n rows (n conditional, then n unconditional)");
+    if (idx_begin < 0 || idx_end > h->cfg.H * h->cfg.W || idx_begin > idx_end)
+        return rqb::fail(RQB200_EINVAL, "ar_sample: bad position span");
+    if (sampled_host && !resume)
+        for (int p = 0; p < idx_begin; p++)
+            if (sampled_host[p]) return rqb::fail(RQB200_EINVAL, "ar_sample: sampled_host must be 0 before the call's first position");
     if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "ar_sample: no CUDA device");
     if (h->cfg.weight_dtype != RQB200_F32 && !h->fast) return rqb::fail(RQB200_EINVAL, "ar_sample: 16-bit weights need the fast tier");
-    if (sampled && !resume && idx_begin > 0 && idx_begin <= h->cfg.H * h->cfg.W)
-        for (int p = 0; p < idx_begin; p++)
-            if (sampled[p]) return rqb::fail(RQB200_EINVAL, "ar_sample_keep: sampled_host must be 0 before the call's first position");
+    const float cfg_s = cfg_n > 0 ? cfg_scale : 0.f;
     h->step_next = -1;                   // sampling reuses the caches a stepped sequence keeps: that sequence ends here
     rqb::g_launches = 0;
     int rc;
     if (h->fast)
         rc = rqb::ar_fast_sample(h->fast, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
                                  noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream,
-                                 cfg_n, cfg_s, keep, sampled);
+                                 cfg_n, cfg_s, keep, sampled_host);
     else
         rc = rqb::ar_sample_impl(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
                                  noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream,
-                                 cfg_n, cfg_s, keep, sampled);
+                                 cfg_n, cfg_s, keep, sampled_host);
     h->last_launches = rqb::g_launches;
     return rc;
-}
-
-extern "C" {
-int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
-                          float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
-                          int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                          void* workspace, size_t workspace_bytes, void* stream) {
-    return ar_sample_span(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise, noise_stride,
-                          logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, 0, 0.f, nullptr, nullptr);
-}
-int rqb200_ar_sample_span_cfg(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
-                              float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
-                              int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                              void* workspace, size_t workspace_bytes, void* stream, float cfg_scale) {
-    if (B < 2 || B % 2) return rqb::fail(RQB200_EINVAL, "ar_sample_cfg: B must be 2n rows (n conditional, then n unconditional), n >= 1");
-    return rqb200_ar_sample_span_keep(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
-                                      noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, nullptr,
-                                      nullptr, B / 2, cfg_scale);
-}
-int rqb200_ar_sample_span_keep(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
-                               float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
-                               int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                               void* workspace, size_t workspace_bytes, void* stream, const uint8_t* keep, const uint8_t* sampled_host,
-                               int cfg_n, float cfg_scale) {
-    if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n))
-        return rqb::fail(RQB200_EINVAL, "ar_sample_cfg: B must be 2n rows (n conditional, then n unconditional), n >= 1");
-    return ar_sample_span(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise, noise_stride,
-                          logits_out, force_codes, out_codes, workspace, workspace_bytes, stream, cfg_n, cfg_n > 0 ? cfg_scale : 0.f, keep,
-                          sampled_host);
-}
-int rqb200_ar_sample(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int start_h, int start_w,
-                     float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
-                     int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
-                     void* workspace, size_t workspace_bytes, void* stream) {
-    if (!h) return rqb::fail(RQB200_EINVAL, "ar_sample: null argument");
-    if (start_h < 0 || start_w < 0 || start_w >= h->cfg.W || start_h > h->cfg.H) return rqb::fail(RQB200_EINVAL, "ar_sample: bad start_loc");
-    const int HW = h->cfg.H * h->cfg.W;
-    return rqb200_ar_sample_span(h, partial, cond, B, std::min(start_h * h->cfg.W + start_w, HW), HW, 0, temperature, top_k_host,
-                                 top_p_host, noise, noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, stream);
 }
 int rqb200_ar_step(rqb200_ar* h, const int64_t* xs, int64_t xs_batch_stride, const int64_t* cond, int B, int pos_h, int pos_w,
                    int d, int restart, float* logits_out, void* workspace, size_t workspace_bytes, void* stream) {
@@ -448,7 +413,7 @@ int rqb200_ar_forward(rqb200_ar* h, const int64_t* codes, const int64_t* cond, i
                       void* workspace, size_t workspace_bytes, void* stream) {
     if (!h || !codes || !logits_out || !workspace) return rqb::fail(RQB200_EINVAL, "ar_forward: null argument");
     if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "ar_forward: no CUDA device");
-    if (!h->fast) return rqb::fail(RQB200_EINVAL, "ar_forward: the batched forward is a fast-tier path (exact tier: teacher-forced rqb200_ar_sample)");
+    if (!h->fast) return rqb::fail(RQB200_EINVAL, "ar_forward: the batched forward is a fast-tier path (exact tier: teacher-forced rqb200_ar_sample_span)");
     rqb::g_launches = 0;
     int rc = rqb::ar_fast_forward(h->fast, codes, cond, B, logits_out, cond_logits_out, workspace, workspace_bytes, (cudaStream_t)stream);
     h->last_launches = rqb::g_launches;

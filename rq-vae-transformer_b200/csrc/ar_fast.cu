@@ -1582,9 +1582,7 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
                    float cfg_s, const uint8_t* keep, const uint8_t* sampled) {
     const rqb200_ar_config& c = f->cfg;
     const int D = c.D, HW = c.H * c.W, cl = c.cond_len;
-    if (B < 1 || B > 256) return fail(RQB200_EINVAL, "ar fast tier: batch must be in [1,256] per call");
-    if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n)) return fail(RQB200_EINVAL, "ar_sample: a guided call takes B = 2 cfg_n rows");
-    if (idx_begin < 0 || idx_end > HW || idx_begin > idx_end) return fail(RQB200_EINVAL, "ar_sample: bad position span");
+    if (B > 256) return fail(RQB200_EINVAL, "ar fast tier: batch must be in [1,256] per call");
     FastWs ws;
     size_t need = fast_layout(*f, B, wsp, ws_bytes, &ws);
     if (need > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_sample: workspace too small");

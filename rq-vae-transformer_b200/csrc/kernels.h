@@ -149,7 +149,7 @@ struct StepState {
     float top_p[8];
 };
 
-// The position plan of a masked sample (rqb200_ar_sample_span_keep): sampled[p] != 0 when some row samples some depth of position p;
+// The position plan of a masked sample (rqb200_ar_sample_span): sampled[p] != 0 when some row samples some depth of position p;
 // sampled == NULL samples every position.  Only sampled positions run the head stack, classifier and sampler; the body consumes the
 // code tokens of the positions between two sampled ones right before the later one's head (positions after the last sampled one
 // are never consumed).
@@ -169,7 +169,7 @@ void ar_fast_destroy(ArFast* f);
 size_t ar_fast_workspace_bytes(const ArFast* f, int B);
 // positions [idx_begin, idx_end) of the raster; resume != 0: continue on the KV state the previous call left in this workspace.
 // cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s.  keep / sampled: the masked-sample
-// plan (null: every token sampled)
+// plan (null: every token sampled).  Arguments already checked by rqb200_ar_sample_span, except B <= 256 and the workspace size.
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
                    float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st, int cfg_n,

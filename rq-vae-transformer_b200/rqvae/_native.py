@@ -89,14 +89,10 @@ def lib():
     L.rqb200_ar_destroy.restype = None
     L.rqb200_ar_workspace_bytes.restype = C.c_size_t
     L.rqb200_ar_workspace_bytes.argtypes = [C.c_void_p, C.c_int]
-    L.rqb200_ar_sample.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
-                                   C.POINTER(C.c_int32), C.POINTER(C.c_float), C.c_void_p, C.c_int64, C.c_void_p,
-                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.rqb200_ar_sample_span.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                         C.POINTER(C.c_int32), C.POINTER(C.c_float), C.c_void_p, C.c_int64, C.c_void_p,
-                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    L.rqb200_ar_sample_span_cfg.argtypes = L.rqb200_ar_sample_span.argtypes + [C.c_float]
-    L.rqb200_ar_sample_span_keep.argtypes = L.rqb200_ar_sample_span.argtypes + [C.c_void_p, C.c_void_p, C.c_int, C.c_float]
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_int, C.c_float]
     L.rqb200_ar_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.rqb200_ar_forward_workspace_bytes.restype = C.c_size_t
@@ -144,7 +140,7 @@ def lib():
 
 EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200_rq_quantize", "rqb200_rq_embed_sum",
            "rqb200_rq_embed_depth", "rqb200_rq_soft_codes", "rqb200_sample_logits", "rqb200_ar_create", "rqb200_ar_destroy",
-           "rqb200_ar_workspace_bytes", "rqb200_ar_sample", "rqb200_ar_sample_span", "rqb200_ar_sample_span_cfg", "rqb200_ar_sample_span_keep", "rqb200_ar_step", "rqb200_ar_forward",
+           "rqb200_ar_workspace_bytes", "rqb200_ar_sample_span", "rqb200_ar_step", "rqb200_ar_forward",
            "rqb200_ar_forward_workspace_bytes", "rqb200_ar_trace", "rqb200_ar_last_launches", "rqb200_vae_create",
            "rqb200_vae_destroy", "rqb200_vae_set_tensor", "rqb200_vae_finalize", "rqb200_vae_workspace_bytes",
            "rqb200_vae_decode", "rqb200_vae_decode_code", "rqb200_vae_encode", "rqb200_vae_last_launches",

@@ -5,7 +5,7 @@ Boundary kept (SURVEY.md section 8b): constructor from an ``RQTransformerConfig`
 ``cached_forward`` :191 (stateful after ``init_cache``: one native token step per call, ``rqb200_ar_step``), ``init_cache`` :289, ``get_block_size``, attributes ``block_size`` / ``block_size_cond`` /
 ``vocab_size``, the losses ``compute_loss`` / ``compute_cond_loss`` / ``compute_codebook_loss`` :371-410, and ``log_prob`` (teacher-forced
 log-likelihoods without the logits, ``rqb200_ar_log_prob``).  The (h,w,d) loop, KV caches, embedding glue, classifier and ``sample_from_logits`` all run inside
-``rqb200_ar_sample`` (csrc/ar_engine.cu): one native call per ``sample``, no per-token host work.
+``rqb200_ar_sample_span`` (csrc/ar_engine.cu): one native call per batch chunk and span of positions, no per-token host work.
 
 Arithmetic tiers: ``amp=False`` -> 'exact' (fp32 weights/activations, FFMA -- the tier the bit-exact-indices gate is
 defined on); ``amp=True`` -> 'fast' (fp16 weights / activations / KV on wgmma tensor cores, fp32 accumulate -- the
@@ -400,9 +400,9 @@ class RQTransformer(Stage2Model):
     def _native_sample(self, partial, model_aux, cond, start_loc, temperature, top_k, top_p, amp, noise=None,
                        return_logits=False, force_codes=None, guidance=None, keep=None):
         """guidance: None, or (s, uncond [B, cond_len] int64) from _guidance -- classifier-free guidance: every image runs a cond and an
-        uncond branch as rows [cond | uncond] of one native call (rqb200_ar_sample_span_cfg), noise stays per image [n_tok, B, V],
+        uncond branch as rows [cond | uncond] of one native call (cfg_n = rows / 2), noise stays per image [n_tok, B, V],
         logits (return_logits) and force_codes hold both branches' rows [2B]: [cond rows | uncond rows].
-        keep: None, or uint8 [B, H, W, D] from _keep_mask -- masked completion (rqb200_ar_sample_span_keep): each batch chunk passes its
+        keep: None, or uint8 [B, H, W, D] from _keep_mask -- masked completion (keep, sampled_host): each batch chunk passes its
         rows of the mask (guided: in both branches' rows) and the positions where any of its rows samples any depth; those position
         lists are formed on the device and read to the host once per call.  The logits of positions a chunk skips are not written."""
         H, W, D = self.block_size
@@ -444,6 +444,7 @@ class RQTransformer(Stage2Model):
                 calls = [(2 * (hi - lo), torch.cat([partial[lo:hi], partial[lo:hi]]), torch.cat([cu[lo:hi], u[lo:hi]]),
                           None if fc is None else torch.cat([fc[lo:hi], fc[B + lo:B + hi]]),
                           torch.empty(2 * (hi - lo), H, W, D, dtype=torch.int64, device=dev)) for lo, hi in bounds]
+            plans = [(None, None)] * len(bounds)                    # per chunk: (sampled_host, keep rows), NULL unless masked
             if keep is not None:
                 HW = H * W
                 sampled = torch.stack([(keep[lo:hi] == 0).reshape(hi - lo, HW, D).any(2).any(0) for lo, hi in bounds])
@@ -478,19 +479,12 @@ class RQTransformer(Stage2Model):
                         noise[t].exponential_(1)
                 tok0 = 0 if draw else (p0 - idx0) * D                  # first token of this span inside `noise`
                 for i, (eng, (lo, hi), (rows, part_c, cond_c, fc_c, out_c)) in enumerate(zip(engines, bounds, calls)):
-                    args = (eng["handle"], off(part_c, 0, HWD, 8), off(cond_c, 0, cl, 8), rows, p0, p1, int(p0 > idx0),
-                            float(temperature), kk, pp, off(noise, lo, V, 4, tok0 * B * V), 0 if noise is None else B * V,
-                            off(logits, 0, V, 4, (p0 - idx0) * D * R * V), off(fc_c, 0, HWD, 8), off(out_c, 0, HWD, 8),
-                            N.ptr(eng["ws"]), eng["ws"].numel(), C.c_void_p(st.cuda_stream))
-                    if keep is not None:
-                        N.check(N.lib().rqb200_ar_sample_span_keep(*args, N.ptr(plans[i][1]), plans[i][0],
-                                                                   0 if guidance is None else rows // 2,
-                                                                   C.c_float(0.0 if guidance is None else guidance[0])),
-                                "ar_sample_keep")
-                    elif guidance is None:
-                        N.check(N.lib().rqb200_ar_sample_span(*args), "ar_sample")
-                    else:
-                        N.check(N.lib().rqb200_ar_sample_span_cfg(*args, C.c_float(guidance[0])), "ar_sample_cfg")
+                    N.check(N.lib().rqb200_ar_sample_span(
+                        eng["handle"], off(part_c, 0, HWD, 8), off(cond_c, 0, cl, 8), rows, p0, p1, int(p0 > idx0),
+                        float(temperature), kk, pp, off(noise, lo, V, 4, tok0 * B * V), 0 if noise is None else B * V,
+                        off(logits, 0, V, 4, (p0 - idx0) * D * R * V), off(fc_c, 0, HWD, 8), off(out_c, 0, HWD, 8),
+                        N.ptr(eng["ws"]), eng["ws"].numel(), C.c_void_p(st.cuda_stream), N.ptr(plans[i][1]), plans[i][0],
+                        0 if guidance is None else rows // 2, C.c_float(0.0 if guidance is None else guidance[0])), "ar_sample")
                     launches += N.lib().rqb200_ar_last_launches(eng["handle"])
             if n_tok == 0:
                 out.copy_(partial)

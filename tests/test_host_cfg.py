@@ -1,6 +1,7 @@
-"""Classifier-free guidance on the host: the entry point is declared, exported and bound, sample() refuses bad guidance arguments with
-ValueError before anything reaches a device, the native entry refuses an odd row count before any CUDA call, and a guided fast-tier
-call is split into equal chunks of at most 128 images."""
+"""Classifier-free guidance on the host: the one sampling entry point is declared, exported and bound with its guidance arguments, the
+entry points it replaced are gone, sample() refuses bad guidance arguments with ValueError before anything reaches a device, the native
+entry refuses a row count that is not 2 cfg_n before any CUDA call, and a guided fast-tier call is split into equal chunks of at most
+128 images."""
 import ctypes as C
 import os
 import re
@@ -13,16 +14,26 @@ from rqvae.models.rqtransformer.transformers import _chunk_bounds
 from tests.test_host_cpu import make_ar
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+SPAN = "rqb200_ar_sample_span"
+PREFIX = SPAN[:-len("_span")]
+# the entry points rqb200_ar_sample_span replaced: the start_loc form, the guided form and the masked form
+REMOVED = (PREFIX, SPAN + "_cfg", SPAN + "_keep")
 
 
-def test_cfg_entry_is_declared_exported_and_bound():
+def test_sample_span_is_the_one_sampling_entry_and_takes_guidance():
     hdr = open(os.path.join(ROOT, "include", "rqb200.h")).read()
-    assert re.search(r"\bint rqb200_ar_sample_span_cfg\s*\(", hdr)
-    assert "rqb200_ar_sample_span_cfg" in N.EXPORTS
-    assert hasattr(C.CDLL(N.LIB_PATH), "rqb200_ar_sample_span_cfg")
+    assert re.search(r"\bint %s\s*\(" % SPAN, hdr)
+    assert SPAN in N.EXPORTS
+    so = C.CDLL(N.LIB_PATH)
+    assert hasattr(so, SPAN)
     L = N.lib()
-    assert L.rqb200_ar_sample_span_cfg.argtypes == L.rqb200_ar_sample_span.argtypes + [C.c_float]
-    assert L.rqb200_version() >= 111
+    argtypes = getattr(L, SPAN).argtypes
+    assert len(argtypes) == 22 and argtypes[-4:] == [C.c_void_p, C.c_void_p, C.c_int, C.c_float]     # keep, sampled_host, cfg_n, cfg_scale
+    assert set(re.findall(r"\b(%s\w*)\s*\(" % PREFIX, hdr)) == {SPAN}
+    assert {n for n in N.EXPORTS if n.startswith(PREFIX)} == {SPAN}
+    for name in REMOVED:
+        assert not hasattr(so, name), name
+    assert L.rqb200_version() >= 113
 
 
 def _errors(model, B, cl):
@@ -65,7 +76,8 @@ def test_guided_chunks_hold_at_most_128_images():
     assert _chunk_bounds(300, N.MODE_FAST) == [(0, 150), (150, 300)]        # unguided: unchanged
 
 
-def test_cfg_entry_refuses_an_odd_row_count_before_any_cuda_call():
+def test_sample_span_refuses_rows_other_than_2_cfg_n_before_any_cuda_call():
+    """B must be 2 cfg_n rows when cfg_n > 0, and cfg_n >= 0: refused with EINVAL before the device is looked at (no GPU here)"""
     torch.manual_seed(0)
     model = make_ar("tiny")
     cfg, w, keep, _ = model._engine_structs(torch.randn(model.vocab_size[0], 256), N.MODE_EXACT)
@@ -75,9 +87,10 @@ def test_cfg_entry_refuses_an_odd_row_count_before_any_cuda_call():
     try:
         kk, pp = (C.c_int32 * 4)(*[512] * 4), (C.c_float * 4)(*[1.0] * 4)
         buf = C.create_string_buffer(64)
-        for B in (0, 1, 3):
-            rc = L.rqb200_ar_sample_span_cfg(h, buf, None, B, 0, 16, 0, 1.0, kk, pp, None, 0, None, None, buf, buf, 64, None,
-                                             C.c_float(1.5))
-            assert rc == N.EINVAL and "2n rows" in L.rqb200_last_error().decode(), B
+        for B, cfg_n in ((0, 1), (1, 1), (3, 1), (4, 1), (2, -1)):
+            rc = L.rqb200_ar_sample_span(h, buf, None, B, 0, 16, 0, 1.0, kk, pp, None, 0, None, None, buf, buf, 64, None, None, None,
+                                         cfg_n, C.c_float(1.5))
+            assert rc == N.EINVAL, (B, cfg_n)
+            assert B < 1 or "2n rows" in L.rqb200_last_error().decode(), (B, cfg_n)
     finally:
         L.rqb200_ar_destroy(h)

@@ -13,14 +13,14 @@ from tests.test_host_cpu import make_ar
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_keep_entries_are_declared_exported_and_bound():
+def test_sample_span_takes_the_keep_arguments_and_append_attn_is_bound():
     hdr = open(os.path.join(ROOT, "include", "rqb200.h")).read()
     L = N.lib()
-    for name in ("rqb200_ar_sample_span_keep", "rqb200_dbg_append_attn"):
+    for name in ("rqb200_ar_sample_span", "rqb200_dbg_append_attn"):
         assert re.search(r"\bint %s\s*\(" % name, hdr)
         assert name in N.EXPORTS
         assert hasattr(C.CDLL(N.LIB_PATH), name)
-    assert L.rqb200_ar_sample_span_keep.argtypes == L.rqb200_ar_sample_span.argtypes + [C.c_void_p, C.c_void_p, C.c_int, C.c_float]
+    assert L.rqb200_ar_sample_span.argtypes[-4:] == [C.c_void_p, C.c_void_p, C.c_int, C.c_float]     # keep, sampled_host, cfg_n, cfg_scale
     assert L.rqb200_version() >= 112
 
 
