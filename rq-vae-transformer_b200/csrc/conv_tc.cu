@@ -11,10 +11,12 @@
 //       which IS the conv's zero padding; no im2col buffer.
 //   N = BN output channels (16 | 64 | 128 | 256), K = taps x Cin walked in 64-channel slabs (one 128 B swizzled row per pixel).
 //
-// Two kernels share the layout and the epilogue:
-//   conv3x3_tc_kernel  every 3x3 stride-1 conv.  Input-stationary within a channel slab: ONE TMA box brings the 8 x TH x NB
-//                      tile plus its one-pixel halo, and the nine taps read it as shifted wgmma operands; only the weight
-//                      slabs stream through the ring (see the comment above the kernel).
+// Three kernels share the layout and the epilogue:
+//   conv3x3_wreg_kernel  3x3 stride-1 convs with Cout % 128 == 0, the GEMM transposed: 128 output channels on the wgmma M side
+//                      with the weight fragments in registers, 256 output pixels on N (see the comment above the kernel).
+//   conv3x3_tc_kernel  the other 3x3 stride-1 convs (conv_out, Cout = 3; Cout = 64).  Input-stationary within a channel slab: ONE
+//                      TMA box brings the 8 x TH x NB tile plus its one-pixel halo, and the nine taps read it as shifted wgmma
+//                      operands; only the weight slabs stream through the ring (see the comment above the kernel).
 //   conv_tc_kernel     1x1 convs, the encoder's stride-2 convs and the rows GEMM: one activation box and one weight slab per
 //                      (tap, slab) k block.
 //
@@ -105,7 +107,9 @@ __device__ __forceinline__ void gn_chunk_stats(const float (&wv)[16], bool valid
 }
 
 // Epilogue of one thread: tile row r (one output pixel), output channels [n0, n0 + 16) in v.  Warp q of the four that share a column
-// half holds the tile's pixels [32 q, 32 q + 32) -- the layout the GroupNorm partial statistics are formed over.
+// half holds the tile's pixels [32 q, 32 q + 32) -- the layout the GroupNorm partial statistics are formed over.  OUT16: the rows
+// GEMM's 16-bit output is possible (conv_tc_kernel); the 3x3 kernels never have it.
+template <bool OUT16>
 __device__ __forceinline__ void ct_epilogue16(const ConvTcParams& p, const float (&v)[16], int n0, int q, int lane, int tx, int ty, int tb,
                                               int b, int y, int x, int64_t pix, bool valid) {
     if (n0 >= p.Cout) return;                                           // (warp-uniform)
@@ -116,7 +120,7 @@ __device__ __forceinline__ void ct_epilogue16(const ConvTcParams& p, const float
             const int n = n0 + i;
             if (n < p.Cout) p.out[(((int64_t)b * p.Cout + n) * p.H + y) * p.W + x] = v[i] + p.bias[n];
         }
-    } else if (p.out16 != nullptr) {
+    } else if (OUT16 && p.out16 != nullptr) {
         if (!valid) return;
         float w[16];
 #pragma unroll
@@ -275,7 +279,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
         const bool valid = (x < p.W) && (y < p.H) && (b < p.B) && (p.m_rows == 0 || pix < p.m_rows);
         tc::drain_acc<BN, CW, 0>(acc, stage, wg, t, [&p, t, nt, tx, ty, tb, b, y, x, pix, valid](const float (&v)[16], int, int c) {
-            ct_epilogue16(p, v, nt * BN + c, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
+            ct_epilogue16<true>(p, v, nt * BN + c, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
         });
     }
 }
@@ -300,9 +304,8 @@ static int launch_conv_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
 // stride (SBO): a shifted descriptor, no reload.  Only the weight slabs [BN x 64] of the nine taps stream through the ring.
 // k order: slab-major, tap-minor.
 //
-// L2 -> smem bytes per 64-channel slab and 128-pixel tile (hi + lo operands): 46 KB halo + 9 x 32 KB weights at BN = 128 ->
-// 166 flop/B, against 96 flop/B (Cout = 128) and 128 flop/B (Cout >= 256, BN = 256) for per-tap A + W reloads; conv_out
-// (BN = 16, Cout = 3): 46 KB + 9 x 4 KB -> 85 flop/B of wgmma work (was 21).
+// L2 -> smem bytes per 64-channel slab and 128-pixel tile (hi + lo operands), conv_out (BN = 16, Cout = 3): 46 KB halo + 9 x 4 KB
+// weights -> 85 flop/B of wgmma work, against 21 for per-tap A + W reloads.
 constexpr int C3_HALO_BYTES = 10 * 10 * 2 * 128;   // per operand; the largest box (TH = 8, NB = 2: 200 pixels; TH = 16: 180)
 
 template <int BN, int FMT, int PASSES>
@@ -322,6 +325,46 @@ __device__ __forceinline__ void c3_mma_kblock(float (&acc)[BN / 2], uint32_t a, 
     for (int j = 0; j < 4; j++)
         tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32, SBO), tc::gmma_desc_k128(b + j * 32),
                                 (PASSES == 3 || !first || j > 0) ? 1u : 0u);
+}
+
+// TMA producer of both 3x3 kernels (one thread): per 64-channel slab ONE halo box (hi [+ lo]) into the next of two halo slots,
+// per tap one [BM x 64] weight slab (hi [+ lo]) into the STAGES-deep ring.  Runs ahead across tiles, so the next tile's operands
+// load during this tile's epilogue.  Halo slot: [X_hi | X_lo], HALO_BYTES apart; weight stage: [W_hi | W_lo], BM x 128 B apart.
+template <int BM, int STAGES, int PASSES, int SLOT_BYTES, int HALO_BYTES>
+__device__ __forceinline__ void c3_produce(const CUtensorMap* tmA, const CUtensorMap* tmB, const CUtensorMap* tmAlo, const CUtensorMap* tmBlo,
+                                           const ConvTcParams& p, uint8_t* smem, uint8_t* wst, uint64_t* full, uint64_t* empty,
+                                           uint64_t* hfull, uint64_t* hempty) {
+    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr int B_BYTES = BM * 64 * 2;
+    constexpr int STAGE_BYTES = NOPS * B_BYTES;
+    const int cslabs = p.Cin / 64;
+    const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
+    const uint32_t halo_tx = NOPS * 10 * (p.TH + 2) * p.NB * 128;
+    uint32_t it = 0, hit = 0;                          // running weight-stage / halo counters across tiles
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+        const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
+        const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
+        const int x0 = tx * 8, y0 = ty * p.TH, b0 = tb * p.NB;
+        for (int sl = 0; sl < cslabs; sl++, hit++) {
+            const int c0 = sl * 64;
+            for (int tap = 0; tap < 9; tap++, it++) {
+                const int s = it % STAGES;
+                tc::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+                tc::mbar_expect_tx(&full[s], STAGE_BYTES);
+                uint8_t* w = wst + s * STAGE_BYTES;
+                tc::tma_load_2d(w, tmB, &full[s], tap * p.Cin + c0, nt * BM, tc::L2_EVICT_LAST);
+                if (PASSES == 3) tc::tma_load_2d(w + B_BYTES, tmBlo, &full[s], tap * p.Cin + c0, nt * BM, tc::L2_EVICT_LAST);
+                if (tap == 0) {                        // the slab's first weights go out before the wait for a halo slot
+                    const int h = hit % 2;
+                    tc::mbar_wait(&hempty[h], ((hit / 2) & 1) ^ 1);
+                    tc::mbar_expect_tx(&hfull[h], halo_tx);
+                    uint8_t* a = smem + h * SLOT_BYTES;
+                    tc::tma_load_4d(a, tmA, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
+                    if (PASSES == 3) tc::tma_load_4d(a + HALO_BYTES, tmAlo, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
+                }
+            }
+        }
+    }
 }
 
 // Two halo slots (the next slab's halo loads during this slab's taps) and STAGES weight stages.
@@ -361,34 +404,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     __syncthreads();
 
     if (warp == 8) {
-        if (lane == 0) {
-            const uint32_t halo_tx = NOPS * 10 * (p.TH + 2) * p.NB * 128;
-            uint32_t it = 0, hit = 0;                          // running weight-stage / halo counters across tiles
-            for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-                const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
-                const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
-                const int x0 = tx * 8, y0 = ty * p.TH, b0 = tb * p.NB;
-                for (int sl = 0; sl < cslabs; sl++, hit++) {
-                    const int c0 = sl * 64;
-                    for (int tap = 0; tap < 9; tap++, it++) {
-                        const int s = it % STAGES;
-                        tc::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
-                        tc::mbar_expect_tx(&full[s], STAGE_BYTES);
-                        uint8_t* w = wst + s * STAGE_BYTES;
-                        tc::tma_load_2d(w, &tmB, &full[s], tap * p.Cin + c0, nt * BN, tc::L2_EVICT_LAST);
-                        if (PASSES == 3) tc::tma_load_2d(w + B_BYTES, &tmBlo, &full[s], tap * p.Cin + c0, nt * BN, tc::L2_EVICT_LAST);
-                        if (tap == 0) {                        // the slab's first weights go out before the wait for a halo slot
-                            const int h = hit % HSLOTS;
-                            tc::mbar_wait(&hempty[h], ((hit / HSLOTS) & 1) ^ 1);
-                            tc::mbar_expect_tx(&hfull[h], halo_tx);
-                            uint8_t* a = smem + h * SLOT_BYTES;
-                            tc::tma_load_4d(a, &tmA, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
-                            if (PASSES == 3) tc::tma_load_4d(a + C3_HALO_BYTES, &tmAlo, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
-                        }
-                    }
-                }
-            }
-        }
+        if (lane == 0) c3_produce<BN, STAGES, PASSES, SLOT_BYTES, C3_HALO_BYTES>(&tmA, &tmB, &tmAlo, &tmBlo, p, smem, wst, full, empty, hfull, hempty);
         return;
     }
 
@@ -435,7 +451,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
         const bool valid = (x < p.W) && (y < p.H) && (b < p.B);
         tc::drain_acc<BN, CW, 0>(acc, stage, wg, t, [&p, t, nt, tx, ty, tb, b, y, x, pix, valid](const float (&v)[16], int, int c) {
-            ct_epilogue16(p, v, nt * BN + c, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
+            ct_epilogue16<false>(p, v, nt * BN + c, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
         });
     }
 }
@@ -452,6 +468,252 @@ static int launch_conv3x3_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, c
     const int grid = total < n_sm ? total : n_sm;
     conv3x3_tc_kernel<BN, STAGES, PASSES><<<grid, CT_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
     return check_launch("conv3x3_tc");
+}
+
+// ------------------------------------------------------------------------------------------------ 3x3 stride-1 convs, Cout % 128 == 0
+// The GEMM transposed: D[cout, pixel] = sum_{slab, tap, c} W[cout, tap, c] X[pixel + tap, c].
+//   M = 128 output channels per tile, 64 per consumer warpgroup.  Each warpgroup ldmatrix-es its W_hi / W_lo fragments of a tap
+//       out of the weight ring and issues register-A wgmma, so the weights cross shared memory once per tap, not once per product.
+//   N = the tile's output pixels in the shared-memory operand: 8 wide x TH rows of NB images (TH = 32 on maps of 32 rows or more:
+//       N = 256; TH = 16: 128; TH = 8, NB = 2: 2 x 64), one wgmma per image.  The halo trick of conv3x3_tc_kernel is unchanged:
+//       one core-matrix group is one 8-pixel output row, 1280 B apart, a tap is a start-address shift, and the TMA's
+//       out-of-bounds fill is the zero padding.
+// Split-fp16 products per k16: W_hi X_lo, W_lo X_hi, W_hi X_hi -- only X is read from shared memory, ~64 B/clk of operand reads at
+// the fp16 rate against ~94 for the pixel-major SS form.  k order (slab-major, tap-minor) and the small-terms-first order of
+// conv3x3_tc_kernel are kept.
+// smem at TH = 32 (PASSES = 3): two halo slots of 2 x 43 KB, ONE 32 KB weight stage, a 16.5 KB epilogue staging buffer and 2 KB of
+// GroupNorm partial sums = 223 KB.
+// The single weight stage is enough because a warpgroup holds two taps' fragments in registers: the producer refills the stage
+// as soon as both warpgroups have loaded tap t, while tap t - 1's and tap t's MMAs run.
+template <int TH, int NB>
+struct C3wTile {
+    static constexpr int NI = 8 * TH;                                          // pixels per wgmma: TH rows of one image
+    static constexpr int NP = NI * NB;                                         // pixels per tile
+    static constexpr int HALO = (10 * (TH + 2) * NB * 128 + 1023) / 1024 * 1024;   // bytes per halo operand (1024 B aligned)
+};
+constexpr int C3W_SP = 128 + 4;                    // epilogue staging row (one pixel, 128 output channels) in floats
+// warps 0-7: two consumer warpgroups, warp 8: TMA producer; warps 9-11 idle.  A whole producer warpgroup lets setmaxnreg move its
+// registers to the consumers (128 accumulators + two taps' fragments per thread): ptxas sizes a wgmma kernel's register budget
+// in warpgroups, so 288 threads would leave 168 registers per thread, as 384 do.  setmaxnreg.inc waits until the CTA's pool (the
+// 168 x 384 registers it was launched with) can grant the increase, so the split must fit that pool.
+constexpr int C3W_THREADS = 384, C3W_REGS_CONSUMER = 240, C3W_REGS_PRODUCER = 24;
+static_assert(256 * C3W_REGS_CONSUMER + 128 * C3W_REGS_PRODUCER <= 168 * C3W_THREADS, "conv3x3_wreg: register split exceeds the pool");
+
+template <int TH, int NB, int FMT, int PASSES>
+__device__ __forceinline__ void c3w_mma_kblock(float (&acc)[C3wTile<TH, NB>::NP / 2], const uint32_t (&fh)[4][4],
+                                               const uint32_t (&fl)[4][4], uint32_t x, bool first) {
+    constexpr int NI = C3wTile<TH, NB>::NI, HALO = C3wTile<TH, NB>::HALO;
+    constexpr uint32_t SBO = 10 * 128, IMG = (TH + 2) * 10 * 128;
+    auto mma = [&acc](const uint32_t (&a)[4], uint32_t xa, uint32_t accumulate) {
+#pragma unroll
+        for (int b = 0; b < NB; b++)
+            tc::WgmmaRA<NI, FMT>::mma(*reinterpret_cast<float(*)[NI / 2]>(&acc[b * (NI / 2)]), a, tc::gmma_desc_k128(xa + b * IMG, SBO),
+                                      accumulate);
+    };
+    if (PASSES == 3) {                                 // small terms first, the dominant product last
+#pragma unroll
+        for (int j = 0; j < 4; j++) mma(fh[j], x + HALO + j * 32, (!first || j > 0) ? 1u : 0u);
+#pragma unroll
+        for (int j = 0; j < 4; j++) mma(fl[j], x + j * 32, 1u);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; j++) mma(fh[j], x + j * 32, (PASSES == 3 || !first || j > 0) ? 1u : 0u);
+}
+
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+
+// smem: [halo slot: X_hi | X_lo] x 2, [W_hi | W_lo] x STAGES (128 rows x 128 B each, SWIZZLE_128B), epilogue staging, barriers.
+template <int TH, int NB, int STAGES, int FMT, int PASSES>
+__global__ void __launch_bounds__(C3W_THREADS, 1)
+conv3x3_wreg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, ConvTcParams p) {
+    using T = C3wTile<TH, NB>;
+    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr int SLOT_BYTES = NOPS * T::HALO;
+    constexpr int B_BYTES = 128 * 128;
+    constexpr int STAGE_BYTES = NOPS * B_BYTES;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* wst = smem + 2 * SLOT_BYTES;
+    float* stage = reinterpret_cast<float*>(wst + STAGES * STAGE_BYTES);          // [32 pixels][C3W_SP]
+    float2* gnred = reinterpret_cast<float2*>(stage + 32 * C3W_SP);               // [8 warps][32 lanes] GroupNorm partial sums
+    uint64_t* full = reinterpret_cast<uint64_t*>(gnred + 256);
+    uint64_t* empty = full + STAGES;
+    uint64_t* hfull = empty + STAGES;
+    uint64_t* hempty = hfull + 2;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nkb = 9 * (p.Cin / 64);
+    const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
+
+    if (warp == 8 && lane == 0) {
+        tc::prefetch_tmap(&tmA);
+        tc::prefetch_tmap(&tmB);
+        // empty[s] / hempty[h]: one arrival per consumer warp -- empty once its fragments are in registers, hempty once its
+        // warpgroup's MMAs reading the halo have completed
+        for (int s = 0; s < STAGES; s++) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 8); }
+        for (int h = 0; h < 2; h++) { tc::mbar_init(&hfull[h], 1); tc::mbar_init(&hempty[h], 8); }
+        tc::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp >= 8) {
+        tc::setmaxnreg_dec<C3W_REGS_PRODUCER>();
+        if (warp == 8 && lane == 0)
+            c3_produce<128, STAGES, PASSES, SLOT_BYTES, T::HALO>(&tmA, &tmB, &tmAlo, &tmBlo, p, smem, wst, full, empty, hfull, hempty);
+        return;
+    }
+    tc::setmaxnreg_inc<C3W_REGS_CONSUMER>();
+
+    // ---- consumer warpgroups 0, 1: output channels [64 wg, 64 wg + 64) of the tile, all NP pixels
+    const int wg = warp >> 2;
+    // ldmatrix.x4 of the m64k16 A fragment: lane l addresses row 16 (warp % 4) + l % 8 + 8 ((l / 8) % 2) of this warpgroup's 64,
+    // 16 B chunk l / 16 + 2 j (k16 step j) of the 128 B swizzled row, stored at chunk (l / 16 + 2 j) ^ (row % 8) -- the byte
+    // offset of step j is lofs ^ 32 j (stages are 1024 B aligned)
+    const uint32_t lofs = (64 * wg + 16 * (warp & 3) + (lane & 7) + 8 * ((lane >> 3) & 1)) * 128 + (((lane >> 4) ^ (lane & 7)) << 4);
+    const uint32_t halo0 = tc::smem_u32(smem), wst0 = tc::smem_u32(wst);
+
+    float acc[T::NP / 2];
+#pragma unroll
+    for (int i = 0; i < T::NP / 2; i++) acc[i] = 0.f;
+    uint32_t frag[2][2][4][4];                          // [tap parity][hi, lo][k16 step][register]
+    uint32_t it = 0, hit = 0;
+    // one k block (tap): fragments of tap kb into frag[F] (their previous reader, tap kb - 2, has completed), MMAs issued, then
+    // wait until tap kb - 1 has completed
+    auto kblock = [&](int kb, uint32_t (&fr)[2][4][4]) {
+        const int tap = kb % 9;
+        if (tap == 0) tc::mbar_wait(&hfull[hit % 2], (hit / 2) & 1);
+        const int s = it % STAGES;
+        tc::mbar_wait(&full[s], (it / STAGES) & 1);
+        const uint32_t w = wst0 + s * STAGE_BYTES + lofs;
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            ldsm_x4(fr[0][j], w ^ (32 * j));
+            if (PASSES == 3) ldsm_x4(fr[1][j], (w + B_BYTES) ^ (32 * j));
+        }
+        const uint32_t x = halo0 + (hit % 2) * SLOT_BYTES + ((tap / 3) * 10 + tap % 3) * 128;
+        tc::wgmma_fence();
+        c3w_mma_kblock<TH, NB, FMT, PASSES>(acc, fr[0], fr[1], x, kb == 0);
+        tc::wgmma_commit();
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&empty[s]);       // the wgmmas above have read the fragments: the stage is free
+        tc::wgmma_wait<1>();
+        if (tap == 0 && kb > 0 && lane == 0) tc::mbar_arrive(&hempty[(hit - 1) % 2]);   // the previous slab's last tap is complete
+        it++;
+        if (tap == 8) hit++;
+    };
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+        for (int kb = 0; kb < nkb; kb += 2) {
+            kblock(kb, frag[0]);
+            if (kb + 1 < nkb) kblock(kb + 1, frag[1]);
+        }
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc);
+        if (lane == 0) tc::mbar_arrive(&hempty[(hit - 1) % 2]);
+
+        // ---- epilogue, 32 pixels at a time through the staging buffer: consumer warp w (0..7) <-> pixels w, w + 8, w + 16, w + 24 of
+        // the chunk, lane <-> output channels [4 lane, 4 lane + 4), so every warp access to the output and the residual is one pixel's
+        // 512 contiguous bytes.  The chunks are the 32-pixel sets the GroupNorm partial statistics are formed over.
+        const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
+        const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
+        const int srow = 2 * (lane & 3), scol = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+        const int n0 = nt * 128 + 4 * lane;
+#pragma unroll
+        for (int c = 0; c < T::NP / 32; c++) {
+#pragma unroll
+            for (int jj = 0; jj < 4; jj++)
+#pragma unroll
+                for (int i = 0; i < 4; i++)
+                    stage[(8 * jj + srow + (i & 1)) * C3W_SP + scol + 8 * (i >> 1)] = acc[4 * (4 * c + jj) + i];
+            tc::bar_sync(1, 256);
+            // pixel 8 r + warp of the chunk: x = tx * 8 + warp, output row y0 + r of image b (TH % 4 == 0: one image per chunk)
+            const int x = tx * 8 + warp, y0 = ty * TH + (4 * c) % TH, b = tb * NB + (4 * c) / TH;
+            const int64_t off = (((int64_t)b * p.H + y0) * p.W + x) * p.Cout + n0;
+            const int rs = p.W * p.Cout;                     // one output row
+            const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0);
+            float4 v[4];
+            unsigned valid = 0;
+#pragma unroll
+            for (int r = 0; r < 4; r++) {
+                if (x < p.W && y0 + r < p.H && b < p.B) valid |= 1u << r;
+                const float4 q = *reinterpret_cast<const float4*>(stage + (8 * r + warp) * C3W_SP + 4 * lane);
+                v[r] = make_float4(q.x + bb.x, q.y + bb.y, q.z + bb.z, q.w + bb.w);
+            }
+            if (p.out_nchw) {
+                const int64_t cs = (int64_t)p.H * p.W;
+#pragma unroll
+                for (int r = 0; r < 4; r++)
+                    if (valid >> r & 1) {
+                        float* o = p.out + (((int64_t)b * p.Cout + n0) * p.H + y0 + r) * p.W + x;
+                        o[0] = v[r].x; o[cs] = v[r].y; o[2 * cs] = v[r].z; o[3 * cs] = v[r].w;
+                    }
+            } else {
+                if (p.residual) {
+#pragma unroll
+                    for (int r = 0; r < 4; r++)
+                        if (valid >> r & 1) {
+                            const float4 rr = *reinterpret_cast<const float4*>(p.residual + off + r * rs);
+                            v[r].x += rr.x; v[r].y += rr.y; v[r].z += rr.z; v[r].w += rr.w;
+                        }
+                }
+#pragma unroll
+                for (int r = 0; r < 4; r++)
+                    if (valid >> r & 1) *reinterpret_cast<float4*>(p.out + off + r * rs) = v[r];
+            }
+            const int cl = p.Cout >> 7;                      // lanes per GroupNorm(32) group: cg = Cout / 32 = 4 cl channels
+            if (p.gn_part != nullptr) {
+                float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+                for (int r = 0; r < 4; r++)
+                    if (valid >> r & 1) {
+                        s1 += (v[r].x + v[r].y) + (v[r].z + v[r].w);
+                        s2 += fmaf(v[r].x, v[r].x, v[r].y * v[r].y) + fmaf(v[r].z, v[r].z, v[r].w * v[r].w);
+                    }
+                for (int m = 1; m < cl; m <<= 1) {
+                    s1 += __shfl_xor_sync(0xffffffffu, s1, m);
+                    s2 += __shfl_xor_sync(0xffffffffu, s2, m);
+                }
+                gnred[warp * 32 + lane] = make_float2(s1, s2);
+            }
+            tc::bar_sync(1, 256);
+            if (p.gn_part != nullptr && warp == 0 && (lane & (cl - 1)) == 0) {     // one lane per group sums the 8 warps' pixels
+                float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+                for (int w = 0; w < 8; w++) {
+                    const float2 q = gnred[w * 32 + lane];
+                    s1 += q.x;
+                    s2 += q.y;
+                }
+                const int chunk = (ty * p.tiles_x + tx) * (TH / 4) + c % (TH / 4);
+                double* o = p.gn_part + (((int64_t)b * p.gn_chunks + chunk) * 32 + n0 / (4 * cl)) * 2;
+                if (b < p.B) { o[0] = (double)s1; o[1] = (double)s2; }
+            }
+        }
+    }
+}
+
+template <int TH, int NB, int STAGES, int FMT, int PASSES>
+static int launch_conv3x3_wreg_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
+                                 const ConvTcParams& p, int n_sm, cudaStream_t st) {
+    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr size_t smem = (size_t)2 * NOPS * C3wTile<TH, NB>::HALO + (size_t)STAGES * NOPS * 128 * 128 + 32 * C3W_SP * 4 + 256 * 8 + 1024 + 256;
+    static_assert(smem <= 227 * 1024, "conv3x3_wreg: shared memory budget");
+    RQB_ENSURE_SMEM(smem, conv3x3_wreg_kernel<TH, NB, STAGES, FMT, PASSES>);
+    const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
+    const int grid = total < n_sm ? total : n_sm;
+    conv3x3_wreg_kernel<TH, NB, STAGES, FMT, PASSES><<<grid, C3W_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
+    return check_launch("conv3x3_wreg");
+}
+
+template <int TH, int NB, int STAGES>
+static int launch_conv3x3_wreg_fmt(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
+                                   bool split, const ConvTcParams& p, int n_sm, cudaStream_t st) {
+    if (split) return p.fmt ? launch_conv3x3_wreg_t<TH, NB, STAGES, 1, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
+                            : launch_conv3x3_wreg_t<TH, NB, STAGES, 0, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+    return p.fmt ? launch_conv3x3_wreg_t<TH, NB, STAGES, 1, 1>(tmA, tmB, tmA, tmB, p, n_sm, st)
+                 : launch_conv3x3_wreg_t<TH, NB, STAGES, 0, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
 }
 
 static int sm_count() {
@@ -473,24 +735,28 @@ bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int 
     return pow2(H) && pow2(W);
 }
 
-// output tile of one CTA, TW x TH x NB = 128 pixels.  3x3 stride 1 (conv3x3_tc_kernel): 8 pixels wide, 16 rows, or 8 rows of
-// NB = 2 images below 16 rows; maps narrower or lower than the tile leave the out-of-range part of it unstored.
-static void conv_tile(int H, int W, int ks, int stride, int& TW, int& TH, int& NB) {
+// output tile of one CTA, TW x TH x NB pixels.  3x3 stride 1, 8 pixels wide: Cout % 128 == 0 (conv3x3_wreg_kernel) 32 rows
+// (256 pixels), 16 rows, or 8 rows of NB = 2 images below 16 rows; other Cout (conv3x3_tc_kernel) 16 rows, or 8 rows of NB = 2
+// images below 16 rows.  Maps narrower or lower than the tile leave the out-of-range part of it unstored.  Else 128 pixels.
+static bool conv3x3_wreg(int Cout, int ks, int stride) { return ks == 3 && stride == 1 && Cout % 128 == 0; }
+
+static void conv_tile(int H, int W, int Cout, int ks, int stride, int& TW, int& TH, int& NB) {
     if (ks == 3 && stride == 1) {
         TW = 8;
-        TH = H > 8 ? 16 : 8;
+        TH = conv3x3_wreg(Cout, ks, stride) && H >= 32 ? 32 : (H > 8 ? 16 : 8);
+        NB = TH == 8 ? 2 : 1;
     } else {
         TW = W < 16 ? W : 16;
         TH = (128 / TW) < H ? (128 / TW) : H;
+        NB = 128 / (TW * TH);
     }
-    NB = 128 / (TW * TH);
 }
 
 // the epilogue can emit the output's GroupNorm(32) partial statistics when the tiles cover the map exactly, every epilogue warp's
 // 32 pixels lie in one image and a 16-channel chunk holds whole groups
 bool conv_tc_gn_fusable(int H, int W, int Cout, int ks, int stride) {
     int TW, TH, NB;
-    conv_tile(H, W, ks, stride, TW, TH, NB);
+    conv_tile(H, W, Cout, ks, stride, TW, TH, NB);
     const int cg = Cout / 32;
     return Cout % 32 == 0 && (cg == 4 || cg == 8 || cg == 16) && W % TW == 0 && H % TH == 0 && TW * TH >= 32 && (H * W) % 32 == 0;
 }
@@ -502,12 +768,11 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
                    cudaStream_t st, int stride, double* gn_part, int fmt) {
     ConvTcParams p = {};
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ks = ks; p.stride = stride; p.fmt = fmt;
-    conv_tile(H, W, ks, stride, p.TW, p.TH, p.NB);
-    if (p.TW * p.TH * p.NB != 128) return fail(RQB200_EINVAL, "conv_tc: feature map extent must be a power of two");
-    p.tiles_x = (int)ceil_div(W, p.TW); p.tiles_y = (int)ceil_div(H, p.TH); p.tiles_b = (int)ceil_div(B, p.NB);
-    // 3x3: at most 128 output channels per tile.  The weight slabs, not the halo, are most of its L2 traffic, so BN = 256 would
-    // save little (178 vs 166 flop/B) and its 128 accumulators per thread spill; BN = 128 also doubles the CTAs of the 8 x 8 maps.
+    conv_tile(H, W, Cout, ks, stride, p.TW, p.TH, p.NB);
     const bool c3 = ks == 3 && stride == 1;
+    if (!c3 && p.TW * p.TH * p.NB != 128) return fail(RQB200_EINVAL, "conv_tc: feature map extent must be a power of two");
+    p.tiles_x = (int)ceil_div(W, p.TW); p.tiles_y = (int)ceil_div(H, p.TH); p.tiles_b = (int)ceil_div(B, p.NB);
+    // 3x3: 128 output channels per tile (conv3x3_wreg_kernel), or 16 | 64 (conv3x3_tc_kernel)
     const int BN = Cout <= 16 ? 16 : (Cout % 256 == 0 && !c3 ? 256 : (Cout % 128 == 0 ? 128 : 64));
     p.n_tiles_n = (int)ceil_div(Cout, BN);
     p.bias = bias; p.residual = residual; p.out = out; p.out_nchw = out_nchw;
@@ -527,20 +792,18 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
         // the halo box: the tile plus one pixel on every side
         RQB_TRY(make_tmap_4d_nhwc(&tmA, X16, (uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B, 64, (uint32_t)p.TW + 2,
                                   (uint32_t)p.TH + 2, (uint32_t)p.NB, 1));
-        if (split) {
+        if (split)
             RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B, 64, (uint32_t)p.TW + 2,
                                       (uint32_t)p.TH + 2, (uint32_t)p.NB, 1));
-            switch (BN) {
-                case 16: return launch_conv3x3_tc_t<16, 8, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-                case 64: return launch_conv3x3_tc_t<64, 4, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-                default: return launch_conv3x3_tc_t<128, 3, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-            }
+        if (conv3x3_wreg(Cout, ks, stride)) {
+            if (p.TH == 32) return launch_conv3x3_wreg_fmt<32, 1, 1>(tmA, tmB, tmAlo, tmBlo, split, p, n_sm, st);
+            if (p.TH == 16) return launch_conv3x3_wreg_fmt<16, 1, 3>(tmA, tmB, tmAlo, tmBlo, split, p, n_sm, st);
+            return launch_conv3x3_wreg_fmt<8, 2, 3>(tmA, tmB, tmAlo, tmBlo, split, p, n_sm, st);
         }
-        switch (BN) {
-            case 16: return launch_conv3x3_tc_t<16, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
-            case 64: return launch_conv3x3_tc_t<64, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
-            default: return launch_conv3x3_tc_t<128, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
-        }
+        if (split) return BN == 16 ? launch_conv3x3_tc_t<16, 8, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
+                                   : launch_conv3x3_tc_t<64, 4, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+        return BN == 16 ? launch_conv3x3_tc_t<16, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st)
+                        : launch_conv3x3_tc_t<64, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
     }
     RQB_TRY(make_tmap_4d_nhwc(&tmA, X16, (uint64_t)Cin, (uint64_t)W * stride, (uint64_t)H * stride, (uint64_t)B, 64, (uint32_t)p.TW,
                               (uint32_t)p.TH, (uint32_t)p.NB, (uint32_t)stride));

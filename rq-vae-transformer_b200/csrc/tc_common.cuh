@@ -94,6 +94,11 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
+// hand registers from one warpgroup to another (all warps of the warpgroup execute it; the kernel's budget must cover the total)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 // named barrier over the `n` threads of the consumer warpgroups (id 0 is __syncthreads)
 __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 

@@ -9,9 +9,9 @@ group it reports:
     tflops        algorithmic TFLOP/s: 2 * B * H * W * Cout * Cin * ks^2 * 3 (the three split-fp16 products) over kernel time
     l2_smem_tbps  the L2 -> shared-memory bytes the kernel's tile plan loads (computed from the shape, not measured) over kernel time
 
-The tile plan is recognised from the kernel name: conv3x3_tc_kernel loads one halo tile per 64-channel slab and streams the
-nine taps' weight slabs; conv_tc_kernel loads an activation box and a weight slab per (tap, slab).  Prints one JSON line with
-the card's name and power limit, read in this run.
+The tile plan is recognised from the kernel name: conv3x3_wreg_kernel (Cout % 128 == 0) and conv3x3_tc_kernel load one halo tile
+per 64-channel slab and stream the nine taps' weight slabs; conv_tc_kernel loads an activation box and a weight slab per (tap,
+slab).  Prints one JSON line with the card's name and power limit, read in this run.
 Usage: python scripts/bench_decode_convs.py [--batch 64] [--reps 3]"""
 import argparse
 import json
@@ -75,7 +75,9 @@ def conv_plan(dd=DD, embed_dim=EMBED_DIM):
 
 
 def block_n(kernel, cout):
-    """output channels per tile (csrc/conv_tc.cu launch_conv_tc): conv3x3_tc_kernel stops at 128"""
+    """output channels per tile (csrc/conv_tc.cu launch_conv_tc): 128 on conv3x3_wreg_kernel, at most 64 on conv3x3_tc_kernel"""
+    if kernel == "conv3x3_wreg_kernel":
+        return 128
     wide = cout % 256 == 0 and not kernel.startswith("conv3x3")
     return 16 if cout <= 16 else (256 if wide else (128 if cout % 128 == 0 else 64))
 
@@ -91,8 +93,8 @@ def plan_bytes(kernel, B, ks, H, W, cin, cout):
     n_tiles = cdiv(cout, bn)
     slabs = cin // 64
     if kernel.startswith("conv3x3"):
-        th = 16 if H >= 16 else 8
-        nbt = 128 // (8 * th)
+        th = 32 if H >= 32 and kernel == "conv3x3_wreg_kernel" else (16 if H >= 16 else 8)
+        nbt = 2 if th == 8 else 1
         tiles = cdiv(W, 8) * cdiv(H, th) * cdiv(B, nbt) * n_tiles
         per_slab = 10 * (th + 2) * nbt * 128 + 9 * bn * 128
         return tiles * slabs * per_slab * ops
@@ -147,7 +149,7 @@ def main():
     kern = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA),
                   key=lambda e: e.time_range.start)
     total_us = sum(e.time_range.elapsed_us() for e in kern)
-    convs = [(e, m.group(1)) for e in kern for m in [re.search(r"\b(conv_tc_kernel|conv3x3_tc_kernel)\b", e.name)] if m]
+    convs = [(e, m.group(1)) for e in kern for m in [re.search(r"\b(conv_tc_kernel|conv3x3_tc_kernel|conv3x3_wreg_kernel)\b", e.name)] if m]
     plan = conv_plan()
     if len(convs) != len(plan):
         raise SystemExit("bench_decode_convs.py: %d conv kernels in the trace, the decoder plan has %d" % (len(convs), len(plan)))
