@@ -300,9 +300,10 @@ int rqb200_dbg_sample_logits(int algo, const float* logits, const float* q, int 
                              float top_p, int64_t* out_idx, void* stream);
 
 /* rqb200_dbg_conv_tc: one launch of the wgmma implicit-GEMM conv (csrc/conv_tc.cu): X NHWC fp16 [B,H,W,Cin], W OHWI fp16
- * [Cout,ks,ks,Cin], stride 1 "same" padding, out f32 NHWC (+bias, +residual) or NCHW when out_nchw.  X16lo / W16lo
- * (both or neither): the fp16 "lo" halves (value - fp16(value)) -> split-fp16, three products per conv.
- * out_nchw bit 1: the operands are bf16 instead of fp16; bits 8..: stride (2: the Downsample conv, H, W the output extent). */
+ * [Cout,ks,ks,Cin], stride 1 "same" padding, out f32 NHWC (+bias, +residual) or NCHW when out_nchw.  X16lo / W16lo (both
+ * required, RQB200_EINVAL when either is NULL): the fp16 "lo" halves (value - fp16(value)) for the split-fp16 products, three
+ * per conv.  Operands are fp16 only: out_nchw bit 1 (bf16) is refused with RQB200_EINVAL.  Both refusals come before any CUDA
+ * call.  out_nchw bits 8..: stride (2: the Downsample conv, H, W the output extent). */
 int rqb200_dbg_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                        const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                        void* stream);

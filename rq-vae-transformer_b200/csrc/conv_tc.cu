@@ -1,8 +1,9 @@
-// P2 "fast" tier -- NHWC implicit-GEMM convolution on wgmma tensor cores (fp16 operands, fp32 accumulate in registers).
+// P2 "fast" tier -- NHWC implicit-GEMM convolution on wgmma tensor cores (split-fp16 operands, fp32 accumulate in registers).
 //
 // Replaces cuDNN's conv behind ResnetBlock / AttnBlock / Upsample / conv_in / conv_out of the decoder (reference:
 // rqvae/models/rqvae/layers.py:100-120,158-182,31-35; modules.py:171-202).  The reference's own GPU path runs these convs
-// with TF32 allowed (10-bit mantissa); fp16 operands carry the same mantissa width.
+// with TF32 allowed (10-bit mantissa).  Every conv takes both operands as fp16 hi + lo pairs and forms three products per k
+// step (see ct_mma_kblock): fp32-class products on the fp16 tensor pipe.
 //
 //   D[pixel, cout] = sum_{tap, cin} A[pixel + tap, cin] * W[cout, tap, cin]
 //
@@ -18,7 +19,8 @@
 //                      TMA box brings the 8 x TH x NB tile plus its one-pixel halo, and the nine taps read it as shifted wgmma
 //                      operands; only the weight slabs stream through the ring (see the comment above the kernel).
 //   conv_tc_kernel     1x1 convs, the encoder's stride-2 convs and the rows GEMM: one activation box and one weight slab per
-//                      (tap, slab) k block.
+//                      (tap, slab) k block.  The rows GEMM (launch_rows_gemm_tc) is the only caller of its single-product
+//                      forms (PASSES == 1) and of bf16 operands (ConvTcParams.fmt == 1).
 //
 // Persistent CTAs (grid = #SMs) loop over (pixel tile, cout tile) pairs; warp 8 = TMA producer, warps 0-7 = two consumer
 // warpgroups, each issuing wgmma m64nBNk16 for 64 of the tile's 128 pixels and then running the epilogue (registers -> shared
@@ -45,7 +47,7 @@ struct ConvTcParams {
     int out_nchw;
     // "rows GEMM" use of the same kernel (launch_rows_gemm_tc: a 1x1 conv over M token rows viewed as 16x8-pixel images):
     void* out16;                   // non-null: 16-bit NHWC output (fmt) instead of `out`, optionally through GELU
-    int gelu, fmt;                 // fmt: 16-bit operand / output format, 0 fp16 (all convs), 1 bf16
+    int gelu, fmt;                 // fmt: 16-bit operand / output format of the rows GEMM, 0 fp16, 1 bf16; every conv is 0 (fp16)
     int64_t m_rows;                // > 0: only pixels (rows) below m_rows are stored
     // GroupNorm(32) statistics of the OUTPUT (bias / residual included), for the GroupNorm that consumes it next (layers.py:16-17,
     // 100-120): every epilogue warp (32 pixels of one image) writes (sum, sum of squares) per group as fp64 to
@@ -57,9 +59,9 @@ struct ConvTcParams {
 constexpr int CT_THREADS = 288;            // warps 0-7: two consumer warpgroups (64 tile rows each), warp 8: TMA producer
 constexpr int CT_A_BYTES = 128 * 64 * 2;
 
-// PASSES == 1: single fp16 product.  PASSES == 3: split-fp16 ("fp16x3") -- both operands are carried as hi + lo fp16 pairs and
-// the accumulator receives A_hi W_hi + A_lo W_hi + A_hi W_lo (the dropped A_lo W_lo term is ~2^-22 relative): fp32-class
-// products on the fp16 tensor pipe, which is what keeps 60 chained convs inside the 1e-3 pixel tolerance.
+// PASSES == 3 (every conv): split-fp16 ("fp16x3") -- both operands are carried as hi + lo fp16 pairs and the accumulator receives
+// A_hi W_hi + A_lo W_hi + A_hi W_lo (the dropped A_lo W_lo term is ~2^-22 relative): fp32-class products on the fp16 tensor pipe,
+// which is what keeps 60 chained convs inside the 1e-3 pixel tolerance.  PASSES == 1: the rows GEMM's single 16-bit product.
 // GroupNorm partial statistics of one 16-channel chunk of a warp's 32 pixels: NV = 2 * (16 / CG) values (the sums, then the sums
 // of squares, of the chunk's 16 / CG groups) are formed per thread and reduced over the 32 lanes with a transpose-reduce
 // (log2(NV) halving steps, then plain butterfly steps): NV + 1 shuffles of depth 5 instead of 5 * NV.  On return `tot` is the total
@@ -308,33 +310,31 @@ static int launch_conv_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
 // weights -> 85 flop/B of wgmma work, against 21 for per-tap A + W reloads.
 constexpr int C3_HALO_BYTES = 10 * 10 * 2 * 128;   // per operand; the largest box (TH = 8, NB = 2: 200 pixels; TH = 16: 180)
 
-template <int BN, int FMT, int PASSES>
+template <int BN>
 __device__ __forceinline__ void c3_mma_kblock(float (&acc)[BN / 2], uint32_t a, uint32_t b, bool first) {
     constexpr int B_BYTES = BN * 64 * 2;
     constexpr uint32_t SBO = 10 * 128;                 // one halo row per core-matrix group
-    if (PASSES == 3) {                                 // small terms first, the dominant product last
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-            tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + C3_HALO_BYTES + j * 32, SBO), tc::gmma_desc_k128(b + j * 32),
-                                    (!first || j > 0) ? 1u : 0u);
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-            tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32, SBO), tc::gmma_desc_k128(b + B_BYTES + j * 32), 1u);
-    }
+    // split-fp16: small terms first, the dominant product last
 #pragma unroll
     for (int j = 0; j < 4; j++)
-        tc::Wgmma<BN, FMT>::mma(acc, tc::gmma_desc_k128(a + j * 32, SBO), tc::gmma_desc_k128(b + j * 32),
-                                (PASSES == 3 || !first || j > 0) ? 1u : 0u);
+        tc::Wgmma<BN, 0>::mma(acc, tc::gmma_desc_k128(a + C3_HALO_BYTES + j * 32, SBO), tc::gmma_desc_k128(b + j * 32),
+                              (!first || j > 0) ? 1u : 0u);
+#pragma unroll
+    for (int j = 0; j < 4; j++)
+        tc::Wgmma<BN, 0>::mma(acc, tc::gmma_desc_k128(a + j * 32, SBO), tc::gmma_desc_k128(b + B_BYTES + j * 32), 1u);
+#pragma unroll
+    for (int j = 0; j < 4; j++)
+        tc::Wgmma<BN, 0>::mma(acc, tc::gmma_desc_k128(a + j * 32, SBO), tc::gmma_desc_k128(b + j * 32), 1u);
 }
 
-// TMA producer of both 3x3 kernels (one thread): per 64-channel slab ONE halo box (hi [+ lo]) into the next of two halo slots,
-// per tap one [BM x 64] weight slab (hi [+ lo]) into the STAGES-deep ring.  Runs ahead across tiles, so the next tile's operands
+// TMA producer of both 3x3 kernels (one thread): per 64-channel slab ONE halo box (hi + lo) into the next of two halo slots,
+// per tap one [BM x 64] weight slab (hi + lo) into the STAGES-deep ring.  Runs ahead across tiles, so the next tile's operands
 // load during this tile's epilogue.  Halo slot: [X_hi | X_lo], HALO_BYTES apart; weight stage: [W_hi | W_lo], BM x 128 B apart.
-template <int BM, int STAGES, int PASSES, int SLOT_BYTES, int HALO_BYTES>
+template <int BM, int STAGES, int SLOT_BYTES, int HALO_BYTES>
 __device__ __forceinline__ void c3_produce(const CUtensorMap* tmA, const CUtensorMap* tmB, const CUtensorMap* tmAlo, const CUtensorMap* tmBlo,
                                            const ConvTcParams& p, uint8_t* smem, uint8_t* wst, uint64_t* full, uint64_t* empty,
                                            uint64_t* hfull, uint64_t* hempty) {
-    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr int NOPS = 2;
     constexpr int B_BYTES = BM * 64 * 2;
     constexpr int STAGE_BYTES = NOPS * B_BYTES;
     const int cslabs = p.Cin / 64;
@@ -353,14 +353,14 @@ __device__ __forceinline__ void c3_produce(const CUtensorMap* tmA, const CUtenso
                 tc::mbar_expect_tx(&full[s], STAGE_BYTES);
                 uint8_t* w = wst + s * STAGE_BYTES;
                 tc::tma_load_2d(w, tmB, &full[s], tap * p.Cin + c0, nt * BM, tc::L2_EVICT_LAST);
-                if (PASSES == 3) tc::tma_load_2d(w + B_BYTES, tmBlo, &full[s], tap * p.Cin + c0, nt * BM, tc::L2_EVICT_LAST);
+                tc::tma_load_2d(w + B_BYTES, tmBlo, &full[s], tap * p.Cin + c0, nt * BM, tc::L2_EVICT_LAST);
                 if (tap == 0) {                        // the slab's first weights go out before the wait for a halo slot
                     const int h = hit % 2;
                     tc::mbar_wait(&hempty[h], ((hit / 2) & 1) ^ 1);
                     tc::mbar_expect_tx(&hfull[h], halo_tx);
                     uint8_t* a = smem + h * SLOT_BYTES;
                     tc::tma_load_4d(a, tmA, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
-                    if (PASSES == 3) tc::tma_load_4d(a + HALO_BYTES, tmAlo, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
+                    tc::tma_load_4d(a + HALO_BYTES, tmAlo, &hfull[h], c0, x0 - 1, y0 - 1, b0, tc::L2_EVICT_NORMAL);
                 }
             }
         }
@@ -369,12 +369,12 @@ __device__ __forceinline__ void c3_produce(const CUtensorMap* tmA, const CUtenso
 
 // Two halo slots (the next slab's halo loads during this slab's taps) and STAGES weight stages.
 // smem: [halo slot: A_hi | A_lo] x 2, [B_hi | B_lo] x STAGES, epilogue staging, barriers.
-template <int BN, int STAGES, int PASSES>
+template <int BN, int STAGES>
 __global__ void __launch_bounds__(CT_THREADS, 1)
 conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, ConvTcParams p) {
     constexpr int B_BYTES = BN * 64 * 2;
-    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr int NOPS = 2;
     constexpr int HSLOTS = 2;
     constexpr int SLOT_BYTES = NOPS * C3_HALO_BYTES;
     constexpr int STAGE_BYTES = NOPS * B_BYTES;
@@ -404,7 +404,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     __syncthreads();
 
     if (warp == 8) {
-        if (lane == 0) c3_produce<BN, STAGES, PASSES, SLOT_BYTES, C3_HALO_BYTES>(&tmA, &tmB, &tmAlo, &tmBlo, p, smem, wst, full, empty, hfull, hempty);
+        if (lane == 0) c3_produce<BN, STAGES, SLOT_BYTES, C3_HALO_BYTES>(&tmA, &tmB, &tmAlo, &tmBlo, p, smem, wst, full, empty, hfull, hempty);
         return;
     }
 
@@ -428,8 +428,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 const uint32_t a = a0 + ((tap / 3) * 10 + tap % 3) * 128, b = tc::smem_u32(wst + s * STAGE_BYTES);
                 const bool first = sl == 0 && tap == 0;
                 tc::wgmma_fence();
-                if (p.fmt) c3_mma_kblock<BN, 1, PASSES>(acc, a, b, first);
-                else c3_mma_kblock<BN, 0, PASSES>(acc, a, b, first);
+                c3_mma_kblock<BN>(acc, a, b, first);
                 tc::wgmma_commit();
                 tc::wgmma_wait<1>();
                 if (!first && lane == 0) {                   // the previous k block's MMAs are complete: free what only it read
@@ -456,17 +455,17 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
 }
 
-template <int BN, int STAGES, int PASSES>
+template <int BN, int STAGES>
 static int launch_conv3x3_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
                                const ConvTcParams& p, int n_sm, cudaStream_t st) {
-    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr int NOPS = 2;
     constexpr size_t smem = (size_t)2 * NOPS * C3_HALO_BYTES + (size_t)STAGES * NOPS * BN * 128 +
                             128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 256;
     static_assert(smem <= 227 * 1024, "conv3x3_tc: shared memory budget");
-    RQB_ENSURE_SMEM(smem, conv3x3_tc_kernel<BN, STAGES, PASSES>);
+    RQB_ENSURE_SMEM(smem, conv3x3_tc_kernel<BN, STAGES>);
     const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
     const int grid = total < n_sm ? total : n_sm;
-    conv3x3_tc_kernel<BN, STAGES, PASSES><<<grid, CT_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
+    conv3x3_tc_kernel<BN, STAGES><<<grid, CT_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
     return check_launch("conv3x3_tc");
 }
 
@@ -481,7 +480,7 @@ static int launch_conv3x3_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, c
 // Split-fp16 products per k16: W_hi X_lo, W_lo X_hi, W_hi X_hi -- only X is read from shared memory, ~64 B/clk of operand reads at
 // the fp16 rate against ~94 for the pixel-major SS form.  k order (slab-major, tap-minor) and the small-terms-first order of
 // conv3x3_tc_kernel are kept.
-// smem at TH = 32 (PASSES = 3): two halo slots of 2 x 43 KB, ONE 32 KB weight stage, a 16.5 KB epilogue staging buffer and 2 KB of
+// smem at TH = 32: two halo slots of 2 x 43 KB, ONE 32 KB weight stage, a 16.5 KB epilogue staging buffer and 2 KB of
 // GroupNorm partial sums = 223 KB.
 // The single weight stage is enough because a warpgroup holds two taps' fragments in registers: the producer refills the stage
 // as soon as both warpgroups have loaded tap t, while tap t - 1's and tap t's MMAs run.
@@ -499,7 +498,7 @@ constexpr int C3W_SP = 128 + 4;                    // epilogue staging row (one 
 constexpr int C3W_THREADS = 384, C3W_REGS_CONSUMER = 240, C3W_REGS_PRODUCER = 24;
 static_assert(256 * C3W_REGS_CONSUMER + 128 * C3W_REGS_PRODUCER <= 168 * C3W_THREADS, "conv3x3_wreg: register split exceeds the pool");
 
-template <int TH, int NB, int FMT, int PASSES>
+template <int TH, int NB>
 __device__ __forceinline__ void c3w_mma_kblock(float (&acc)[C3wTile<TH, NB>::NP / 2], const uint32_t (&fh)[4][4],
                                                const uint32_t (&fl)[4][4], uint32_t x, bool first) {
     constexpr int NI = C3wTile<TH, NB>::NI, HALO = C3wTile<TH, NB>::HALO;
@@ -507,17 +506,16 @@ __device__ __forceinline__ void c3w_mma_kblock(float (&acc)[C3wTile<TH, NB>::NP 
     auto mma = [&acc](const uint32_t (&a)[4], uint32_t xa, uint32_t accumulate) {
 #pragma unroll
         for (int b = 0; b < NB; b++)
-            tc::WgmmaRA<NI, FMT>::mma(*reinterpret_cast<float(*)[NI / 2]>(&acc[b * (NI / 2)]), a, tc::gmma_desc_k128(xa + b * IMG, SBO),
-                                      accumulate);
+            tc::WgmmaRA<NI>::mma(*reinterpret_cast<float(*)[NI / 2]>(&acc[b * (NI / 2)]), a, tc::gmma_desc_k128(xa + b * IMG, SBO),
+                                 accumulate);
     };
-    if (PASSES == 3) {                                 // small terms first, the dominant product last
+    // split-fp16: small terms first, the dominant product last
 #pragma unroll
-        for (int j = 0; j < 4; j++) mma(fh[j], x + HALO + j * 32, (!first || j > 0) ? 1u : 0u);
+    for (int j = 0; j < 4; j++) mma(fh[j], x + HALO + j * 32, (!first || j > 0) ? 1u : 0u);
 #pragma unroll
-        for (int j = 0; j < 4; j++) mma(fl[j], x + j * 32, 1u);
-    }
+    for (int j = 0; j < 4; j++) mma(fl[j], x + j * 32, 1u);
 #pragma unroll
-    for (int j = 0; j < 4; j++) mma(fh[j], x + j * 32, (PASSES == 3 || !first || j > 0) ? 1u : 0u);
+    for (int j = 0; j < 4; j++) mma(fh[j], x + j * 32, 1u);
 }
 
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
@@ -525,12 +523,12 @@ __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
 }
 
 // smem: [halo slot: X_hi | X_lo] x 2, [W_hi | W_lo] x STAGES (128 rows x 128 B each, SWIZZLE_128B), epilogue staging, barriers.
-template <int TH, int NB, int STAGES, int FMT, int PASSES>
+template <int TH, int NB, int STAGES>
 __global__ void __launch_bounds__(C3W_THREADS, 1)
 conv3x3_wreg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, ConvTcParams p) {
     using T = C3wTile<TH, NB>;
-    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr int NOPS = 2;
     constexpr int SLOT_BYTES = NOPS * T::HALO;
     constexpr int B_BYTES = 128 * 128;
     constexpr int STAGE_BYTES = NOPS * B_BYTES;
@@ -562,7 +560,7 @@ conv3x3_wreg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     if (warp >= 8) {
         tc::setmaxnreg_dec<C3W_REGS_PRODUCER>();
         if (warp == 8 && lane == 0)
-            c3_produce<128, STAGES, PASSES, SLOT_BYTES, T::HALO>(&tmA, &tmB, &tmAlo, &tmBlo, p, smem, wst, full, empty, hfull, hempty);
+            c3_produce<128, STAGES, SLOT_BYTES, T::HALO>(&tmA, &tmB, &tmAlo, &tmBlo, p, smem, wst, full, empty, hfull, hempty);
         return;
     }
     tc::setmaxnreg_inc<C3W_REGS_CONSUMER>();
@@ -591,11 +589,11 @@ conv3x3_wreg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             ldsm_x4(fr[0][j], w ^ (32 * j));
-            if (PASSES == 3) ldsm_x4(fr[1][j], (w + B_BYTES) ^ (32 * j));
+            ldsm_x4(fr[1][j], (w + B_BYTES) ^ (32 * j));
         }
         const uint32_t x = halo0 + (hit % 2) * SLOT_BYTES + ((tap / 3) * 10 + tap % 3) * 128;
         tc::wgmma_fence();
-        c3w_mma_kblock<TH, NB, FMT, PASSES>(acc, fr[0], fr[1], x, kb == 0);
+        c3w_mma_kblock<TH, NB>(acc, fr[0], fr[1], x, kb == 0);
         tc::wgmma_commit();
         __syncwarp();
         if (lane == 0) tc::mbar_arrive(&empty[s]);       // the wgmmas above have read the fragments: the stage is free
@@ -694,26 +692,17 @@ conv3x3_wreg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     }
 }
 
-template <int TH, int NB, int STAGES, int FMT, int PASSES>
+template <int TH, int NB, int STAGES>
 static int launch_conv3x3_wreg_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
                                  const ConvTcParams& p, int n_sm, cudaStream_t st) {
-    constexpr int NOPS = PASSES == 3 ? 2 : 1;
+    constexpr int NOPS = 2;
     constexpr size_t smem = (size_t)2 * NOPS * C3wTile<TH, NB>::HALO + (size_t)STAGES * NOPS * 128 * 128 + 32 * C3W_SP * 4 + 256 * 8 + 1024 + 256;
     static_assert(smem <= 227 * 1024, "conv3x3_wreg: shared memory budget");
-    RQB_ENSURE_SMEM(smem, conv3x3_wreg_kernel<TH, NB, STAGES, FMT, PASSES>);
+    RQB_ENSURE_SMEM(smem, conv3x3_wreg_kernel<TH, NB, STAGES>);
     const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
     const int grid = total < n_sm ? total : n_sm;
-    conv3x3_wreg_kernel<TH, NB, STAGES, FMT, PASSES><<<grid, C3W_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
+    conv3x3_wreg_kernel<TH, NB, STAGES><<<grid, C3W_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
     return check_launch("conv3x3_wreg");
-}
-
-template <int TH, int NB, int STAGES>
-static int launch_conv3x3_wreg_fmt(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
-                                   bool split, const ConvTcParams& p, int n_sm, cudaStream_t st) {
-    if (split) return p.fmt ? launch_conv3x3_wreg_t<TH, NB, STAGES, 1, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
-                            : launch_conv3x3_wreg_t<TH, NB, STAGES, 0, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-    return p.fmt ? launch_conv3x3_wreg_t<TH, NB, STAGES, 1, 1>(tmA, tmB, tmA, tmB, p, n_sm, st)
-                 : launch_conv3x3_wreg_t<TH, NB, STAGES, 0, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
 }
 
 static int sm_count() {
@@ -761,13 +750,14 @@ bool conv_tc_gn_fusable(int H, int W, int Cout, int ks, int stride) {
     return Cout % 32 == 0 && (cg == 4 || cg == 8 || cg == 16) && W % TW == 0 && H % TH == 0 && TW * TH >= 32 && (H * W) % 32 == 0;
 }
 
-// X: NHWC 16-bit [B,H*stride,W*stride,Cin]; Wt: [Cout, ks, ks, Cin] 16-bit; out fp32 [B,H,W,Cout].  X16lo/W16lo non-null ->
-// split-fp16 (3 products).  H, W are the OUTPUT extent.  fmt: 0 fp16 operands, 1 bf16.
+// X: NHWC fp16 [B,H*stride,W*stride,Cin]; Wt: [Cout, ks, ks, Cin] fp16; out fp32 [B,H,W,Cout].  X16lo / W16lo (required): their
+// fp16 lo halves, for the split-fp16 products.  H, W are the OUTPUT extent.
 int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                    const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
-                   cudaStream_t st, int stride, double* gn_part, int fmt) {
+                   cudaStream_t st, int stride, double* gn_part) {
+    if (X16lo == nullptr || W16lo == nullptr) return fail(RQB200_EINVAL, "conv_tc: the lo halves X16lo and W16lo are required");
     ConvTcParams p = {};
-    p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ks = ks; p.stride = stride; p.fmt = fmt;
+    p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ks = ks; p.stride = stride;
     conv_tile(H, W, Cout, ks, stride, p.TW, p.TH, p.NB);
     const bool c3 = ks == 3 && stride == 1;
     if (!c3 && p.TW * p.TH * p.NB != 128) return fail(RQB200_EINVAL, "conv_tc: feature map extent must be a power of two");
@@ -782,46 +772,33 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
         p.gn_part = gn_part;
         p.gn_chunks = H * W / 32;
     }
-    const bool split = X16lo != nullptr && W16lo != nullptr;
     CUtensorMap tmA, tmB, tmAlo, tmBlo;
     RQB_TRY(make_tmap_2d(&tmB, W16, 1, (uint64_t)ks * ks * Cin, (uint64_t)Cout, (uint64_t)ks * ks * Cin * 2, 64, (uint32_t)BN));
-    if (split)
-        RQB_TRY(make_tmap_2d(&tmBlo, W16lo, 1, (uint64_t)ks * ks * Cin, (uint64_t)Cout, (uint64_t)ks * ks * Cin * 2, 64, (uint32_t)BN));
+    RQB_TRY(make_tmap_2d(&tmBlo, W16lo, 1, (uint64_t)ks * ks * Cin, (uint64_t)Cout, (uint64_t)ks * ks * Cin * 2, 64, (uint32_t)BN));
     const int n_sm = sm_count();
     if (c3) {
         // the halo box: the tile plus one pixel on every side
         RQB_TRY(make_tmap_4d_nhwc(&tmA, X16, (uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B, 64, (uint32_t)p.TW + 2,
                                   (uint32_t)p.TH + 2, (uint32_t)p.NB, 1));
-        if (split)
-            RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B, 64, (uint32_t)p.TW + 2,
-                                      (uint32_t)p.TH + 2, (uint32_t)p.NB, 1));
+        RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B, 64, (uint32_t)p.TW + 2,
+                                  (uint32_t)p.TH + 2, (uint32_t)p.NB, 1));
         if (conv3x3_wreg(Cout, ks, stride)) {
-            if (p.TH == 32) return launch_conv3x3_wreg_fmt<32, 1, 1>(tmA, tmB, tmAlo, tmBlo, split, p, n_sm, st);
-            if (p.TH == 16) return launch_conv3x3_wreg_fmt<16, 1, 3>(tmA, tmB, tmAlo, tmBlo, split, p, n_sm, st);
-            return launch_conv3x3_wreg_fmt<8, 2, 3>(tmA, tmB, tmAlo, tmBlo, split, p, n_sm, st);
+            if (p.TH == 32) return launch_conv3x3_wreg_t<32, 1, 1>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+            if (p.TH == 16) return launch_conv3x3_wreg_t<16, 1, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+            return launch_conv3x3_wreg_t<8, 2, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
         }
-        if (split) return BN == 16 ? launch_conv3x3_tc_t<16, 8, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
-                                   : launch_conv3x3_tc_t<64, 4, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-        return BN == 16 ? launch_conv3x3_tc_t<16, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st)
-                        : launch_conv3x3_tc_t<64, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
+        return BN == 16 ? launch_conv3x3_tc_t<16, 8>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
+                        : launch_conv3x3_tc_t<64, 4>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
     }
     RQB_TRY(make_tmap_4d_nhwc(&tmA, X16, (uint64_t)Cin, (uint64_t)W * stride, (uint64_t)H * stride, (uint64_t)B, 64, (uint32_t)p.TW,
                               (uint32_t)p.TH, (uint32_t)p.NB, (uint32_t)stride));
-    if (split) {
-        RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)W * stride, (uint64_t)H * stride, (uint64_t)B, 64,
-                                  (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.NB, (uint32_t)stride));
-        switch (BN) {
-            case 16: return launch_conv_tc_t<16, 5, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-            case 64: return launch_conv_tc_t<64, 4, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-            case 128: return launch_conv_tc_t<128, 3, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-            default: return launch_conv_tc_t<256, 2, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
-        }
-    }
+    RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)W * stride, (uint64_t)H * stride, (uint64_t)B, 64,
+                              (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.NB, (uint32_t)stride));
     switch (BN) {
-        case 16: return launch_conv_tc_t<16, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
-        case 64: return launch_conv_tc_t<64, 8, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
-        case 128: return launch_conv_tc_t<128, 6, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
-        default: return launch_conv_tc_t<256, 4, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
+        case 16: return launch_conv_tc_t<16, 5, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+        case 64: return launch_conv_tc_t<64, 4, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+        case 128: return launch_conv_tc_t<128, 3, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+        default: return launch_conv_tc_t<256, 2, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
     }
 }
 
@@ -979,26 +956,25 @@ int launch_cast_f16(const float* X, void* Y16, void* Y16lo, int B, int H, int W,
 }  // namespace rqb
 
 // diagnostic entry point: one conv through the wgmma path (tests/test_gpu_tc.py, tests/test_gpu_conv3x3.py)
-// out_nchw bit 0: NCHW output; bit 1: bf16 operands; bits 8.. : stride (0/1 -> 1, 2 -> the Downsample conv; then H, W are the
-// OUTPUT extent)
+// out_nchw bit 0: NCHW output; bit 1 (bf16 operands) is refused: the convs take fp16 only; bits 8.. : stride (0/1 -> 1, 2 -> the
+// Downsample conv; then H, W are the OUTPUT extent)
 extern "C" int rqb200_dbg_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                                   const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                                   void* stream) {
-    const int stride = (out_nchw >> 8) > 1 ? (out_nchw >> 8) : 1;
-    if (!rqb::conv_tc_supported(H, W, Cin, Cout, ks, stride, 0)) return rqb::fail(RQB200_EINVAL, "conv_tc: unsupported shape");
-    return rqb::launch_conv_tc(X16, W16, X16lo, W16lo, bias, residual, out, B, H, W, Cin, Cout, ks, out_nchw & 1, (cudaStream_t)stream,
-                               stride, nullptr, (out_nchw >> 1) & 1);
+    return rqb200_dbg_conv_tc_gn(X16, W16, X16lo, W16lo, bias, residual, out, nullptr, B, H, W, Cin, Cout, ks, out_nchw, stream);
 }
 
 // diagnostic entry point: one conv with the GroupNorm(32) partial statistics of its output emitted by the epilogue
-// (tests/test_gpu_conv3x3.py); gn_part holds B * (H * W / 32) * 32 * 2 doubles.  out_nchw bits as above (NCHW is rejected).
+// (tests/test_gpu_conv3x3.py, tests/test_gpu_vae_kernels.py); gn_part holds B * (H * W / 32) * 32 * 2 doubles, or is null (no
+// statistics).  out_nchw bits as above (NCHW is rejected with gn_part).
 extern "C" int rqb200_dbg_conv_tc_gn(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                                      const float* residual, float* out, double* gn_part, int B, int H, int W, int Cin, int Cout, int ks,
                                      int out_nchw, void* stream) {
     const int stride = (out_nchw >> 8) > 1 ? (out_nchw >> 8) : 1;
     if (!rqb::conv_tc_supported(H, W, Cin, Cout, ks, stride, 0)) return rqb::fail(RQB200_EINVAL, "conv_tc: unsupported shape");
+    if (out_nchw & 2) return rqb::fail(RQB200_EINVAL, "conv_tc: bf16 operands are not supported (fp16 only)");
     return rqb::launch_conv_tc(X16, W16, X16lo, W16lo, bias, residual, out, B, H, W, Cin, Cout, ks, out_nchw & 1, (cudaStream_t)stream,
-                               stride, gn_part, (out_nchw >> 1) & 1);
+                               stride, gn_part);
 }
 
 // diagnostic entry point: the rows GEMM (tests/test_gpu_tc.py).  X must have ceil(M/128)*128 readable rows.

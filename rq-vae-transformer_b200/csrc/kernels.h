@@ -79,7 +79,7 @@ int launch_gn_stats(const float* X, double* stats_ws, int B, int HW, int C, cuda
 bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int in_nchw);
 int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                    const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
-                   cudaStream_t st, int stride = 1, double* gn_part = nullptr, int fmt = 0);
+                   cudaStream_t st, int stride = 1, double* gn_part = nullptr);
 bool conv_tc_gn_fusable(int H, int W, int Cout, int ks, int stride);
 int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                         int gelu, int fmt, int64_t M, int N_out, int K, cudaStream_t st);

@@ -23,7 +23,6 @@ struct rqb200_vae {
     std::unordered_map<std::string, VTensor> t;
     bool finalized = false;
     bool fast_ok = false;     // FAST mode and every decoder channel count is a multiple of 128
-    bool split = false;       // split-fp16 (3 products per conv): "<key>.weight_lo" tensors registered
     bool enc_fast = false;    // the encoder's convs were registered in fp16 as well: encode on the wgmma path
     bool gn_fuse = true;      // conv epilogues emit the next GroupNorm's partial statistics (mode bit RQB200_VAE_NO_GN_FUSE clears it)
     int64_t last_launches = 0;
@@ -45,7 +44,7 @@ struct Operand {
 
 // One walk per network serves both tiers: the tier lives in operand / norm / conv, each of which branches on `fast`.  The
 // exact tier runs every conv and GroupNorm on the fp32 FFMA kernels; the fast tier (fast_ok: every channel count a multiple of
-// 128) runs them on the wgmma implicit GEMM with fp16 operands.
+// 128) runs them on the wgmma implicit GEMM with split-fp16 operands: each wgmma conv needs "<key>.weight_lo" beside its weight.
 struct VaeRun {
     rqb200_vae* h;
     cudaStream_t st;
@@ -55,7 +54,7 @@ struct VaeRun {
     double* gn_ws;
     std::string missing;
     __half* h16[2] = {nullptr, nullptr};      // fp16 conv operands (GN output / cast / upsampled cast)
-    __half* l16[2] = {nullptr, nullptr};      // their fp16 'lo' halves (split-fp16 products); null -> single product
+    __half* l16[2] = {nullptr, nullptr};      // their fp16 'lo' halves (split-fp16 products)
     float* zq = nullptr;                      // decode_code's staging buffer for the embedded codes
     bool fast = false;                        // the walk's tier, set by decode / encode
 
@@ -100,24 +99,20 @@ struct VaeRun {
              int stride, bool feeds_gn, int out_nchw) {
         const ConvGeom g = vae_conv_geom(B, H, W, Cin, Cout, ks, stride, in.upsample, in.nchw, out_nchw);
         const int Ho = g.Ho, Wo = g.Wo;
-        const VTensor* w = get(name + ".weight", (int64_t)Cout * ks * ks * Cin);
+        const int64_t wn = (int64_t)Cout * ks * ks * Cin;
+        const VTensor* w = get(name + ".weight", wn);
         const VTensor* b = get(name + ".bias", Cout);
+        const VTensor* wl = in.slot < 0 ? nullptr : get(name + ".weight_lo", wn);
         note_act((int64_t)Ho * Wo, Cout);
         if (dry || !w || !b) return 0;
         if (in.slot < 0) return launch_conv(in.x, w->ptr, w->dtype, (const float*)b->ptr, resid, out, g, st);
-        if (w->dtype != RQB200_F16) return fail(RQB200_ESTATE, "vae fast tier: conv weights must be fp16: " + name);
-        const __half* in_lo = nullptr;
-        const void* w_lo = nullptr;
-        if (h->split) {
-            const VTensor* wl = get(name + ".weight_lo", (int64_t)Cout * ks * ks * Cin);
-            if (!wl) return 0;
-            w_lo = wl->ptr;
-            in_lo = l16[in.slot];
-        }
+        if (!wl) return 0;
+        if (w->dtype != RQB200_F16 || wl->dtype != RQB200_F16)
+            return fail(RQB200_ESTATE, "vae fast tier: conv weights and their lo halves must be fp16: " + name);
         const bool fuse = feeds_gn && h->gn_fuse && !out_nchw && conv_tc_gn_fusable(Ho, Wo, Cout, ks, stride);
         stats_buf = fuse ? out : nullptr;
         stats_chunks = fuse ? Ho * Wo / 32 : 0;
-        return launch_conv_tc(h16[in.slot], w->ptr, in_lo, w_lo, (const float*)b->ptr, resid, out, B, Ho, Wo, Cin, Cout, ks, out_nchw, st,
+        return launch_conv_tc(h16[in.slot], w->ptr, l16[in.slot], wl->ptr, (const float*)b->ptr, resid, out, B, Ho, Wo, Cin, Cout, ks, out_nchw, st,
                               stride, fuse ? gn_ws : nullptr);
     }
 
@@ -243,7 +238,7 @@ static size_t vae_layout(const rqb200_vae* h, int B, void* base, size_t cap, Vae
         __half* p16 = a.take<__half>((size_t)B * h->max_act);
         if (run) run->h16[i] = p16;
     }
-    if (h->split)
+    if (h->fast_ok)
         for (int i = 0; i < 2; i++) {
             __half* p16 = a.take<__half>((size_t)B * h->max_act);
             if (run) run->l16[i] = p16;
@@ -282,7 +277,6 @@ int rqb200_vae_finalize(rqb200_vae* h) {
                   c.out_ch == 3 && r > 0 && (r & (r - 1)) == 0;
         h->fast_ok = ok;
         h->gn_fuse = !(c.mode & RQB200_VAE_NO_GN_FUSE);
-        h->split = ok && h->t.find("decoder.conv_in.weight_lo") != h->t.end();
     }
     {
         auto it = h->t.find("encoder.conv_out.weight");

@@ -37,7 +37,6 @@ class RQVAE(Stage1Model):
         self.post_quant_conv = nn.Conv2d(embed_dim, ddconfig["z_channels"], 1)
         self.loss_type, self.latent_loss_weight = loss_type, latent_loss_weight
         self.precision = None            # None -> _native.default_precision() ('auto' == exact until told otherwise)
-        self.split_fp16 = True           # fast tier: 3-product split-fp16 convs (keeps 60 chained convs within 1e-3)
         self._eng = {}                   # (device, mode) -> dict(handle, tensors, ws)
         self._eng_fp = None              # parameter fingerprint the cached engines were built from
         self.last_launches = 0
@@ -72,7 +71,7 @@ class RQVAE(Stage1Model):
         if fp != self._eng_fp:               # weights changed behind the module's own hooks (wrapper load, in-place write)
             self._invalidate_native()
             self._eng_fp = fp
-        key = (str(device), mode, self.split_fp16)
+        key = (str(device), mode)
         if key in self._eng:
             return self._eng[key]
         L = N.lib()
@@ -107,8 +106,7 @@ class RQVAE(Stage1Model):
             if mode == N.MODE_FAST and not name.startswith("encoder.conv_in"):
                 hi = w.to(torch.float16)
                 reg(name, hi)
-                if self.split_fp16:
-                    reg(name + "_lo", (w - hi.float()).to(torch.float16))
+                reg(name + "_lo", (w - hi.float()).to(torch.float16))
             else:
                 reg(name, w)          # exact tier, and the encoder's conv_in in every tier (fp32 FFMA kernels)
 

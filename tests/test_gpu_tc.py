@@ -73,13 +73,10 @@ def test_gemm_tc_large_m_row_chunks(N_out, K, M):
     (2, 8, 8, 256, 512, 3, 0, 0), (3, 16, 16, 512, 512, 1, 0, 1), (1, 64, 64, 256, 256, 3, 0, 1),
     (2, 256, 256, 128, 128, 3, 0, 1), (2, 256, 256, 128, 3, 3, 1, 0), (5, 8, 8, 512, 1536, 1, 0, 0),
     (1, 32, 32, 512, 256, 3, 0, 0), (2, 128, 128, 256, 128, 1, 0, 0)])
-@pytest.mark.parametrize("split", [0, 1])
-def test_conv_tc_matches_fp32_conv(B, H, W, Cin, Cout, ks, nchw, res, split):
+def test_conv_tc_matches_fp32_conv(B, H, W, Cin, Cout, ks, nchw, res):
     g = torch.Generator().manual_seed(B * 1000 + H + Cin + Cout)
     x = torch.randn(B, Cin, H, W, generator=g)
     w = torch.randn(Cout, Cin, ks, ks, generator=g) / (Cin * ks * ks) ** 0.5
-    if not split:                       # single product: operands ARE fp16 values
-        x, w = x.to(torch.float16).float(), w.to(torch.float16).float()
     bias = torch.randn(Cout, generator=g)
     R = torch.randn(B, Cout, H, W, generator=g)
     ref = torch.nn.functional.conv2d(x.double().to(DEV), w.double().to(DEV), bias.double().to(DEV), padding=ks // 2).float()
@@ -88,8 +85,7 @@ def test_conv_tc_matches_fp32_conv(B, H, W, Cin, Cout, ks, nchw, res, split):
     x_nhwc = x.permute(0, 2, 3, 1).contiguous().to(DEV)
     w_ohwi = w.permute(0, 2, 3, 1).contiguous().to(DEV)
     x_hi, w_hi = x_nhwc.half(), w_ohwi.half()
-    x_lo = (x_nhwc - x_hi.float()).half() if split else None
-    w_lo = (w_ohwi - w_hi.float()).half() if split else None
+    x_lo, w_lo = (x_nhwc - x_hi.float()).half(), (w_ohwi - w_hi.float()).half()
     r_nhwc = R.permute(0, 2, 3, 1).contiguous().to(DEV) if res else None
     out = torch.full((B, Cout, H, W) if nchw else (B, H, W, Cout), float("nan"), device=DEV)
     L = N.lib()
@@ -97,33 +93,29 @@ def test_conv_tc_matches_fp32_conv(B, H, W, Cin, Cout, ks, nchw, res, split):
                                  B, H, W, Cin, Cout, ks, nchw, N.stream_ptr()))
     torch.cuda.synchronize()
     got = out if nchw else out.permute(0, 3, 1, 2)
-    # fp32 accumulate of exact fp16 products (split: of fp32-class products): summation order only
-    torch.testing.assert_close(got, ref, rtol=1e-4 if split else 2e-3, atol=1e-4 if split else 2e-3)
+    # fp32 accumulate of fp32-class (split-fp16) products: summation order only
+    torch.testing.assert_close(got, ref, rtol=1e-4, atol=1e-4)
 
 
 @pytest.mark.parametrize("B,Ho,Cin,Cout", [(2, 128, 128, 128), (3, 8, 512, 512), (1, 32, 256, 256), (2, 16, 64, 128)])
-@pytest.mark.parametrize("split", [0, 1])
-def test_conv_tc_stride2_downsample(B, Ho, Cin, Cout, split):
+def test_conv_tc_stride2_downsample(B, Ho, Cin, Cout):
     """layers.py:50-57: F.pad(x, (0,1,0,1)) + 3x3 stride-2 conv, as the same implicit GEMM through an element-strided tensor map"""
     g = torch.Generator().manual_seed(B * 100 + Ho + Cin)
     Hi = 2 * Ho
     x = torch.randn(B, Cin, Hi, Hi, generator=g)
     w = torch.randn(Cout, Cin, 3, 3, generator=g) / (Cin * 9) ** 0.5
-    if not split:
-        x, w = x.half().float(), w.half().float()
     bias = torch.randn(Cout, generator=g)
     ref = torch.nn.functional.conv2d(torch.nn.functional.pad(x.double().to(DEV), (0, 1, 0, 1)), w.double().to(DEV), bias.double().to(DEV),
                                      stride=2).float()
     x_nhwc = x.permute(0, 2, 3, 1).contiguous().to(DEV)
     w_ohwi = w.permute(0, 2, 3, 1).contiguous().to(DEV)
     x_hi, w_hi = x_nhwc.half(), w_ohwi.half()
-    x_lo = (x_nhwc - x_hi.float()).half() if split else None
-    w_lo = (w_ohwi - w_hi.float()).half() if split else None
+    x_lo, w_lo = (x_nhwc - x_hi.float()).half(), (w_ohwi - w_hi.float()).half()
     out = torch.full((B, Ho, Ho, Cout), float("nan"), device=DEV)
     N.check(N.lib().rqb200_dbg_conv_tc(N.ptr(x_hi), N.ptr(w_hi), N.ptr(x_lo), N.ptr(w_lo), N.ptr(bias.to(DEV)), None, N.ptr(out),
                                        B, Ho, Ho, Cin, Cout, 3, 2 << 8, N.stream_ptr()))
     torch.cuda.synchronize()
-    torch.testing.assert_close(out.permute(0, 3, 1, 2), ref, rtol=1e-4 if split else 2e-3, atol=1e-4 if split else 2e-3)
+    torch.testing.assert_close(out.permute(0, 3, 1, 2), ref, rtol=1e-4, atol=1e-4)
 
 
 @pytest.mark.parametrize("M,N_out,K", [(257, 1536, 1536), (2048, 4608, 1536), (1000, 1280, 5120), (4096, 256, 256), (130, 128, 64), (700, 512, 512),

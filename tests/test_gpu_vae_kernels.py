@@ -238,10 +238,12 @@ def conv_gn_inputs(B, H, W, Cin, Cout, seed, r=None, needles=False):
 
 
 def fused_stats(x, w, bias, res, B, H, W, Cin, Cout):
-    """one conv through rqb200_dbg_conv_tc_gn: (its output, the guarded workspace (buffer, view) holding its partial statistics)"""
+    """one conv through rqb200_dbg_conv_tc_gn: (its output, the guarded workspace (buffer, view) holding its partial statistics).
+    x and w are fp16 values, so their split-fp16 lo halves are zero."""
     ws = nan_guarded((ws_doubles(B, H * W),), torch.float64)
     ofull, out = nan_guarded((B, H, W, Cout), torch.float32)
-    N.check(N.lib().rqb200_dbg_conv_tc_gn(N.ptr(x), N.ptr(w), None, None, N.ptr(bias), N.ptr(res), N.ptr(out), N.ptr(ws[1]), B, H, W,
+    x_lo, w_lo = torch.zeros_like(x), torch.zeros_like(w)
+    N.check(N.lib().rqb200_dbg_conv_tc_gn(N.ptr(x), N.ptr(w), N.ptr(x_lo), N.ptr(w_lo), N.ptr(bias), N.ptr(res), N.ptr(out), N.ptr(ws[1]), B, H, W,
                                           Cin, Cout, 3, 0, N.stream_ptr()), "dbg_conv_tc_gn")
     torch.cuda.synchronize()
     assert guard_intact(ofull, out.numel()) and guard_intact(ws[0], ws[1].numel())
