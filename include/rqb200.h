@@ -285,6 +285,15 @@ int rqb200_dbg_gemm_tc(const void* W16, const void* X16, const float* bias, cons
  *   chunks of 128. */
 int rqb200_dbg_gemm_tc_fp8(const void* W8_packed, const float* scale, const void* X16, const float* bias, const float* residual,
                            void* out, int out_is_16, int gelu, float* partial, int N_out, int K, int B, int splits, void* stream);
+/* rqb200_dbg_gemm_tc_epi: one launch of the same GEMM with the epilogue options the AR engine passes (its w_in / w_head launches):
+ *   W: 16-bit [N_out,K] (fmt 0 fp16, 1 bf16) when scale == NULL, else packed E4M3 tiles with row scales scale [N_out] (fmt 0).
+ *   acc[b, n] = sum_k W[n,k] X[b,k] (times scale[n]); mode 0: out f32 [B,N_out] = acc + bias[n] * bias_scale + residual[row0 *
+ *   res_row_stride + r * ld_res + n] with r = b / res_div (res_div > 1) or b, row0 = *res_row_ptr (a device int) or 0 when
+ *   res_row_ptr == NULL (residual nullable; ld_res = 0 broadcasts one row); mode 1: acc + bias * bias_scale rounded to 16 bits; mode 2:
+ *   gelu_erf of it; mode 3: partial [splits,B,N_out] f32 = the per-split accumulators (B <= 256).  Modes 0-2 take splits == 1. */
+int rqb200_dbg_gemm_tc_epi(const void* W, const float* scale, const void* X16, int mode, const float* bias, float bias_scale,
+                           const float* residual, int64_t ld_res, int res_div, const int* res_row_ptr, int64_t res_row_stride,
+                           void* out, float* partial, int N_out, int K, int B, int splits, int fmt, void* stream);
 
 /* rqb200_dbg_rq_quantize: rqb200_rq_quantize with the kernel form forced: 1 = csrc/rq_search.cu (2x4 register tile), 2 =
  * csrc/rq_search2.cu (8x8 register tile, 2-CTA clusters splitting the codebook; fails with RQB200_EINVAL for shapes it does not
@@ -300,9 +309,10 @@ int rqb200_dbg_sample_logits(int algo, const float* logits, const float* q, int 
                              float top_p, int64_t* out_idx, void* stream);
 
 /* rqb200_dbg_conv_tc: one launch of the wgmma implicit-GEMM conv (csrc/conv_tc.cu): X NHWC fp16 [B,H,W,Cin], W OHWI fp16
- * [Cout,ks,ks,Cin], stride 1 "same" padding, out f32 NHWC (+bias, +residual) or NCHW when out_nchw.  X16lo / W16lo (both
+ * [Cout,ks,ks,Cin], stride 1 "same" padding, out f32 NHWC (+bias, +residual; Cout % 16 == 0) or NCHW when out_nchw (+bias only:
+ * a residual is refused with RQB200_EINVAL).  X16lo / W16lo (both
  * required, RQB200_EINVAL when either is NULL): the fp16 "lo" halves (value - fp16(value)) for the split-fp16 products, three
- * per conv.  Operands are fp16 only: out_nchw bit 1 (bf16) is refused with RQB200_EINVAL.  Both refusals come before any CUDA
+ * per conv.  Operands are fp16 only: out_nchw bit 1 (bf16) is refused with RQB200_EINVAL.  Every refusal comes before any CUDA
  * call.  out_nchw bits 8..: stride (2: the Downsample conv, H, W the output extent). */
 int rqb200_dbg_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                        const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,

@@ -716,10 +716,11 @@ static int sm_count() {
     return n;
 }
 
-bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int in_nchw) {
+bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int in_nchw, int out_nchw) {
     if ((stride != 1 && !(stride == 2 && ks == 3)) || in_nchw || (ks != 1 && ks != 3)) return false;
     if (Cin % 64 != 0) return false;
-    if (Cout != 3 && Cout % 128 != 0 && Cout != 64) return false;     // bias/residual float4 path needs Cout % 16 == 0
+    if (Cout != 3 && Cout % 128 != 0 && Cout != 64) return false;
+    if (!out_nchw && Cout % 16 != 0) return false;       // the NHWC epilogue reads bias / residual and stores 16 channels at a time
     auto pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
     return pow2(H) && pow2(W);
 }
@@ -756,6 +757,9 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
                    const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                    cudaStream_t st, int stride, double* gn_part) {
     if (X16lo == nullptr || W16lo == nullptr) return fail(RQB200_EINVAL, "conv_tc: the lo halves X16lo and W16lo are required");
+    // the NHWC epilogue moves 16 channels per access (past the end of `out` unless Cout % 16 == 0); the NCHW one adds no residual
+    if (!out_nchw && Cout % 16 != 0) return fail(RQB200_EINVAL, "conv_tc: an NHWC output needs Cout % 16 == 0");
+    if (out_nchw && residual != nullptr) return fail(RQB200_EINVAL, "conv_tc: an NCHW output takes no residual");
     ConvTcParams p = {};
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ks = ks; p.stride = stride;
     conv_tile(H, W, Cout, ks, stride, p.TW, p.TH, p.NB);
@@ -971,7 +975,7 @@ extern "C" int rqb200_dbg_conv_tc_gn(const void* X16, const void* W16, const voi
                                      const float* residual, float* out, double* gn_part, int B, int H, int W, int Cin, int Cout, int ks,
                                      int out_nchw, void* stream) {
     const int stride = (out_nchw >> 8) > 1 ? (out_nchw >> 8) : 1;
-    if (!rqb::conv_tc_supported(H, W, Cin, Cout, ks, stride, 0)) return rqb::fail(RQB200_EINVAL, "conv_tc: unsupported shape");
+    if (!rqb::conv_tc_supported(H, W, Cin, Cout, ks, stride, 0, out_nchw & 1)) return rqb::fail(RQB200_EINVAL, "conv_tc: unsupported shape");
     if (out_nchw & 2) return rqb::fail(RQB200_EINVAL, "conv_tc: bf16 operands are not supported (fp16 only)");
     return rqb::launch_conv_tc(X16, W16, X16lo, W16lo, bias, residual, out, B, H, W, Cin, Cout, ks, out_nchw & 1, (cudaStream_t)stream,
                                stride, gn_part);

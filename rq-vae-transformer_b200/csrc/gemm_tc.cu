@@ -428,7 +428,8 @@ int launch_gemm_tc(const StreamedWeight& w, const CUtensorMap& tmX, GemmTcParams
 
 }  // namespace rqb
 
-// ---- diagnostic entry points (tests/test_gpu_tc.py, tests/test_gpu_fp8.py, bench.py's roofline leg): one GEMM through the streamer
+// ---- diagnostic entry points (tests/test_gpu_tc.py, tests/test_gpu_fp8.py, tests/test_gpu_tc_kernels.py, bench.py's roofline leg): one
+// GEMM through the streamer
 
 // the GEMM over B activation rows X16 [B, K] fp16 / bf16 with the epilogue the arguments select
 static int dbg_gemm_tc(const rqb::StreamedWeight& w, const void* X16, const float* bias, const float* residual, void* out, int out_is_16,
@@ -458,4 +459,25 @@ extern "C" int rqb200_dbg_gemm_tc_fp8(const void* W8_packed, const float* scale,
     rqb::StreamedWeight w;
     RQB_TRY(rqb::make_streamed_weight(&w, true, W8_packed, scale, N_out, K));
     return dbg_gemm_tc(w, X16, bias, residual, out, out_is_16, gelu, partial, B, splits, 0, stream);
+}
+
+// the streamer with every epilogue option the AR engine uses (w_in's bias_scale and broadcast / indexed position rows, res_div of the
+// batched w_in), through the same launcher as the engine's GEMMs
+extern "C" int rqb200_dbg_gemm_tc_epi(const void* W, const float* scale, const void* X16, int mode, const float* bias, float bias_scale,
+                                      const float* residual, int64_t ld_res, int res_div, const int* res_row_ptr, int64_t res_row_stride,
+                                      void* out, float* partial, int N_out, int K, int B, int splits, int fmt, void* stream) {
+    using namespace rqb;
+    if (mode < GT_F32 || mode > GT_PARTIAL) return fail(RQB200_EINVAL, "dbg_gemm_tc_epi: mode must be 0..3");
+    if ((mode == GT_PARTIAL) != (partial != nullptr)) return fail(RQB200_EINVAL, "dbg_gemm_tc_epi: a partial buffer exactly in mode 3");
+    StreamedWeight w;
+    RQB_TRY(make_streamed_weight(&w, scale != nullptr, W, scale, N_out, K));
+    if (B < 1) return fail(RQB200_EINVAL, "gemm_tc: no activation rows");
+    CUtensorMap tx;
+    RQB_TRY(make_tmap_2d(&tx, X16, 1, (uint64_t)w.K, (uint64_t)B, (uint64_t)w.K * 2, 64, (uint32_t)gemm_tc_chunk_rows(w, B)));
+    GemmTcParams p = {};
+    p.B = B; p.splits = splits; p.mode = mode; p.fmt = fmt;
+    p.bias = bias; p.bias_scale = bias_scale;
+    p.residual = residual; p.ld_res = ld_res; p.res_div = res_div; p.res_row_ptr = res_row_ptr; p.res_row_stride = res_row_stride;
+    p.out = out; p.ld_out = N_out; p.partial = partial;
+    return launch_gemm_tc(w, tx, p, false, (cudaStream_t)stream);
 }

@@ -76,7 +76,7 @@ int launch_vae_attn(const float* qkv, float* out, int B, int HW, int C, cudaStre
 size_t groupnorm_ws_doubles(int B, int HW);
 int launch_gn_stats(const float* X, double* stats_ws, int B, int HW, int C, cudaStream_t st);
 // conv_tc.cu -- wgmma implicit-GEMM conv (fast tier), the large-M rows GEMM on the same kernel, and the fp16 operand producers
-bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int in_nchw);
+bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int in_nchw, int out_nchw);
 int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const void* W16lo, const float* bias,
                    const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                    cudaStream_t st, int stride = 1, double* gn_part = nullptr);

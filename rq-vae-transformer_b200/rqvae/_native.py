@@ -121,6 +121,8 @@ def lib():
     L.rqb200_dbg_gemm_tc.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     L.rqb200_dbg_gemm_tc_fp8.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p] + [C.c_int] * 4 + [C.c_void_p]
+    L.rqb200_dbg_gemm_tc_epi.argtypes = [C.c_void_p] * 3 + [C.c_int, C.c_void_p, C.c_float, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
+                                         C.c_int64, C.c_void_p, C.c_void_p] + [C.c_int] * 5 + [C.c_void_p]
     L.rqb200_dbg_conv_tc.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     L.rqb200_dbg_conv_tc_gn.argtypes = [C.c_void_p] * 8 + [C.c_int] * 7 + [C.c_void_p]
@@ -144,7 +146,7 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_ar_forward_workspace_bytes", "rqb200_ar_trace", "rqb200_ar_last_launches", "rqb200_vae_create",
            "rqb200_vae_destroy", "rqb200_vae_set_tensor", "rqb200_vae_finalize", "rqb200_vae_workspace_bytes",
            "rqb200_vae_decode", "rqb200_vae_decode_code", "rqb200_vae_encode", "rqb200_vae_last_launches",
-           "rqb200_dbg_gemm_tc", "rqb200_dbg_gemm_tc_fp8", "rqb200_dbg_conv_tc", "rqb200_dbg_conv_tc_gn", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
+           "rqb200_dbg_gemm_tc", "rqb200_dbg_gemm_tc_fp8", "rqb200_dbg_gemm_tc_epi", "rqb200_dbg_conv_tc", "rqb200_dbg_conv_tc_gn", "rqb200_dbg_rq_quantize", "rqb200_dbg_sample_logits",
            "rqb200_dbg_rows_gemm", "rqb200_rq_quantize_depthwise", "rqb200_rq_embed_sum_depthwise",
            "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise", "rqb200_ar_log_prob",
            "rqb200_ar_log_prob_workspace_bytes", "rqb200_dbg_log_prob_rows", "rqb200_dbg_attn_step", "rqb200_dbg_prefill_attn", "rqb200_dbg_append_attn",

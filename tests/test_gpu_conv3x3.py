@@ -1,5 +1,6 @@
-"""The input-stationary 3x3 stride-1 conv (conv3x3_tc_kernel, csrc/conv_tc.cu) on every 3x3 shape the ImageNet / FFHQ (f16) and f8
-decoders run, against an fp64 conv of the very operands the kernel multiplies (hi + lo: the split-fp16 products)."""
+"""The 3x3 stride-1 convs (csrc/conv_tc.cu) on every 3x3 shape the ImageNet / FFHQ (f16) and f8 decoders run, against an fp64 conv
+of the very operands the kernel multiplies (hi + lo: the split-fp16 products).  Cout % 128 == 0 -- every shape here but Cout = 3 and
+64 -- runs conv3x3_wreg_kernel; conv_out (Cout = 3) and Cout = 64 run the input-stationary conv3x3_tc_kernel."""
 import pytest
 import torch
 
