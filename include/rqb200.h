@@ -269,6 +269,17 @@ int rqb200_vae_decode_code(rqb200_vae* h, const int64_t* codes, int B, float* ou
 int rqb200_vae_encode(rqb200_vae* h, const float* x, int B, float* z_e, void* workspace, size_t workspace_bytes,
                       void* stream);
 int64_t rqb200_vae_last_launches(const rqb200_vae* h);
+/* Any image size (the reference's RQ-VAE is fully convolutional): the same calls on B images of H x W pixels, H and W positive
+ * multiples of f = 2^(n_levels - 1) (RQB200_EINVAL otherwise; the workspace query returns 0).  Which levels carry an AttnBlock
+ * follows the configured resolution ladder, as in the reference.  The calls above are these at H = W = resolution. */
+size_t rqb200_vae_workspace_bytes_hw(const rqb200_vae* h, int B, int H, int W);
+/* x [B,in_channels,H,W] f32 NCHW -> z_e [B,H/f,W/f,embed_dim] f32 NHWC */
+int rqb200_vae_encode_hw(rqb200_vae* h, const float* x, int B, int H, int W, float* z_e, void* workspace, size_t workspace_bytes,
+                         void* stream);
+/* z_q [B,hl,wl,embed_dim] f32 NHWC (hl, wl the latent extent) -> out [B,out_ch,hl f,wl f] f32 NCHW; its workspace is
+ * rqb200_vae_workspace_bytes_hw(h, B, hl f, wl f) */
+int rqb200_vae_decode_hw(rqb200_vae* h, const float* z_q, int B, int hl, int wl, float* out, void* workspace, size_t workspace_bytes,
+                         void* stream);
 
 /* ------------------------------------------------------------------------------------------------ diagnostics
  * Single-kernel entry points used by tests/ and bench.py's roofline leg; not part of the reference-facing surface.
@@ -394,6 +405,9 @@ int rqb200_dbg_cast_f16(const float* X, void* Y16, void* Y16lo, int B, int H, in
  *   keys of (q k^T * float(1 / sqrt(C))) v, single head.  RQB200_EINVAL, with nothing launched, when the C + HW floats of the query
  *   and its scores do not fit in shared memory beside the kernel's static shared memory within 48 KB (C + HW > about 12000). */
 int rqb200_dbg_vae_attn(const float* qkv, float* out, int B, int HW, int C, void* stream);
+/* rqb200_dbg_vae_attn_tc: the same attention on the tensor-core kernel the fast tier runs on maps past 1024 tokens (fp16 operands,
+ *   fp32 scores, softmax and accumulators; no shared-memory limit on HW).  C must be 128, 256, 384 or 512 (RQB200_EINVAL). */
+int rqb200_dbg_vae_attn_tc(const float* qkv, float* out, int B, int HW, int C, void* stream);
 
 #ifdef __cplusplus
 }

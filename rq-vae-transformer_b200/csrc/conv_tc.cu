@@ -721,13 +721,14 @@ bool conv_tc_supported(int H, int W, int Cin, int Cout, int ks, int stride, int 
     if (Cin % 64 != 0) return false;
     if (Cout != 3 && Cout % 128 != 0 && Cout != 64) return false;
     if (!out_nchw && Cout % 16 != 0) return false;       // the NHWC epilogue reads bias / residual and stores 16 channels at a time
-    auto pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
-    return pow2(H) && pow2(W);
+    return H > 0 && W > 0;
 }
 
 // output tile of one CTA, TW x TH x NB pixels.  3x3 stride 1, 8 pixels wide: Cout % 128 == 0 (conv3x3_wreg_kernel) 32 rows
 // (256 pixels), 16 rows, or 8 rows of NB = 2 images below 16 rows; other Cout (conv3x3_tc_kernel) 16 rows, or 8 rows of NB = 2
-// images below 16 rows.  Maps narrower or lower than the tile leave the out-of-range part of it unstored.  Else 128 pixels.
+// images below 16 rows.  Else (conv_tc_kernel) 128 pixels: TW and TH the powers of two at or above W and H, capped at 16 and
+// 128 / TW.  Maps narrower or lower than the tile, or not a multiple of it, leave the out-of-range part of it unstored; the TMA
+// box reads zeros there.
 static bool conv3x3_wreg(int Cout, int ks, int stride) { return ks == 3 && stride == 1 && Cout % 128 == 0; }
 
 static void conv_tile(int H, int W, int Cout, int ks, int stride, int& TW, int& TH, int& NB) {
@@ -736,8 +737,9 @@ static void conv_tile(int H, int W, int Cout, int ks, int stride, int& TW, int& 
         TH = conv3x3_wreg(Cout, ks, stride) && H >= 32 ? 32 : (H > 8 ? 16 : 8);
         NB = TH == 8 ? 2 : 1;
     } else {
-        TW = W < 16 ? W : 16;
-        TH = (128 / TW) < H ? (128 / TW) : H;
+        auto pow2_ceil = [](int v) { int p = 1; while (p < v) p *= 2; return p; };
+        TW = pow2_ceil(W < 16 ? W : 16);
+        TH = pow2_ceil(H < 128 / TW ? H : 128 / TW);
         NB = 128 / (TW * TH);
     }
 }
@@ -764,7 +766,6 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ks = ks; p.stride = stride;
     conv_tile(H, W, Cout, ks, stride, p.TW, p.TH, p.NB);
     const bool c3 = ks == 3 && stride == 1;
-    if (!c3 && p.TW * p.TH * p.NB != 128) return fail(RQB200_EINVAL, "conv_tc: feature map extent must be a power of two");
     p.tiles_x = (int)ceil_div(W, p.TW); p.tiles_y = (int)ceil_div(H, p.TH); p.tiles_b = (int)ceil_div(B, p.NB);
     // 3x3: 128 output channels per tile (conv3x3_wreg_kernel), or 16 | 64 (conv3x3_tc_kernel)
     const int BN = Cout <= 16 ? 16 : (Cout % 256 == 0 && !c3 ? 256 : (Cout % 128 == 0 ? 128 : 64));

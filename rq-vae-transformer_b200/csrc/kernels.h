@@ -73,6 +73,8 @@ int launch_conv(const float* X, const void* W, int wdtype, const float* bias, co
 int launch_groupnorm_silu(const float* X, const float* gamma, const float* beta, float* Y, double* stats_ws, int B, int HW,
                           int C, int silu, cudaStream_t st);
 int launch_vae_attn(const float* qkv, float* out, int B, int HW, int C, cudaStream_t st);
+// vae_attn_tc.cu -- the same attention on the tensor cores (fp16 operands, fp32 softmax and accumulators), C = 128 | 256 | 384 | 512
+int launch_vae_attn_tc(const float* qkv, float* out, int B, int HW, int C, cudaStream_t st);
 size_t groupnorm_ws_doubles(int B, int HW);
 int launch_gn_stats(const float* X, double* stats_ws, int B, int HW, int C, cudaStream_t st);
 // conv_tc.cu -- wgmma implicit-GEMM conv (fast tier), the large-M rows GEMM on the same kernel, and the fp16 operand producers

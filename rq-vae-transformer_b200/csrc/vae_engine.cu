@@ -26,8 +26,9 @@ struct rqb200_vae {
     bool enc_fast = false;    // the encoder's convs were registered in fp16 as well: encode on the wgmma path
     bool gn_fuse = true;      // conv epilogues emit the next GroupNorm's partial statistics (mode bit RQB200_VAE_NO_GN_FUSE clears it)
     int64_t last_launches = 0;
-    int64_t max_act = 0;      // max H*W*C per image over all activations
-    int64_t max_gn_hw = 0;
+    // the activation sizes of the last pixel extent a workspace was laid out for (vae_layout's dry walk, cached)
+    mutable int ext_h = 0, ext_w = 0;
+    mutable int64_t ext_act = 0, ext_gn_hw = 0;
     rqb::RqTables codebooks{};   // decode_code's embedding tables, resolved by finalize from "codebook" or "codebook.<d>"
 };
 
@@ -61,6 +62,9 @@ struct VaeRun {
     // fast tier: a conv whose output feeds a GroupNorm emits that GroupNorm's partial statistics from its epilogue
     const float* stats_buf = nullptr;         // conv output whose statistics sit in gn_ws
     int stats_chunks = 0;
+    // what a dry walk measures for the workspace
+    int64_t max_act = 0;                      // max H*W*C per image over all activations
+    int64_t max_gn_hw = 0;
 
     const VTensor* get(const std::string& k, int64_t numel) {
         auto it = h->t.find(k);
@@ -70,7 +74,7 @@ struct VaeRun {
         }
         return &it->second;
     }
-    void note_act(int64_t hw, int64_t c) { if (hw * c > h->max_act) h->max_act = hw * c; }
+    void note_act(int64_t hw, int64_t c) { if (hw * c > max_act) max_act = hw * c; }
 
     // x as a conv operand: itself on the exact tier; on the fast tier its fp16 copy, cast into slot (x2 nearest upsampled if asked)
     int operand(const float* x, int H, int W, int C, int slot, int upsample, Operand* o) {
@@ -83,7 +87,7 @@ struct VaeRun {
     int norm(const std::string& name, const float* in, float* out, int HW, int C, int silu, Operand* o) {
         const VTensor* g = get(name + ".weight", C);
         const VTensor* b = get(name + ".bias", C);
-        if (HW > h->max_gn_hw) h->max_gn_hw = HW;
+        if (HW > max_gn_hw) max_gn_hw = HW;
         note_act(HW, C);
         *o = fast ? Operand{nullptr, 0, 0, 0} : Operand{out, -1, 0, 0};
         if (dry || !g || !b) return 0;
@@ -140,107 +144,137 @@ struct VaeRun {
         RQB_TRY(norm(p + ".norm", buf[cur], buf[a], H * W, C, 0, &x));
         // fused q|k|v 1x1 conv: key "<p>.qkv" registered by the host binding ([3C,1,1,C] / [3C])
         RQB_TRY(conv(p + ".qkv", x, buf[b], nullptr, H, W, C, 3 * C, 1, 1, false, 0));
-        if (!dry && missing.empty()) RQB_TRY(launch_vae_attn(buf[b], buf[a], B, H * W, C, st));
+        // the fast tier runs maps past 1024 tokens on the tensor-core kernel; up to 1024 (every shipped VAE at its configured
+        // resolution) both tiers keep the fp32 kernel
+        if (!dry && missing.empty())
+            RQB_TRY(fast && H * W > 1024 ? launch_vae_attn_tc(buf[b], buf[a], B, H * W, C, st) : launch_vae_attn(buf[b], buf[a], B, H * W, C, st));
         RQB_TRY(operand(buf[a], H, W, C, 0, 0, &x));
         RQB_TRY(conv(p + ".proj_out", x, buf[c], buf[cur], H, W, C, C, 1, 1, true, 0));
         cur = c;
         return 0;
     }
-    bool has_attn(int res) const {
-        for (int i = 0; i < h->cfg.n_attn_res; i++) if (h->cfg.attn_resolutions[i] == res) return true;
+    // which levels carry an AttnBlock follows the CONFIGURED resolution ladder (the reference's Encoder / Decoder decide it at
+    // construction from ddconfig["resolution"], modules.py:29-50,117-160), whatever extent the call walks
+    bool has_attn(int cres) const {
+        for (int i = 0; i < h->cfg.n_attn_res; i++) if (h->cfg.attn_resolutions[i] == cres) return true;
         return false;
     }
 
-    // Decoder.forward (modules.py:171-202) preceded by post_quant_conv (rqvae.py:87).  z NHWC [B,r,r,embed_dim].
-    int decode(const float* z, float* out) {
+    // Decoder.forward (modules.py:171-202) preceded by post_quant_conv (rqvae.py:87).  z NHWC [B,H,W,embed_dim], H x W the latent
+    // extent; out NCHW [B,out_ch,H f,W f].  cres: the level's resolution in the configured ladder.
+    int decode(const float* z, float* out, int H, int W) {
         fast = h->fast_ok;
         const rqb200_vae_config& c = h->cfg;
         const int nl = c.n_levels, nb = c.num_res_blocks;
-        int res = c.resolution >> (nl - 1), ch = c.ch * c.ch_mult[nl - 1], cur = 0;
+        int cres = c.resolution >> (nl - 1), ch = c.ch * c.ch_mult[nl - 1], cur = 0;
         Operand x;
-        RQB_TRY(operand(z, res, res, c.embed_dim, 0, 0, &x));
-        RQB_TRY(conv("post_quant_conv", x, buf[1], nullptr, res, res, c.embed_dim, c.z_channels, 1, 1, false, 0));
-        RQB_TRY(operand(buf[1], res, res, c.z_channels, 0, 0, &x));
-        RQB_TRY(conv("decoder.conv_in", x, buf[0], nullptr, res, res, c.z_channels, ch, 3, 1, true, 0));
-        RQB_TRY(resblock("decoder.mid.block_1", cur, res, res, ch, ch));
-        RQB_TRY(attnblock("decoder.mid.attn_1", cur, res, res, ch));
-        RQB_TRY(resblock("decoder.mid.block_2", cur, res, res, ch, ch));
+        RQB_TRY(operand(z, H, W, c.embed_dim, 0, 0, &x));
+        RQB_TRY(conv("post_quant_conv", x, buf[1], nullptr, H, W, c.embed_dim, c.z_channels, 1, 1, false, 0));
+        RQB_TRY(operand(buf[1], H, W, c.z_channels, 0, 0, &x));
+        RQB_TRY(conv("decoder.conv_in", x, buf[0], nullptr, H, W, c.z_channels, ch, 3, 1, true, 0));
+        RQB_TRY(resblock("decoder.mid.block_1", cur, H, W, ch, ch));
+        RQB_TRY(attnblock("decoder.mid.attn_1", cur, H, W, ch));
+        RQB_TRY(resblock("decoder.mid.block_2", cur, H, W, ch, ch));
         for (int lvl = nl - 1; lvl >= 0; lvl--) {
             const int cout = c.ch * c.ch_mult[lvl];
             const std::string p = "decoder.up." + std::to_string(lvl);
             for (int b = 0; b <= nb; b++) {
-                RQB_TRY(resblock(p + ".block." + std::to_string(b), cur, res, res, ch, cout));
+                RQB_TRY(resblock(p + ".block." + std::to_string(b), cur, H, W, ch, cout));
                 ch = cout;
-                if (has_attn(res)) RQB_TRY(attnblock(p + ".attn." + std::to_string(b), cur, res, res, ch));
+                if (has_attn(cres)) RQB_TRY(attnblock(p + ".attn." + std::to_string(b), cur, H, W, ch));
             }
             if (lvl != 0) {
                 const int nxt = (cur + 1) & 3;
-                RQB_TRY(operand(buf[cur], res, res, ch, 1, 1, &x));
-                RQB_TRY(conv(p + ".upsample.conv", x, buf[nxt], nullptr, res, res, ch, ch, 3, 1, true, 0));
+                RQB_TRY(operand(buf[cur], H, W, ch, 1, 1, &x));
+                RQB_TRY(conv(p + ".upsample.conv", x, buf[nxt], nullptr, H, W, ch, ch, 3, 1, true, 0));
                 cur = nxt;
-                res *= 2;
+                cres *= 2;
+                H *= 2;
+                W *= 2;
             }
         }
-        RQB_TRY(norm("decoder.norm_out", buf[cur], buf[(cur + 1) & 3], res * res, ch, 1, &x));
-        return conv("decoder.conv_out", x, out, nullptr, res, res, ch, c.out_ch, 3, 1, false, 1);
+        RQB_TRY(norm("decoder.norm_out", buf[cur], buf[(cur + 1) & 3], H * W, ch, 1, &x));
+        return conv("decoder.conv_out", x, out, nullptr, H, W, ch, c.out_ch, 3, 1, false, 1);
     }
 
-    // Encoder.forward (modules.py:73-98) followed by quant_conv (rqvae.py:82).  x NCHW -> z_e NHWC.  The fast tier needs the
-    // encoder's convs registered in fp16 (enc_fast); conv_in (Cin = 3, NCHW fp32 input, 0.3 % of the encoder's flops) runs the
-    // fp32 FFMA kernel on both tiers.
-    int encode(const float* x, float* z_e) {
+    // Encoder.forward (modules.py:73-98) followed by quant_conv (rqvae.py:82).  x NCHW [B,in_channels,H,W] -> z_e NHWC
+    // [B,H/f,W/f,embed_dim].  The fast tier needs the encoder's convs registered in fp16 (enc_fast); conv_in (Cin = 3, NCHW fp32
+    // input, 0.3 % of the encoder's flops) runs the fp32 FFMA kernel on both tiers.
+    int encode(const float* x, float* z_e, int H, int W) {
         fast = h->fast_ok && h->enc_fast;
         const rqb200_vae_config& c = h->cfg;
         const int nl = c.n_levels, nb = c.num_res_blocks;
-        int res = c.resolution, ch = c.ch, cur = 0;
-        RQB_TRY(conv("encoder.conv_in", Operand{x, -1, 0, 1}, buf[0], nullptr, res, res, c.in_channels, ch, 3, 1, false, 0));
+        int cres = c.resolution, ch = c.ch, cur = 0;
+        RQB_TRY(conv("encoder.conv_in", Operand{x, -1, 0, 1}, buf[0], nullptr, H, W, c.in_channels, ch, 3, 1, false, 0));
         Operand o;
         for (int lvl = 0; lvl < nl; lvl++) {
             const int cout = c.ch * c.ch_mult[lvl];
             const std::string p = "encoder.down." + std::to_string(lvl);
             for (int b = 0; b < nb; b++) {
-                RQB_TRY(resblock(p + ".block." + std::to_string(b), cur, res, res, ch, cout));
+                RQB_TRY(resblock(p + ".block." + std::to_string(b), cur, H, W, ch, cout));
                 ch = cout;
-                if (has_attn(res)) RQB_TRY(attnblock(p + ".attn." + std::to_string(b), cur, res, res, ch));
+                if (has_attn(cres)) RQB_TRY(attnblock(p + ".attn." + std::to_string(b), cur, H, W, ch));
             }
             if (lvl != nl - 1) {
                 const int nxt = (cur + 1) & 3;
-                RQB_TRY(operand(buf[cur], res, res, ch, 1, 0, &o));
-                RQB_TRY(conv(p + ".downsample.conv", o, buf[nxt], nullptr, res, res, ch, ch, 3, 2, true, 0));
+                RQB_TRY(operand(buf[cur], H, W, ch, 1, 0, &o));
+                RQB_TRY(conv(p + ".downsample.conv", o, buf[nxt], nullptr, H, W, ch, ch, 3, 2, true, 0));
                 cur = nxt;
-                res /= 2;
+                cres /= 2;
+                H /= 2;
+                W /= 2;
             }
         }
-        RQB_TRY(resblock("encoder.mid.block_1", cur, res, res, ch, ch));
-        RQB_TRY(attnblock("encoder.mid.attn_1", cur, res, res, ch));
-        RQB_TRY(resblock("encoder.mid.block_2", cur, res, res, ch, ch));
+        RQB_TRY(resblock("encoder.mid.block_1", cur, H, W, ch, ch));
+        RQB_TRY(attnblock("encoder.mid.attn_1", cur, H, W, ch));
+        RQB_TRY(resblock("encoder.mid.block_2", cur, H, W, ch, ch));
         float* zc = buf[(cur + 2) & 3];
-        RQB_TRY(norm("encoder.norm_out", buf[cur], buf[(cur + 1) & 3], res * res, ch, 1, &o));
-        RQB_TRY(conv("encoder.conv_out", o, zc, nullptr, res, res, ch, c.z_channels, 3, 1, false, 0));
-        RQB_TRY(operand(zc, res, res, c.z_channels, 0, 0, &o));
-        return conv("quant_conv", o, z_e, nullptr, res, res, c.z_channels, c.embed_dim, 1, 1, false, 0);
+        RQB_TRY(norm("encoder.norm_out", buf[cur], buf[(cur + 1) & 3], H * W, ch, 1, &o));
+        RQB_TRY(conv("encoder.conv_out", o, zc, nullptr, H, W, ch, c.z_channels, 3, 1, false, 0));
+        RQB_TRY(operand(zc, H, W, c.z_channels, 0, 0, &o));
+        return conv("quant_conv", o, z_e, nullptr, H, W, c.z_channels, c.embed_dim, 1, 1, false, 0);
     }
 };
 
-static size_t vae_layout(const rqb200_vae* h, int B, void* base, size_t cap, VaeRun* run) {
+// the downsampling factor f = 2^(n_levels - 1): an image's H and W must be positive multiples of it
+static int vae_factor(const rqb200_vae* h) { return 1 << (h->cfg.n_levels - 1); }
+static bool vae_extent_ok(const rqb200_vae* h, int H, int W) {
+    const int f = vae_factor(h);
+    return H > 0 && W > 0 && H % f == 0 && W % f == 0;
+}
+
+// the workspace of a call on B images of H x W pixels: the activation sizes come from a dry walk of both networks at that extent;
+// decode_code's zq staging stays at the configured latent grid
+static size_t vae_layout(const rqb200_vae* h, int B, int H, int W, void* base, size_t cap, VaeRun* run) {
+    if (H != h->ext_h || W != h->ext_w) {
+        VaeRun d{const_cast<rqb200_vae*>(h), nullptr, 1, true, {nullptr, nullptr, nullptr, nullptr}, nullptr, ""};
+        const int f = vae_factor(h);
+        d.decode(nullptr, nullptr, H / f, W / f);
+        d.encode(nullptr, nullptr, H, W);
+        h->ext_h = H;
+        h->ext_w = W;
+        h->ext_act = d.max_act;
+        h->ext_gn_hw = d.max_gn_hw;
+    }
+    const int64_t max_act = h->ext_act;
     Arena a(base, cap);
     for (int i = 0; i < 4; i++) {
-        float* p = a.take<float>((size_t)B * h->max_act);
+        float* p = a.take<float>((size_t)B * max_act);
         if (run) run->buf[i] = p;
     }
-    double* g = a.take<double>(groupnorm_ws_doubles(B, (int)h->max_gn_hw));
+    double* g = a.take<double>(groupnorm_ws_doubles(B, (int)h->ext_gn_hw));
     if (run) run->gn_ws = g;
     const rqb200_vae_config& c = h->cfg;
     int r = c.resolution >> (c.n_levels - 1);
     float* zq = a.take<float>((size_t)B * r * r * c.embed_dim);
     if (run) run->zq = zq;
     for (int i = 0; i < 2; i++) {
-        __half* p16 = a.take<__half>((size_t)B * h->max_act);
+        __half* p16 = a.take<__half>((size_t)B * max_act);
         if (run) run->h16[i] = p16;
     }
     if (h->fast_ok)
         for (int i = 0; i < 2; i++) {
-            __half* p16 = a.take<__half>((size_t)B * h->max_act);
+            __half* p16 = a.take<__half>((size_t)B * max_act);
             if (run) run->l16[i] = p16;
         }
     return a.off + 256;
@@ -268,13 +302,13 @@ int rqb200_vae_set_tensor(rqb200_vae* h, const char* key, const void* ptr, int d
 int rqb200_vae_finalize(rqb200_vae* h) {
     if (!h) return rqb::fail(RQB200_EINVAL, "vae_finalize: null handle");
     rqb::VaeRun run{h, nullptr, 1, true, {nullptr, nullptr, nullptr, nullptr}, nullptr, ""};
-    h->max_act = 0;
-    h->max_gn_hw = 0;
+    h->ext_h = h->ext_w = 0;
     {
         const rqb200_vae_config& c = h->cfg;
-        int r = c.resolution >> (c.n_levels - 1);
+        if (c.resolution < 1 || c.resolution % rqb::vae_factor(h))
+            return rqb::fail(RQB200_EINVAL, "vae_finalize: resolution must be a positive multiple of 2^(n_levels - 1)");
         bool ok = (c.mode & 0xff) == RQB200_MODE_FAST && c.ch % 128 == 0 && c.z_channels % 128 == 0 && c.embed_dim % 128 == 0 &&
-                  c.out_ch == 3 && r > 0 && (r & (r - 1)) == 0;
+                  c.out_ch == 3;
         h->fast_ok = ok;
         h->gn_fuse = !(c.mode & RQB200_VAE_NO_GN_FUSE);
     }
@@ -282,8 +316,9 @@ int rqb200_vae_finalize(rqb200_vae* h) {
         auto it = h->t.find("encoder.conv_out.weight");
         h->enc_fast = h->fast_ok && it != h->t.end() && it->second.dtype == RQB200_F16;
     }
-    run.decode(nullptr, nullptr);
-    run.encode(nullptr, nullptr);
+    const int R = h->cfg.resolution, f = rqb::vae_factor(h);
+    run.decode(nullptr, nullptr, R / f, R / f);
+    run.encode(nullptr, nullptr, R, R);
     if (!run.missing.empty()) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor " + run.missing);
     {
         const rqb200_vae_config& c = h->cfg;
@@ -311,49 +346,75 @@ int rqb200_vae_finalize(rqb200_vae* h) {
 
 size_t rqb200_vae_workspace_bytes(const rqb200_vae* h, int B) {
     if (!h || !h->finalized || B <= 0) return 0;
-    return rqb::vae_layout(h, B, nullptr, 0, nullptr);
+    return rqb::vae_layout(h, B, h->cfg.resolution, h->cfg.resolution, nullptr, 0, nullptr);
 }
 
-static int vae_prepare(rqb200_vae* h, int B, void* ws, size_t ws_bytes, void* stream, rqb::VaeRun* run) {
+size_t rqb200_vae_workspace_bytes_hw(const rqb200_vae* h, int B, int H, int W) {
+    if (!h || !h->finalized || B <= 0 || !rqb::vae_extent_ok(h, H, W)) return 0;
+    return rqb::vae_layout(h, B, H, W, nullptr, 0, nullptr);
+}
+
+// H, W: the call's pixel extent
+static int vae_prepare(rqb200_vae* h, int B, int H, int W, void* ws, size_t ws_bytes, void* stream, rqb::VaeRun* run) {
     if (!h || !ws) return rqb::fail(RQB200_EINVAL, "vae: null argument");
     if (!h->finalized) return rqb::fail(RQB200_ESTATE, "vae: engine not finalised");
     if (B <= 0) return rqb::fail(RQB200_EINVAL, "vae: B must be > 0");
+    if (!rqb::vae_extent_ok(h, H, W))
+        return rqb::fail(RQB200_EINVAL, "vae: H and W must be positive multiples of 2^(n_levels - 1) = " + std::to_string(rqb::vae_factor(h)));
     if (rqb200_device_count() <= 0) return rqb::fail(RQB200_ENODEV, "vae: no CUDA device");
     *run = rqb::VaeRun{h, (cudaStream_t)stream, B, false, {nullptr, nullptr, nullptr, nullptr}, nullptr, ""};
-    size_t need = rqb::vae_layout(h, B, ws, ws_bytes, run);
+    size_t need = rqb::vae_layout(h, B, H, W, ws, ws_bytes, run);
     if (need > ws_bytes) return rqb::fail(RQB200_EWORKSPACE, "vae: workspace too small");
     rqb::g_launches = 0;
     return 0;
 }
 
-int rqb200_vae_decode(rqb200_vae* h, const float* z_q, int B, float* out, void* workspace, size_t workspace_bytes,
-                      void* stream) {
+int rqb200_vae_decode_hw(rqb200_vae* h, const float* z_q, int B, int hl, int wl, float* out, void* workspace, size_t workspace_bytes,
+                         void* stream) {
+    if (!h) return rqb::fail(RQB200_EINVAL, "vae: null argument");
+    if (hl <= 0 || wl <= 0) return rqb::fail(RQB200_EINVAL, "vae_decode: the latent extent must be positive");
+    const int f = rqb::vae_factor(h);
+    if ((int64_t)hl * f > (1 << 20) || (int64_t)wl * f > (1 << 20)) return rqb::fail(RQB200_EINVAL, "vae_decode: latent extent too large");
     rqb::VaeRun run;
-    RQB_TRY(vae_prepare(h, B, workspace, workspace_bytes, stream, &run));
-    int rc = run.decode(z_q, out);
+    RQB_TRY(vae_prepare(h, B, hl * f, wl * f, workspace, workspace_bytes, stream, &run));
+    int rc = run.decode(z_q, out, hl, wl);
     h->last_launches = rqb::g_launches;
     return rc;
 }
 
+int rqb200_vae_decode(rqb200_vae* h, const float* z_q, int B, float* out, void* workspace, size_t workspace_bytes,
+                      void* stream) {
+    if (!h) return rqb::fail(RQB200_EINVAL, "vae: null argument");
+    const int r = h->cfg.resolution / rqb::vae_factor(h);
+    return rqb200_vae_decode_hw(h, z_q, B, r, r, out, workspace, workspace_bytes, stream);
+}
+
 int rqb200_vae_decode_code(rqb200_vae* h, const int64_t* codes, int B, float* out, void* workspace,
                            size_t workspace_bytes, void* stream) {
+    if (!h) return rqb::fail(RQB200_EINVAL, "vae: null argument");
     rqb::VaeRun run;
-    RQB_TRY(vae_prepare(h, B, workspace, workspace_bytes, stream, &run));
     const rqb200_vae_config& c = h->cfg;
+    RQB_TRY(vae_prepare(h, B, c.resolution, c.resolution, workspace, workspace_bytes, stream, &run));
     int r = c.resolution >> (c.n_levels - 1);
     RQB_TRY(rqb::launch_rq_embed(codes, h->codebooks, (int64_t)B * r * r, c.depth, c.embed_dim, run.zq, true, (cudaStream_t)stream));
-    int rc = run.decode(run.zq, out);
+    int rc = run.decode(run.zq, out, r, r);
+    h->last_launches = rqb::g_launches;
+    return rc;
+}
+
+int rqb200_vae_encode_hw(rqb200_vae* h, const float* x, int B, int H, int W, float* z_e, void* workspace, size_t workspace_bytes,
+                         void* stream) {
+    rqb::VaeRun run;
+    RQB_TRY(vae_prepare(h, B, H, W, workspace, workspace_bytes, stream, &run));
+    int rc = run.encode(x, z_e, H, W);
     h->last_launches = rqb::g_launches;
     return rc;
 }
 
 int rqb200_vae_encode(rqb200_vae* h, const float* x, int B, float* z_e, void* workspace, size_t workspace_bytes,
                       void* stream) {
-    rqb::VaeRun run;
-    RQB_TRY(vae_prepare(h, B, workspace, workspace_bytes, stream, &run));
-    int rc = run.encode(x, z_e);
-    h->last_launches = rqb::g_launches;
-    return rc;
+    if (!h) return rqb::fail(RQB200_EINVAL, "vae: null argument");
+    return rqb200_vae_encode_hw(h, x, B, h->cfg.resolution, h->cfg.resolution, z_e, workspace, workspace_bytes, stream);
 }
 int64_t rqb200_vae_last_launches(const rqb200_vae* h) { return h ? h->last_launches : 0; }
 
@@ -400,5 +461,14 @@ int rqb200_dbg_vae_attn(const float* qkv, float* out, int B, int HW, int C, void
     if (!qkv || !out) return fail(RQB200_EINVAL, "dbg_vae_attn: null argument");
     if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_vae_attn: no CUDA device");
     return launch_vae_attn(qkv, out, B, HW, C, (cudaStream_t)stream);
+}
+
+int rqb200_dbg_vae_attn_tc(const float* qkv, float* out, int B, int HW, int C, void* stream) {
+    using namespace rqb;
+    if (B < 1 || HW < 1 || C < 1) return fail(RQB200_EINVAL, "dbg_vae_attn_tc: need B, HW, C >= 1");
+    if (!qkv || !out) return fail(RQB200_EINVAL, "dbg_vae_attn_tc: null argument");
+    if (C != 128 && C != 256 && C != 384 && C != 512) return fail(RQB200_EINVAL, "dbg_vae_attn_tc: C must be 128, 256, 384 or 512");
+    if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_vae_attn_tc: no CUDA device");
+    return launch_vae_attn_tc(qkv, out, B, HW, C, (cudaStream_t)stream);
 }
 }

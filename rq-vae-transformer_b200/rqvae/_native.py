@@ -116,6 +116,10 @@ def lib():
     L.rqb200_vae_workspace_bytes.argtypes = [C.c_void_p, C.c_int]
     for fn in (L.rqb200_vae_decode, L.rqb200_vae_decode_code, L.rqb200_vae_encode):
         fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.rqb200_vae_workspace_bytes_hw.restype = C.c_size_t
+    L.rqb200_vae_workspace_bytes_hw.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
+    for fn in (L.rqb200_vae_decode_hw, L.rqb200_vae_encode_hw):
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.rqb200_vae_last_launches.restype = C.c_int64
     L.rqb200_vae_last_launches.argtypes = [C.c_void_p]
     L.rqb200_dbg_gemm_tc.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
@@ -136,6 +140,7 @@ def lib():
     L.rqb200_dbg_groupnorm.argtypes = [C.c_int] + [C.c_void_p] * 7 + [C.c_int64] + [C.c_int] * 4 + [C.c_void_p]
     L.rqb200_dbg_cast_f16.argtypes = [C.c_void_p] * 3 + [C.c_int] * 5 + [C.c_void_p]
     L.rqb200_dbg_vae_attn.argtypes = [C.c_void_p] * 2 + [C.c_int] * 3 + [C.c_void_p]
+    L.rqb200_dbg_vae_attn_tc.argtypes = [C.c_void_p] * 2 + [C.c_int] * 3 + [C.c_void_p]
     _lib = L
     return L
 
@@ -151,7 +156,8 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_rq_embed_depth_depthwise", "rqb200_dbg_rq_quantize_depthwise", "rqb200_ar_log_prob",
            "rqb200_ar_log_prob_workspace_bytes", "rqb200_dbg_log_prob_rows", "rqb200_dbg_attn_step", "rqb200_dbg_prefill_attn", "rqb200_dbg_append_attn",
            "rqb200_dbg_ln", "rqb200_dbg_act_reduce", "rqb200_dbg_vae_conv", "rqb200_dbg_groupnorm", "rqb200_dbg_cast_f16",
-           "rqb200_dbg_vae_attn"]
+           "rqb200_dbg_vae_attn", "rqb200_vae_workspace_bytes_hw", "rqb200_vae_encode_hw", "rqb200_vae_decode_hw",
+           "rqb200_dbg_vae_attn_tc"]
 
 
 def check(rc, what=""):

@@ -141,45 +141,66 @@ class RQVAE(Stage1Model):
         self._eng[key] = eng
         return eng
 
-    def _ws(self, eng, B, device):
-        need = N.lib().rqb200_vae_workspace_bytes(eng["handle"], B)
+    def _ws(self, eng, B, device, hw):
+        """the workspace for B images of hw = (H, W) pixels; the largest buffer so far is kept"""
+        need = N.lib().rqb200_vae_workspace_bytes_hw(eng["handle"], B, *hw)
         ws = eng["ws"].get("buf")
         if ws is None or ws.numel() < need:
             eng["ws"]["buf"] = ws = torch.empty(need, dtype=torch.uint8, device=device)
         return ws, need
 
-    def _run(self, fn_name, x, out_shape):
+    def _run(self, fn_name, x, out_shape, hw, ext=()):
+        """one native call on x -> out_shape.  hw: the call's pixel extent (H, W); ext: the extent arguments the *_hw entry points
+        take after B"""
         N.require_cuda(x)
         eng = self._engine(x.device)
         B = x.shape[0]
         out = torch.empty(out_shape, dtype=torch.float32, device=x.device)
         with torch.cuda.device(x.device):
-            ws, need = self._ws(eng, B, x.device)
+            ws, need = self._ws(eng, B, x.device, hw)
             fn = getattr(N.lib(), fn_name)
-            N.check(fn(eng["handle"], N.ptr(x), B, N.ptr(out), N.ptr(ws), ws.numel(), N.stream_ptr(x.device)), fn_name)
+            N.check(fn(eng["handle"], N.ptr(x), B, *ext, N.ptr(out), N.ptr(ws), ws.numel(), N.stream_ptr(x.device)), fn_name)
         self.last_launches = N.lib().rqb200_vae_last_launches(eng["handle"])
         N.launch_count["total"] += self.last_launches
         return out
 
     # ------------------------------------------------------------------ reference surface
-    def _latent_hw(self):
-        dd = self.ddconfig
-        r = dd["resolution"] // 2 ** (len(dd["ch_mult"]) - 1)
-        return r
+    def downsample_factor(self):
+        """f = 2^(len(ch_mult) - 1): an image of H x W pixels has an H/f x W/f latent"""
+        return 2 ** (len(self.ddconfig["ch_mult"]) - 1)
+
+    def _check_input(self, t, channels, what, f):
+        """ValueError unless t is [B, ..] 4-D with `channels` at dim 1 (what == 'image', NCHW) or dim 3 (NHWC latent) and both spatial
+        extents positive multiples of f -> (H, W)"""
+        if t.dim() != 4:
+            raise ValueError("RQVAE: the %s must be 4-D, got shape %s" % (what, tuple(t.shape)))
+        nchw = what == "image"
+        c = t.shape[1] if nchw else t.shape[3]
+        H, W = (t.shape[2], t.shape[3]) if nchw else (t.shape[1], t.shape[2])
+        if c != channels:
+            raise ValueError("RQVAE: the %s has %d channels, the model takes %d (shape %s)" % (what, c, channels, tuple(t.shape)))
+        if t.shape[0] < 1 or H < 1 or W < 1 or H % f or W % f:
+            raise ValueError("RQVAE: the %s's extent %d x %d is not a positive multiple of %d (shape %s)" % (what, H, W, f, tuple(t.shape)))
+        return H, W
 
     @torch.no_grad()
     def encode(self, x):
-        """rqvae.py:80-83: [B,3,R,R] -> z_e [B,h,w,embed_dim] NHWC contiguous"""
+        """rqvae.py:80-83: [B,in_channels,H,W] -> z_e [B,H/f,W/f,embed_dim] NHWC contiguous, at any H, W the downsampling
+        factor f = downsample_factor() divides (the reference's encoder is fully convolutional)"""
+        f = self.downsample_factor()
+        H, W = self._check_input(x, self.ddconfig["in_channels"], "image", f)
         x = x.float().contiguous()
-        r = self._latent_hw()
-        return self._run("rqb200_vae_encode", x, (x.shape[0], r, r, self.embed_dim))
+        return self._run("rqb200_vae_encode_hw", x, (x.shape[0], H // f, W // f, self.embed_dim), (H, W), (H, W))
 
     @torch.no_grad()
     def decode(self, z_q):
-        """rqvae.py:85-89: z_q [B,h,w,embed_dim] NHWC -> [B,out_ch,R,R]"""
+        """rqvae.py:85-89: z_q [B,h,w,embed_dim] NHWC -> [B,out_ch,h f,w f], at any latent extent h, w >= 1.  A code map of
+        another grid than code_shape decodes as decode(quantizer.embed_code_with_depth(code, True)[0].sum(-2)), as in the
+        reference (decode_code itself keeps the configured code_shape)."""
+        h, w = self._check_input(z_q, self.embed_dim, "latent", 1)
         z_q = z_q.float().contiguous()
-        dd = self.ddconfig
-        return self._run("rqb200_vae_decode", z_q, (z_q.shape[0], dd["out_ch"], dd["resolution"], dd["resolution"]))
+        f = self.downsample_factor()
+        return self._run("rqb200_vae_decode_hw", z_q, (z_q.shape[0], self.ddconfig["out_ch"], h * f, w * f), (h * f, w * f), (h, w))
 
     @torch.no_grad()
     def forward(self, xs):
@@ -202,7 +223,8 @@ class RQVAE(Stage1Model):
         dd = self.ddconfig
         if tuple(self.quantizer.shape_divisor[:2]) != (1, 1):
             return self.decode(self.quantizer.embed_code(code))
-        return self._run("rqb200_vae_decode_code", code, (code.shape[0], dd["out_ch"], dd["resolution"], dd["resolution"]))
+        R = dd["resolution"]
+        return self._run("rqb200_vae_decode_code", code, (code.shape[0], dd["out_ch"], R, R), (R, R))
 
     def get_recon_imgs(self, xs_real, xs_recon):
         return xs_real * 0.5 + 0.5, torch.clamp(xs_recon * 0.5 + 0.5, 0, 1)
