@@ -281,6 +281,46 @@ int rqb200_vae_encode_hw(rqb200_vae* h, const float* x, int B, int H, int W, flo
 int rqb200_vae_decode_hw(rqb200_vae* h, const float* z_q, int B, int hl, int wl, float* out, void* workspace, size_t workspace_bytes,
                          void* stream);
 
+/* ------------------------------------------------------------------------------------------------ FID Inception-v3
+ * InceptionV3 (rqvae/metrics/inception.py, use_fid_inception=True): the pytorch-fid Inception-v3 behind FID, as a static layer plan
+ * (csrc/inception_engine.cu).  Tensors are registered under the reference's InceptionV3 state_dict keys as they are (fp32, device):
+ * "<layer>.conv.weight" OIHW and "<layer>.bn.{weight,bias,running_mean,running_var}" for every BasicConv2d of blocks 0..last_block,
+ * plus "fc.weight" [1008, 2048] / "fc.bias" when last_block == 3.  rqb200_inception_finalize names the first missing or mis-sized
+ * key, then folds each BatchNorm (eps 0.001) into its conv in fp64 on `stream`, into the caller's parameter buffer of
+ * rqb200_inception_params_bytes(h) bytes, which must stay alive and unchanged while the engine is used.  Two tiers:
+ * RQB200_MODE_EXACT runs every conv on fp32 FFMA; RQB200_MODE_FAST runs every conv but Conv2d_1a_3x3 (Cin = 3, fp32 FFMA on both
+ * tiers) on the wgmma implicit GEMM with split-fp16 operands (three fp16 products per k step, fp32 accumulate).  ABI 116 added
+ * this section. */
+typedef struct rqb200_inception rqb200_inception;
+typedef struct {
+    int32_t last_block; /* 0..3: the deepest block the engine holds (InceptionV3's max(output_blocks)) */
+    int32_t mode;       /* RQB200_MODE_EXACT or RQB200_MODE_FAST */
+} rqb200_inception_config;
+
+/* rqb200_inception_forward flags */
+#define RQB200_INC_RESIZE 1      /* bilinear resize (align_corners=False) to 299 x 299 first; else H, W >= 75 */
+#define RQB200_INC_NORMALIZE 2   /* x -> 2 x - 1 */
+#define RQB200_INC_OUT0 4        /* write block 0's output (64 channels) to out0; OUT1 = 8, OUT2 = 16 (192, 768 channels) */
+#define RQB200_INC_OUT1 8
+#define RQB200_INC_OUT2 16
+#define RQB200_INC_OUT3 32       /* write the pooled features [B, 2048] to out3 */
+#define RQB200_INC_LOGITS 64     /* write fc's logits [B, 1008] to logits (last_block == 3) */
+
+rqb200_inception* rqb200_inception_create(const rqb200_inception_config* cfg);
+void rqb200_inception_destroy(rqb200_inception* h);
+int rqb200_inception_set_tensor(rqb200_inception* h, const char* key, const void* ptr, int dtype, int64_t numel);
+size_t rqb200_inception_params_bytes(const rqb200_inception* h);
+int rqb200_inception_finalize(rqb200_inception* h, void* params, size_t params_bytes, void* stream);
+/* the workspace of rqb200_inception_forward on B images of H x W with these flags; 0 for an extent the network does not take.  A
+ * batch whose activations exceed 2 GiB runs in chunks of as many images as fit, so the workspace stops growing with B there. */
+size_t rqb200_inception_workspace_bytes(rqb200_inception* h, int B, int H, int W, int flags);
+/* x NCHW [B, 3, H, W] f32 in [0, 1] (the reference's input).  Block k's output, NCHW [B, C_k, h_k, w_k] (C = 64, 192, 768), goes to
+ * out_k when flags has RQB200_INC_OUT<k>; out3 [B, 2048] and logits [B, 1008] likewise.  An image's outputs do not depend on the other
+ * images of the batch. */
+int rqb200_inception_forward(rqb200_inception* h, const float* x, int B, int H, int W, int flags, float* out0, float* out1, float* out2,
+                             float* out3, float* logits, void* workspace, size_t workspace_bytes, void* stream);
+int64_t rqb200_inception_last_launches(const rqb200_inception* h);
+
 /* ------------------------------------------------------------------------------------------------ diagnostics
  * Single-kernel entry points used by tests/ and bench.py's roofline leg; not part of the reference-facing surface.
  * rqb200_dbg_gemm_tc: one launch of the wgmma weight-streaming GEMM (csrc/gemm_tc.cu):
@@ -408,6 +448,28 @@ int rqb200_dbg_vae_attn(const float* qkv, float* out, int B, int HW, int C, void
 /* rqb200_dbg_vae_attn_tc: the same attention on the tensor-core kernel the fast tier runs on maps past 1024 tokens (fp16 operands,
  *   fp32 scores, softmax and accumulators; no shared-memory limit on HW).  C must be 128, 256, 384 or 512 (RQB200_EINVAL). */
 int rqb200_dbg_vae_attn_tc(const float* qkv, float* out, int B, int HW, int C, void* stream);
+
+/* The Inception engine's kernels (csrc/inception_engine.cu), one launch each through the launcher the engine calls.  Maps are NHWC f32.
+ * rqb200_dbg_inception_conv: conv + bias + ReLU of X [B, H, W, Cin] with Wt OHWI [Cout, kh, kw, Cin] f32 (BatchNorm already folded),
+ *   zero padding pad_h rows above and below, pad_w columns left and right, stride `stride`; output pixel m's channel n goes to
+ *   out[m * ldy + yoff + n] (nothing else is written), Ho = (H + 2 pad_h - kh) / stride + 1, Wo alike. */
+int rqb200_dbg_inception_conv(const float* X, const float* Wt, const float* bias, float* out, int B, int H, int W, int Cin, int Cout,
+                              int kh, int kw, int pad_h, int pad_w, int stride, int ldy, int yoff, void* stream);
+/* rqb200_dbg_inception_conv_tc: the fast tier's conv (csrc/conv_tc.cu inc_conv_tc_kernel) with the same geometry and output placement:
+ *   X16 / X16lo NHWC [B, H, W, Cin] fp16 hi / lo, W16 / W16lo OHWI [Cout, kh, kw, Cin] fp16 hi / lo, Cin % 8 == 0, Cout, ldy and yoff
+ *   multiples of 16, stride 1 or 2; ReLU(A_hi W_hi + A_lo W_hi + A_hi W_lo + bias) to out (fp32, nullable) and its fp16 hi / lo to
+ *   out_hi / out_lo (both or neither), at out[m * ldy + yoff + n]. */
+int rqb200_dbg_inception_conv_tc(const void* X16, const void* X16lo, const void* W16, const void* W16lo, const float* bias, float* out,
+                                 void* out_hi, void* out_lo, int B, int H, int W, int Cin, int Cout, int kh, int kw, int pad_h, int pad_w,
+                                 int stride, int ldy, int yoff, void* stream);
+/* rqb200_dbg_inception_input: x NCHW [B, 3, H, W] -> y NHWC [B, 299, 299, 3] (resize) or [B, H, W, 3], then 2 v - 1 when normalize. */
+int rqb200_dbg_inception_input(const float* x, float* y, int B, int H, int W, int resize, int normalize, void* stream);
+/* rqb200_dbg_inception_pool: 3x3 pool of X [B, H, W, C] with stride and pad (0 | 1) into channels [yoff, yoff + C) of rows of ldy
+ *   floats; mode 0 max (padding acts as -inf), 1 average over the in-map pixels (count_include_pad=False). */
+int rqb200_dbg_inception_pool(int mode, const float* X, float* Y, int B, int H, int W, int C, int stride, int pad, int ldy, int yoff,
+                              void* stream);
+/* rqb200_dbg_inception_gap: Y [B, C] = the mean of X [B, HW, C] over HW. */
+int rqb200_dbg_inception_gap(const float* X, float* Y, int B, int HW, int C, void* stream);
 
 #ifdef __cplusplus
 }

@@ -18,7 +18,10 @@ constexpr int CB_M = 64, CB_N = 64, CB_K = 16, C_THREADS = 256;
 template <typename WT>
 __device__ __forceinline__ float w_at(const WT* p, int64_t i) { return to_f32<WT>(p[i]); }
 
-template <typename WT>
+// INC = false: the VAE's form (one symmetric pad, output rows of Cout).  INC = true: the Inception engine's form -- separate
+// pad_h / pad_w (1x7, 7x1, 1x3, 3x1 and 5x5 kernels), bias + ReLU, and the output written into channels [yoff, yoff + Cout) of
+// rows of ldy floats (a branch's slice of its block's concat buffer).  A separate instantiation, so the VAE's launches keep their code.
+template <typename WT, bool INC = false>
 __global__ void __launch_bounds__(C_THREADS)
 conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const float* __restrict__ bias, const float* R,
                   float* Y, ConvGeom g) {
@@ -51,7 +54,7 @@ conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const f
             if (mvalid && kk < K) {
                 int tap = kk / g.Cin, ci = kk % g.Cin;
                 int ky = tap / g.KW, kx = tap % g.KW;
-                int uy = oy * g.stride + ky - g.pad, ux = ox * g.stride + kx - g.pad;
+                int uy = oy * g.stride + ky - g.pad, ux = ox * g.stride + kx - (INC ? g.pad_w : g.pad);
                 if (uy >= 0 && uy < Hv && ux >= 0 && ux < Wv) {
                     int iy = g.upsample ? (uy >> 1) : uy, ix = g.upsample ? (ux >> 1) : ux;
                     float4 v = *reinterpret_cast<const float4*>(X + (((int64_t)b * g.Hi + iy) * g.Wi + ix) * g.Cin + ci);
@@ -65,7 +68,7 @@ conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const f
                 if (mvalid && k < K) {
                     int tap = k / g.Cin, ci = k % g.Cin;
                     int ky = tap / g.KW, kx = tap % g.KW;
-                    int uy = oy * g.stride + ky - g.pad, ux = ox * g.stride + kx - g.pad;
+                    int uy = oy * g.stride + ky - g.pad, ux = ox * g.stride + kx - (INC ? g.pad_w : g.pad);
                     if (uy >= 0 && uy < Hv && ux >= 0 && ux < Wv) {
                         int iy = g.upsample ? (uy >> 1) : uy, ix = g.upsample ? (ux >> 1) : ux;
                         av[i] = g.in_nchw ? X[(((int64_t)b * g.Cin + ci) * g.Hi + iy) * g.Wi + ix]
@@ -104,6 +107,10 @@ conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const f
             int n = n0 + tx * 4 + j;
             if (n >= N) continue;
             float v = acc[i][j] + (bias ? bias[n] : 0.f);
+            if (INC) {
+                Y[mm * g.ldy + g.yoff + n] = fmaxf(v, 0.f);
+                continue;
+            }
             if (R) v = R[mm * N + n] + v;                                  // x + h  (layers.py:120,182)
             if (g.out_nchw) Y[(((int64_t)bb * N + n) * g.Ho + oyy) * g.Wo + oxx] = v;
             else Y[mm * N + n] = v;
@@ -112,7 +119,7 @@ conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const f
 }
 
 ConvGeom vae_conv_geom(int B, int H, int W, int Cin, int Cout, int ks, int stride, int upsample, int in_nchw, int out_nchw) {
-    ConvGeom g;
+    ConvGeom g{};
     g.B = B; g.Hi = H; g.Wi = W; g.Cin = Cin; g.Cout = Cout; g.KH = g.KW = ks; g.stride = stride;
     g.upsample = upsample; g.in_nchw = in_nchw; g.out_nchw = out_nchw;
     g.pad = (ks == 3 && stride == 1) ? 1 : 0;
@@ -135,6 +142,16 @@ int launch_conv(const float* X, const void* W, int wdtype, const float* bias, co
     else
         return fail(RQB200_EINVAL, "conv: unsupported weight dtype");
     return check_launch("conv_igemm");
+}
+
+// conv + bias + ReLU of the Inception engine (conv_igemm_kernel<float, true>): fp32 weights, NHWC input (or NCHW when g.in_nchw),
+// output rows of g.ldy floats from channel g.yoff
+int launch_conv_relu(const float* X, const float* W, const float* bias, float* Y, const ConvGeom& g, cudaStream_t st) {
+    const int64_t M = (int64_t)g.B * g.Ho * g.Wo;
+    if (M <= 0) return 0;
+    dim3 grid((unsigned)ceil_div(M, CB_M), (unsigned)ceil_div(g.Cout, CB_N));
+    conv_igemm_kernel<float, true><<<grid, C_THREADS, 0, st>>>(X, W, bias, nullptr, Y, g);
+    return check_launch("conv_igemm_relu");
 }
 
 // ------------------------------------------------------------------------------------------------ GroupNorm(32) (+SiLU)

@@ -833,6 +833,188 @@ int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, con
     return launch_conv_tc_t<128, 6, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
 }
 
+// ------------------------------------------------------------------------------------------------ Inception convs (fast tier)
+// The Inception engine's convs on conv_tc_kernel's layout, generalised: any KH x KW with separate top/bottom and left/right zero
+// padding (the tap's box starts at x * stride + kx - pad_w, y * stride + ky - pad_h; TMA zero-fills every box element at a negative
+// or past-the-end coordinate, which IS the padding), stride-2 "valid" convs, and Cin % 8 == 0 rather than % 64: the activation's
+// tensor map has the true channel extent Cin, so the last 64-channel slab's channels past Cin are zero-filled in A and multiply the
+// next tap's weights (or the weight map's own zero fill) to zero.  That keeps the activations unpadded, so the engine's concat
+// buffers stay exactly the reference's channel layout.  Epilogue: bias + ReLU, stored at channel yoff of rows of ldy as fp32 and
+// as the next conv's fp16 hi / lo operands (no cast pass between convs).
+struct IncTcParams {
+    int B, H, W, Cin, Cout;        // H, W: OUTPUT extent
+    int KH, KW, pad_h, pad_w, stride;
+    int TW, TH, NB;
+    int tiles_x, tiles_y, tiles_b, n_tiles_n;
+    const float* bias;
+    float* out;                    // fp32 [B, H, W, ldy] or null
+    __half* out_hi;                // fp16 hi / lo of the same values, [B, H, W, ldy], or null
+    __half* out_lo;
+    int ldy, yoff;
+};
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(CT_THREADS, 1)
+inc_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, IncTcParams p) {
+    constexpr int B_BYTES = BN * 64 * 2;
+    constexpr int STAGE_BYTES = 2 * (CT_A_BYTES + B_BYTES);
+    constexpr int OFF_B = 2 * CT_A_BYTES;                    // [A_hi | A_lo | B_hi | B_lo]
+    constexpr int CW = BN < 32 ? BN : 32;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    float* stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(stage + 128 * (CW + 4));
+    uint64_t* empty = full + STAGES;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int cslabs = (p.Cin + 63) / 64;
+    const int nkb = p.KH * p.KW * cslabs;
+    const int sx = p.stride;
+    const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_b;
+    const int total = m_tiles * p.n_tiles_n;
+
+    if (warp == 8 && lane == 0) {
+        tc::prefetch_tmap(&tmA);
+        tc::prefetch_tmap(&tmB);
+        for (int s = 0; s < STAGES; s++) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 8); }
+        tc::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        if (lane == 0) {
+            uint32_t it = 0;
+            for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+                const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
+                const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
+                const int x0 = tx * p.TW, y0 = ty * p.TH, b0 = tb * p.NB;
+                for (int kb = 0; kb < nkb; kb++, it++) {
+                    const int s = it % STAGES;
+                    tc::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+                    const int tap = kb / cslabs, c0 = (kb % cslabs) * 64;
+                    const int ky = tap / p.KW, kx = tap % p.KW;
+                    const int ix = x0 * sx + kx - p.pad_w, iy = y0 * sx + ky - p.pad_h;
+                    tc::mbar_expect_tx(&full[s], STAGE_BYTES);
+                    uint8_t* st = smem + s * STAGE_BYTES;
+                    tc::tma_load_4d(st, &tmA, &full[s], c0, ix, iy, b0, tc::L2_EVICT_NORMAL);
+                    tc::tma_load_4d(st + CT_A_BYTES, &tmAlo, &full[s], c0, ix, iy, b0, tc::L2_EVICT_NORMAL);
+                    tc::tma_load_2d(st + OFF_B, &tmB, &full[s], tap * p.Cin + c0, nt * BN, tc::L2_EVICT_LAST);
+                    tc::tma_load_2d(st + OFF_B + B_BYTES, &tmBlo, &full[s], tap * p.Cin + c0, nt * BN, tc::L2_EVICT_LAST);
+                }
+            }
+        }
+        return;
+    }
+
+    const int wg = warp >> 2, t = threadIdx.x;
+    const int r = t & 127;
+    const int rx = r % p.TW, ry = (r / p.TW) % p.TH, rb = r / (p.TW * p.TH);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+        for (int kb = 0; kb < nkb; kb++, it++) {
+            const int s = it % STAGES;
+            tc::mbar_wait(&full[s], (it / STAGES) & 1);
+            const uint32_t a = tc::smem_u32(smem + s * STAGE_BYTES) + wg * (64 * 128), b = tc::smem_u32(smem + s * STAGE_BYTES + OFF_B);
+            tc::wgmma_fence();
+            ct_mma_kblock<BN, 0, 3>(acc, a, b, kb == 0);
+            tc::wgmma_commit();
+            tc::wgmma_wait<1>();
+            if (kb > 0 && lane == 0) tc::mbar_arrive(&empty[(it - 1) % STAGES]);
+        }
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc);
+        if (lane == 0) tc::mbar_arrive(&empty[(it - 1) % STAGES]);
+
+        const int nt = tile % p.n_tiles_n, mt = tile / p.n_tiles_n;
+        const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tb = mt / (p.tiles_x * p.tiles_y);
+        const int x = tx * p.TW + rx, y = ty * p.TH + ry, b = tb * p.NB + rb;
+        const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
+        const bool valid = (x < p.W) && (y < p.H) && (b < p.B);
+        tc::drain_acc<BN, CW, 0>(acc, stage, wg, t, [&p, nt, pix, valid](const float (&v)[16], int, int c) {
+            const int n0 = nt * BN + c;
+            if (n0 >= p.Cout || !valid) return;                     // Cout % 16 == 0: a 16-channel chunk is all in or all out
+            float w[16];
+#pragma unroll
+            for (int i = 0; i < 16; i += 4) {
+                const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
+                w[i] = fmaxf(v[i] + bb.x, 0.f); w[i + 1] = fmaxf(v[i + 1] + bb.y, 0.f);
+                w[i + 2] = fmaxf(v[i + 2] + bb.z, 0.f); w[i + 3] = fmaxf(v[i + 3] + bb.w, 0.f);
+            }
+            const int64_t o = pix * p.ldy + p.yoff + n0;
+            if (p.out) {
+#pragma unroll
+                for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(p.out + o + i) = make_float4(w[i], w[i + 1], w[i + 2], w[i + 3]);
+            }
+            if (p.out_hi) {
+                uint32_t hi[8], lo[8];
+#pragma unroll
+                for (int i = 0; i < 8; i++) {
+                    const __half2 h = __floats2half2_rn(w[2 * i], w[2 * i + 1]);
+                    const float2 hf = __half22float2(h);
+                    const __half2 l = __floats2half2_rn(w[2 * i] - hf.x, w[2 * i + 1] - hf.y);
+                    hi[i] = *reinterpret_cast<const uint32_t*>(&h);
+                    lo[i] = *reinterpret_cast<const uint32_t*>(&l);
+                }
+                uint4* dh = reinterpret_cast<uint4*>(p.out_hi + o);
+                dh[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                dh[1] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+                uint4* dl = reinterpret_cast<uint4*>(p.out_lo + o);
+                dl[0] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+                dl[1] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+            }
+        });
+    }
+}
+
+template <int BN, int STAGES>
+static int launch_inc_conv_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
+                                const IncTcParams& p, int n_sm, cudaStream_t st) {
+    constexpr size_t smem = (size_t)STAGES * 2 * (CT_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 256;
+    static_assert(smem <= 227 * 1024, "inc_conv_tc: shared memory budget");
+    RQB_ENSURE_SMEM(smem, inc_conv_tc_kernel<BN, STAGES>);
+    const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
+    inc_conv_tc_kernel<BN, STAGES><<<total < n_sm ? total : n_sm, CT_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
+    return check_launch("inc_conv_tc");
+}
+
+int launch_inc_conv_tc(const void* X16, const void* X16lo, const void* W16, const void* W16lo, const float* bias, float* out,
+                       void* out_hi, void* out_lo, int B, int Hi, int Wi, int Cin, int Cout, int KH, int KW, int pad_h, int pad_w,
+                       int stride, int ldy, int yoff, cudaStream_t st) {
+    if (!X16 || !X16lo || !W16 || !W16lo || !bias || (!out && !out_hi) || (out_hi && !out_lo))
+        return fail(RQB200_EINVAL, "inc_conv_tc: need both operand halves, a bias and an fp32 or an fp16 hi + lo output");
+    if (Cin % 8 || Cout % 16 || ldy % 16 || yoff % 16 || yoff + Cout > ldy || (stride != 1 && stride != 2) || KH < 1 || KW < 1 ||
+        pad_h < 0 || pad_w < 0)
+        return fail(RQB200_EINVAL, "inc_conv_tc: need Cin % 8 == 0, Cout, ldy, yoff % 16 == 0, yoff + Cout <= ldy, stride 1 | 2");
+    IncTcParams p = {};
+    p.B = B; p.Cin = Cin; p.Cout = Cout; p.KH = KH; p.KW = KW; p.pad_h = pad_h; p.pad_w = pad_w; p.stride = stride;
+    p.H = (Hi + 2 * pad_h - KH) / stride + 1;
+    p.W = (Wi + 2 * pad_w - KW) / stride + 1;
+    if (B < 1 || p.H < 1 || p.W < 1) return fail(RQB200_EINVAL, "inc_conv_tc: empty output");
+    auto pow2_ceil = [](int v) { int q = 1; while (q < v) q *= 2; return q; };
+    p.TW = pow2_ceil(p.W < 16 ? p.W : 16);
+    p.TH = pow2_ceil(p.H < 128 / p.TW ? p.H : 128 / p.TW);
+    p.NB = 128 / (p.TW * p.TH);
+    p.tiles_x = (int)ceil_div(p.W, p.TW); p.tiles_y = (int)ceil_div(p.H, p.TH); p.tiles_b = (int)ceil_div(B, p.NB);
+    const int BN = Cout >= 128 ? 128 : 64;
+    p.n_tiles_n = (int)ceil_div(Cout, BN);
+    p.bias = bias; p.out = out; p.out_hi = (__half*)out_hi; p.out_lo = (__half*)out_lo; p.ldy = ldy; p.yoff = yoff;
+    const uint64_t K = (uint64_t)KH * KW * Cin;
+    CUtensorMap tmA, tmB, tmAlo, tmBlo;
+    RQB_TRY(make_tmap_2d(&tmB, W16, 1, K, (uint64_t)Cout, K * 2, 64, (uint32_t)BN));
+    RQB_TRY(make_tmap_2d(&tmBlo, W16lo, 1, K, (uint64_t)Cout, K * 2, 64, (uint32_t)BN));
+    RQB_TRY(make_tmap_4d_nhwc(&tmA, X16, (uint64_t)Cin, (uint64_t)Wi, (uint64_t)Hi, (uint64_t)B, 64, (uint32_t)p.TW, (uint32_t)p.TH,
+                              (uint32_t)p.NB, (uint32_t)stride));
+    RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)Wi, (uint64_t)Hi, (uint64_t)B, 64, (uint32_t)p.TW, (uint32_t)p.TH,
+                              (uint32_t)p.NB, (uint32_t)stride));
+    const int n_sm = sm_count();
+    return BN == 128 ? launch_inc_conv_tc_t<128, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
+                     : launch_inc_conv_tc_t<64, 4>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+}
+
 // ------------------------------------------------------------------------------------------------ fp16 operand producers
 // 4 fp32 values -> fp16 hi (+ optional fp16 lo = value - hi)
 __device__ __forceinline__ void store_split4(__half* hi, __half* lo, const float (&v)[4]) {

@@ -64,12 +64,17 @@ struct ConvGeom {
     int upsample;            // 1: the conv reads nearest-x2-upsampled input (layers.py:31-35)
     int out_nchw;            // 1: write [B,Cout,Ho,Wo] (final conv_out)
     int in_nchw;             // 1: read [B,Cin,Hi,Wi] (encoder conv_in)
+    // launch_conv_relu only (the Inception engine): pad is the top/bottom pad and pad_w the left/right one; the output pixel m's
+    // channel n goes to Y[m * ldy + yoff + n]
+    int pad_w;
+    int ldy, yoff;
 };
 // the geometry of one conv of the VAE layer plan (vae_engine.cu): H, W the input extent before the optional nearest x2 upsample;
 // Ho, Wo = the (upsampled) extent / stride; pad 1 for a 3x3 stride-1 conv, else 0 (stride 2: the Downsample's implicit (0,1,0,1))
 ConvGeom vae_conv_geom(int B, int H, int W, int Cin, int Cout, int ks, int stride, int upsample, int in_nchw, int out_nchw);
 int launch_conv(const float* X, const void* W, int wdtype, const float* bias, const float* R, float* Y, const ConvGeom& g,
                 cudaStream_t st);
+int launch_conv_relu(const float* X, const float* W, const float* bias, float* Y, const ConvGeom& g, cudaStream_t st);
 int launch_groupnorm_silu(const float* X, const float* gamma, const float* beta, float* Y, double* stats_ws, int B, int HW,
                           int C, int silu, cudaStream_t st);
 int launch_vae_attn(const float* qkv, float* out, int B, int HW, int C, cudaStream_t st);
@@ -83,6 +88,11 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
                    const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ks, int out_nchw,
                    cudaStream_t st, int stride = 1, double* gn_part = nullptr);
 bool conv_tc_gn_fusable(int H, int W, int Cout, int ks, int stride);
+// the Inception engine's fast-tier conv (conv_tc.cu, inc_conv_tc_kernel): X NHWC [B, Hi, Wi, Cin] fp16 hi + lo, W OHWI [Cout, KH, KW, Cin]
+// fp16 hi + lo, out[pix * ldy + yoff + n] = ReLU(conv + bias) as fp32 (out) and / or fp16 hi + lo (out_hi, out_lo)
+int launch_inc_conv_tc(const void* X16, const void* X16lo, const void* W16, const void* W16lo, const float* bias, float* out,
+                       void* out_hi, void* out_lo, int B, int Hi, int Wi, int Cin, int Cout, int KH, int KW, int pad_h, int pad_w,
+                       int stride, int ldy, int yoff, cudaStream_t st);
 int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                         int gelu, int fmt, int64_t M, int N_out, int K, cudaStream_t st);
 int launch_groupnorm_f16(const float* X, const float* gamma, const float* beta, void* Y16, void* Y16lo, double* stats_ws, int B,

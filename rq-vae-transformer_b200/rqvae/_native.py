@@ -157,7 +157,10 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_ar_log_prob_workspace_bytes", "rqb200_dbg_log_prob_rows", "rqb200_dbg_attn_step", "rqb200_dbg_prefill_attn", "rqb200_dbg_append_attn",
            "rqb200_dbg_ln", "rqb200_dbg_act_reduce", "rqb200_dbg_vae_conv", "rqb200_dbg_groupnorm", "rqb200_dbg_cast_f16",
            "rqb200_dbg_vae_attn", "rqb200_vae_workspace_bytes_hw", "rqb200_vae_encode_hw", "rqb200_vae_decode_hw",
-           "rqb200_dbg_vae_attn_tc"]
+           "rqb200_dbg_vae_attn_tc", "rqb200_inception_create", "rqb200_inception_destroy", "rqb200_inception_set_tensor",
+           "rqb200_inception_params_bytes", "rqb200_inception_finalize", "rqb200_inception_workspace_bytes", "rqb200_inception_forward",
+           "rqb200_inception_last_launches", "rqb200_dbg_inception_conv", "rqb200_dbg_inception_conv_tc", "rqb200_dbg_inception_input", "rqb200_dbg_inception_pool",
+           "rqb200_dbg_inception_gap"]
 
 
 def check(rc, what=""):
