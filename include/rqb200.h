@@ -188,13 +188,24 @@ size_t rqb200_ar_workspace_bytes(const rqb200_ar* h, int B);
  * right before b's head: on the fast tier in one batched pass at sequence offset cond_len + a when b - a is at least a few tokens
  * (token by token with RQB200_AR_SEQUENTIAL_PREFILL), on the exact tier token by token.  That grouping depends on sampled_host alone, so
  * a call split into spans gives the codes of one span bit for bit.
- * Fast tier: B <= 256 rows per call (a guided call: n <= 128 images).  The null pointers, B, cfg_n, the span and sampled_host are
- * checked before any CUDA call.  ABI 113 appended the last four arguments: a caller built against an older header must pass them. */
+ * Sliding-window sampling of a canvas larger than the grid: canvas_h x canvas_w = Ht x Wt with Ht >= H, Wt >= W (H x W: the
+ *   grid, today's call).  partial, force_codes and out_codes are then [B, Ht, Wt, D], keep [B, Ht*Wt, D], sampled_host [Ht*Wt], and
+ *   idx_begin / idx_end and the noise / logits_out token indices count canvas positions in raster order.  The token at canvas (i, j, d)
+ *   is sampled as the model's token (i - r0, j - c0, d) of the H x W window with origin
+ *       r0 = clamp(i - floor(H/2), 0, Ht - H),   c0 = clamp(j - floor(W/2), 0, Wt - W),
+ *   seeing the cond prefix, the window's positions before it in window raster order (read from the canvas as it stands) and its own
+ *   depths < d -- nothing outside its window.  Consecutive sampled positions with one origin continue one KV cache (one segment); a new
+ *   origin restarts the body with a prefill of the window's prefix.  The workspace is the grid's (rqb200_ar_workspace_bytes).
+ *   canvas_h * canvas_w * D must not exceed RQB200_CANVAS_MAX_CODES.
+ * Fast tier: B <= 256 rows per call (a guided call: n <= 128 images).  The null pointers, B, cfg_n, the canvas, the span and
+ * sampled_host are checked before any CUDA call.  ABI 113 appended keep .. cfg_scale and ABI 117 canvas_h and canvas_w: a caller built
+ * against an older header must pass them (the grid's H and W for today's call). */
+#define RQB200_CANVAS_MAX_CODES 2147483647LL   /* canvas_h * canvas_w * D: canvas positions and offsets are 32-bit */
 int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                           float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
                           void* workspace, size_t workspace_bytes, void* stream, const uint8_t* keep, const uint8_t* sampled_host,
-                          int cfg_n, float cfg_scale);
+                          int cfg_n, float cfg_scale, int canvas_h, int canvas_w);
 /* RQTransformer.cached_forward (transformers.py:190-287): the logits of ONE token (h, w, d) into logits_out [B,V] f32.
  *   xs: the caller's code map, int64, batch row b at xs + b*xs_batch_stride, positions in raster order, D codes each
  *       (only the codes this step consumes are read: position idx-1 when d == 0, codes 0..d-1 of position idx when d > 0;

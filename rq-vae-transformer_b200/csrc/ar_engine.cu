@@ -78,15 +78,16 @@ static int run_stack(const rqb200_ar* h, const std::vector<rqb200_block_weights>
 }
 
 // ws.LIN[(b*J + j)*D + d, :] = the body input embedding of code d at position j0 + j: input_mlp(e_d) (transformers.py:219-220), or
-// the tok_emb row of the code (:222, EMB_TOK_INPUT)
-static int body_inputs(const rqb200_ar* h, const int64_t* codes, int B, int j0, int J, ArWs& ws, cudaStream_t st) {
+// the tok_emb row of the code (:222, EMB_TOK_INPUT).  cv (nullable): the positions are window positions of a canvas (kernels.h); this
+// and the functions below pass it to the code gathers.
+static int body_inputs(const rqb200_ar* h, const int64_t* codes, int B, int j0, int J, ArWs& ws, cudaStream_t st, const CanvasMap* cv) {
     const rqb200_ar_config& c = h->cfg;
     const rqb200_ar_weights& w = h->w;
     const int E = c.embed_dim, D = c.D, HW = c.H * c.W, C = c.code_dim, K = c.codebook_size;
     if (c.embed_variant & RQB200_EMB_TOK_INPUT)
         return launch_code_emb(codes, w.tok_emb, (c.embed_variant & RQB200_EMB_TUPLE) ? (int64_t)c.vocab * E : 0, B, HW, D, c.vocab, E,
-                               j0, J, ws.LIN, st);
-    RQB_TRY(launch_code_emb(codes, w.codebook, c.codebook_per_depth ? (int64_t)K * C : 0, B, HW, D, K, C, j0, J, ws.EMB, st));
+                               j0, J, ws.LIN, st, cv);
+    RQB_TRY(launch_code_emb(codes, w.codebook, c.codebook_per_depth ? (int64_t)K * C : 0, B, HW, D, K, C, j0, J, ws.EMB, st, cv));
     return launch_linear(ws.EMB, C, w.w_in, c.weight_dtype, w.b_in, nullptr, ws.LIN, E, B * J * D, E, C, 0, st);
 }
 
@@ -111,14 +112,15 @@ static const char* check_e4m3_weights(const rqb200_ar_config& c, const rqb200_ar
 }
 
 // prefill: tokens [cond (cl) | xs_emb[0 .. idx0-1]] through the body (transformers.py:224-239); ws.CTX = the last token's output
-static int prefill_prefix(const rqb200_ar* h, const int64_t* codes, const int64_t* cond, int B, int idx0, ArWs& ws, cudaStream_t st) {
+static int prefill_prefix(const rqb200_ar* h, const int64_t* codes, const int64_t* cond, int B, int idx0, ArWs& ws, cudaStream_t st,
+                          const CanvasMap* cv = nullptr) {
     const rqb200_ar_config& c = h->cfg;
     const rqb200_ar_weights& w = h->w;
     const int E = c.embed_dim, D = c.D, cl = c.cond_len, Tb = cl + c.H * c.W;
     const int Tn0 = cl + idx0;
     RQB_TRY(launch_cond_token(cond, w.cond_emb, w.pos_emb_cond, B, cl, c.vocab_cond, E, Tn0, ws.X, st));
     if (idx0 > 0) {
-        RQB_TRY(body_inputs(h, codes, B, 0, idx0, ws, st));
+        RQB_TRY(body_inputs(h, codes, B, 0, idx0, ws, st, cv));
         RQB_TRY(launch_body_token(ws.LIN, w.pos_emb_hw, B, D, E, 0, idx0, cl, Tn0, ws.X, st));
     }
     RQB_TRY(run_stack(h, h->body, ws, B, Tn0, 0, Tb, ws.kc_body, ws.vc_body, st));
@@ -126,10 +128,10 @@ static int prefill_prefix(const rqb200_ar* h, const int64_t* codes, const int64_
 }
 
 // decode step of the body on the token of position idx-1 (transformers.py:240-242); ws.CTX = its output
-static int body_step(const rqb200_ar* h, const int64_t* codes, int B, int idx, ArWs& ws, cudaStream_t st) {
+static int body_step(const rqb200_ar* h, const int64_t* codes, int B, int idx, ArWs& ws, cudaStream_t st, const CanvasMap* cv = nullptr) {
     const rqb200_ar_config& c = h->cfg;
     const int E = c.embed_dim, cl = c.cond_len, Tb = cl + c.H * c.W;
-    RQB_TRY(body_inputs(h, codes, B, idx - 1, 1, ws, st));
+    RQB_TRY(body_inputs(h, codes, B, idx - 1, 1, ws, st, cv));
     RQB_TRY(launch_body_token(ws.LIN, h->w.pos_emb_hw, B, c.D, E, idx - 1, 1, 0, 1, ws.X, st));
     RQB_TRY(run_stack(h, h->body, ws, B, 1, cl + idx - 1, Tb, ws.kc_body, ws.vc_body, st));
     RQB_CUDA(cudaMemcpyAsync(ws.CTX, ws.X, (size_t)B * E * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -137,7 +139,8 @@ static int body_step(const rqb200_ar* h, const int64_t* codes, int B, int idx, A
 }
 
 // head depth d of position idx: its token, the head stack (cache rows [0, d) from the earlier depths) and the classifier -> lg [B,V]
-static int head_depth(const rqb200_ar* h, const int64_t* codes, int B, int idx, int d, ArWs& ws, float* lg, cudaStream_t st) {
+static int head_depth(const rqb200_ar* h, const int64_t* codes, int B, int idx, int d, ArWs& ws, float* lg, cudaStream_t st,
+                      const CanvasMap* cv = nullptr) {
     const rqb200_ar_config& c = h->cfg;
     const rqb200_ar_weights& w = h->w;
     const int E = c.embed_dim, D = c.D, HW = c.H * c.W, C = c.code_dim, V = c.vocab, K = c.codebook_size, wd = c.weight_dtype;
@@ -148,11 +151,11 @@ static int head_depth(const rqb200_ar* h, const int64_t* codes, int B, int idx, 
     if (d == 0) {
         RQB_TRY(launch_row_add(ws.CTX, E, 0, w.pos_emb_d, B, E, ws.X, st));                         // ctx + pos_emb_d[0]
     } else if (ev & RQB200_EMB_TOK_HEAD) {
-        RQB_TRY(launch_head_cumsum(codes, w.tok_emb, tes, B, HW, D, V, E, idx, d, ws.TOK, st, true));  // tok_emb(code_{d-1})
+        RQB_TRY(launch_head_cumsum(codes, w.tok_emb, tes, B, HW, D, V, E, idx, d, ws.TOK, st, true, cv));  // tok_emb(code_{d-1})
         RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
     } else {
         // head_mlp(cumsum_{i<d} e_i), or head_mlp(e_{d-1}) without cumsum_depth_ctx
-        RQB_TRY(launch_head_cumsum(codes, w.codebook, cbs, B, HW, D, K, C, idx, d, ws.EMB, st, (ev & RQB200_EMB_NO_CUMSUM) != 0));
+        RQB_TRY(launch_head_cumsum(codes, w.codebook, cbs, B, HW, D, K, C, idx, d, ws.EMB, st, (ev & RQB200_EMB_NO_CUMSUM) != 0, cv));
         RQB_TRY(launch_linear(ws.EMB, C, w.w_head, wd, w.b_head, nullptr, ws.TOK, E, B, E, C, 0, st));
         RQB_TRY(launch_row_add(ws.TOK, E, 0, w.pos_emb_d + (int64_t)d * E, B, E, ws.X, st));
     }
@@ -166,37 +169,49 @@ static int head_depth(const rqb200_ar* h, const int64_t* codes, int B, int idx, 
 // positions [idx0, idx_end) of the raster; resume != 0: no prefill, continue on the caches / context left in this workspace.
 // cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s (the sampler forms the guided logits).
 // keep / sampled: the masked-sample plan of the fast tier (kernels.h), with one body step per appended code token.
+// Ht x Wt: the canvas (H x W: the grid).  Positions are canvas positions; a canvas is walked in segments as on the fast tier
+// (ar_fast_sample): a new window origin restarts the body with a prefill of the window's prefix.
 // B >= 1 and a span within the raster: rqb200_ar_sample_span checks them, ar_log_prob_impl forms them.
 static int ar_sample_impl(rqb200_ar* h, const int64_t* partial, const int64_t* cond, int B, int idx0, int idx_end, int resume,
                           float temperature, const int32_t* top_k, const float* top_p, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force, int64_t* out, void* wsp,
-                          size_t ws_bytes, cudaStream_t st, int cfg_n, float cfg_s, const uint8_t* keep, const uint8_t* sampled) {
+                          size_t ws_bytes, cudaStream_t st, int cfg_n, float cfg_s, const uint8_t* keep, const uint8_t* sampled,
+                          int Ht, int Wt) {
     const rqb200_ar_config& c = h->cfg;
-    const int D = c.D, HW = c.H * c.W, V = c.vocab;
+    const int D = c.D, V = c.vocab;
+    const int64_t row = (int64_t)Ht * Wt * D;         // codes per batch row
+    CanvasMap cm{c.W, Wt, 0, Ht * Wt};
+    const CanvasMap* cv = (Ht != c.H || Wt != c.W) ? &cm : nullptr;
     ArWs ws;
     size_t need = ar_layout(c, B, wsp, ws_bytes, &ws);
     if (need > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_sample: workspace too small");
-    const int64_t code_bytes = (int64_t)B * HW * D * sizeof(int64_t);
+    const int64_t code_bytes = (int64_t)B * row * sizeof(int64_t);
     if (!resume && out != partial) RQB_CUDA(cudaMemcpyAsync(out, partial, code_bytes, cudaMemcpyDeviceToDevice, st));   // xs = partial_sample.clone()
     if (idx0 >= idx_end) return 0;
 
     int prev = resume ? plan_prev(sampled, idx0) : -1;     // the last sampled position before this span; none: prefill at the first
+    int prev_p = -1;                                        // its window position
+    if (prev >= 0) win_locate(prev, c.H, c.W, Wt, Ht, &cm.org, &prev_p);
     for (int idx = idx0; idx < idx_end; idx++) {
         if (!plan_sampled(sampled, idx)) continue;
-        if (prev < 0)
-            RQB_TRY(prefill_prefix(h, out, cond, B, idx, ws, st));
-        else
-            for (int j = prev + 1; j <= idx; j++) RQB_TRY(body_step(h, out, B, j, ws, st));   // decode steps on positions prev .. idx-1
+        int org, p;
+        win_locate(idx, c.H, c.W, Wt, Ht, &org, &p);
+        if (prev < 0 || org != cm.org) {
+            cm.org = org;
+            RQB_TRY(prefill_prefix(h, out, cond, B, p, ws, st, cv));
+        } else {
+            for (int j = prev_p + 1; j <= p; j++) RQB_TRY(body_step(h, out, B, j, ws, st, cv));   // decode steps on positions prev_p .. p-1
+        }
         for (int d = 0; d < D; d++) {
             const int64_t step = (int64_t)(idx - idx0) * D + d;
             float* lg = logits_out ? logits_out + step * (int64_t)B * V : ws.LOGITS;
-            RQB_TRY(head_depth(h, out, B, idx, d, ws, lg, st));
+            RQB_TRY(head_depth(h, out, B, p, d, ws, lg, st, cv));
             const float* q = noise ? noise + step * noise_stride : nullptr;
-            const int64_t off = (int64_t)idx * D + d;
-            RQB_TRY(launch_sample(lg, q, B, V, temperature, top_k[d], top_p[d], out + off, force ? force + off : nullptr,
-                                  (int64_t)HW * D, st, 1, cfg_n, cfg_s, keep ? keep + off : nullptr));
+            const int64_t off = cm.at(0, p) * D + d;
+            RQB_TRY(launch_sample(lg, q, B, V, temperature, top_k[d], top_p[d], out + off, force ? force + off : nullptr, row, st, 1, cfg_n,
+                                  cfg_s, keep ? keep + off : nullptr));
         }
-        prev = idx;
+        prev = idx; prev_p = p;
     }
     return 0;
 }
@@ -262,7 +277,7 @@ static int ar_log_prob_impl(rqb200_ar* h, const int64_t* codes, const int64_t* c
     for (int p0 = 0; p0 < HW; p0 += (int)P) {
         const int p1 = (int)std::min<int64_t>(p0 + P, HW), n_pos = p1 - p0, steps = n_pos * D;
         RQB_TRY(ar_sample_impl(h, codes, cond, B, p0, p1, p0 > 0, 1.f, top_k.data(), top_p.data(), nullptr, 0, sp.logits, codes, ws.CODES,
-                               wsp, ws_bytes, st, 0, 0.f, nullptr, nullptr));
+                               wsp, ws_bytes, st, 0, 0.f, nullptr, nullptr, c.H, c.W));
         // row (step, b), step = (idx - p0)*D + d  <-  codes[b][p0*D + step]
         RQB_TRY(launch_gather_targets(codes, 1, steps, B, 0, 1, HWD, (int64_t)p0 * D, sp.tgt, st));
         RQB_TRY(launch_logprob_rows(sp.logits, V, V, (int64_t)steps * B, sp.tgt, 1, sp.lp, st));
@@ -344,13 +359,17 @@ int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* c
                           float temperature, const int32_t* top_k_host, const float* top_p_host, const float* noise,
                           int64_t noise_stride, float* logits_out, const int64_t* force_codes, int64_t* out_codes,
                           void* workspace, size_t workspace_bytes, void* stream, const uint8_t* keep, const uint8_t* sampled_host,
-                          int cfg_n, float cfg_scale) {
+                          int cfg_n, float cfg_scale, int canvas_h, int canvas_w) {
     if (!h || (!partial && !resume) || !out_codes || !top_k_host || !top_p_host || !workspace)
         return rqb::fail(RQB200_EINVAL, "ar_sample: null argument");
     if (B < 1) return rqb::fail(RQB200_EINVAL, "ar_sample: B must be > 0");
     if (cfg_n < 0 || (cfg_n > 0 && B != 2 * cfg_n))
         return rqb::fail(RQB200_EINVAL, "ar_sample: cfg_n must be 0, or n >= 1 with B = 2n rows (n conditional, then n unconditional)");
-    if (idx_begin < 0 || idx_end > h->cfg.H * h->cfg.W || idx_begin > idx_end)
+    if (canvas_h < h->cfg.H || canvas_w < h->cfg.W)
+        return rqb::fail(RQB200_EINVAL, "ar_sample: the canvas must be at least the model's grid (canvas_h >= H, canvas_w >= W)");
+    if ((int64_t)canvas_h * canvas_w * h->cfg.D > RQB200_CANVAS_MAX_CODES)
+        return rqb::fail(RQB200_EINVAL, "ar_sample: canvas_h * canvas_w * D must be at most RQB200_CANVAS_MAX_CODES (2^31 - 1)");
+    if (idx_begin < 0 || idx_end > canvas_h * canvas_w || idx_begin > idx_end)
         return rqb::fail(RQB200_EINVAL, "ar_sample: bad position span");
     if (sampled_host && !resume)
         for (int p = 0; p < idx_begin; p++)
@@ -364,11 +383,11 @@ int rqb200_ar_sample_span(rqb200_ar* h, const int64_t* partial, const int64_t* c
     if (h->fast)
         rc = rqb::ar_fast_sample(h->fast, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
                                  noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream,
-                                 cfg_n, cfg_s, keep, sampled_host);
+                                 cfg_n, cfg_s, keep, sampled_host, canvas_h, canvas_w);
     else
         rc = rqb::ar_sample_impl(h, partial, cond, B, idx_begin, idx_end, resume, temperature, top_k_host, top_p_host, noise,
                                  noise_stride, logits_out, force_codes, out_codes, workspace, workspace_bytes, (cudaStream_t)stream,
-                                 cfg_n, cfg_s, keep, sampled_host);
+                                 cfg_n, cfg_s, keep, sampled_host, canvas_h, canvas_w);
     h->last_launches = rqb::g_launches;
     return rc;
 }

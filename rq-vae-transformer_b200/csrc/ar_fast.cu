@@ -709,6 +709,8 @@ cond_tok_kernel(const StepState* __restrict__ stt, const float* __restrict__ con
 // code i is looked up in cb + i * cb_dstride (0: one shared codebook; K*C: per-depth codebooks stacked [D,K,C]).
 // last_only: code nd-1 alone instead of codes 0..nd-1 (cumsum_depth_ctx = false: the head input of depth d is e_{d-1}, :250-255).
 // stt is not __restrict__: the previous kernel writes it, and a read-only (non-coherent) load may be scheduled above pdl_wait().
+// CV: the positions are window positions, read from the canvas through stt->cv (kernels.h); else stt->codes is [B, HW, D].
+template <bool CV>
 __global__ void __launch_bounds__(64)
 code_sum_kernel(const StepState* stt, const float* __restrict__ cb, int64_t cb_dstride, int HW, int D, int K, int C,
                 int mode, int pos0, h16* __restrict__ out, int bf, int last_only) {
@@ -721,7 +723,7 @@ code_sum_kernel(const StepState* stt, const float* __restrict__ cb, int64_t cb_d
     for (int c = threadIdx.x; c < C; c += 64) {
         float a = 0.f;
         for (int i = last_only ? nd - 1 : 0; i < nd; i++) {
-            int64_t k = stt->codes[((int64_t)b * HW + pos) * D + i];
+            int64_t k = stt->codes[(CV ? stt->cv.at(b, pos) : (int64_t)b * HW + pos) * D + i];
             k = k < 0 ? 0 : (k >= K ? K - 1 : k);
             a += cb[i * cb_dstride + k * C + c];
         }
@@ -736,7 +738,8 @@ static int64_t cb_dstride(const rqb200_ar_config& c) { return c.codebook_per_dep
 //   where 0: stt->idx - 1 (the body step's token),  1: stt->idx (a head step's token),  2: pos0 + blockIdx.y (batched rows),
 // row = blockIdx.y * B + b (token-major, like code_sum_kernel).  The body token sums all D codes with pos = pos_emb_hw (pos_stride E);
 // the head token of depth d is code d-1 alone with pos = pos_emb_d + d*E (pos_stride 0).  E % 4 == 0.
-// stt is not __restrict__ (see code_sum_kernel).
+// stt is not __restrict__ (see code_sum_kernel).  CV: as code_sum_kernel.
+template <bool CV>
 __global__ void __launch_bounds__(128)
 tok_gather_kernel(const StepState* stt, const float* __restrict__ tok, int64_t tok_dstride, int HW, int D, int V, int E, int d0, int nd,
                   int where, int pos0, const float* __restrict__ pos, int64_t pos_stride, float* __restrict__ out) {
@@ -744,7 +747,7 @@ tok_gather_kernel(const StepState* stt, const float* __restrict__ tok, int64_t t
     tc::pdl_wait();
     const int b = blockIdx.x, B = gridDim.x;
     const int p = where == 2 ? pos0 + blockIdx.y : (where == 0 ? stt->idx - 1 : stt->idx);
-    const int64_t* kr = stt->codes + ((int64_t)b * HW + p) * D;
+    const int64_t* kr = stt->codes + (CV ? stt->cv.at(b, p) : (int64_t)b * HW + p) * D;
     int64_t rows[8];
 #pragma unroll
     for (int i = 0; i < 8; i++)
@@ -784,6 +787,13 @@ __global__ void __launch_bounds__(256) logits_copy_kernel(const StepState* __res
     for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) dst[i] = lg[i];
 }
 
+// a new segment of a canvas: the body sequence restarts (s = idx = 0) on the window at canvas offset org
+__global__ void segment_kernel(StepState* stt, int org) {
+    tc::pdl_launch_dependents();
+    tc::pdl_wait();
+    if (threadIdx.x == 0) { stt->s = 0; stt->idx = 0; stt->cv.org = org; }
+}
+
 // keep_pos != 0: a resumed span keeps the position counters the previous span left behind
 __global__ void init_state_kernel(StepState* dst, StepState v, int keep_pos) {
     if (threadIdx.x == 0) {
@@ -818,8 +828,12 @@ struct FastLayer {
     StreamedWeight qkv, proj, fc1, fc2;
 };
 
-// G_HEAD_STEP + d: head depth d alone with its logits copied out (rqb200_ar_step), d < 8
-enum { G_COND = 0, G_CODE = 1, G_HEAD = 2, G_HEAD_LOGITS = 3, G_HEAD_STEP = 4, G_COUNT = G_HEAD_STEP + 8 };
+// G_HEAD_STEP + d: head depth d alone with its logits copied out (rqb200_ar_step), d < 8.  G_CODE_CV .. G_HEAD_LOGITS_CV: G_CODE ..
+// G_HEAD_LOGITS on a canvas (their gathers and sampler address the window through StepState::cv); they share their grid twins' trace
+// slots, so the trace buffer keeps G_COUNT graphs' worth.
+enum { G_COND = 0, G_CODE = 1, G_HEAD = 2, G_HEAD_LOGITS = 3, G_HEAD_STEP = 4, G_COUNT = G_HEAD_STEP + 8,
+       G_CODE_CV = G_COUNT, G_HEAD_CV, G_HEAD_LOGITS_CV, G_ALL };
+static int grid_twin(int which) { return which < G_COUNT ? which : which - G_CODE_CV + G_CODE; }
 
 struct ArFast {
     rqb200_ar_config cfg;
@@ -834,8 +848,8 @@ struct ArFast {
     void* ws_base = nullptr;
     int B = 0;
     CUtensorMap tx_xn, tx_att, tx_h, tx_s;
-    cudaGraphExec_t graphs[G_COUNT] = {};
-    int64_t n_nodes[G_COUNT] = {};       // kernels recorded in each graph (for the launch counter)
+    cudaGraphExec_t graphs[G_ALL] = {};
+    int64_t n_nodes[G_ALL] = {};       // kernels recorded in each graph (for the launch counter)
     cudaStream_t cap_stream = nullptr;   // capture never happens on the caller's stream (it may be the legacy default stream)
     // launch options (cfg.flags), set by ar_fast_create and never changed afterwards.  use_pdl and trace are the single-token chain's;
     // a batched pass states each launch's PDL attribute at the launch and is never traced.
@@ -1032,7 +1046,7 @@ static int fast_stack(const ArFast& f, const std::vector<rqb200_block_weights>& 
     return 0;
 }
 
-static int record_body(ArFast& f, FastWs& ws, bool cond_token, cudaStream_t st) {
+static int record_body(ArFast& f, FastWs& ws, bool cond_token, bool cv, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const rqb200_ar_weights& w = f.w;
     const int E = c.embed_dim, B = f.B, HW = c.H * c.W, Tb = c.cond_len + HW;
@@ -1041,11 +1055,12 @@ static int record_body(ArFast& f, FastWs& ws, bool cond_token, cudaStream_t st) 
                            w.pos_emb_cond, c.cond_len, c.vocab_cond, E, ws.XB));
     } else if (c.embed_variant & RQB200_EMB_TOK_INPUT) {
         // x = sum_d tok_emb(code_d) + pos_emb_hw[idx-1]           (transformers.py:222,225)
-        RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, 1), dim3(128), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.tok_emb,
-                           tok_dstride(c), HW, c.D, c.vocab, E, 0, c.D, 0, 0, w.pos_emb_hw, (int64_t)E, ws.XB));
+        RQB_TRY(launch_pdl(cv ? tok_gather_kernel<true> : tok_gather_kernel<false>, dim3(B, 1), dim3(128), (size_t)0, st, f.use_pdl,
+                           (const StepState*)ws.state, w.tok_emb, tok_dstride(c), HW, c.D, c.vocab, E, 0, c.D, 0, 0, w.pos_emb_hw, (int64_t)E,
+                           ws.XB));
     } else {
-        RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
-                           cb_dstride(c), HW, c.D, c.codebook_size, c.code_dim, 0, 0, ws.S, f.bf, 0));
+        RQB_TRY(launch_pdl(cv ? code_sum_kernel<true> : code_sum_kernel<false>, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl,
+                           (const StepState*)ws.state, w.codebook, cb_dstride(c), HW, c.D, c.codebook_size, c.code_dim, 0, 0, ws.S, f.bf, 0));
         // x = W_in (sum_d e_d) + D b_in + pos_emb_hw[idx-1]       (bias counted D times, transformers.py:220,225)
         RQB_TRY(gemm(f, "w_in", f.w_in, f.tx_s, B, 1, GT_F32, w.b_in, (float)c.D, ws.XB, nullptr, w.pos_emb_hw - E /* row idx-1 */, 0,
                      &ws.state->idx, E, st));
@@ -1057,7 +1072,7 @@ static int record_body(ArFast& f, FastWs& ws, bool cond_token, cudaStream_t st) 
 
 // head depth d of the position stt->idx: its token, the head stack (cache rows [0, d) from the earlier depths of this position) and
 // the classifier -> ws.LOGITS
-static int record_head_depth(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
+static int record_head_depth(ArFast& f, FastWs& ws, int d, bool cv, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const rqb200_ar_weights& w = f.w;
     const int E = c.embed_dim, B = f.B, HW = c.H * c.W, D = c.D, V = c.vocab;
@@ -1068,13 +1083,13 @@ static int record_head_depth(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
     } else {
         if (c.embed_variant & RQB200_EMB_TOK_HEAD) {
             // token = tok_emb(code_{d-1}) + pos_emb_d[d]                                    (transformers.py:257,267)
-            RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, 1), dim3(128), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
-                               w.tok_emb, tok_dstride(c), HW, D, c.vocab, E, d - 1, 1, 1, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
+            RQB_TRY(launch_pdl(cv ? tok_gather_kernel<true> : tok_gather_kernel<false>, dim3(B, 1), dim3(128), (size_t)0, st, f.use_pdl,
+                               (const StepState*)ws.state, w.tok_emb, tok_dstride(c), HW, D, c.vocab, E, d - 1, 1, 1, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
                                ws.XH));
         } else {
             // token = head_mlp(sum_{i<d} e_i, or e_{d-1} alone) + pos_emb_d[d]              (transformers.py:250-255,267)
-            RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl, (const StepState*)ws.state, w.codebook,
-                               cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf,
+            RQB_TRY(launch_pdl(cv ? code_sum_kernel<true> : code_sum_kernel<false>, dim3(B, 1), dim3(64), (size_t)0, st, f.use_pdl,
+                               (const StepState*)ws.state, w.codebook, cb_dstride(c), HW, D, c.codebook_size, c.code_dim, d, 0, ws.S, f.bf,
                                (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
             RQB_TRY(gemm(f, "w_head", f.w_head, f.tx_s, B, 1, GT_F32, w.b_head, 1.f, ws.XH, nullptr,
                          w.pos_emb_d + (int64_t)d * E, 0, nullptr, 0, st));
@@ -1090,15 +1105,15 @@ static int record_head_depth(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
     return 0;
 }
 
-static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st) {
+static int record_head(ArFast& f, FastWs& ws, bool with_logits, bool cv, cudaStream_t st) {
     const rqb200_ar_config& c = f.cfg;
     const int B = f.B, HW = c.H * c.W, D = c.D, V = c.vocab;
     for (int d = 0; d < D; d++) {
-        RQB_TRY(record_head_depth(f, ws, d, st));
+        RQB_TRY(record_head_depth(f, ws, d, cv, st));
         if (with_logits)
             RQB_TRY(launch_pdl(logits_copy_kernel, dim3(64), dim3(256), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
                                (const float*)ws.LOGITS, d, (int64_t)B * V));
-        RQB_TRY(launch_sample_dyn(ws.LOGITS, ws.state, d, B, V, HW, D, st, f.use_pdl));
+        RQB_TRY(launch_sample_dyn(ws.LOGITS, ws.state, d, B, V, HW, D, st, f.use_pdl, cv));
     }
     RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, f.use_pdl, ws.state, 0, 1, D));
     return 0;
@@ -1107,7 +1122,7 @@ static int record_head(ArFast& f, FastWs& ws, bool with_logits, cudaStream_t st)
 // the single-token step's head graph: depth d only, its logits to stt->logits_out (stt->step == 0), no sampler; the code of depth d
 // comes from the caller at the next step.  Launch for launch the depth-d part of record_head: the same logits, bit for bit.
 static int record_head_step(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
-    RQB_TRY(record_head_depth(f, ws, d, st));
+    RQB_TRY(record_head_depth(f, ws, d, false, st));
     RQB_TRY(launch_pdl(logits_copy_kernel, dim3(64), dim3(256), (size_t)0, st, f.use_pdl, (const StepState*)ws.state,
                        (const float*)ws.LOGITS, 0, (int64_t)f.B * f.cfg.vocab));
     if (d == f.cfg.D - 1) RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, f.use_pdl, ws.state, 0, 1, 0));
@@ -1116,10 +1131,12 @@ static int record_head_step(ArFast& f, FastWs& ws, int d, cudaStream_t st) {
 
 static int record(ArFast& f, FastWs& ws, int which, cudaStream_t st) {
     f.tr_base = ws.trace;
-    f.tr_next = f.tr_graph_base[which];
-    int rc = which == G_COND ? record_body(f, ws, true, st) : which == G_CODE ? record_body(f, ws, false, st)
-           : which >= G_HEAD_STEP ? record_head_step(f, ws, which - G_HEAD_STEP, st)
-                                  : record_head(f, ws, which == G_HEAD_LOGITS, st);
+    f.tr_next = f.tr_graph_base[grid_twin(which)];
+    const bool cv = which >= G_COUNT;
+    const int kind = grid_twin(which);
+    int rc = kind == G_COND ? record_body(f, ws, true, false, st) : kind == G_CODE ? record_body(f, ws, false, cv, st)
+           : kind >= G_HEAD_STEP ? record_head_step(f, ws, kind - G_HEAD_STEP, st)
+                                 : record_head(f, ws, kind == G_HEAD_LOGITS, cv, st);
     // trace slots: every graph owns TR_PER_GRAPH of the buffer
     return rc;
 }
@@ -1143,7 +1160,7 @@ static int capture(ArFast& f, FastWs& ws, int which, cudaGraphExec_t* out) {
 }
 
 static void drop_graphs(ArFast& f) {
-    for (int i = 0; i < G_COUNT; i++) {
+    for (int i = 0; i < G_ALL; i++) {
         if (f.graphs[i]) cudaGraphExecDestroy(f.graphs[i]);
         f.graphs[i] = nullptr;
     }
@@ -1323,7 +1340,9 @@ static int stack_batched(const ArFast& f, const std::vector<rqb200_block_weights
 // body input tokens [T0, T0 + T) of every batch row into X (token-major, token T0 + r in rows r * B ..): token s < cond_len is a cond
 // token (transformers.py:224), token s >= cond_len carries the summed input embeddings of the codes of position s - cond_len (:219-225).
 // The cond tokens' kernel reads their index from state->s, which must equal T0.
-static int body_tokens_batched(const ArFast& f, const StepState* state, float* X, h16* S, int B, int T, cudaStream_t st, int T0 = 0) {
+// cv: the code tokens are window positions, gathered from the canvas through state->cv.
+static int body_tokens_batched(const ArFast& f, const StepState* state, float* X, h16* S, int B, int T, cudaStream_t st, int T0 = 0,
+                               bool cv = false) {
     const rqb200_ar_config& c = f.cfg;
     const rqb200_ar_weights& w = f.w;
     const int E = c.embed_dim, HW = c.H * c.W, cl = c.cond_len;
@@ -1335,11 +1354,11 @@ static int body_tokens_batched(const ArFast& f, const StepState* state, float* X
     float* Xc = X + (int64_t)n_cond * B * E;
     if (n_code > 0 && (c.embed_variant & RQB200_EMB_TOK_INPUT)) {
         // row (j, b) = sum_d tok_emb(code_d of position j) + pos_emb_hw[j]                   (:222,225)
-        RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, n_code), dim3(128), (size_t)0, st, false, state, w.tok_emb, tok_dstride(c), HW, c.D,
-                           c.vocab, E, 0, c.D, 2, pos0, w.pos_emb_hw, (int64_t)E, Xc));
+        RQB_TRY(launch_pdl(cv ? tok_gather_kernel<true> : tok_gather_kernel<false>, dim3(B, n_code), dim3(128), (size_t)0, st, false, state,
+                           w.tok_emb, tok_dstride(c), HW, c.D, c.vocab, E, 0, c.D, 2, pos0, w.pos_emb_hw, (int64_t)E, Xc));
     } else if (n_code > 0) {
-        RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, n_code), dim3(64), (size_t)0, st, false, state, w.codebook, cb_dstride(c), HW, c.D,
-                           c.codebook_size, c.code_dim, -c.D, pos0, S, f.bf, 0));
+        RQB_TRY(launch_pdl(cv ? code_sum_kernel<true> : code_sum_kernel<false>, dim3(B, n_code), dim3(64), (size_t)0, st, false, state,
+                           w.codebook, cb_dstride(c), HW, c.D, c.codebook_size, c.code_dim, -c.D, pos0, S, f.bf, 0));
         const int64_t Mc = (int64_t)B * n_code;
         GemmTcParams e = epilogue(GT_F32, w.b_in, Xc, w.pos_emb_hw + (int64_t)pos0 * E, E);
         e.bias_scale = (float)c.D;       // (the bias is counted D times, as in the single-token step)
@@ -1352,12 +1371,12 @@ static int body_tokens_batched(const ArFast& f, const StepState* state, float* X
 // ---- batched body pass: body tokens [T0, T0 + T) of every batch row in one pass, on the KV cache rows [0, T0) earlier passes or steps
 // left (state.s == T0).  Leaves ws.XB = the last token's output rows, the KV cache rows [T0, T0 + T) written, state.s = T0 + T.  The
 // prefill is T0 = 0; an append of a run of kept positions' code tokens to the cache is T0 > 0.
-static int body_batched(const ArFast& f, FastWs& ws, int T0, int T, cudaStream_t st) {
+static int body_batched(const ArFast& f, FastWs& ws, int T0, int T, cudaStream_t st, bool cv = false) {
     const rqb200_ar_config& c = f.cfg;
     const int E = c.embed_dim, B = f.B, HW = c.H * c.W, cl = c.cond_len, Tb = cl + HW;
     const int64_t M = (int64_t)B * T;
     if (M > ws.Mmax || T0 + T > Tb) return fail(RQB200_EINVAL, "ar fast tier: too many tokens for the batched body pass");
-    RQB_TRY(body_tokens_batched(f, ws.state, ws.PX, ws.PS, B, T, st, T0));
+    RQB_TRY(body_tokens_batched(f, ws.state, ws.PX, ws.PS, B, T, st, T0, cv));
     BatchBufs bb = {ws.PX, ws.PXN, ws.PQKV, ws.PATT, ws.PH};
     RQB_TRY(stack_batched(f, f.body, f.lbody, bb, B, T, ws.kc_body, ws.vc_body, (int64_t)B * c.n_head * Tb * 64, Tb, st, T0));
     RQB_CUDA(cudaMemcpyAsync(ws.XB, ws.PX + (int64_t)(T - 1) * B * E, (size_t)B * E * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -1421,12 +1440,12 @@ static int forward_passes(const ArFast& f, const FwdWs& ws, const int64_t* codes
     RQB_TRY(ln_rows(G, ws.BX + (int64_t)(cl - 1) * B * E, w.pos_emb_d, ws.HX, nof, nof, nullptr, E, f.bf, f.n_sm, st));
     for (int d = 1; d < D; d++) {
         if (c.embed_variant & RQB200_EMB_TOK_HEAD) {        // tok_emb(code_{d-1}) + pos_emb_d[d]        (:164,177)
-            RQB_TRY(launch_pdl(tok_gather_kernel, dim3(B, HW), dim3(128), (size_t)0, st, false, (const StepState*)ws.state, w.tok_emb,
+            RQB_TRY(launch_pdl(tok_gather_kernel<false>, dim3(B, HW), dim3(128), (size_t)0, st, false, (const StepState*)ws.state, w.tok_emb,
                                tok_dstride(c), HW, D, V, E, d - 1, 1, 2, 0, w.pos_emb_d + (int64_t)d * E, (int64_t)0,
                                ws.HX + (int64_t)d * G * E));
             continue;
         }
-        RQB_TRY(launch_pdl(code_sum_kernel, dim3(B, HW), dim3(64), (size_t)0, st, false, (const StepState*)ws.state, w.codebook,
+        RQB_TRY(launch_pdl(code_sum_kernel<false>, dim3(B, HW), dim3(64), (size_t)0, st, false, (const StepState*)ws.state, w.codebook,
                            cb_dstride(c), HW, D, c.codebook_size, c.code_dim, -d, 0, ws.S, f.bf,
                            (c.embed_variant & RQB200_EMB_NO_CUMSUM) ? 1 : 0));
         RQB_TRY(linear_rows(f, f.w_head, ws.S, G, G, true,
@@ -1553,10 +1572,12 @@ static int run_graph(ArFast& f, FastWs& ws, int which, cudaStream_t st) {
 
 // prefill: cond tokens, then (start_loc resume) the code tokens of positions < idx_begin (transformers.py:237-239), from a StepState
 // with s = idx = 0.  Leaves state.idx = idx_begin, state.s = cond_len + idx_begin, ws.XB = the last prefix token's output rows.
-static int prefill_prefix(ArFast& f, FastWs& ws, int idx_begin, cudaStream_t st) {
+// cv: the positions are those of the canvas window state.cv (code_graph is then G_CODE_CV).
+static int prefill_prefix(ArFast& f, FastWs& ws, int idx_begin, cudaStream_t st, bool cv = false) {
     const int T0 = f.cfg.cond_len + idx_begin;
+    const int code_graph = cv ? G_CODE_CV : G_CODE;
     if (f.batched_prefill && T0 >= 4 && (int64_t)f.B * T0 <= ws.Mmax) {
-        RQB_TRY(body_batched(f, ws, 0, T0, st));
+        RQB_TRY(body_batched(f, ws, 0, T0, st, cv));
         // state.idx must equal idx_begin for the first head graph
         if (idx_begin > 0) RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, idx_begin, 0));
     } else {
@@ -1565,7 +1586,7 @@ static int prefill_prefix(ArFast& f, FastWs& ws, int idx_begin, cudaStream_t st)
         // state.idx must equal (position whose codes feed the body) + 1 while replaying the code-token graph
         for (int j = 1; j <= idx_begin; j++) {
             RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, 1, 0));
-            RQB_TRY(run_graph(f, ws, G_CODE, st));
+            RQB_TRY(run_graph(f, ws, code_graph, st));
         }
     }
     return 0;
@@ -1576,18 +1597,22 @@ static int prefill_prefix(ArFast& f, FastWs& ws, int idx_begin, cudaStream_t st)
 // an H100 80GB HBM3 at 700 W, runs of exactly k: batched / token by token = 1.03 at k = 5, 0.90 at k = 6, 0.68 at k = 8.
 constexpr int APPEND_BATCHED_MIN = 6;
 
+// A canvas larger than the grid is walked in segments: consecutive sampled positions whose windows share an origin continue one KV
+// cache (the window positions between them are appended as kept code tokens, as on the grid); a new origin restarts the body sequence
+// with a prefill of the window's prefix.  On the grid every origin is 0: one segment, the grid graphs, the launches of a grid call.
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
                    float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st, int cfg_n,
-                   float cfg_s, const uint8_t* keep, const uint8_t* sampled) {
+                   float cfg_s, const uint8_t* keep, const uint8_t* sampled, int Ht, int Wt) {
     const rqb200_ar_config& c = f->cfg;
-    const int D = c.D, HW = c.H * c.W, cl = c.cond_len;
+    const int D = c.D, cl = c.cond_len;
+    const bool cv = Ht != c.H || Wt != c.W;
     if (B > 256) return fail(RQB200_EINVAL, "ar fast tier: batch must be in [1,256] per call");
     FastWs ws;
     size_t need = fast_layout(*f, B, wsp, ws_bytes, &ws);
     if (need > ws_bytes) return fail(RQB200_EWORKSPACE, "ar_sample: workspace too small");
     if (!resume && out != partial)
-        RQB_CUDA(cudaMemcpyAsync(out, partial, (size_t)B * HW * D * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+        RQB_CUDA(cudaMemcpyAsync(out, partial, (size_t)B * Ht * Wt * D * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
     int first = idx_begin;                            // the span's first sampled position
     while (first < idx_end && !plan_sampled(sampled, first)) first++;
     if (first >= idx_end) return 0;                   // nothing to sample: `out` holds partial
@@ -1598,6 +1623,10 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
         if (prev >= 0) return fail(RQB200_ESTATE, "ar_sample: resume on a workspace / batch the engine is not bound to");
         RQB_TRY(bind(*f, ws, wsp, B));
     }
+    // the current segment's window origin and the window position of prev (on the grid: 0 and prev)
+    int cur_org = 0, prev_p = -1;
+    win_locate(prev >= 0 ? prev : first, c.H, c.W, Wt, Ht, &cur_org, &prev_p);
+    if (prev < 0) prev_p = -1;
     StepState h = {};
     h.s = 0; h.idx = 0; h.step = 0;
     h.cond = cond; h.codes = out; h.force = force; h.noise = noise; h.logits_out = logits_out; h.noise_stride = noise_stride;
@@ -1605,12 +1634,14 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
     h.cfg_n = cfg_n; h.cfg_scale = cfg_s;        // (the head graphs' samplers read them: no recapture between guided and unguided calls)
     h.keep = keep;
     for (int d = 0; d < D; d++) { h.top_k[d] = top_k[d]; h.top_p[d] = top_p[d]; }
+    h.cv = CanvasMap{c.W, Wt, cur_org, Ht * Wt};
     RQB_TRY(launch_pdl(init_state_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, h, prev >= 0 ? 1 : 0));
     if (f->trace && prev < 0) RQB_CUDA(cudaMemsetAsync(ws.trace, 0, (size_t)4 * TR_CAP * sizeof(long long), st));
-    const int head_graph = logits_out ? G_HEAD_LOGITS : G_HEAD;
-    // the host's copy of state.idx / state.step: a head graph leaves idx one past its position; step counts the span's tokens, sampled
-    // or not, so that noise and logits_out stay indexed by token
-    int cur_idx = prev >= 0 ? prev + 1 : 0, cur_step = 0;
+    const int head_graph = logits_out ? (cv ? G_HEAD_LOGITS_CV : G_HEAD_LOGITS) : (cv ? G_HEAD_CV : G_HEAD);
+    const int code_graph = cv ? G_CODE_CV : G_CODE;
+    // the host's copy of state.idx / state.step: a head graph leaves idx one past its (window) position; step counts the span's canvas
+    // tokens, sampled or not, so that noise and logits_out stay indexed by token
+    int cur_idx = prev >= 0 ? prev_p + 1 : 0, cur_step = 0;
     auto advance_to = [&](int idx, int step) -> int {
         if (idx == cur_idx && step == cur_step) return 0;
         RQB_TRY(launch_pdl(advance_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, 0, idx - cur_idx, step - cur_step));
@@ -1619,21 +1650,28 @@ int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B
     };
     for (int b = first; b < idx_end; b++) {
         if (!plan_sampled(sampled, b)) continue;
+        int org, p;
+        win_locate(b, c.H, c.W, Wt, Ht, &org, &p);
+        if (prev >= 0 && org != cur_org) {                                 // a new window: its body sequence starts over
+            RQB_TRY(launch_pdl(segment_kernel, dim3(1), dim3(32), (size_t)0, st, false, ws.state, org));
+            cur_org = org; cur_idx = 0;
+            prev = -1;
+        }
         if (prev < 0) {
-            RQB_TRY(prefill_prefix(*f, ws, b, st));                        // cond tokens and positions [0, b); state.idx = b
-            cur_idx = b;
-        } else if (f->batched_prefill && b - prev >= APPEND_BATCHED_MIN && (int64_t)B * (b - prev) <= ws.Mmax) {
-            RQB_TRY(body_batched(*f, ws, cl + prev, b - prev, st));       // the code tokens of positions [prev, b) in one pass
+            RQB_TRY(prefill_prefix(*f, ws, p, st, cv));                    // cond tokens and window positions [0, p); state.idx = p
+            cur_idx = p;
+        } else if (f->batched_prefill && p - prev_p >= APPEND_BATCHED_MIN && (int64_t)B * (p - prev_p) <= ws.Mmax) {
+            RQB_TRY(body_batched(*f, ws, cl + prev_p, p - prev_p, st, cv)); // the code tokens of window positions [prev_p, p) in one pass
         } else {
-            for (int j = prev; j < b; j++) {                               // one body step each (state.idx == j + 1: position j)
+            for (int j = prev_p; j < p; j++) {                             // one body step each (state.idx == j + 1: position j)
                 RQB_TRY(advance_to(j + 1, cur_step));
-                RQB_TRY(run_graph(*f, ws, G_CODE, st));
+                RQB_TRY(run_graph(*f, ws, code_graph, st));
             }
         }
-        RQB_TRY(advance_to(b, (b - idx_begin) * D));
+        RQB_TRY(advance_to(p, (b - idx_begin) * D));
         RQB_TRY(run_graph(*f, ws, head_graph, st));                        // D head steps + sampling; advances idx, step
-        cur_idx = b + 1; cur_step += D;
-        prev = b;
+        cur_idx = p + 1; cur_step += D;
+        prev = b; prev_p = p;
     }
     return 0;
 }

@@ -10,7 +10,7 @@
 //                       scale folded into K :87, causal mask :89-91, softmax :92, att @ V :95)
 //   embedding kernels . transformers.py:217-232 (body token = sum_d input_mlp(e_d) + pos_emb_hw, bias counted D
 //                       times), :249-270 (head token = head_mlp(cumsum_d e) + pos_emb_d / spatial ctx + pos_emb_d[0])
-#include "common.cuh"
+#include "kernels.h"
 
 namespace rqb {
 
@@ -180,11 +180,13 @@ int launch_attn_cached(const float* qkv, float* kc, float* vc, float* out, int B
 
 // ------------------------------------------------------------------------------------------------ embedding glue
 // out[(b*J + (j-j0))*D + d, :] = codebook_d[codes[b, j, d], :]   for j in [j0, j0+J); codebook_d = cb + d * cb_dstride
+// CV: j is a window position, read from the canvas through cv (kernels.h); else codes is [B, HW, D]
+template <bool CV>
 __global__ void code_emb_kernel(const int64_t* __restrict__ codes, const float* __restrict__ cb, int64_t cb_dstride, int HW, int D,
-                                int K, int C, int j0, int J, float* __restrict__ out) {
+                                int K, int C, int j0, int J, float* __restrict__ out, CanvasMap cv) {
     int r = blockIdx.x;                         // over B*J*D
     int d = r % D, j = (r / D) % J, b = r / (D * J);
-    int64_t k = codes[((int64_t)b * HW + j0 + j) * D + d];
+    int64_t k = codes[(CV ? cv.at(b, j0 + j) : (int64_t)b * HW + j0 + j) * D + d];
     k = k < 0 ? 0 : (k >= K ? K - 1 : k);
     const float* e = cb + d * cb_dstride + k * C;
     for (int c = threadIdx.x; c < C; c += blockDim.x) out[(int64_t)r * C + c] = e[c];
@@ -212,15 +214,16 @@ __global__ void cond_token_kernel(const int64_t* __restrict__ cond, const float*
         X[((int64_t)b * Tn + s) * E + e] = cond_emb[c * E + e] + pos_cond[(int64_t)s * E + e];
 }
 // head input for depth d >= 1: out[b,:] = e_0 + e_1 + ... + e_{d-1} (sequential, torch.cumsum order); last_only: e_{d-1} alone
-// (cumsum_depth_ctx = false, or the row of a token embedding table when cb is tok_emb)
+// (cumsum_depth_ctx = false, or the row of a token embedding table when cb is tok_emb).  CV: as code_emb_kernel
+template <bool CV>
 __global__ void head_cumsum_kernel(const int64_t* __restrict__ codes, const float* __restrict__ cb, int64_t cb_dstride, int HW, int D,
-                                   int K, int C, int j, int d, int last_only, float* __restrict__ out) {
+                                   int K, int C, int j, int d, int last_only, float* __restrict__ out, CanvasMap cv) {
     int b = blockIdx.x;
     const int i0 = last_only ? d - 1 : 0;
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
         float a = 0.f;
         for (int i = i0; i < d; i++) {
-            int64_t k = codes[((int64_t)b * HW + j) * D + i];
+            int64_t k = codes[(CV ? cv.at(b, j) : (int64_t)b * HW + j) * D + i];
             k = k < 0 ? 0 : (k >= K ? K - 1 : k);
             float e = cb[i * cb_dstride + k * C + c];
             a = (i == i0) ? e : a + e;
@@ -237,9 +240,12 @@ __global__ void row_add_kernel(const float* __restrict__ in, int64_t in_row_stri
 }
 
 int launch_code_emb(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j0, int J,
-                    float* out, cudaStream_t st) {
+                    float* out, cudaStream_t st, const CanvasMap* cv) {
     if (B * J * D <= 0) return 0;
-    code_emb_kernel<<<B * J * D, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j0, J, out);
+    if (cv)
+        code_emb_kernel<true><<<B * J * D, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j0, J, out, *cv);
+    else
+        code_emb_kernel<false><<<B * J * D, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j0, J, out, CanvasMap{});
     return check_launch("code_emb");
 }
 int launch_body_token(const float* lin, const float* pos_hw, int B, int D, int E, int j0, int J, int s0, int Tn, float* X,
@@ -254,8 +260,11 @@ int launch_cond_token(const int64_t* cond, const float* cond_emb, const float* p
     return check_launch("cond_token");
 }
 int launch_head_cumsum(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j, int d,
-                       float* out, cudaStream_t st, bool last_only) {
-    head_cumsum_kernel<<<B, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j, d, last_only ? 1 : 0, out);
+                       float* out, cudaStream_t st, bool last_only, const CanvasMap* cv) {
+    if (cv)
+        head_cumsum_kernel<true><<<B, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j, d, last_only ? 1 : 0, out, *cv);
+    else
+        head_cumsum_kernel<false><<<B, 64, 0, st>>>(codes, cb, cb_dstride, HW, D, K, C, j, d, last_only ? 1 : 0, out, CanvasMap{});
     return check_launch("head_cumsum");
 }
 int launch_row_add(const float* in, int64_t in_row_stride, int64_t in_off, const float* pos, int B, int E, float* out,

@@ -17,6 +17,30 @@ struct RqTables {
 // host arrays of n device pointers / sizes -> RqTables; fails unless 1 <= n <= RQ_MAX_TABLES, every K > 0 and no pointer is null
 int make_rq_tables(RqTables* out, const float* const* cb_host, const int32_t* K_host, int n);
 
+// Sliding-window sampling of a code map larger than the model's grid (rqb200_ar_sample_span with a canvas): the token at canvas
+// position (i, j) is sampled as the model's token (i - r0, j - c0) of the grid-sized window with origin (r0, c0) = (win_origin(i, H, Ht),
+// win_origin(j, W, Wt)).  The window's position p (raster order in the H x W grid) lies at canvas position org + (p / gw) * cw + p % gw
+// of its batch row, org = r0 * cw + c0; a batch row holds chw canvas positions.  Kernels that gather codes take it as a template switch:
+// their grid instantiation addresses [B, H*W, D] exactly as before.
+struct CanvasMap {
+    int gw;         // the model grid's width W
+    int cw;         // the canvas width Wt
+    int org;        // the window's origin, r0 * Wt + c0
+    int chw;        // canvas positions per batch row, Ht * Wt
+    __host__ __device__ __forceinline__ int64_t at(int64_t b, int p) const { return b * chw + org + (p / gw) * cw + p % gw; }
+};
+// the window origin along one axis: the window of n cells that centres coordinate i (floor(n/2) cells before it), clamped to [0, nt - n]
+inline int win_origin(int i, int n, int nt) {
+    const int r = i - n / 2;
+    return r < 0 ? 0 : (r > nt - n ? nt - n : r);
+}
+// canvas position idx (raster order in Ht x Wt) -> its window's origin org and its position p inside the window
+inline void win_locate(int idx, int H, int W, int Wt, int Ht, int* org, int* p) {
+    const int i = idx / Wt, j = idx % Wt, r0 = win_origin(i, H, Ht), c0 = win_origin(j, W, Wt);
+    *org = r0 * Wt + c0;
+    *p = (i - r0) * W + (j - c0);
+}
+
 // rq_search.cu
 int launch_rq_quantize(const float* x, const RqTables& tabs, int64_t N, int C, int D, int64_t* codes, float* quant_list,
                        float* resid_out, cudaStream_t st, int form = 0);
@@ -44,14 +68,14 @@ int launch_attn_cached(const float* qkv, float* kc, float* vc, float* out, int B
                        int nh, cudaStream_t st);
 // cb_dstride: floats between depth d's table and depth d+1's (0: one shared [K,C] table; K*C: a [D,K,C] per-depth stack)
 int launch_code_emb(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j0, int J,
-                    float* out, cudaStream_t st);
+                    float* out, cudaStream_t st, const CanvasMap* cv = nullptr);
 int launch_body_token(const float* lin, const float* pos_hw, int B, int D, int E, int j0, int J, int s0, int Tn, float* X,
                       cudaStream_t st);
 int launch_cond_token(const int64_t* cond, const float* cond_emb, const float* pos_cond, int B, int cond_len, int vocab_cond,
                       int E, int Tn, float* X, cudaStream_t st);
 // last_only: code d-1 alone instead of the sum over codes 0..d-1
 int launch_head_cumsum(const int64_t* codes, const float* cb, int64_t cb_dstride, int B, int HW, int D, int K, int C, int j, int d,
-                       float* out, cudaStream_t st, bool last_only = false);
+                       float* out, cudaStream_t st, bool last_only = false, const CanvasMap* cv = nullptr);
 int launch_row_add(const float* in, int64_t in_row_stride, int64_t in_off, const float* pos, int B, int E, float* out,
                    cudaStream_t st);
 // conv_kernels.cu
@@ -159,6 +183,7 @@ struct StepState {
     const uint8_t* keep;      // [B, HW, D] nonzero: the token keeps the code `codes` was initialised with (the sampler writes nothing); or null
     int top_k[8];
     float top_p[8];
+    CanvasMap cv;             // sliding-window sampling: where the window of the current segment lies in `codes` (canvas graphs only)
 };
 
 // The position plan of a masked sample (rqb200_ar_sample_span): sampled[p] != 0 when some row samples some depth of position p;
@@ -172,7 +197,9 @@ inline int plan_prev(const uint8_t* sampled, int p) {
         if (plan_sampled(sampled, i)) return i;
     return -1;
 }
-int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, int V, int HW, int D, cudaStream_t st, bool pdl);
+// canvas: the sampler writes the canvas position of stt->idx through stt->cv (the canvas graphs), else position stt->idx of [B, HW, D]
+int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, int V, int HW, int D, cudaStream_t st, bool pdl,
+                      bool canvas = false);
 
 struct ArFast;
 ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, const rqb200_block_weights* body,
@@ -181,11 +208,12 @@ void ar_fast_destroy(ArFast* f);
 size_t ar_fast_workspace_bytes(const ArFast* f, int B);
 // positions [idx_begin, idx_end) of the raster; resume != 0: continue on the KV state the previous call left in this workspace.
 // cfg_n > 0: classifier-free guidance over B = 2 cfg_n rows [cond | uncond] with scale cfg_s.  keep / sampled: the masked-sample
-// plan (null: every token sampled).  Arguments already checked by rqb200_ar_sample_span, except B <= 256 and the workspace size.
+// plan (null: every token sampled).  Ht x Wt: the canvas (H x W: the grid).  Arguments already checked by rqb200_ar_sample_span, except
+// B <= 256 and the workspace size.
 int ar_fast_sample(ArFast* f, const int64_t* partial, const int64_t* cond, int B, int idx_begin, int idx_end, int resume,
                    float temperature, const int32_t* top_k, const float* top_p, const float* noise, int64_t noise_stride,
                    float* logits_out, const int64_t* force, int64_t* out, void* wsp, size_t ws_bytes, cudaStream_t st, int cfg_n,
-                   float cfg_s, const uint8_t* keep, const uint8_t* sampled);
+                   float cfg_s, const uint8_t* keep, const uint8_t* sampled, int Ht, int Wt);
 // the logits of ONE token (idx, d) into logits_out [B,V] (rqb200_ar_step; arguments already checked by the caller)
 int ar_fast_step(ArFast* f, const int64_t* xs, int64_t xs_stride, const int64_t* cond, int B, int idx, int d, int restart,
                  float* logits_out, void* wsp, size_t ws_bytes, cudaStream_t st);

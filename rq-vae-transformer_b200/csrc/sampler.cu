@@ -53,6 +53,8 @@ __device__ __forceinline__ bool item_before(const SortItem& a, const SortItem& b
     return (a.p > b.p) || (a.p == b.p && a.idx < b.idx);
 }
 
+// CV (the fast tier's canvas graphs): the token's code lives at the canvas position of stt->idx (stt->cv, kernels.h)
+template <bool CV>
 __global__ void __launch_bounds__(SMP_THREADS, 1)
 sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise, int V, float temperature, int top_k,
               float top_p, int64_t* __restrict__ out_idx, const int64_t* __restrict__ force, int64_t out_stride,
@@ -82,10 +84,10 @@ sample_kernel(const float* __restrict__ logits, const float* __restrict__ qnoise
     if (stt != nullptr && stt->cfg_n > 0 && row >= stt->cfg_n && stt->force == nullptr) return;
     tc::pdl_wait();
     if (stt != nullptr) {   // fast AR tier: per-token pointers and settings come from the device-resident StepState
-        const int64_t off = (int64_t)stt->idx * dyn_D + dyn_d;
+        const int64_t off = (CV ? stt->cv.at(0, stt->idx) : (int64_t)stt->idx) * dyn_D + dyn_d;
         out_idx = stt->codes + off;
         force = stt->force ? stt->force + off : nullptr;
-        out_stride = (int64_t)dyn_HW * dyn_D;
+        out_stride = (int64_t)(CV ? stt->cv.chw : dyn_HW) * dyn_D;
         qnoise = stt->noise ? stt->noise + (int64_t)(stt->step + dyn_d) * stt->noise_stride : nullptr;
         temperature = stt->temperature;
         top_k = stt->top_k[dyn_d];
@@ -437,20 +439,27 @@ int launch_sample(const float* logits, const float* q, int B, int V, float tempe
     int vpad = 1;
     while (vpad < V) vpad <<= 1;
     size_t smem = (size_t)V * sizeof(float) + (top_p < 1.0f ? (size_t)vpad * sizeof(SortItem) : 0);
-    RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel);
+    RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel<false>);
     const int grid = (cfg_n > 0 && force == nullptr) ? cfg_n : B;
-    sample_kernel<<<grid, SMP_THREADS, smem, st>>>(logits, q, V, temperature, top_k, top_p, out_idx, force, out_stride, nullptr, 0, 0,
+    sample_kernel<false><<<grid, SMP_THREADS, smem, st>>>(logits, q, V, temperature, top_k, top_p, out_idx, force, out_stride, nullptr, 0, 0,
                                                    0, algo, cfg_n, cfg_s, keep);
     return check_launch("sample_logits");
 }
 
-int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, int V, int HW, int D, cudaStream_t st, bool pdl) {
+int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, int V, int HW, int D, cudaStream_t st, bool pdl,
+                      bool canvas) {
     if (V <= 0 || V > SMP_MAXV) return fail(RQB200_EINVAL, "sample: V must be in [1,16384]");
     int vpad = 1;
     while (vpad < V) vpad <<= 1;
     size_t smem = (size_t)V * sizeof(float) + (size_t)vpad * sizeof(SortItem);   // top_p is only known on the device
-    RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel);
-    return launch_pdl(sample_kernel, dim3(B), dim3(SMP_THREADS), smem, st, pdl, logits, (const float*)nullptr, V, 1.0f, 0, 1.0f,
+    if (canvas) {
+        RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel<true>);
+        return launch_pdl(sample_kernel<true>, dim3(B), dim3(SMP_THREADS), smem, st, pdl, logits, (const float*)nullptr, V, 1.0f, 0, 1.0f,
+                          (int64_t*)nullptr, (const int64_t*)nullptr, (int64_t)0, stt, d, HW, D, SAMPLER_ALGO_DEFAULT, 0, 0.0f,
+                          (const uint8_t*)nullptr);
+    }
+    RQB_ENSURE_SMEM(SMP_MAXV * 12, sample_kernel<false>);
+    return launch_pdl(sample_kernel<false>, dim3(B), dim3(SMP_THREADS), smem, st, pdl, logits, (const float*)nullptr, V, 1.0f, 0, 1.0f,
                       (int64_t*)nullptr, (const int64_t*)nullptr, (int64_t)0, stt, d, HW, D, SAMPLER_ALGO_DEFAULT, 0, 0.0f,
                       (const uint8_t*)nullptr);
 }

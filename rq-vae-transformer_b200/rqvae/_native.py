@@ -89,6 +89,8 @@ def lib():
     L.rqb200_ar_destroy.restype = None
     L.rqb200_ar_workspace_bytes.restype = C.c_size_t
     L.rqb200_ar_workspace_bytes.argtypes = [C.c_void_p, C.c_int]
+    # the arguments up to cfg_scale (ABI 113).  ABI 117 appended canvas_h and canvas_w (C int): every caller passes them after
+    # these as C.c_int values, which ctypes forwards as declared-int arguments of the same call.
     L.rqb200_ar_sample_span.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                         C.POINTER(C.c_int32), C.POINTER(C.c_float), C.c_void_p, C.c_int64, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,

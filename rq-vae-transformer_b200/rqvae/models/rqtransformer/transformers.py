@@ -373,13 +373,15 @@ class RQTransformer(Stage2Model):
             raise ValueError("rqb200: uncond entries must lie in [0, %d)" % self.vocab_size_cond)
         return float(cfg_scale), u
 
-    def _keep_mask(self, keep_mask, B, start_loc):
+    def _keep_mask(self, keep_mask, B, start_loc, canvas=None):
         """sample()'s keep_mask checked before any kernel runs and laid out for the engine: None, or a contiguous uint8 [B, H, W, D] with
         the start_loc prefix kept too.  Raises ValueError for a mask that is not a bool tensor, does not broadcast to [B, H, W, D] or lies
-        on another device than the model."""
+        on another device than the model.  canvas: (Ht, Wt) of a canvas larger than the grid, which then takes the place of (H, W)."""
         if keep_mask is None:
             return None
         H, W, D = self.block_size
+        if canvas is not None:
+            H, W = canvas
         if not isinstance(keep_mask, torch.Tensor) or keep_mask.dtype != torch.bool:
             raise ValueError("rqb200: keep_mask must be a torch.bool tensor, got %s" % getattr(keep_mask, "dtype", type(keep_mask)))
         if keep_mask.device != self.pos_emb_hw.device:
@@ -405,7 +407,7 @@ class RQTransformer(Stage2Model):
         keep: None, or uint8 [B, H, W, D] from _keep_mask -- masked completion (keep, sampled_host): each batch chunk passes its
         rows of the mask (guided: in both branches' rows) and the positions where any of its rows samples any depth; those position
         lists are formed on the device and read to the host once per call.  The logits of positions a chunk skips are not written."""
-        H, W, D = self.block_size
+        H, W, D = partial.shape[1:]         # the canvas: the model's grid, or larger (sliding-window sampling)
         B = partial.shape[0]
         dev = self.pos_emb_hw.device
         self._check_computable()
@@ -484,7 +486,7 @@ class RQTransformer(Stage2Model):
                         float(temperature), kk, pp, off(noise, lo, V, 4, tok0 * B * V), 0 if noise is None else B * V,
                         off(logits, 0, V, 4, (p0 - idx0) * D * R * V), off(fc_c, 0, HWD, 8), off(out_c, 0, HWD, 8),
                         N.ptr(eng["ws"]), eng["ws"].numel(), C.c_void_p(st.cuda_stream), N.ptr(plans[i][1]), plans[i][0],
-                        0 if guidance is None else rows // 2, C.c_float(0.0 if guidance is None else guidance[0])), "ar_sample")
+                        0 if guidance is None else rows // 2, C.c_float(0.0 if guidance is None else guidance[0]), C.c_int(H), C.c_int(W)), "ar_sample")
                     launches += N.lib().rqb200_ar_last_launches(eng["handle"])
             if n_tok == 0:
                 out.copy_(partial)
@@ -523,10 +525,20 @@ class RQTransformer(Stage2Model):
         before start_loc are kept as always.  Every other token is sampled as sample() would, seeing the kept codes before it in raster
         order (and none after it), and every token still takes its Exp(1) draw.  Positions where nothing is sampled skip the head stack;
         their codes reach the body in one batched pass per run on the fast tier.  Which positions those are is read to the host once
-        per call.  Composes with guidance, both tiers and every fast weight format."""
-        assert self.block_size == partial_sample.shape[1:]
+        per call.  Composes with guidance, both tiers and every fast weight format.
+        Canvases larger than the grid (sliding-window sampling): ``partial_sample`` [B, Ht, Wt, D] with Ht >= H, Wt >= W returns
+        [B, Ht, Wt, D].  The token at canvas (i, j, d) is sampled as the model's token (i - r0, j - c0, d) of the H x W window with origin
+        r0 = clamp(i - H // 2, 0, Ht - H), c0 = clamp(j - W // 2, 0, Wt - W) (Taming Transformers' rule at even sizes), seeing the cond
+        prefix, the window's positions before it and its own depths < d, read from the canvas as it stands -- nothing outside its
+        window.  ``start_loc`` is in canvas coordinates and ``keep_mask`` broadcasts to [B, Ht, Wt, D] (outpainting: keep the encoded
+        part).  Ht * Wt * D may not exceed 2^31 - 1.  On the grid itself this is the call above, launch for launch."""
+        shp = partial_sample.shape
+        assert len(shp) == 4 and shp[1] >= self.block_size[0] and shp[2] >= self.block_size[1] and shp[3] == self.block_size[2]
+        if shp[1] * shp[2] * shp[3] > CANVAS_MAX_CODES:
+            raise ValueError("rqb200: a canvas of %d x %d x %d codes is past the engine's index range (Ht * Wt * D <= 2^31 - 1)"
+                             % (shp[1], shp[2], shp[3]))
         guidance = self._guidance(partial_sample.shape[0], cfg_scale, uncond)
-        keep = self._keep_mask(keep_mask, partial_sample.shape[0], start_loc)
+        keep = self._keep_mask(keep_mask, partial_sample.shape[0], start_loc, canvas=(shp[1], shp[2]))
         self.init_cache()
         out = self._native_sample(partial_sample, model_aux, cond, start_loc, temperature, top_k, top_p, amp, guidance=guidance,
                                   keep=keep)
@@ -760,6 +772,10 @@ class RQTransformer(Stage2Model):
         else:
             tokenwise = torch.nn.functional.cross_entropy(logits, targets.reshape(-1), reduction="none")
         return tokenwise.reshape(-1, D).mean(dim=0)
+
+
+# the engine's canvas limit (RQB200_CANVAS_MAX_CODES, include/rqb200.h): Ht * Wt * D, the codes of one batch row of a canvas
+CANVAS_MAX_CODES = (1 << 31) - 1
 
 
 def _chunk_bounds(B, mode, limit=256):

@@ -94,7 +94,7 @@ def per_position_ms(ar, vae, cond, B):
     def span(p0, p1, resume):
         N.check(N.lib().rqb200_ar_sample_span(eng["handle"], N.ptr(part), N.ptr(cond), B, p0, p1, resume, 1.0, kk, pp, null, 0, null,
                                               null, N.ptr(out), N.ptr(eng["ws"]), eng["ws"].numel(), C.c_void_p(st.cuda_stream),
-                                              None, None, 0, C.c_float(0.0)),
+                                              None, None, 0, C.c_float(0.0), C.c_int(H), C.c_int(W)),
                 "ar_sample_span")
 
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
