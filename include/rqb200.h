@@ -332,12 +332,63 @@ int rqb200_inception_forward(rqb200_inception* h, const float* x, int B, int H, 
                              float* out3, float* logits, void* workspace, size_t workspace_bytes, void* stream);
 int64_t rqb200_inception_last_launches(const rqb200_inception* h);
 
+/* ------------------------------------------------------------------------------------------------ CLIP ViT
+ * OpenAI's CLIP ViT image and text encoders (the model behind the reference's rqvae/metrics/clip_score.py) as a static layer plan
+ * (csrc/clip_engine.cu).  Tensors are registered under OpenAI's state_dict keys as they are (fp32, device): visual.conv1.weight,
+ * visual.class_embedding, visual.positional_embedding, visual.ln_pre.*, visual.transformer.resblocks.N.{ln_1, attn.in_proj_*,
+ * attn.out_proj.*, ln_2, mlp.c_fc.*, mlp.c_proj.*}, visual.ln_post.*, visual.proj, token_embedding.weight, positional_embedding,
+ * transformer.resblocks.N.*, ln_final.*, text_projection.  rqb200_clip_finalize names the first missing or mis-sized key, then packs
+ * conv1 (K padded to a multiple of 64), the transposed projections and, on the fast tier, fp16 copies of every GEMM weight into the
+ * caller's buffer of rqb200_clip_params_bytes(h) bytes, which must stay alive and unchanged (as must the registered tensors) while
+ * the engine is used.  Heads = width / 64.  RQB200_MODE_EXACT: fp32 FFMA throughout.  RQB200_MODE_FAST: fp16 operands on the wgmma
+ * GEMMs (fp32 accumulate), fp32 residual stream, LayerNorm and softmax; widths must be multiples of 128.  ABI 118 added this section. */
+typedef struct rqb200_clip rqb200_clip;
+typedef struct {
+    int32_t vision_width, vision_layers, vision_patch, vision_resolution;
+    int32_t text_width, text_layers, context_length, vocab_size;
+    int32_t embed_dim;
+    int32_t mode;       /* RQB200_MODE_EXACT or RQB200_MODE_FAST */
+} rqb200_clip_config;
+
+/* rqb200_clip_encode_image flags */
+#define RQB200_CLIP_PREPROCESS 1   /* x = NCHW pixels in [0, 1] at any H x W: (x * 255) truncated to uint8 (inputs clamped to [0, 1] first),
+                                    * Pillow's bicubic resize of the shorter side to R, centre crop R x R, (u / 255 - mean) / std;
+                                    * bit-exact to the PIL / torchvision route.  Else x = an already-normalised [B, 3, R, R] batch. */
+
+rqb200_clip* rqb200_clip_create(const rqb200_clip_config* cfg);
+void rqb200_clip_destroy(rqb200_clip* h);
+int rqb200_clip_set_tensor(rqb200_clip* h, const char* key, const void* ptr, int dtype, int64_t numel);
+size_t rqb200_clip_params_bytes(const rqb200_clip* h);
+int rqb200_clip_finalize(rqb200_clip* h, void* params, size_t params_bytes, void* stream);
+/* workspaces of one encode call; 0 for an input the call refuses */
+size_t rqb200_clip_workspace_bytes(rqb200_clip* h, int B, int H, int W, int flags);
+size_t rqb200_clip_text_workspace_bytes(rqb200_clip* h, int N);
+/* image features [B, embed_dim] fp32 of x (see RQB200_CLIP_PREPROCESS) */
+int rqb200_clip_encode_image(rqb200_clip* h, const float* x, int B, int H, int W, int flags, float* feat_out, void* workspace,
+                             size_t workspace_bytes, void* stream);
+/* text features [N, embed_dim] fp32 of tokens [N, context_length] int64 (ids in [0, vocab_size)), pooled at tokens.argmax(-1) */
+int rqb200_clip_encode_text(rqb200_clip* h, const int64_t* tokens, int N, float* feat_out, void* workspace, size_t workspace_bytes,
+                            void* stream);
+/* out[i] = F.cosine_similarity(img_feat[i], txt_feat[i]) (eps 1e-8) for n rows of dim floats */
+int rqb200_clip_cosine(const float* img_feat, const float* txt_feat, int n, int dim, float* out, void* stream);
+int64_t rqb200_clip_last_launches(const rqb200_clip* h);
+/* the host resize plan of an H x W input at resolution R: out6 = {resized H, resized W, crop top, crop left, horizontal taps per
+ * output pixel (0: that pass is skipped), vertical taps} */
+int rqb200_clip_resize_plan(int H, int W, int R, int32_t* out6);
+
 /* ------------------------------------------------------------------------------------------------ diagnostics
  * Single-kernel entry points used by tests/ and bench.py's roofline leg; not part of the reference-facing surface.
  * rqb200_dbg_gemm_tc: one launch of the wgmma weight-streaming GEMM (csrc/gemm_tc.cu):
  *   out[b, n] = act(sum_k W[n,k] X[b,k] + bias[n]) (+ residual[b,n]);  W [N_out,K], X [B,K] both 16-bit: fmt 0 = fp16, 1 = bf16;
+ *   act (16-bit output only): gelu 0 none, 1 exact GELU, 2 QuickGELU x * sigmoid(1.702 x) (16-bit weights; ABI 118);
  *   partial != NULL: partial [splits,B,N_out] f32 receives the per-split sums instead (no bias / act / residual; B <= 256).
  *   B > 256 (splits == 1) runs as row chunks of 256 (the batched-prefill / teacher-forced-forward shape). */
+/* rqb200_dbg_clip_preprocess: the CLIP preprocessing of x [B, 3, H, W] at resolution R: u8_out [B, 3, R, R] the uint8 crop, norm_out
+ * [B, 3, R, R] fp32 the normalised tensor (either nullable).  rqb200_dbg_clip_attn: the exact tier's fp32 attention, qkv [T * G, 3E]
+ * token-major -> out [T * G, E]; rqb200_dbg_clip_attn_flash: the fast tier's (prefill_attn_flash_kernel, fp16).  causal 0 / 1. */
+int rqb200_dbg_clip_preprocess(const float* x, int B, int H, int W, int R, uint8_t* u8_out, float* norm_out, void* stream);
+int rqb200_dbg_clip_attn(const float* qkv, float* out, int G, int T, int E, int causal, void* stream);
+int rqb200_dbg_clip_attn_flash(const void* qkv16, void* att16, int G, int T, int E, int causal, void* stream);
 int rqb200_dbg_gemm_tc(const void* W16, const void* X16, const float* bias, const float* residual, void* out,
                        int out_is_16, int gelu, float* partial, int N_out, int K, int B, int splits, int fmt, void* stream);
 /* rqb200_dbg_gemm_tc_fp8: the same GEMM with FP8 (E4M3) weights and fp16 activations:
@@ -389,7 +440,8 @@ int rqb200_dbg_conv_tc_gn(const void* X16, const void* W16, const void* X16lo, c
 
 /* rqb200_dbg_rows_gemm: the large-M GEMM of the batched prefill / forward passes (csrc/conv_tc.cu launch_rows_gemm_tc: persistent
  * 128 x BN tiles, wgmma): out[m,n] = act(sum_k X[m,k] W[n,k] + bias[n]) (+ residual[m,n]).  X [ceil(M/128)*128, K] and
- * W [N_out,K] 16-bit (fmt 0 fp16 / 1 bf16); exactly one of out_f32 / out_16; gelu applies to out_16 only. */
+ * W [N_out,K] 16-bit (fmt 0 fp16 / 1 bf16); exactly one of out_f32 / out_16; gelu (0 none, 1 exact GELU,
+ * 2 QuickGELU since ABI 118) applies to out_16 only. */
 int rqb200_dbg_rows_gemm(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                          int gelu, int fmt, int64_t M, int N_out, int K, void* stream);
 

@@ -499,7 +499,9 @@ constexpr int PM_ROW = 144;                           // bytes per staged row (6
 // ldmatrix.trans.  Key tiles are visited in a fixed order: run-to-run deterministic.  When kc != NULL the CTA of query tile i writes
 // the cache rows T0 + t of its tile's new tokens t (every new row exactly once).  At T0 = 0 every tile but the diagonal one is
 // unmasked, as in the plain prefill.
-template <bool BF>
+// CAUSAL == false (the CLIP vision tower; T0 = 0, no cache): every query sees keys [0, T0 + T); the key tile that holds the last key
+// masks the zero-filled rows past it explicitly (causality no longer does).
+template <bool BF, bool CAUSAL = true>
 __global__ void __launch_bounds__(128)
 prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16* __restrict__ vc, h16* __restrict__ att, int G, int T, int E,
                           int nh, int Tmax, int T0) {
@@ -543,7 +545,7 @@ prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16
     const int r0 = qt * 64 + 16 * w + (lane >> 2), r1 = r0 + 8;          // new-token rows; sequence rows T0 + r0, T0 + r1
     const int q0 = T0 + r0, q1 = T0 + r1;
     // the last key tile of this query tile: the one holding its last real query's key (rows past T see keys up to it, never beyond)
-    const int kt_last = (T0 + min(qt * 64 + 63, T - 1)) >> 6;
+    const int kt_last = CAUSAL ? (T0 + min(qt * 64 + 63, T - 1)) >> 6 : (T0 + T - 1) >> 6;
     uint32_t qa[4][4];
     float oacc[8][4];
 #pragma unroll
@@ -580,15 +582,17 @@ prefill_attn_flash_kernel(const h16* __restrict__ qkv, h16* __restrict__ kc, h16
             }
         }
         // ---- scale (+ causal mask where the tile holds keys past this tile's first query row), new row maxima
-        const bool masked = kt * 64 + 63 > T0 + qt * 64;
+        const bool masked = CAUSAL ? kt * 64 + 63 > T0 + qt * 64 : kt * 64 + 63 >= T0 + T;
+        // the last key a row sees: its own sequence index (causal), else the last token
+        const int lim0 = CAUSAL ? q0 : T0 + T - 1, lim1 = CAUSAL ? q1 : T0 + T - 1;
         float t0 = m0, t1 = m1;
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             const int c0 = kt * 64 + 8 * j + (lane & 3) * 2;
-            sacc[j][0] = (!masked || c0 <= q0) ? sacc[j][0] * 0.125f : -INFINITY;
-            sacc[j][1] = (!masked || c0 + 1 <= q0) ? sacc[j][1] * 0.125f : -INFINITY;
-            sacc[j][2] = (!masked || c0 <= q1) ? sacc[j][2] * 0.125f : -INFINITY;
-            sacc[j][3] = (!masked || c0 + 1 <= q1) ? sacc[j][3] * 0.125f : -INFINITY;
+            sacc[j][0] = (!masked || c0 <= lim0) ? sacc[j][0] * 0.125f : -INFINITY;
+            sacc[j][1] = (!masked || c0 + 1 <= lim0) ? sacc[j][1] * 0.125f : -INFINITY;
+            sacc[j][2] = (!masked || c0 <= lim1) ? sacc[j][2] * 0.125f : -INFINITY;
+            sacc[j][3] = (!masked || c0 + 1 <= lim1) ? sacc[j][3] * 0.125f : -INFINITY;
             t0 = fmaxf(t0, fmaxf(sacc[j][0], sacc[j][1]));
             t1 = fmaxf(t1, fmaxf(sacc[j][2], sacc[j][3]));
         }
@@ -1311,6 +1315,22 @@ static int prefill_attn(const h16* qkv, h16* kc, h16* vc, h16* att, int G, int T
     const dim3 grid((unsigned)((int64_t)ceil_div(T, 64) * G * nh));     // 64-query tiles over 64-key tiles, online softmax
     if (bf) return launch_pdl(prefill_attn_flash_kernel<true>, grid, dim3(128), (size_t)0, st, pdl, qkv, kc, vc, att, G, T, E, nh, Tmax, T0);
     return launch_pdl(prefill_attn_flash_kernel<false>, grid, dim3(128), (size_t)0, st, pdl, qkv, kc, vc, att, G, T, E, nh, Tmax, T0);
+}
+
+// The CLIP engine's pieces of the batched pass (fp16, no KV cache): the tiled attention over G groups of T tokens, causal (text) or
+// not (vision), and the warp-per-row LayerNorm to fp16 at every row count.
+int launch_attn_flash_f16(const h16* qkv, h16* att, int G, int T, int E, bool causal, cudaStream_t st) {
+    const dim3 grid((unsigned)((int64_t)ceil_div(T, 64) * G * (E / 64)));
+    if (causal) return launch_pdl(prefill_attn_flash_kernel<false>, grid, dim3(128), (size_t)0, st, false, qkv, (h16*)nullptr,
+                                  (h16*)nullptr, att, G, T, E, E / 64, 0, 0);
+    return launch_pdl(prefill_attn_flash_kernel<false, false>, grid, dim3(128), (size_t)0, st, false, qkv, (h16*)nullptr, (h16*)nullptr,
+                      att, G, T, E, E / 64, 0, 0);
+}
+int launch_ln_rows_f16(int64_t rows, const float* x, const float* g, const float* be, h16* xn, int E, cudaStream_t st) {
+    int dev = 0, n_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    return ln_rows_warp(rows, x, nullptr, nullptr, g, be, xn, E, 0, n_sm > 0 ? n_sm : 132, st);
 }
 
 // T new tokens of G groups at sequence offset T0 through one stack; cache rows [T0, T0 + T) written when kc != NULL (T0 > 0 needs kc)

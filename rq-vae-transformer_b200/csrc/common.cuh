@@ -150,6 +150,8 @@ __device__ __forceinline__ h16 pack_h16(float a, int bf) {
 
 // GELU in the exact erf form (F.gelu's default, the reference's gelu='v1')
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+// CLIP's QuickGELU, x * sigmoid(1.702 x), with an IEEE division so the exact tier's value does not depend on build flags
+__device__ __forceinline__ float quick_gelu(float x) { return __fdiv_rn(x, 1.0f + expf(-1.702f * x)); }
 
 template <typename T>
 __device__ __forceinline__ float to_f32(T v);

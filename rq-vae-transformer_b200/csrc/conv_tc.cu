@@ -110,8 +110,9 @@ __device__ __forceinline__ void gn_chunk_stats(const float (&wv)[16], bool valid
 
 // Epilogue of one thread: tile row r (one output pixel), output channels [n0, n0 + 16) in v.  Warp q of the four that share a column
 // half holds the tile's pixels [32 q, 32 q + 32) -- the layout the GroupNorm partial statistics are formed over.  OUT16: the rows
-// GEMM's 16-bit output is possible (conv_tc_kernel); the 3x3 kernels never have it.
-template <bool OUT16>
+// GEMM's 16-bit output is possible (conv_tc_kernel); the 3x3 kernels never have it.  QG: that output's activation is QuickGELU
+// (x * sigmoid(1.702 x), the CLIP engine's c_fc) rather than p.gelu's exact GELU.
+template <bool OUT16, bool QG = false>
 __device__ __forceinline__ void ct_epilogue16(const ConvTcParams& p, const float (&v)[16], int n0, int q, int lane, int tx, int ty, int tb,
                                               int b, int y, int x, int64_t pix, bool valid) {
     if (n0 >= p.Cout) return;                                           // (warp-uniform)
@@ -130,7 +131,10 @@ __device__ __forceinline__ void ct_epilogue16(const ConvTcParams& p, const float
             const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
             w[i] = v[i] + bb.x; w[i + 1] = v[i + 1] + bb.y; w[i + 2] = v[i + 2] + bb.z; w[i + 3] = v[i + 3] + bb.w;
         }
-        if (p.gelu) {
+        if (QG) {
+#pragma unroll
+            for (int i = 0; i < 16; i++) w[i] = quick_gelu(w[i]);
+        } else if (p.gelu) {
 #pragma unroll
             for (int i = 0; i < 16; i++) w[i] = gelu_erf(w[i]);
         }
@@ -193,7 +197,7 @@ __device__ __forceinline__ void ct_mma_kblock(float (&acc)[BN / 2], uint32_t a, 
                                 (PASSES == 3 || !first || j > 0) ? 1u : 0u);
 }
 
-template <int BN, int STAGES, int PASSES>
+template <int BN, int STAGES, int PASSES, bool QG = false>
 __global__ void __launch_bounds__(CT_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, ConvTcParams p) {
@@ -281,20 +285,20 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int64_t pix = ((int64_t)b * p.H + y) * p.W + x;
         const bool valid = (x < p.W) && (y < p.H) && (b < p.B) && (p.m_rows == 0 || pix < p.m_rows);
         tc::drain_acc<BN, CW, 0>(acc, stage, wg, t, [&p, t, nt, tx, ty, tb, b, y, x, pix, valid](const float (&v)[16], int, int c) {
-            ct_epilogue16<true>(p, v, nt * BN + c, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
+            ct_epilogue16<true, QG>(p, v, nt * BN + c, (t >> 5) & 3, t & 31, tx, ty, tb, b, y, x, pix, valid);
         });
     }
 }
 
-template <int BN, int STAGES, int PASSES>
+template <int BN, int STAGES, int PASSES, bool QG = false>
 static int launch_conv_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
                             const ConvTcParams& p, int n_sm, cudaStream_t st) {
     constexpr size_t smem = (size_t)STAGES * (PASSES == 3 ? 2 : 1) * (CT_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 256;
     static_assert(smem <= 227 * 1024, "conv_tc: shared memory budget");
-    RQB_ENSURE_SMEM(smem, conv_tc_kernel<BN, STAGES, PASSES>);
+    RQB_ENSURE_SMEM(smem, conv_tc_kernel<BN, STAGES, PASSES, QG>);
     const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
     const int grid = total < n_sm ? total : n_sm;
-    conv_tc_kernel<BN, STAGES, PASSES><<<grid, CT_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
+    conv_tc_kernel<BN, STAGES, PASSES, QG><<<grid, CT_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
     return check_launch("conv_tc");
 }
 
@@ -811,6 +815,7 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
 // -- a 1x1 "conv" over ceil(M/128) images of 16x8 pixels.  The batched prefill / teacher-forced forward passes of the AR tier
 // (csrc/ar_fast.cu) use it for M > 256: persistent CTAs, 128 x BN tiles, operand loads of the next tile overlapped with
 // this tile's epilogue -- what gemm_tc_kernel (a weight streamer built for M <= 256) does not have.
+// gelu: 0 none, 1 exact GELU, 2 QuickGELU (16-bit output only).
 // X [M_alloc, K] 16-bit with M_alloc >= ceil(M/128)*128 rows readable; exactly one of out_f32 / out_16 non-null;
 // residual (f32, may alias out_f32) only with out_f32.  N_out % 128 == 0, K % 64 == 0.
 int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
@@ -829,6 +834,10 @@ int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, con
     RQB_TRY(make_tmap_4d_nhwc(&tmA, X16, (uint64_t)K, 16, 8, (uint64_t)p.B, 64, 16, 8, 1, 1));
     RQB_TRY(make_tmap_2d(&tmB, W16, 1, (uint64_t)K, (uint64_t)N_out, (uint64_t)K * 2, 64, (uint32_t)BN));
     const int n_sm = sm_count();
+    if (gelu == 2) {
+        if (BN == 256) return launch_conv_tc_t<256, 4, 1, true>(tmA, tmB, tmA, tmB, p, n_sm, st);
+        return launch_conv_tc_t<128, 6, 1, true>(tmA, tmB, tmA, tmB, p, n_sm, st);
+    }
     if (BN == 256) return launch_conv_tc_t<256, 4, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
     return launch_conv_tc_t<128, 6, 1>(tmA, tmB, tmA, tmB, p, n_sm, st);
 }

@@ -13,7 +13,7 @@ int fail(int code, const std::string& msg) {
 
 extern "C" {
 const char* rqb200_last_error(void) { return rqb::g_err.c_str(); }
-int rqb200_version(void) { return 117; }
+int rqb200_version(void) { return 118; }
 int rqb200_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }

@@ -90,7 +90,8 @@ __device__ __forceinline__ void gt_epilogue_cols(const GemmTcParams& p, const fl
             if (MODE == GT_F32 && res != nullptr) x += res[(rdiv ? (int64_t)((m0 + col) / rdiv) : (int64_t)(m0 + col)) * res_ld];
             if (MODE == GT_PARTIAL || MODE == GT_F32) out_f[(int64_t)col * ld] = x;
             else if (MODE == GT_H16) out_h[(int64_t)col * ld] = pack_h16(x, p.fmt);
-            else out_h[(int64_t)col * ld] = pack_h16(gelu_erf(x), p.fmt);
+            else if (MODE == GT_H16_GELU) out_h[(int64_t)col * ld] = pack_h16(gelu_erf(x), p.fmt);
+            else out_h[(int64_t)col * ld] = pack_h16(quick_gelu(x), p.fmt);
         }
     }
 }
@@ -248,7 +249,8 @@ struct GtFormat<GT_E4M3> {
 };
 
 // ---------------------------------------------------------------- the streamer
-template <int BN, int WF>
+// QG: the 16-bit activation epilogue applies QuickGELU (GT_H16_QGELU) instead of the exact GELU; every other mode is the same code
+template <int BN, int WF, bool QG = false>
 __global__ void __launch_bounds__(GT_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ typename GtFormat<WF>::Arg W, const __grid_constant__ CUtensorMap tmX, GemmTcParams p) {
     using F = GtFormat<WF>;
@@ -365,20 +367,20 @@ gemm_tc_kernel(const __grid_constant__ typename GtFormat<WF>::Arg W, const __gri
             case GT_PARTIAL: gt_epilogue<GT_PARTIAL>(p, v, n, split, m0, nb, col0); break;
             case GT_F32: gt_epilogue<GT_F32>(p, v, n, split, m0, nb, col0); break;
             case GT_H16: gt_epilogue<GT_H16>(p, v, n, split, m0, nb, col0); break;
-            default: gt_epilogue<GT_H16_GELU>(p, v, n, split, m0, nb, col0); break;
+            default: gt_epilogue<QG ? GT_H16_QGELU : GT_H16_GELU>(p, v, n, split, m0, nb, col0); break;
         }
     });
     if (tr && t == 0) p.trace[3] = tc::gtimer();
 }
 
-template <int BN, int WF>
+template <int BN, int WF, bool QG = false>
 static int launch_gemm_tc_t(const typename GtFormat<WF>::Arg& w, const CUtensorMap& tmX, const GemmTcParams& p, bool pdl,
                             cudaStream_t st) {
     using F = GtFormat<WF>;
     constexpr size_t smem = (size_t)F::stages(BN) * (F::A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 512;
     static_assert(smem <= 227 * 1024, "gemm_tc: shared memory budget");
-    RQB_ENSURE_SMEM(smem, gemm_tc_kernel<BN, WF>);
-    return launch_pdl(gemm_tc_kernel<BN, WF>, dim3((unsigned)(ceil_div(p.N_out, 128) * p.splits), (unsigned)ceil_div(p.B, BN)),
+    RQB_ENSURE_SMEM(smem, gemm_tc_kernel<BN, WF, QG>);
+    return launch_pdl(gemm_tc_kernel<BN, WF, QG>, dim3((unsigned)(ceil_div(p.N_out, 128) * p.splits), (unsigned)ceil_div(p.B, BN)),
                       dim3(GT_THREADS), smem, st, pdl, w, tmX, p);
 }
 
@@ -391,6 +393,17 @@ static int launch_gemm_tc_bn(const typename GtFormat<WF>::Arg& w, const CUtensor
         case 64: return launch_gemm_tc_t<64, WF>(w, tmX, p, pdl, st);
         case 128: return launch_gemm_tc_t<128, WF>(w, tmX, p, pdl, st);
         default: return launch_gemm_tc_t<(WF == GT_E4M3 ? 128 : 256), WF>(w, tmX, p, pdl, st);      // (256 rows: 16-bit weights only)
+    }
+}
+
+// GT_H16_QGELU (the CLIP engine's c_fc): 16-bit weights only
+static int launch_gemm_tc_qgelu(const CUtensorMap& w, const CUtensorMap& tmX, const GemmTcParams& p, int bn, bool pdl, cudaStream_t st) {
+    switch (bn) {
+        case 16: return launch_gemm_tc_t<16, GT_W16, true>(w, tmX, p, pdl, st);
+        case 32: return launch_gemm_tc_t<32, GT_W16, true>(w, tmX, p, pdl, st);
+        case 64: return launch_gemm_tc_t<64, GT_W16, true>(w, tmX, p, pdl, st);
+        case 128: return launch_gemm_tc_t<128, GT_W16, true>(w, tmX, p, pdl, st);
+        default: return launch_gemm_tc_t<256, GT_W16, true>(w, tmX, p, pdl, st);
     }
 }
 
@@ -422,6 +435,10 @@ int launch_gemm_tc(const StreamedWeight& w, const CUtensorMap& tmX, GemmTcParams
     if (p.mode != GT_PARTIAL && p.splits != 1) return fail(RQB200_EINVAL, "gemm_tc: direct epilogues need splits == 1");
     const int bn = gemm_tc_chunk_rows(w, p.B);
     if (ceil_div(p.B, bn) > 65535) return fail(RQB200_EINVAL, "gemm_tc: more than 65535 row chunks");
+    if (p.mode == GT_H16_QGELU) {
+        if (w.e4m3()) return fail(RQB200_EINVAL, "gemm_tc: the QuickGELU epilogue takes 16-bit weights only");
+        return launch_gemm_tc_qgelu(w.tm, tmX, p, bn, pdl, st);
+    }
     if (w.e4m3()) return launch_gemm_tc_bn<GT_E4M3>(GtE4m3Tiles{w.q8, w.s8}, tmX, p, bn, pdl, st);
     return launch_gemm_tc_bn<GT_W16>(w.tm, tmX, p, bn, pdl, st);
 }
@@ -440,7 +457,8 @@ static int dbg_gemm_tc(const rqb::StreamedWeight& w, const void* X16, const floa
     GemmTcParams p = {};
     p.B = B; p.splits = splits; p.fmt = fmt;
     p.bias = bias; p.bias_scale = 1.f; p.residual = residual; p.ld_res = w.N_out; p.out = out; p.ld_out = w.N_out; p.partial = partial;
-    p.mode = (splits > 1 || partial != nullptr) ? GT_PARTIAL : (out_is_16 ? (gelu ? GT_H16_GELU : GT_H16) : GT_F32);
+    p.mode = (splits > 1 || partial != nullptr) ? GT_PARTIAL
+                                                 : (out_is_16 ? (gelu == 2 ? GT_H16_QGELU : gelu ? GT_H16_GELU : GT_H16) : GT_F32);
     if (p.mode == GT_PARTIAL && partial == nullptr) return fail(RQB200_EINVAL, "dbg_gemm_tc: splits > 1 needs a partial buffer");
     return launch_gemm_tc(w, tx, p, false, (cudaStream_t)stream);
 }

@@ -126,7 +126,8 @@ int make_tmap_4d_nhwc(CUtensorMap* out, const void* base, uint64_t C, uint64_t W
                       uint32_t box_w, uint32_t box_h, uint32_t box_b, uint32_t stride = 1);
 
 // gemm_tc.cu -- wgmma weight-streaming GEMM (fast tier)
-enum GemmTcMode { GT_F32 = 0, GT_H16 = 1, GT_H16_GELU = 2, GT_PARTIAL = 3 };
+// GT_H16_QGELU: QuickGELU x * sigmoid(1.702 x) (CLIP's MLP) instead of the exact GELU; 16-bit weights, splits == 1
+enum GemmTcMode { GT_F32 = 0, GT_H16 = 1, GT_H16_GELU = 2, GT_PARTIAL = 3, GT_H16_QGELU = 4 };
 struct GemmTcParams {
     int N_out, K, B, splits, mode;   // B = activation rows (batch rows of the cached step, or B*T tokens of a prefill / forward pass)
     int fmt;                      // 16-bit operand / output format: 0 = fp16 (the reference's autocast class), 1 = bf16
@@ -200,6 +201,11 @@ inline int plan_prev(const uint8_t* sampled, int p) {
 // canvas: the sampler writes the canvas position of stt->idx through stt->cv (the canvas graphs), else position stt->idx of [B, HW, D]
 int launch_sample_dyn(const float* logits, const StepState* stt, int d, int B, int V, int HW, int D, cudaStream_t st, bool pdl,
                       bool canvas = false);
+
+// ar_fast.cu, for the CLIP engine: prefill_attn_flash_kernel over G groups of T tokens (qkv token-major [T*G, 3E] fp16, bias added;
+// head dim 64; causal or not) -> att [T*G, E] fp16; LayerNorm (eps 1e-5) of fp32 rows x [rows, E] -> xn fp16 (E % 4 == 0)
+int launch_attn_flash_f16(const h16* qkv, h16* att, int G, int T, int E, bool causal, cudaStream_t st);
+int launch_ln_rows_f16(int64_t rows, const float* x, const float* g, const float* be, h16* xn, int E, cudaStream_t st);
 
 struct ArFast;
 ArFast* ar_fast_create(const rqb200_ar_config& cfg, const rqb200_ar_weights& w, const rqb200_block_weights* body,

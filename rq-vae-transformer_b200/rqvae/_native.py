@@ -162,7 +162,10 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_dbg_vae_attn_tc", "rqb200_inception_create", "rqb200_inception_destroy", "rqb200_inception_set_tensor",
            "rqb200_inception_params_bytes", "rqb200_inception_finalize", "rqb200_inception_workspace_bytes", "rqb200_inception_forward",
            "rqb200_inception_last_launches", "rqb200_dbg_inception_conv", "rqb200_dbg_inception_conv_tc", "rqb200_dbg_inception_input", "rqb200_dbg_inception_pool",
-           "rqb200_dbg_inception_gap"]
+           "rqb200_dbg_inception_gap", "rqb200_clip_create", "rqb200_clip_destroy", "rqb200_clip_set_tensor", "rqb200_clip_params_bytes",
+           "rqb200_clip_finalize", "rqb200_clip_workspace_bytes", "rqb200_clip_text_workspace_bytes", "rqb200_clip_encode_image",
+           "rqb200_clip_encode_text", "rqb200_clip_cosine", "rqb200_clip_last_launches", "rqb200_clip_resize_plan",
+           "rqb200_dbg_clip_preprocess", "rqb200_dbg_clip_attn", "rqb200_dbg_clip_attn_flash"]
 
 
 def check(rc, what=""):
