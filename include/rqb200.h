@@ -376,6 +376,38 @@ int64_t rqb200_clip_last_launches(const rqb200_clip* h);
  * output pixel (0: that pass is skipped), vertical taps} */
 int rqb200_clip_resize_plan(int H, int W, int R, int32_t* out6);
 
+/* ------------------------------------------------------------------------------------------------ LPIPS
+ * LPIPS (rqvae/losses/vqgan/lpips.py: the VGG16 perceptual distance) forward as a static layer plan (csrc/lpips_engine.cu).  Tensors
+ * are registered under the reference's LPIPS state_dict keys as they are (fp32, device): "scaling_layer.shift" / "scaling_layer.scale"
+ * [3], "net.slice<s>.<i>.weight" OIHW / ".bias" for the 13 convs of VGG16's features[:30] (net.slice1.0 .. net.slice5.28), and
+ * "lin<k>.model.1.weight" [1, C_k, 1, 1] (use_dropout=True) or "lin<k>.model.0.weight" (use_dropout=False), C = 64, 128, 256, 512, 512.
+ * rqb200_lpips_finalize names the first missing or mis-sized key, then packs OHWI conv weights (fast tier: with their fp16 hi / lo
+ * halves), the biases, the lin weights and the scaling buffers on `stream` into the caller's buffer of rqb200_lpips_params_bytes(h)
+ * bytes, which must stay alive and unchanged while the engine is used.  Two tiers: RQB200_MODE_EXACT runs every conv on fp32 FFMA;
+ * RQB200_MODE_FAST runs every conv but conv1_1 (Cin = 3, fp32 FFMA on both tiers) on the wgmma implicit GEMM with split-fp16 operands
+ * (three fp16 products per k step, fp32 accumulate).  The head (normalisation, squared difference, lin) runs in fp32 on both tiers and
+ * the spatial average in fp64.  This section is additive and leaves rqb200_version() at 118, the value existing callers pin; a
+ * caller finds it by looking up the rqb200_lpips_create symbol. */
+typedef struct rqb200_lpips rqb200_lpips;
+typedef struct {
+    int32_t mode;       /* RQB200_MODE_EXACT or RQB200_MODE_FAST */
+} rqb200_lpips_config;
+
+rqb200_lpips* rqb200_lpips_create(const rqb200_lpips_config* cfg);
+void rqb200_lpips_destroy(rqb200_lpips* h);
+int rqb200_lpips_set_tensor(rqb200_lpips* h, const char* key, const void* ptr, int dtype, int64_t numel);
+size_t rqb200_lpips_params_bytes(const rqb200_lpips* h);
+int rqb200_lpips_finalize(rqb200_lpips* h, void* params, size_t params_bytes, void* stream);
+/* the workspace of rqb200_lpips_forward on B pairs of H x W; 0 unless B >= 1 and H, W >= 16.  A batch whose activations exceed 2 GiB
+ * runs in chunks of as many pairs as fit, so the workspace stops growing with B there. */
+size_t rqb200_lpips_workspace_bytes(rqb200_lpips* h, int B, int H, int W);
+/* x0 (input), x1 (target) NCHW [B, 3, H, W] f32 in [-1, 1], H, W >= 16.  layer_out [B, 5] (nullable): each tap's spatial average of
+ * the lin output (relu1_2 .. relu5_3); val_out [B]: their sum, the reference's LPIPS(x0, x1, reduction='none').  A pair's values do not
+ * depend on the other pairs of the batch, and swapping x0 and x1 gives the same bits. */
+int rqb200_lpips_forward(rqb200_lpips* h, const float* x0, const float* x1, int B, int H, int W, float* layer_out, float* val_out,
+                         void* workspace, size_t workspace_bytes, void* stream);
+int64_t rqb200_lpips_last_launches(const rqb200_lpips* h);
+
 /* ------------------------------------------------------------------------------------------------ diagnostics
  * Single-kernel entry points used by tests/ and bench.py's roofline leg; not part of the reference-facing surface.
  * rqb200_dbg_gemm_tc: one launch of the wgmma weight-streaming GEMM (csrc/gemm_tc.cu):
@@ -533,6 +565,21 @@ int rqb200_dbg_inception_pool(int mode, const float* X, float* Y, int B, int H, 
                               void* stream);
 /* rqb200_dbg_inception_gap: Y [B, C] = the mean of X [B, HW, C] over HW. */
 int rqb200_dbg_inception_gap(const float* X, float* Y, int B, int HW, int C, void* stream);
+
+/* The LPIPS engine's kernels (csrc/lpips_engine.cu), one launch each through the launcher the engine calls.  Maps are NHWC f32.
+ * rqb200_dbg_lpips_input: x0, x1 NCHW [n, 3, H, W] -> y NHWC [2n, H, W, 3] (images [0, n) from x0, [n, 2n) from x1), each
+ *   (x - shift[c]) / scale[c] (shift, scale [3] f32 on the device). */
+int rqb200_dbg_lpips_input(const float* x0, const float* x1, const float* shift, const float* scale, float* y, int n, int H, int W,
+                           void* stream);
+/* rqb200_dbg_lpips_pool: 2x2 stride-2 max pool of X [N, H, W, C] (C % 4 == 0) into Y [N, H/2, W/2, C] f32 and / or its fp16 halves
+ *   Yhi = fp16(v), Ylo = fp16(v - Yhi) (nullable, both or neither). */
+int rqb200_dbg_lpips_pool(const float* X, float* Y, void* Yhi, void* Ylo, int N, int H, int W, int C, void* stream);
+/* rqb200_dbg_lpips_head: F [2n, hw, C] (image b and image b + n form pair b), w [C] -> d [n, hw] = sum_c w[c] (a_c / (|a| + 1e-10) -
+ *   t_c / (|t| + 1e-10))^2 per pixel. */
+int rqb200_dbg_lpips_head(const float* F, const float* w, float* d, int n, int hw, int C, void* stream);
+/* rqb200_dbg_lpips_mean: tap k's spatial average of d [n, hw] in fp64: tapmean [n, 5] (f64) entry k, layer_out [n, 5] (nullable) its
+ *   f32 value, and at k == 4 val [n] = the sum of tapmean's five entries. */
+int rqb200_dbg_lpips_mean(const float* d, int n, int hw, int k, double* tapmean, float* layer_out, float* val, void* stream);
 
 #ifdef __cplusplus
 }

@@ -165,7 +165,10 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_dbg_inception_gap", "rqb200_clip_create", "rqb200_clip_destroy", "rqb200_clip_set_tensor", "rqb200_clip_params_bytes",
            "rqb200_clip_finalize", "rqb200_clip_workspace_bytes", "rqb200_clip_text_workspace_bytes", "rqb200_clip_encode_image",
            "rqb200_clip_encode_text", "rqb200_clip_cosine", "rqb200_clip_last_launches", "rqb200_clip_resize_plan",
-           "rqb200_dbg_clip_preprocess", "rqb200_dbg_clip_attn", "rqb200_dbg_clip_attn_flash"]
+           "rqb200_dbg_clip_preprocess", "rqb200_dbg_clip_attn", "rqb200_dbg_clip_attn_flash", "rqb200_lpips_create",
+           "rqb200_lpips_destroy", "rqb200_lpips_set_tensor", "rqb200_lpips_params_bytes", "rqb200_lpips_finalize",
+           "rqb200_lpips_workspace_bytes", "rqb200_lpips_forward", "rqb200_lpips_last_launches", "rqb200_dbg_lpips_input",
+           "rqb200_dbg_lpips_pool", "rqb200_dbg_lpips_head", "rqb200_dbg_lpips_mean"]
 
 
 def check(rc, what=""):
