@@ -12,7 +12,6 @@
 #include <cmath>
 #include <cstring>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "kernels.h"
@@ -271,14 +270,7 @@ __global__ void __launch_bounds__(128) clip_cosine_kernel(const float* __restric
     if (lane == 0) out[r] = d;
 }
 
-static unsigned clip_grid(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(ceil_div(n, 256), 1), 8192); }
-
 // ------------------------------------------------------------------------------------------------ the engine
-struct ClipTensor {
-    const void* ptr;
-    int dtype;
-    int64_t numel;
-};
 // one linear layer: fp32 weight [N, K] and bias (the caller's tensors) and, fast tier, its fp16 copy behind a streamer tensor map
 struct ClipLinear {
     const float* w = nullptr;
@@ -304,7 +296,7 @@ struct ClipTower {
 struct rqb200_clip {
     rqb200_clip_config cfg;
     bool fast = false;
-    std::unordered_map<std::string, rqb::ClipTensor> t;
+    rqb::TensorTable t;
     rqb::ClipTower vis, txt;
     int Kp = 0;                    // conv1's K = 3 P^2, padded to a multiple of 64
     rqb::ClipLinear conv1;         // w = [width, Kp] fp32 in params (zero-padded), b = zeros
@@ -358,7 +350,7 @@ __global__ void clip_pack_kernel(const float* __restrict__ src, int rows, int co
     }
 }
 static int clip_pack(const float* src, int rows, int cols, int ld_dst, bool transpose, float* d32, __half* d16, cudaStream_t st) {
-    clip_pack_kernel<<<clip_grid((int64_t)rows * cols), 256, 0, st>>>(src, rows, cols, ld_dst, transpose ? 1 : 0, d32, d16);
+    clip_pack_kernel<<<grid_1d((int64_t)rows * cols), 256, 0, st>>>(src, rows, cols, ld_dst, transpose ? 1 : 0, d32, d16);
     return check_launch("clip_pack");
 }
 
@@ -403,7 +395,7 @@ static int clip_linear(const rqb200_clip* h, const ClipLinear& L, int64_t M, con
     if (!h->fast) {
         RQB_TRY(launch_linear(x32, L.K, L.w, RQB200_F32, L.b, res, out32, L.N, (int)M, L.N, L.K, 0, st));
         if (act == 2) {
-            clip_quick_gelu_kernel<<<clip_grid(M * L.N), 256, 0, st>>>(out32, M * L.N);
+            clip_quick_gelu_kernel<<<grid_1d(M * L.N), 256, 0, st>>>(out32, M * L.N);
             RQB_TRY(check_launch("clip_quick_gelu"));
         }
         return 0;
@@ -469,9 +461,9 @@ static int clip_preprocess(const ClipPrep& pp, const float* x, int B, int H, int
     ClipAxis ah{q, q + pp.hlo.size(), q + pp.hlo.size() + pp.hn.size(), pp.ksh, pp.left};
     q += pp.hlo.size() + pp.hn.size() + pp.hk.size();
     ClipAxis av{q, q + pp.vlo.size(), q + pp.vlo.size() + pp.vn.size(), pp.ksv, pp.top};
-    clip_resize_h_kernel<<<clip_grid((int64_t)B * 3 * H * R), 256, 0, st>>>(x, tmp, B, H, W, R, ah);
+    clip_resize_h_kernel<<<grid_1d((int64_t)B * 3 * H * R), 256, 0, st>>>(x, tmp, B, H, W, R, ah);
     RQB_TRY(check_launch("clip_resize_h"));
-    clip_resize_v_kernel<<<clip_grid((int64_t)B * 3 * R * R), 256, 0, st>>>(tmp, B, H, R, av, u8, nchw, rows32, rows16, P, ld);
+    clip_resize_v_kernel<<<grid_1d((int64_t)B * 3 * R * R), 256, 0, st>>>(tmp, B, H, R, av, u8, nchw, rows32, rows16, P, ld);
     return check_launch("clip_resize_v");
 }
 
@@ -521,7 +513,7 @@ void rqb200_clip_destroy(rqb200_clip* h) { delete h; }
 
 int rqb200_clip_set_tensor(rqb200_clip* h, const char* key, const void* ptr, int dtype, int64_t numel) {
     if (!h || !key || !ptr) return rqb::fail(RQB200_EINVAL, "clip_set_tensor: null argument");
-    h->t[key] = rqb::ClipTensor{ptr, dtype, numel};
+    h->t.set(key, ptr, dtype, numel);
     h->finalized = false;
     return 0;
 }
@@ -535,14 +527,7 @@ int rqb200_clip_finalize(rqb200_clip* h, void* params, size_t params_bytes, void
     if (!h) return fail(RQB200_EINVAL, "clip_finalize: null handle");
     h->finalized = false;
     const rqb200_clip_config& c = h->cfg;
-    auto get = [&](const std::string& k, int64_t numel, const float** out) -> int {
-        auto it = h->t.find(k);
-        if (it == h->t.end()) return fail(RQB200_ESTATE, "clip_finalize: tensor " + k + " (missing)");
-        if (it->second.numel != numel) return fail(RQB200_ESTATE, "clip_finalize: tensor " + k + " (wrong size)");
-        if (it->second.dtype != RQB200_F32) return fail(RQB200_EINVAL, "clip_finalize: tensor " + k + " must be fp32");
-        *out = (const float*)it->second.ptr;
-        return 0;
-    };
+    auto get = [h](const std::string& k, int64_t numel, const float** out) { return h->t.get_f32("clip_finalize", k, numel, out); };
     const int vw = c.vision_width, tw = c.text_width, P = c.vision_patch, D = c.embed_dim;
     const float *conv1 = nullptr, *cls = nullptr, *vpos = nullptr, *lnpre_w = nullptr, *lnpre_b = nullptr, *vproj = nullptr;
     const float *tok = nullptr, *tpos = nullptr, *tproj = nullptr;
@@ -660,15 +645,15 @@ int rqb200_clip_encode_image(rqb200_clip* h, const float* x, int B, int H, int W
     else if (h->Kp != 3 * P * P) RQB_CUDA(cudaMemsetAsync(b.rows32, 0, (size_t)B * np * h->Kp * 4, st));
     if (prep) RQB_TRY(clip_preprocess(pp, x, B, H, W, R, b.tmp, b.tabs, nullptr, nullptr, b.rows32, (__half*)b.rows16, P, h->Kp, st));
     else {
-        clip_patch_rows_kernel<<<clip_grid((int64_t)B * 3 * R * R), 256, 0, st>>>(x, B, R, P, h->Kp, b.rows32, (__half*)b.rows16);
+        clip_patch_rows_kernel<<<grid_1d((int64_t)B * 3 * R * R), 256, 0, st>>>(x, B, R, P, h->Kp, b.rows32, (__half*)b.rows16);
         RQB_TRY(check_launch("clip_patch_rows"));
     }
     // conv1 -> token rows 1.. (rows t * B + g), then class token + positional embedding, ln_pre (fp32, in place)
     RQB_TRY(clip_linear(h, h->conv1, (int64_t)B * np, b.rows32, b.rows16, b.X + (int64_t)B * E, nullptr, nullptr, 0, st));
-    const float *cls = (const float*)h->t.at("visual.class_embedding").ptr, *pos = (const float*)h->t.at("visual.positional_embedding").ptr;
-    clip_vis_embed_kernel<<<clip_grid((int64_t)B * T * E), 256, 0, st>>>(b.X, cls, pos, B, T, E);
+    const float *cls = (const float*)h->t.find("visual.class_embedding")->ptr, *pos = (const float*)h->t.find("visual.positional_embedding")->ptr;
+    clip_vis_embed_kernel<<<grid_1d((int64_t)B * T * E), 256, 0, st>>>(b.X, cls, pos, B, T, E);
     RQB_TRY(check_launch("clip_vis_embed"));
-    RQB_TRY(launch_layernorm(b.X, E, (const float*)h->t.at("visual.ln_pre.weight").ptr, (const float*)h->t.at("visual.ln_pre.bias").ptr, b.X,
+    RQB_TRY(launch_layernorm(b.X, E, (const float*)h->t.find("visual.ln_pre.weight")->ptr, (const float*)h->t.find("visual.ln_pre.bias")->ptr, b.X,
                              E, B * T, E, st));
     RQB_TRY(clip_blocks(h, h->vis, b, B, false, st));
     // token 0 of every image: rows 0 .. B - 1
@@ -692,8 +677,8 @@ int rqb200_clip_encode_text(rqb200_clip* h, const int64_t* tokens, int N, float*
     if (clip_layout(h, h->txt, N, 0, 0, 0, 0, ws, &b) > ws_bytes)
         return fail(RQB200_EWORKSPACE, "clip_encode_text: workspace smaller than rqb200_clip_text_workspace_bytes");
     g_launches = 0;
-    clip_txt_embed_kernel<<<clip_grid((int64_t)N * T * E), 256, 0, st>>>(b.X, tokens, (const float*)h->t.at("token_embedding.weight").ptr,
-                                                                        (const float*)h->t.at("positional_embedding").ptr, N, T, E, c.vocab_size);
+    clip_txt_embed_kernel<<<grid_1d((int64_t)N * T * E), 256, 0, st>>>(b.X, tokens, (const float*)h->t.find("token_embedding.weight")->ptr,
+                                                                        (const float*)h->t.find("positional_embedding")->ptr, N, T, E, c.vocab_size);
     RQB_TRY(check_launch("clip_txt_embed"));
     RQB_TRY(clip_blocks(h, h->txt, b, N, true, st));
     float* gathered = h->fast ? (float*)b.XN : b.XN32;            // [N, E] fp32 scratch (XN holds at least 2 N T E bytes)

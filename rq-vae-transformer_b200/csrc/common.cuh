@@ -5,6 +5,7 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <algorithm>
 #include <atomic>
 #include <string>
 
@@ -70,6 +71,15 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaS
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
+
+// the grid of a 256-thread grid-stride launch over n elements: one CTA per 256 elements, at least 1 and at most 8192
+inline unsigned grid_1d(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(ceil_div(n, 256), 1), 8192); }
+// the items (images, pairs) a layer-plan call runs at once: as many as fit in 2 GiB of workspace, at least 1 and at most B; a larger
+// batch runs in chunks of that many inside one call
+inline int chunk_items(int B, size_t bytes_per_item) {
+    const int64_t fit = std::max<int64_t>(1, (int64_t)((size_t(2) << 30) / bytes_per_item));
+    return (int)std::min<int64_t>(B, fit);
+}
 
 // bump allocator over the caller's workspace
 struct Arena {
@@ -146,6 +156,17 @@ __device__ __forceinline__ h16 pack_h16(float a, int bf) {
     }
     __half h = __float2half_rn(a);
     return *reinterpret_cast<h16*>(&h);
+}
+
+// The split-fp16 form of the fast tier's conv operands and weights: hi = fp16(v), lo = fp16(v - hi)
+__device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
+    hi = __float2half_rn(v);
+    lo = __float2half_rn(v - __half2float(hi));
+}
+__device__ __forceinline__ void split_f16x2(float a, float b, __half2& hi, __half2& lo) {
+    hi = __floats2half2_rn(a, b);
+    const float2 f = __half22float2(hi);
+    lo = __floats2half2_rn(a - f.x, b - f.y);
 }
 
 // GELU in the exact erf form (F.gelu's default, the reference's gelu='v1')

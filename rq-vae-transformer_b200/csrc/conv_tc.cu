@@ -962,9 +962,8 @@ inc_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
                 uint32_t hi[8], lo[8];
 #pragma unroll
                 for (int i = 0; i < 8; i++) {
-                    const __half2 h = __floats2half2_rn(w[2 * i], w[2 * i + 1]);
-                    const float2 hf = __half22float2(h);
-                    const __half2 l = __floats2half2_rn(w[2 * i] - hf.x, w[2 * i + 1] - hf.y);
+                    __half2 h, l;
+                    split_f16x2(w[2 * i], w[2 * i + 1], h, l);
                     hi[i] = *reinterpret_cast<const uint32_t*>(&h);
                     lo[i] = *reinterpret_cast<const uint32_t*>(&l);
                 }
@@ -1100,11 +1099,7 @@ __global__ void __launch_bounds__(256) gn_apply_f16_kernel(const float* __restri
         }
         __half2 h[4], l[4];
 #pragma unroll
-        for (int k = 0; k < 4; k++) {
-            h[k] = __floats2half2_rn(v[2 * k], v[2 * k + 1]);
-            const float2 f = __half22float2(h[k]);
-            l[k] = __floats2half2_rn(v[2 * k] - f.x, v[2 * k + 1] - f.y);
-        }
+        for (int k = 0; k < 4; k++) split_f16x2(v[2 * k], v[2 * k + 1], h[k], l[k]);
         *reinterpret_cast<uint4*>(Yb + (size_t)i * 8) = *reinterpret_cast<uint4*>(h);
         if (Lb) *reinterpret_cast<uint4*>(Lb + (size_t)i * 8) = *reinterpret_cast<uint4*>(l);
     }

@@ -9,8 +9,6 @@
 // (FIDInceptionC), blocks.3.{0,1,2} = Mixed_7a (InceptionD), Mixed_7b (FIDInceptionE_1), Mixed_7c (FIDInceptionE_2), and fc.
 // Differences in execution, not arithmetic: activations are NHWC fp32; every branch writes straight into its channel slice of
 // the block's output (torch.cat is never a copy); the bilinear resize, 2x - 1 and NCHW -> NHWC are one pass.
-#include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "kernels.h"
@@ -20,8 +18,6 @@ namespace rqb {
 constexpr int INC_RES = 299;                       // F.interpolate(size=(299, 299)) of resize_input
 constexpr int INC_MIN_EXTENT = 75;                 // smallest H, W every layer accepts (Mixed_7a's stride-2 3x3 needs 3 pixels)
 constexpr double INC_BN_EPS = 1e-3;                // BasicConv2d's BatchNorm2d(eps=0.001)
-constexpr size_t INC_CHUNK_BYTES = size_t(2) << 30;   // a call's workspace covers at most this many bytes of images; larger
-                                                      // batches run in chunks of as many images as fit
 constexpr int INC_FEAT = 2048, INC_CLASSES = 1008;
 
 // ------------------------------------------------------------------------------------------------ kernels
@@ -79,11 +75,7 @@ __global__ void inc_pool_kernel(const float* __restrict__ X, float* __restrict__
         }
         const float v = mode == 0 ? acc : acc / (float)cnt;
         Y[m * ldy + yoff + c] = v;
-        if (Yhi) {                                     // fast tier: the next conv's fp16 operand halves too
-            const __half h = __float2half_rn(v);
-            Yhi[m * ldy + yoff + c] = h;
-            Ylo[m * ldy + yoff + c] = __float2half_rn(v - __half2float(h));
-        }
+        if (Yhi) split_f16(v, Yhi[m * ldy + yoff + c], Ylo[m * ldy + yoff + c]);   // fast tier: the next conv's operand halves too
     }
 }
 
@@ -108,41 +100,15 @@ __global__ void inc_to_nchw_kernel(const float* __restrict__ X, float* __restric
     }
 }
 
-// BatchNorm folded into the conv, in fp64: s = gamma / sqrt(var + eps); w' (OHWI) = w (OIHW) s; b' = beta - mean s
-__global__ void inc_fold_bn_kernel(const float* __restrict__ w, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                   const float* __restrict__ mean, const float* __restrict__ var, float* __restrict__ wo,
-                                   float* __restrict__ bo, __half* __restrict__ whi, __half* __restrict__ wlo, int Cout, int Cin,
-                                   int KH, int KW) {
-    const int64_t n = (int64_t)Cout * KH * KW * Cin;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const int ci = (int)(i % Cin);
-        const int kx = (int)((i / Cin) % KW), ky = (int)((i / Cin / KW) % KH), o = (int)(i / Cin / KW / KH);
-        const double s = (double)gamma[o] / sqrt((double)var[o] + INC_BN_EPS);
-        const float f = (float)((double)w[(((int64_t)o * Cin + ci) * KH + ky) * KW + kx] * s);
-        wo[i] = f;
-        if (whi) {                                     // the fast tier's split-fp16 weight: hi = fp16(f), lo = fp16(f - hi)
-            const __half h = __float2half_rn(f);
-            whi[i] = h;
-            wlo[i] = __float2half_rn(f - __half2float(h));
-        }
-        if (i < Cout) {
-            const double so = (double)gamma[i] / sqrt((double)var[i] + INC_BN_EPS);
-            bo[i] = (float)((double)beta[i] - (double)mean[i] * so);
-        }
-    }
-}
-
-static unsigned grid_of(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(ceil_div(n, 256), 1), 8192); }
-
 int launch_inc_input(const float* x, float* y, int B, int H, int W, int resize, int normalize, cudaStream_t st) {
     const int Ho = resize ? INC_RES : H, Wo = resize ? INC_RES : W;
-    inc_input_kernel<<<grid_of((int64_t)B * Ho * Wo * 3), 256, 0, st>>>(x, y, B, H, W, Ho, Wo, resize, normalize);
+    inc_input_kernel<<<grid_1d((int64_t)B * Ho * Wo * 3), 256, 0, st>>>(x, y, B, H, W, Ho, Wo, resize, normalize);
     return check_launch("inc_input");
 }
 int launch_inc_pool(const float* X, float* Y, int B, int H, int W, int C, int stride, int pad, int mode, int ldy, int yoff,
                     cudaStream_t st, __half* Yhi = nullptr, __half* Ylo = nullptr) {
     const int Ho = (H + 2 * pad - 3) / stride + 1, Wo = (W + 2 * pad - 3) / stride + 1;
-    inc_pool_kernel<<<grid_of((int64_t)B * Ho * Wo * C), 256, 0, st>>>(X, Y, B, H, W, C, Ho, Wo, stride, pad, mode, ldy, yoff, Yhi, Ylo);
+    inc_pool_kernel<<<grid_1d((int64_t)B * Ho * Wo * C), 256, 0, st>>>(X, Y, B, H, W, C, Ho, Wo, stride, pad, mode, ldy, yoff, Yhi, Ylo);
     return check_launch(mode == 0 ? "inc_maxpool" : "inc_avgpool");
 }
 int launch_inc_gap(const float* X, float* Y, int B, int HW, int C, cudaStream_t st) {
@@ -151,11 +117,6 @@ int launch_inc_gap(const float* X, float* Y, int B, int HW, int C, cudaStream_t 
 }
 
 // ------------------------------------------------------------------------------------------------ layer plan
-struct IncTensor {
-    const void* ptr;
-    int dtype;
-    int64_t numel;
-};
 // one BasicConv2d: its folded OHWI weight and bias live at w_off / b_off (floats) of the folded-parameter buffer
 struct IncConv {
     std::string name;
@@ -167,14 +128,11 @@ struct IncConv {
 
 struct rqb200_inception {
     rqb200_inception_config cfg;
-    std::unordered_map<std::string, rqb::IncTensor> t;
+    rqb::TensorTable t;
     std::vector<rqb::IncConv> convs;              // plan order
     std::unordered_map<std::string, int> conv_at;
-    int64_t params_floats = 0;
+    rqb::SplitParams par;                         // the folded weights and biases (bound at finalize)
     bool fast = false;                            // RQB200_MODE_FAST
-    const float* params = nullptr;                // folded weights (finalize): fp32, then (fast) the fp16 hi and lo copies
-    const __half* params_hi = nullptr;
-    const __half* params_lo = nullptr;
     bool finalized = false;
     int64_t last_launches = 0;
 };
@@ -207,34 +165,22 @@ struct IncRun {
     // BasicConv2d name: x NHWC [B, H, W, Cin] -> y rows of ldy floats from channel yoff; (H, W) becomes the output extent
     int conv(const std::string& name, const float* x, int& H, int& W, int Cin, float* y, int ldy, int yoff, int Cout, int kh, int kw,
              int ph, int pw, int stride) {
-        const int Ho = (H + 2 * ph - kh) / stride + 1, Wo = (W + 2 * pw - kw) / stride + 1;
-        note((int64_t)Ho * Wo, ldy);
+        const ConvGeom g = conv_geom(B, H, W, Cin, Cout, kh, kw, ph, pw, stride, ldy, yoff);
+        note((int64_t)g.Ho * g.Wo, ldy);
         if (mode == 0) {
-            IncConv c{name, Cin, Cout, kh, kw, h->params_floats, 0};
-            h->params_floats += (int64_t)Cout * kh * kw * Cin;
-            h->params_floats = (int64_t)align_up((size_t)h->params_floats, 64);
-            c.b_off = h->params_floats;
-            h->params_floats = (int64_t)align_up((size_t)(h->params_floats + Cout), 64);
+            const int64_t w_off = h->par.take((int64_t)Cout * kh * kw * Cin);
             h->conv_at[name] = (int)h->convs.size();
-            h->convs.push_back(c);
+            h->convs.push_back(IncConv{name, Cin, Cout, kh, kw, w_off, h->par.take(Cout)});
         }
         if (mode == 2) {
+            // Conv2d_1a_3x3 reads the staged fp32 input (no fp16 operand): fp32 FFMA on both tiers
             const IncConv& c = h->convs[h->conv_at.at(name)];
-            ConvGeom g{};
-            g.B = B; g.Hi = H; g.Wi = W; g.Cin = Cin; g.Ho = Ho; g.Wo = Wo; g.Cout = Cout; g.KH = kh; g.KW = kw; g.stride = stride;
-            g.pad = ph; g.pad_w = pw; g.ldy = ldy; g.yoff = yoff;
             const int sx = slot(x), sy = slot(y);
-            if (h->fast && sx >= 0)
-                RQB_TRY(launch_inc_conv_tc(hi[sx], lo[sx], h->params_hi + c.w_off, h->params_lo + c.w_off, h->params + c.b_off, y, hi[sy],
-                                           lo[sy], B, H, W, Cin, Cout, kh, kw, ph, pw, stride, ldy, yoff, st));
-            else {
-                RQB_TRY(launch_conv_relu(x, h->params + c.w_off, h->params + c.b_off, y, g, st));
-                // fast tier: Conv2d_1a_3x3 (Cin = 3, the staged fp32 input) runs on fp32 FFMA; its output becomes the next operand
-                if (h->fast) RQB_TRY(launch_cast_f16(y, hi[sy], lo[sy], B, Ho, Wo, ldy, 0, st));
-            }
+            RQB_TRY(launch_plan_conv(h->fast, h->par, c.w_off, c.b_off, x, sx >= 0 ? hi[sx] : nullptr, sx >= 0 ? lo[sx] : nullptr, y, hi[sy],
+                                     lo[sy], g, st));
         }
-        H = Ho;
-        W = Wo;
+        H = g.Ho;
+        W = g.Wo;
         return 0;
     }
     int conv1(const std::string& name, const float* x, int H, int W, int Cin, float* y, int ldy, int yoff, int Cout) {
@@ -261,7 +207,7 @@ struct IncRun {
     int emit(int k, const float* y, int H, int W, int C) {
         if (mode != 2 || !out_nchw[k]) return 0;
         const int64_t hw = (int64_t)H * W;
-        inc_to_nchw_kernel<<<grid_of(B * hw * C), 256, 0, st>>>(y, out_nchw[k] + out_b0 * hw * C, B, (int)hw, C);
+        inc_to_nchw_kernel<<<grid_1d(B * hw * C), 256, 0, st>>>(y, out_nchw[k] + out_b0 * hw * C, B, (int)hw, C);
         return check_launch("inc_to_nchw");
     }
 
@@ -383,10 +329,6 @@ static int64_t inc_max_act(rqb200_inception* h, int Hs, int Ws) {
 static size_t inc_image_bytes(int Hs, int Ws, int64_t max_act, bool fast) {
     return ((size_t)Hs * Ws * 3 + 4 * (size_t)max_act + INC_FEAT) * sizeof(float) + (fast ? 8 * (size_t)max_act * sizeof(__half) : 0);
 }
-static int inc_chunk(int B, size_t per_image) {
-    const int64_t fit = std::max<int64_t>(1, (int64_t)(INC_CHUNK_BYTES / per_image));
-    return (int)std::min<int64_t>(B, fit);
-}
 static size_t inc_layout(int n, int Hs, int Ws, int64_t max_act, bool fast, void* base, size_t cap, float** x0, IncRun* run) {
     Arena ar(base, cap);
     float* p = ar.take<float>((size_t)n * Hs * Ws * 3);
@@ -427,59 +369,42 @@ void rqb200_inception_destroy(rqb200_inception* h) { delete h; }
 
 int rqb200_inception_set_tensor(rqb200_inception* h, const char* key, const void* ptr, int dtype, int64_t numel) {
     if (!h || !key || !ptr) return rqb::fail(RQB200_EINVAL, "inception_set_tensor: null argument");
-    h->t[key] = rqb::IncTensor{ptr, dtype, numel};
+    h->t.set(key, ptr, dtype, numel);
     h->finalized = false;
     return 0;
 }
 
-// fp32 folded weights and biases; the fast tier adds their fp16 hi and lo copies at the same element offsets
 size_t rqb200_inception_params_bytes(const rqb200_inception* h) {
-    return h ? (size_t)h->params_floats * (sizeof(float) + (h->fast ? 2 * sizeof(__half) : 0)) : 0;
+    return h ? h->par.bytes(h->fast) : 0;
 }
 
 int rqb200_inception_finalize(rqb200_inception* h, void* params, size_t params_bytes, void* stream) {
     using namespace rqb;
     if (!h) return fail(RQB200_EINVAL, "inception_finalize: null handle");
     h->finalized = false;
-    auto get = [&](const std::string& k, int64_t numel, const IncTensor** out) -> int {
-        auto it = h->t.find(k);
-        if (it == h->t.end()) return fail(RQB200_ESTATE, "inception_finalize: tensor " + k + " (missing)");
-        if (it->second.numel != numel) return fail(RQB200_ESTATE, "inception_finalize: tensor " + k + " (wrong size)");
-        if (it->second.dtype != RQB200_F32) return fail(RQB200_EINVAL, "inception_finalize: tensor " + k + " must be fp32");
-        *out = &it->second;
-        return 0;
-    };
-    std::vector<const IncTensor*> ts(h->convs.size() * 5);
+    const char* who = "inception_finalize";
+    std::vector<const float*> ts(h->convs.size() * 5);
     for (size_t i = 0; i < h->convs.size(); i++) {
         const IncConv& c = h->convs[i];
-        RQB_TRY(get(c.name + ".conv.weight", (int64_t)c.cout * c.cin * c.kh * c.kw, &ts[i * 5]));
+        RQB_TRY(h->t.get_f32(who, c.name + ".conv.weight", (int64_t)c.cout * c.cin * c.kh * c.kw, &ts[i * 5]));
         static const char* bn[4] = {".bn.weight", ".bn.bias", ".bn.running_mean", ".bn.running_var"};
-        for (int j = 0; j < 4; j++) RQB_TRY(get(c.name + bn[j], c.cout, &ts[i * 5 + 1 + j]));
+        for (int j = 0; j < 4; j++) RQB_TRY(h->t.get_f32(who, c.name + bn[j], c.cout, &ts[i * 5 + 1 + j]));
     }
     if (h->cfg.last_block == 3) {
-        const IncTensor* d;
-        RQB_TRY(get("fc.weight", (int64_t)INC_CLASSES * INC_FEAT, &d));
-        RQB_TRY(get("fc.bias", INC_CLASSES, &d));
+        const float* d;
+        RQB_TRY(h->t.get_f32(who, "fc.weight", (int64_t)INC_CLASSES * INC_FEAT, &d));
+        RQB_TRY(h->t.get_f32(who, "fc.bias", INC_CLASSES, &d));
     }
     if (!params) return fail(RQB200_EINVAL, "inception_finalize: null parameter buffer");
     if (params_bytes < rqb200_inception_params_bytes(h))
         return fail(RQB200_EWORKSPACE, "inception_finalize: parameter buffer smaller than rqb200_inception_params_bytes");
     if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "inception_finalize: no CUDA device");
-    float* P = (float*)params;
-    __half* Ph = h->fast ? (__half*)(P + h->params_floats) : nullptr;
-    __half* Pl = h->fast ? Ph + h->params_floats : nullptr;
-    for (size_t i = 0; i < h->convs.size(); i++) {
+    h->par.bind(params, h->fast);
+    for (size_t i = 0; i < h->convs.size(); i++) {       // each BatchNorm folded into its conv
         const IncConv& c = h->convs[i];
-        const int64_t n = (int64_t)c.cout * c.kh * c.kw * c.cin;
-        inc_fold_bn_kernel<<<grid_of(n), 256, 0, (cudaStream_t)stream>>>(
-            (const float*)ts[i * 5]->ptr, (const float*)ts[i * 5 + 1]->ptr, (const float*)ts[i * 5 + 2]->ptr,
-            (const float*)ts[i * 5 + 3]->ptr, (const float*)ts[i * 5 + 4]->ptr, P + c.w_off, P + c.b_off, Ph ? Ph + c.w_off : nullptr,
-            Pl ? Pl + c.w_off : nullptr, c.cout, c.cin, c.kh, c.kw);
-        RQB_TRY(check_launch("inc_fold_bn"));
+        RQB_TRY(launch_conv_prep(ts[i * 5], nullptr, &ts[i * 5 + 1], INC_BN_EPS, h->par, c.w_off, c.b_off, c.cout, c.cin, c.kh, c.kw,
+                                 (cudaStream_t)stream));
     }
-    h->params = P;
-    h->params_hi = Ph;
-    h->params_lo = Pl;
     h->finalized = true;
     return 0;
 }
@@ -491,7 +416,7 @@ size_t rqb200_inception_workspace_bytes(rqb200_inception* h, int B, int H, int W
     staged_extent(H, W, flags, &Hs, &Ws);
     if (Hs < INC_MIN_EXTENT || Ws < INC_MIN_EXTENT) return 0;
     const int64_t ma = inc_max_act(h, Hs, Ws);
-    return inc_layout(inc_chunk(B, inc_image_bytes(Hs, Ws, ma, h->fast)), Hs, Ws, ma, h->fast, nullptr, 0, nullptr, nullptr);
+    return inc_layout(chunk_items(B, inc_image_bytes(Hs, Ws, ma, h->fast)), Hs, Ws, ma, h->fast, nullptr, 0, nullptr, nullptr);
 }
 
 int rqb200_inception_forward(rqb200_inception* h, const float* x, int B, int H, int W, int flags, float* out0, float* out1, float* out2,
@@ -517,15 +442,15 @@ int rqb200_inception_forward(rqb200_inception* h, const float* x, int B, int H, 
     if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "inception_forward: no CUDA device");
     const cudaStream_t st = (cudaStream_t)stream;
     const int64_t ma = inc_max_act(h, Hs, Ws);
-    const int chunk = inc_chunk(B, inc_image_bytes(Hs, Ws, ma, h->fast));
+    const int chunk = chunk_items(B, inc_image_bytes(Hs, Ws, ma, h->fast));
     IncRun run{h, st, chunk, 2};
     for (int k = 0; k < 3; k++) run.out_nchw[k] = outs[k];
     float* x0 = nullptr;
     if (inc_layout(chunk, Hs, Ws, ma, h->fast, workspace, workspace_bytes, &x0, &run) > workspace_bytes)
         return fail(RQB200_EWORKSPACE, "inception_forward: workspace smaller than rqb200_inception_workspace_bytes");
     g_launches = 0;
-    const float* fc_w = want_logits ? (const float*)h->t.at("fc.weight").ptr : nullptr;
-    const float* fc_b = want_logits ? (const float*)h->t.at("fc.bias").ptr : nullptr;
+    const float* fc_w = want_logits ? (const float*)h->t.find("fc.weight")->ptr : nullptr;
+    const float* fc_b = want_logits ? (const float*)h->t.find("fc.bias")->ptr : nullptr;
     int rc = 0;
     for (int b0 = 0; b0 < B && rc == 0; b0 += chunk) {
         const int n = std::min(chunk, B - b0);
@@ -558,13 +483,7 @@ int rqb200_dbg_inception_conv(const float* X, const float* Wt, const float* bias
     if (H + 2 * pad_h < kh || W + 2 * pad_w < kw) return fail(RQB200_EINVAL, "dbg_inception_conv: kernel larger than the padded input");
     if (!X || !Wt || !bias || !out) return fail(RQB200_EINVAL, "dbg_inception_conv: null argument");
     if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "dbg_inception_conv: no CUDA device");
-    ConvGeom g{};
-    g.B = B; g.Hi = H; g.Wi = W; g.Cin = Cin; g.Cout = Cout; g.KH = kh; g.KW = kw; g.stride = stride; g.pad = pad_h; g.pad_w = pad_w;
-    g.Ho = (H + 2 * pad_h - kh) / stride + 1;
-    g.Wo = (W + 2 * pad_w - kw) / stride + 1;
-    g.ldy = ldy;
-    g.yoff = yoff;
-    return launch_conv_relu(X, Wt, bias, out, g, (cudaStream_t)stream);
+    return launch_conv_relu(X, Wt, bias, out, conv_geom(B, H, W, Cin, Cout, kh, kw, pad_h, pad_w, stride, ldy, yoff), (cudaStream_t)stream);
 }
 
 int rqb200_dbg_inception_conv_tc(const void* X16, const void* X16lo, const void* W16, const void* W16lo, const float* bias, float* out,

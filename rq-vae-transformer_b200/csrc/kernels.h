@@ -2,6 +2,9 @@
 #pragma once
 #include <cuda.h>
 
+#include <string>
+#include <unordered_map>
+
 #include "common.cuh"
 
 namespace rqb {
@@ -93,6 +96,17 @@ struct ConvGeom {
     int pad_w;
     int ldy, yoff;
 };
+// the geometry of one conv of the Inception and LPIPS layer plans (launch_conv_relu / launch_plan_conv): x NHWC [B, H, W, Cin], a kh x kw
+// kernel with pads ph (top / bottom) and pw (left / right), output rows of ldy floats from channel yoff
+inline ConvGeom conv_geom(int B, int H, int W, int Cin, int Cout, int kh, int kw, int ph, int pw, int stride, int ldy, int yoff) {
+    ConvGeom g{};
+    g.B = B; g.Hi = H; g.Wi = W; g.Cin = Cin; g.Cout = Cout; g.KH = kh; g.KW = kw; g.stride = stride; g.pad = ph; g.pad_w = pw;
+    g.Ho = (H + 2 * ph - kh) / stride + 1;
+    g.Wo = (W + 2 * pw - kw) / stride + 1;
+    g.ldy = ldy;
+    g.yoff = yoff;
+    return g;
+}
 // the geometry of one conv of the VAE layer plan (vae_engine.cu): H, W the input extent before the optional nearest x2 upsample;
 // Ho, Wo = the (upsampled) extent / stride; pad 1 for a 3x3 stride-1 conv, else 0 (stride 2: the Downsample's implicit (0,1,0,1))
 ConvGeom vae_conv_geom(int B, int H, int W, int Cin, int Cout, int ks, int stride, int upsample, int in_nchw, int out_nchw);
@@ -124,6 +138,51 @@ int launch_groupnorm_f16(const float* X, const float* gamma, const float* beta, 
 int launch_cast_f16(const float* X, void* Y16, void* Y16lo, int B, int H, int W, int C, int upsample, cudaStream_t st);
 int make_tmap_4d_nhwc(CUtensorMap* out, const void* base, uint64_t C, uint64_t W, uint64_t H, uint64_t B, uint32_t box_c,
                       uint32_t box_w, uint32_t box_h, uint32_t box_b, uint32_t stride = 1);
+
+// plan.cu -- what the layer-plan engines (VAE, Inception, CLIP, LPIPS) share
+// The caller's tensors of one engine by state_dict key (rqb200_<engine>_set_tensor); the engine reads them at finalize
+struct PlanTensor {
+    const void* ptr;
+    int dtype;
+    int64_t numel;
+};
+struct TensorTable {
+    std::unordered_map<std::string, PlanTensor> t;
+    void set(const char* key, const void* ptr, int dtype, int64_t numel) { t[key] = PlanTensor{ptr, dtype, numel}; }
+    const PlanTensor* find(const std::string& key) const;      // null when the key was never set
+    // *out = the fp32 data of key, registered with numel elements; else fails with "<who>: tensor <key> (missing)" / "(wrong size)"
+    // (RQB200_ESTATE) or "must be fp32" (RQB200_EINVAL)
+    int get_f32(const char* who, const std::string& key, int64_t numel, const float** out) const;
+};
+// The parameter buffer of the Inception and LPIPS engines: `floats` fp32 values, then on the fast tier their fp16 hi and lo halves
+// (split_f16) at the same element offsets.  Each region a plan takes starts at a multiple of 64 floats.
+struct SplitParams {
+    int64_t floats = 0;
+    float* f32 = nullptr;           // bind()
+    __half* hi = nullptr;           // null on the exact tier
+    __half* lo = nullptr;
+    int64_t take(int64_t n) {
+        const int64_t o = floats;
+        floats = (int64_t)align_up((size_t)(o + n), 64);
+        return o;
+    }
+    size_t bytes(bool fast) const { return (size_t)floats * (sizeof(float) + (fast ? 2 * sizeof(__half) : 0)); }
+    void bind(void* params, bool fast) {
+        f32 = (float*)params;
+        hi = fast ? (__half*)(f32 + floats) : nullptr;
+        lo = fast ? hi + floats : nullptr;
+    }
+};
+// finalize of one plan conv: w OIHW [Cout, Cin, KH, KW] -> P.f32 + w_off OHWI and, on the fast tier (P.hi set), its split-fp16 halves
+// at the same offset; the bias -> P.f32 + b_off.  bn = {gamma, beta, running_mean, running_var} (nullable): the BatchNorm after the
+// conv, folded in fp64 (s = gamma / sqrt(var + bn_eps), w' = w s, b' = beta - mean s); without it w and bias are stored unchanged.
+int launch_conv_prep(const float* w, const float* bias, const float* const* bn, double bn_eps, const SplitParams& P, int64_t w_off,
+                     int64_t b_off, int Cout, int Cin, int KH, int KW, cudaStream_t st);
+// One plan conv + bias + ReLU, weights at w_off / bias at b_off of P.  The fast tier with the input's fp16 hi / lo operands (x_hi set)
+// runs inc_conv_tc_kernel, writing y (fp32) and / or y_hi / y_lo (either nullable); otherwise the fp32 FFMA kernel reads x and
+// writes y, and on the fast tier y's rows are then cast into y_hi / y_lo for the next conv.
+int launch_plan_conv(bool fast, const SplitParams& P, int64_t w_off, int64_t b_off, const float* x, const __half* x_hi,
+                     const __half* x_lo, float* y, __half* y_hi, __half* y_lo, const ConvGeom& g, cudaStream_t st);
 
 // gemm_tc.cu -- wgmma weight-streaming GEMM (fast tier)
 // GT_H16_QGELU: QuickGELU x * sigmoid(1.702 x) (CLIP's MLP) instead of the exact GELU; 16-bit weights, splits == 1

@@ -5,8 +5,6 @@
 // (relu1_2 .. relu5_3) write fp32; on the fast tier every other conv writes the next conv's fp16 hi / lo operands only, and the pools
 // read a tap's fp32 map and write those operands.  The head (normalize_tensor, squared difference, lin) runs in fp32 on both tiers; the
 // spatial average is a fixed-order fp64 sum, so a pair's value does not depend on the batch around it.
-#include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "kernels.h"
@@ -16,8 +14,6 @@ namespace rqb {
 constexpr int LP_MIN_EXTENT = 16;                    // four 2x2 pools must leave relu5_3 at least 1 x 1
 constexpr int LP_TAPS = 5;
 constexpr int LP_CHNS[LP_TAPS] = {64, 128, 256, 512, 512};
-constexpr size_t LP_CHUNK_BYTES = size_t(2) << 30;   // a call's workspace covers at most this many bytes of pairs; larger batches
-                                                     // run in chunks of as many pairs as fit
 constexpr float LP_EPS = 1e-10f;                     // normalize_tensor's eps
 
 // ------------------------------------------------------------------------------------------------ kernels
@@ -54,9 +50,9 @@ __global__ void lpips_pool_kernel(const float* __restrict__ X, float* __restrict
         const int64_t o = m * C + c;
         if (Y) *reinterpret_cast<float4*>(Y + o) = make_float4(v[0], v[1], v[2], v[3]);
         if (Yhi) {
-            const __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);
-            const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-            const __half2 l0 = __floats2half2_rn(v[0] - f0.x, v[1] - f0.y), l1 = __floats2half2_rn(v[2] - f1.x, v[3] - f1.y);
+            __half2 h0, h1, l0, l1;
+            split_f16x2(v[0], v[1], h0, l0);
+            split_f16x2(v[2], v[3], h1, l1);
             reinterpret_cast<__half2*>(Yhi + o)[0] = h0;
             reinterpret_cast<__half2*>(Yhi + o)[1] = h1;
             reinterpret_cast<__half2*>(Ylo + o)[0] = l0;
@@ -128,32 +124,13 @@ __global__ void __launch_bounds__(LP_MEAN_THREADS) lpips_mean_kernel(const float
     }
 }
 
-// finalize: a conv weight OIHW [Cout, Cin, 3, 3] -> OHWI fp32 (wo) and, on the fast tier, its split-fp16 halves
-__global__ void lpips_pack_kernel(const float* __restrict__ w, float* __restrict__ wo, __half* __restrict__ whi, __half* __restrict__ wlo,
-                                  int Cout, int Cin) {
-    const int64_t total = (int64_t)Cout * 9 * Cin;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int ci = (int)(i % Cin), tap = (int)((i / Cin) % 9);
-        const int64_t o = i / Cin / 9;
-        const float f = w[(o * Cin + ci) * 9 + tap];
-        wo[i] = f;
-        if (whi) {
-            const __half h = __float2half_rn(f);
-            whi[i] = h;
-            wlo[i] = __float2half_rn(f - __half2float(h));
-        }
-    }
-}
-
-static unsigned lp_grid(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(ceil_div(n, 256), 1), 8192); }
-
 int launch_lpips_input(const float* x0, const float* x1, const float* shift, const float* scale, float* y, int n, int H, int W,
                        cudaStream_t st) {
-    lpips_input_kernel<<<lp_grid(2 * (int64_t)n * H * W * 3), 256, 0, st>>>(x0, x1, shift, scale, y, n, H, W);
+    lpips_input_kernel<<<grid_1d(2 * (int64_t)n * H * W * 3), 256, 0, st>>>(x0, x1, shift, scale, y, n, H, W);
     return check_launch("lpips_input");
 }
 int launch_lpips_pool(const float* X, float* Y, __half* Yhi, __half* Ylo, int N, int H, int W, int C, cudaStream_t st) {
-    lpips_pool_kernel<<<lp_grid((int64_t)N * (H / 2) * (W / 2) * (C / 4)), 256, 0, st>>>(X, Y, Yhi, Ylo, N, H, W, C);
+    lpips_pool_kernel<<<grid_1d((int64_t)N * (H / 2) * (W / 2) * (C / 4)), 256, 0, st>>>(X, Y, Yhi, Ylo, N, H, W, C);
     return check_launch("lpips_pool");
 }
 int launch_lpips_head(const float* F, const float* w, float* d, int n, int hw, int C, cudaStream_t st) {
@@ -167,11 +144,6 @@ int launch_lpips_mean(const float* d, int n, int hw, int k, double* tapmean, flo
 }
 
 // ------------------------------------------------------------------------------------------------ layer plan
-struct LpTensor {
-    const void* ptr;
-    int dtype;
-    int64_t numel;
-};
 // one 3x3 pad-1 conv + bias + ReLU of vgg16.features: its OHWI weight and bias at w_off / b_off (floats) of the parameter buffer
 struct LpConv {
     std::string name;           // "net.slice<s>.<index>"
@@ -184,15 +156,12 @@ struct LpConv {
 
 struct rqb200_lpips {
     rqb200_lpips_config cfg;
-    std::unordered_map<std::string, rqb::LpTensor> t;
+    rqb::TensorTable t;
     std::vector<rqb::LpConv> convs;               // plan order
     int64_t lin_off[rqb::LP_TAPS];                // lin{k}'s weight [C_k]
     int64_t shift_off = 0, scale_off = 0;         // ScalingLayer's buffers [3]
-    int64_t params_floats = 0;
+    rqb::SplitParams par;                         // bound at finalize
     bool fast = false;                            // RQB200_MODE_FAST
-    const float* params = nullptr;                // finalize: fp32, then (fast) the fp16 hi and lo copies at the same element offsets
-    const __half* params_hi = nullptr;
-    const __half* params_lo = nullptr;
     bool finalized = false;
     int64_t last_launches = 0;
 };
@@ -204,22 +173,17 @@ static void lp_plan(rqb200_lpips* h) {
     static const int idx[13] = {0, 2, 5, 7, 10, 12, 14, 17, 19, 21, 24, 26, 28};
     static const int slice[13] = {1, 1, 2, 2, 3, 3, 3, 4, 4, 4, 5, 5, 5};
     static const int cout[13] = {64, 64, 128, 128, 256, 256, 256, 512, 512, 512, 512, 512, 512};
-    auto take = [h](int64_t n) {
-        const int64_t o = h->params_floats;
-        h->params_floats = (int64_t)align_up((size_t)(o + n), 64);
-        return o;
-    };
     int cin = 3;
     for (int i = 0; i < 13; i++) {
         LpConv c{"net.slice" + std::to_string(slice[i]) + "." + std::to_string(idx[i]), cin, cout[i], i == 12 || slice[i] != slice[i + 1], 0, 0};
-        c.w_off = take((int64_t)c.cout * 9 * c.cin);
-        c.b_off = take(c.cout);
+        c.w_off = h->par.take((int64_t)c.cout * 9 * c.cin);
+        c.b_off = h->par.take(c.cout);
         h->convs.push_back(c);
         cin = cout[i];
     }
-    for (int k = 0; k < LP_TAPS; k++) h->lin_off[k] = take(LP_CHNS[k]);
-    h->shift_off = take(3);
-    h->scale_off = take(3);
+    for (int k = 0; k < LP_TAPS; k++) h->lin_off[k] = h->par.take(LP_CHNS[k]);
+    h->shift_off = h->par.take(3);
+    h->scale_off = h->par.take(3);
 }
 
 // per pair: two staged images; exact: two fp32 activation buffers per image, fast: one plus two fp16 hi / lo operand pairs; the head's
@@ -229,10 +193,6 @@ static size_t lp_pair_bytes(int H, int W, bool fast) {
     const size_t ma = (size_t)lp_max_act(H, W), hw = (size_t)H * W;
     return 2 * (hw * 3 + (fast ? 1 : 2) * ma) * sizeof(float) + (fast ? 2 * 4 * ma * sizeof(__half) : 0) + hw * sizeof(float) +
            LP_TAPS * sizeof(double);
-}
-static int lp_chunk(int B, int H, int W, bool fast) {
-    const int64_t fit = std::max<int64_t>(1, (int64_t)(LP_CHUNK_BYTES / lp_pair_bytes(H, W, fast)));
-    return (int)std::min<int64_t>(B, fit);
 }
 struct LpBufs {
     float* x0 = nullptr;          // staged input [2n, H, W, 3]
@@ -262,7 +222,7 @@ static size_t lp_layout(int n, int H, int W, bool fast, void* base, size_t cap, 
 // one chunk of n pairs: x0 / x1 NCHW [n, 3, H, W] -> layer_out [n, 5] (nullable), val [n]
 static int lp_run(rqb200_lpips* h, const LpBufs& bf, const float* x0, const float* x1, int n, int H, int W, float* layer_out, float* val,
                   cudaStream_t st) {
-    const float* P = h->params;
+    const float* P = h->par.f32;
     const int N = 2 * n;
     RQB_TRY(launch_lpips_input(x0, x1, P + h->shift_off, P + h->scale_off, bf.x0, n, H, W, st));
     const float* in = bf.x0;      // the current fp32 map (exact tier; the staged input and the taps on both tiers)
@@ -271,21 +231,15 @@ static int lp_run(rqb200_lpips* h, const LpBufs& bf, const float* x0, const floa
     for (size_t i = 0; i < h->convs.size(); i++) {
         const LpConv& c = h->convs[i];
         float* out = h->fast ? bf.f[0] : (in == bf.f[0] ? bf.f[1] : bf.f[0]);
-        if (c.cin == 3 || !h->fast) {
-            ConvGeom g{};
-            g.B = N; g.Hi = H; g.Wi = W; g.Cin = c.cin; g.Ho = H; g.Wo = W; g.Cout = c.cout; g.KH = 3; g.KW = 3; g.stride = 1;
-            g.pad = 1; g.pad_w = 1; g.ldy = c.cout; g.yoff = 0;
-            RQB_TRY(launch_conv_relu(in, P + c.w_off, P + c.b_off, out, g, st));
-            // fast tier: conv1_1's output becomes the next conv's operand
-            if (h->fast) RQB_TRY(launch_cast_f16(out, bf.hi[0], bf.lo[0], N, H, W, c.cout, 0, st));
-            cs = 0;
-        } else {
-            const int os = 1 - cs;
-            RQB_TRY(launch_inc_conv_tc(bf.hi[cs], bf.lo[cs], h->params_hi + c.w_off, h->params_lo + c.w_off, P + c.b_off,
-                                       c.tap ? out : nullptr, c.tap ? nullptr : bf.hi[os], c.tap ? nullptr : bf.lo[os], N, H, W, c.cin,
-                                       c.cout, 3, 3, 1, 1, 1, c.cout, 0, st));
-            cs = os;
-        }
+        // conv1_1 reads the staged fp32 input (no fp16 operand): fp32 FFMA on both tiers.  On the wgmma path only the taps write
+        // fp32, the other convs only the next conv's operands.
+        const __half* xh = c.cin == 3 ? nullptr : bf.hi[cs];
+        const bool tc = h->fast && xh;
+        const int os = 1 - cs;
+        RQB_TRY(launch_plan_conv(h->fast, h->par, c.w_off, c.b_off, in, xh, bf.lo[cs], tc && !c.tap ? nullptr : out,
+                                 tc && c.tap ? nullptr : bf.hi[os], tc && c.tap ? nullptr : bf.lo[os],
+                                 conv_geom(N, H, W, c.cin, c.cout, 3, 3, 1, 1, 1, c.cout, 0), st));
+        cs = os;
         in = out;
         if (!c.tap) continue;
         RQB_TRY(launch_lpips_head(in, P + h->lin_off[tap], bf.d, n, H * W, c.cout, st));
@@ -322,68 +276,52 @@ void rqb200_lpips_destroy(rqb200_lpips* h) { delete h; }
 
 int rqb200_lpips_set_tensor(rqb200_lpips* h, const char* key, const void* ptr, int dtype, int64_t numel) {
     if (!h || !key || !ptr) return rqb::fail(RQB200_EINVAL, "lpips_set_tensor: null argument");
-    h->t[key] = rqb::LpTensor{ptr, dtype, numel};
+    h->t.set(key, ptr, dtype, numel);
     h->finalized = false;
     return 0;
 }
 
 size_t rqb200_lpips_params_bytes(const rqb200_lpips* h) {
-    return h ? (size_t)h->params_floats * (sizeof(float) + (h->fast ? 2 * sizeof(__half) : 0)) : 0;
+    return h ? h->par.bytes(h->fast) : 0;
 }
 
 int rqb200_lpips_finalize(rqb200_lpips* h, void* params, size_t params_bytes, void* stream) {
     using namespace rqb;
     if (!h) return fail(RQB200_EINVAL, "lpips_finalize: null handle");
     h->finalized = false;
-    auto get = [&](const std::string& k, int64_t numel, const LpTensor** out) -> int {
-        auto it = h->t.find(k);
-        if (it == h->t.end()) return fail(RQB200_ESTATE, "lpips_finalize: tensor " + k + " (missing)");
-        if (it->second.numel != numel) return fail(RQB200_ESTATE, "lpips_finalize: tensor " + k + " (wrong size)");
-        if (it->second.dtype != RQB200_F32) return fail(RQB200_EINVAL, "lpips_finalize: tensor " + k + " must be fp32");
-        *out = &it->second;
-        return 0;
-    };
-    std::vector<const LpTensor*> ts(h->convs.size() * 2);
+    const char* who = "lpips_finalize";
+    std::vector<const float*> ts(h->convs.size() * 2);
     for (size_t i = 0; i < h->convs.size(); i++) {
         const LpConv& c = h->convs[i];
-        RQB_TRY(get(c.name + ".weight", (int64_t)c.cout * c.cin * 9, &ts[2 * i]));
-        RQB_TRY(get(c.name + ".bias", c.cout, &ts[2 * i + 1]));
+        RQB_TRY(h->t.get_f32(who, c.name + ".weight", (int64_t)c.cout * c.cin * 9, &ts[2 * i]));
+        RQB_TRY(h->t.get_f32(who, c.name + ".bias", c.cout, &ts[2 * i + 1]));
     }
-    const LpTensor* lin[LP_TAPS];
+    const float* lin[LP_TAPS];
     for (int k = 0; k < LP_TAPS; k++) {
         // lin<k>.model.1.weight with the Dropout in front (use_dropout=True), lin<k>.model.0.weight without
         const std::string p = "lin" + std::to_string(k) + ".model.";
-        RQB_TRY(get(h->t.count(p + "1.weight") ? p + "1.weight" : p + "0.weight", LP_CHNS[k], &lin[k]));
+        RQB_TRY(h->t.get_f32(who, h->t.find(p + "1.weight") ? p + "1.weight" : p + "0.weight", LP_CHNS[k], &lin[k]));
     }
-    const LpTensor *shift, *scale;
-    RQB_TRY(get("scaling_layer.shift", 3, &shift));
-    RQB_TRY(get("scaling_layer.scale", 3, &scale));
+    const float *shift, *scale;
+    RQB_TRY(h->t.get_f32(who, "scaling_layer.shift", 3, &shift));
+    RQB_TRY(h->t.get_f32(who, "scaling_layer.scale", 3, &scale));
     if (!params) return fail(RQB200_EINVAL, "lpips_finalize: null parameter buffer");
     if (params_bytes < rqb200_lpips_params_bytes(h))
         return fail(RQB200_EWORKSPACE, "lpips_finalize: parameter buffer smaller than rqb200_lpips_params_bytes");
     if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "lpips_finalize: no CUDA device");
     const cudaStream_t st = (cudaStream_t)stream;
-    float* P = (float*)params;
-    __half* Ph = h->fast ? (__half*)(P + h->params_floats) : nullptr;
-    __half* Pl = h->fast ? Ph + h->params_floats : nullptr;
-    auto copy = [&](float* dst, const LpTensor* s) -> int {
-        RQB_CUDA(cudaMemcpyAsync(dst, s->ptr, (size_t)s->numel * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    h->par.bind(params, h->fast);
+    auto copy = [&](int64_t off, const float* s, int64_t n) -> int {
+        RQB_CUDA(cudaMemcpyAsync(h->par.f32 + off, s, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
         return 0;
     };
     for (size_t i = 0; i < h->convs.size(); i++) {
         const LpConv& c = h->convs[i];
-        lpips_pack_kernel<<<lp_grid((int64_t)c.cout * 9 * c.cin), 256, 0, st>>>((const float*)ts[2 * i]->ptr, P + c.w_off,
-                                                                             Ph ? Ph + c.w_off : nullptr, Pl ? Pl + c.w_off : nullptr,
-                                                                             c.cout, c.cin);
-        RQB_TRY(check_launch("lpips_pack"));
-        RQB_TRY(copy(P + c.b_off, ts[2 * i + 1]));
+        RQB_TRY(launch_conv_prep(ts[2 * i], ts[2 * i + 1], nullptr, 0.0, h->par, c.w_off, c.b_off, c.cout, c.cin, 3, 3, st));
     }
-    for (int k = 0; k < LP_TAPS; k++) RQB_TRY(copy(P + h->lin_off[k], lin[k]));
-    RQB_TRY(copy(P + h->shift_off, shift));
-    RQB_TRY(copy(P + h->scale_off, scale));
-    h->params = P;
-    h->params_hi = Ph;
-    h->params_lo = Pl;
+    for (int k = 0; k < LP_TAPS; k++) RQB_TRY(copy(h->lin_off[k], lin[k], LP_CHNS[k]));
+    RQB_TRY(copy(h->shift_off, shift, 3));
+    RQB_TRY(copy(h->scale_off, scale, 3));
     h->finalized = true;
     return 0;
 }
@@ -391,7 +329,7 @@ int rqb200_lpips_finalize(rqb200_lpips* h, void* params, size_t params_bytes, vo
 size_t rqb200_lpips_workspace_bytes(rqb200_lpips* h, int B, int H, int W) {
     using namespace rqb;
     if (!h || B <= 0 || H < LP_MIN_EXTENT || W < LP_MIN_EXTENT) return 0;
-    return lp_layout(lp_chunk(B, H, W, h->fast), H, W, h->fast, nullptr, 0, nullptr);
+    return lp_layout(chunk_items(B, lp_pair_bytes(H, W, h->fast)), H, W, h->fast, nullptr, 0, nullptr);
 }
 
 int rqb200_lpips_forward(rqb200_lpips* h, const float* x0, const float* x1, int B, int H, int W, float* layer_out, float* val_out,
@@ -403,7 +341,7 @@ int rqb200_lpips_forward(rqb200_lpips* h, const float* x0, const float* x1, int 
         return fail(RQB200_EINVAL, "lpips_forward: need B >= 1 and H, W >= 16");
     if (rqb200_device_count() <= 0) return fail(RQB200_ENODEV, "lpips_forward: no CUDA device");
     const cudaStream_t st = (cudaStream_t)stream;
-    const int chunk = lp_chunk(B, H, W, h->fast);
+    const int chunk = chunk_items(B, lp_pair_bytes(H, W, h->fast));
     LpBufs bf;
     if (lp_layout(chunk, H, W, h->fast, workspace, workspace_bytes, &bf) > workspace_bytes)
         return fail(RQB200_EWORKSPACE, "lpips_forward: workspace smaller than rqb200_lpips_workspace_bytes");

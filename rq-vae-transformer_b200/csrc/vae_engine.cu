@@ -6,21 +6,13 @@
 // Differences in execution, not arithmetic: activations stay NHWC end to end (the reference permutes NHWC<->NCHW at
 // rqvae.py:82,86), the nearest-x2 upsample and the (0,1,0,1) pad are folded into conv indexing, q/k/v 1x1 convs run as
 // one Cout=3C GEMM, and the whole batch is decoded in one pass (the reference's callers decode image by image).
-#include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "kernels.h"
 
-struct VTensor {
-    const void* ptr;
-    int dtype;
-    int64_t numel;
-};
-
 struct rqb200_vae {
     rqb200_vae_config cfg;
-    std::unordered_map<std::string, VTensor> t;
+    rqb::TensorTable t;
     bool finalized = false;
     bool fast_ok = false;     // FAST mode and every decoder channel count is a multiple of 128
     bool enc_fast = false;    // the encoder's convs were registered in fp16 as well: encode on the wgmma path
@@ -66,13 +58,13 @@ struct VaeRun {
     int64_t max_act = 0;                      // max H*W*C per image over all activations
     int64_t max_gn_hw = 0;
 
-    const VTensor* get(const std::string& k, int64_t numel) {
-        auto it = h->t.find(k);
-        if (it == h->t.end() || it->second.numel != numel) {
-            if (missing.empty()) missing = k + (it == h->t.end() ? " (missing)" : " (wrong size)");
+    const PlanTensor* get(const std::string& k, int64_t numel) {
+        const PlanTensor* p = h->t.find(k);
+        if (!p || p->numel != numel) {
+            if (missing.empty()) missing = k + (!p ? " (missing)" : " (wrong size)");
             return nullptr;
         }
-        return &it->second;
+        return p;
     }
     void note_act(int64_t hw, int64_t c) { if (hw * c > max_act) max_act = hw * c; }
 
@@ -85,8 +77,8 @@ struct VaeRun {
     // GroupNorm (+ SiLU) of in: into out on the exact tier, into slot 0 on the fast tier (from fused statistics where the
     // producing conv emitted them)
     int norm(const std::string& name, const float* in, float* out, int HW, int C, int silu, Operand* o) {
-        const VTensor* g = get(name + ".weight", C);
-        const VTensor* b = get(name + ".bias", C);
+        const PlanTensor* g = get(name + ".weight", C);
+        const PlanTensor* b = get(name + ".bias", C);
         if (HW > max_gn_hw) max_gn_hw = HW;
         note_act(HW, C);
         *o = fast ? Operand{nullptr, 0, 0, 0} : Operand{out, -1, 0, 0};
@@ -104,9 +96,9 @@ struct VaeRun {
         const ConvGeom g = vae_conv_geom(B, H, W, Cin, Cout, ks, stride, in.upsample, in.nchw, out_nchw);
         const int Ho = g.Ho, Wo = g.Wo;
         const int64_t wn = (int64_t)Cout * ks * ks * Cin;
-        const VTensor* w = get(name + ".weight", wn);
-        const VTensor* b = get(name + ".bias", Cout);
-        const VTensor* wl = in.slot < 0 ? nullptr : get(name + ".weight_lo", wn);
+        const PlanTensor* w = get(name + ".weight", wn);
+        const PlanTensor* b = get(name + ".bias", Cout);
+        const PlanTensor* wl = in.slot < 0 ? nullptr : get(name + ".weight_lo", wn);
         note_act((int64_t)Ho * Wo, Cout);
         if (dry || !w || !b) return 0;
         if (in.slot < 0) return launch_conv(in.x, w->ptr, w->dtype, (const float*)b->ptr, resid, out, g, st);
@@ -294,7 +286,7 @@ void rqb200_vae_destroy(rqb200_vae* h) { delete h; }
 
 int rqb200_vae_set_tensor(rqb200_vae* h, const char* key, const void* ptr, int dtype, int64_t numel) {
     if (!h || !key || !ptr) return rqb::fail(RQB200_EINVAL, "vae_set_tensor: null argument");
-    h->t[key] = VTensor{ptr, dtype, numel};
+    h->t.set(key, ptr, dtype, numel);
     h->finalized = false;
     return 0;
 }
@@ -313,8 +305,8 @@ int rqb200_vae_finalize(rqb200_vae* h) {
         h->gn_fuse = !(c.mode & RQB200_VAE_NO_GN_FUSE);
     }
     {
-        auto it = h->t.find("encoder.conv_out.weight");
-        h->enc_fast = h->fast_ok && it != h->t.end() && it->second.dtype == RQB200_F16;
+        const rqb::PlanTensor* w = h->t.find("encoder.conv_out.weight");
+        h->enc_fast = h->fast_ok && w && w->dtype == RQB200_F16;
     }
     const int R = h->cfg.resolution, f = rqb::vae_factor(h);
     run.decode(nullptr, nullptr, R / f, R / f);
@@ -322,7 +314,7 @@ int rqb200_vae_finalize(rqb200_vae* h) {
     if (!run.missing.empty()) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor " + run.missing);
     {
         const rqb200_vae_config& c = h->cfg;
-        const bool shared = h->t.count("codebook") != 0, per_depth = h->t.count("codebook.0") != 0;
+        const bool shared = h->t.find("codebook") != nullptr, per_depth = h->t.find("codebook.0") != nullptr;
         if (!shared && !per_depth) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor codebook (missing)");
         if (shared && per_depth) return rqb::fail(RQB200_EINVAL, "vae_finalize: both codebook and codebook.<d> registered");
         if (per_depth && (c.depth < 1 || c.depth > rqb::RQ_MAX_TABLES))
@@ -331,11 +323,11 @@ int rqb200_vae_finalize(rqb200_vae* h) {
         int32_t ks[rqb::RQ_MAX_TABLES];
         const int n = shared ? 1 : c.depth;
         for (int d = 0; d < n; d++) {
-            auto it = h->t.find(shared ? std::string("codebook") : "codebook." + std::to_string(d));
-            if (it == h->t.end()) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor codebook." + std::to_string(d) + " (missing)");
-            ptrs[d] = (const float*)it->second.ptr;
-            ks[d] = shared ? c.codebook_size : (int32_t)(it->second.numel / c.embed_dim);
-            if (!shared && (int64_t)ks[d] * c.embed_dim != it->second.numel)
+            const rqb::PlanTensor* cb = h->t.find(shared ? std::string("codebook") : "codebook." + std::to_string(d));
+            if (!cb) return rqb::fail(RQB200_ESTATE, "vae_finalize: tensor codebook." + std::to_string(d) + " (missing)");
+            ptrs[d] = (const float*)cb->ptr;
+            ks[d] = shared ? c.codebook_size : (int32_t)(cb->numel / c.embed_dim);
+            if (!shared && (int64_t)ks[d] * c.embed_dim != cb->numel)
                 return rqb::fail(RQB200_EINVAL, "vae_finalize: codebook." + std::to_string(d) + " is not [K, embed_dim]");
         }
         RQB_TRY(rqb::make_rq_tables(&h->codebooks, ptrs, ks, n));

@@ -294,4 +294,101 @@ def param_fingerprint(module):
     return hash(tuple((t.data_ptr(), t._version) for t in list(module.parameters()) + list(module.buffers())))
 
 
+class EngineCache:
+    """Mixin for an nn.Module whose forward runs in native engines built from its parameters.  The engines live in ``_eng`` (key ->
+    {"handle", ...}) and are destroyed through ``_DESTROY`` (the C function's name) when the module moves (``_apply``), loads a
+    state_dict, is collected, or its parameters change in a way its own hooks do not see (``_cached_engine``'s fingerprint)."""
+    _DESTROY = None
+
+    def __init__(self, *a, **k):
+        super().__init__(*a, **k)
+        self.precision = None            # None -> default_precision() ('auto' == exact unless the module says otherwise)
+        self._eng = {}
+        self._eng_fp = None              # the fingerprint the cached engines were built from
+        self.last_launches = 0
+
+    def _invalidate_native(self):
+        for e in self._eng.values():
+            getattr(lib(), self._DESTROY)(e["handle"])
+        self._eng = {}
+
+    def _apply(self, fn, *a, **k):
+        self._invalidate_native()
+        return super()._apply(fn, *a, **k)
+
+    def load_state_dict(self, *a, **k):
+        self._invalidate_native()
+        return super().load_state_dict(*a, **k)
+
+    def __del__(self):
+        try:
+            self._invalidate_native()
+        except Exception:
+            pass
+
+    def _mode(self):
+        p = self.precision or default_precision()
+        return MODE_FAST if p == "fast" else MODE_EXACT
+
+    def _cached_engine(self, key, fingerprint, build):
+        """the engine under key, made by build() when absent; every engine is dropped first when fingerprint differs from the one
+        they were built from (weights changed behind the module's own hooks: a wrapper's load, an in-place write)"""
+        if fingerprint != self._eng_fp:
+            self._invalidate_native()
+            self._eng_fp = fingerprint
+        if key not in self._eng:
+            self._eng[key] = build()
+        return self._eng[key]
+
+
+def bind_plan_engine(L, prefix, cfg_type):
+    """ctypes signatures of the lifecycle every layer-plan engine rqb200_<prefix>_* shares: create (from a cfg_type), destroy,
+    set_tensor, params_bytes, finalize and last_launches"""
+    fn = lambda name: getattr(L, "rqb200_%s_%s" % (prefix, name))
+    fn("create").restype = C.c_void_p
+    fn("create").argtypes = [C.POINTER(cfg_type)]
+    fn("destroy").argtypes = [C.c_void_p]
+    fn("destroy").restype = None
+    fn("set_tensor").argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int64]
+    fn("params_bytes").restype = C.c_size_t
+    fn("params_bytes").argtypes = [C.c_void_p]
+    fn("finalize").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    fn("last_launches").restype = C.c_int64
+    fn("last_launches").argtypes = [C.c_void_p]
+
+
+def plan_engine(L, prefix, cfg, tensors, device):
+    """a layer-plan engine rqb200_<prefix>_* (L bound by bind_plan_engine) on device: created from cfg, every tensor of {key: tensor}
+    registered as a contiguous fp32 copy, its parameter buffer allocated and finalized -> {"handle", "keep", "params", "ws"}"""
+    fn = lambda name: getattr(L, "rqb200_%s_%s" % (prefix, name))
+    handle = fn("create")(C.byref(cfg))
+    if not handle:
+        raise NativeError("rqb200_%s_create: %s" % (prefix, L.rqb200_last_error().decode()))
+    eng = {"handle": handle, "keep": {}, "ws": None}
+    try:
+        for k, v in tensors.items():
+            require_cuda(v)
+            t = v.detach().float().contiguous()
+            eng["keep"][k] = t
+            check(fn("set_tensor")(handle, k.encode(), ptr(t), dtype_code(t), t.numel()), prefix + "_set_tensor")
+        eng["params"] = params = torch.empty(fn("params_bytes")(handle), dtype=torch.uint8, device=device)
+        with torch.cuda.device(device):
+            check(fn("finalize")(handle, ptr(params), params.numel(), stream_ptr(device)), prefix + "_finalize")
+    except BaseException:
+        fn("destroy")(handle)
+        raise
+    return eng
+
+
+def workspace(eng, need, device, refused=None):
+    """eng["ws"] grown to at least `need` bytes on device; a growing buffer is released before the larger one is allocated.  need == 0
+    is the engine refusing the call's arguments: NativeError(refused), unless refused is None and the engine's own call reports it."""
+    if need == 0 and refused is not None:
+        raise NativeError(refused)
+    if eng["ws"] is None or eng["ws"].numel() < need:
+        eng["ws"] = None
+        eng["ws"] = torch.empty(need, dtype=torch.uint8, device=device)
+    return eng["ws"]
+
+
 launch_count = {"total": 0}      # kernels launched by our library through this binding (bench.py's gpu_launches)

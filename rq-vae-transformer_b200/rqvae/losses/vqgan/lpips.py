@@ -23,7 +23,7 @@ VGG_SLICES = (((0, 64), (2, 64)), ((5, 128), (7, 128)), ((10, 256), (12, 256), (
               ((24, 512), (26, 512), (28, 512)))
 
 
-class LPIPS(nn.Module):
+class LPIPS(N.EngineCache, nn.Module):
     """Learned perceptual metric (the reference's class; compute in the native engine, forward only).
 
     ``precision``: None (the default: RQB200_PRECISION, 'auto' = exact) or 'exact' run every conv on fp32 FFMA; 'fast' runs them (but the
@@ -40,10 +40,6 @@ class LPIPS(nn.Module):
         self.lin3 = NetLinLayer(self.chns[3], use_dropout=use_dropout)
         self.lin4 = NetLinLayer(self.chns[4], use_dropout=use_dropout)
         self.use_dropout = use_dropout
-        self.precision = None
-        self._eng = {}
-        self._eng_fp = None
-        self.last_launches = 0
         self.load_from_pretrained()
         for param in self.parameters():
             param.requires_grad = False
@@ -63,55 +59,12 @@ class LPIPS(nn.Module):
         return model
 
     # ------------------------------------------------------------------ native engine plumbing
-    def _invalidate_native(self):
-        for e in self._eng.values():
-            N.lib().rqb200_lpips_destroy(e["handle"])
-        self._eng = {}
-
-    def _apply(self, fn, *a, **k):
-        self._invalidate_native()
-        return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, *a, **k):
-        self._invalidate_native()
-        return super().load_state_dict(*a, **k)
-
-    def __del__(self):
-        try:
-            self._invalidate_native()
-        except Exception:
-            pass
-
-    def _mode(self):
-        p = self.precision or N.default_precision()
-        return N.MODE_FAST if p == "fast" else N.MODE_EXACT
+    _DESTROY = "rqb200_lpips_destroy"
 
     def _engine(self, device):
         mode = self._mode()
-        fp = N.param_fingerprint(self)
-        if fp != self._eng_fp:
-            self._invalidate_native()
-            self._eng_fp = fp
-        key = (str(device), mode)
-        if key in self._eng:
-            return self._eng[key]
-        L = _lib()
-        cfg = LpipsConfig(mode)
-        handle = L.rqb200_lpips_create(C.byref(cfg))
-        if not handle:
-            raise N.NativeError("rqb200_lpips_create: " + L.rqb200_last_error().decode())
-        eng = {"handle": handle, "keep": {}, "ws": None}
-        self._eng[key] = eng
-        for k, v in self.state_dict().items():
-            N.require_cuda(v)
-            t = v.detach().float().contiguous()
-            eng["keep"][k] = t
-            N.check(L.rqb200_lpips_set_tensor(handle, k.encode(), N.ptr(t), N.dtype_code(t), t.numel()), "lpips_set_tensor")
-        params = torch.empty(L.rqb200_lpips_params_bytes(handle), dtype=torch.uint8, device=device)
-        eng["params"] = params
-        with torch.cuda.device(device):
-            N.check(L.rqb200_lpips_finalize(handle, N.ptr(params), params.numel(), N.stream_ptr(device)), "lpips_finalize")
-        return eng
+        return self._cached_engine((str(device), mode), N.param_fingerprint(self),
+                                   lambda: N.plan_engine(_lib(), "lpips", LpipsConfig(mode), self.state_dict(), device))
 
     def _check(self, input, target, reduction):
         for name, t in (("input", input), ("target", target)):
@@ -147,13 +100,8 @@ class LPIPS(nn.Module):
         layers = torch.empty(B, 5, dtype=torch.float32, device=x0.device)
         val = torch.empty(B, dtype=torch.float32, device=x0.device)
         with torch.cuda.device(x0.device):
-            need = L.rqb200_lpips_workspace_bytes(eng["handle"], B, H, W)
-            if need == 0:
-                raise N.NativeError("rqb200_lpips_workspace_bytes: extent %d x %d refused" % (H, W))
-            if eng["ws"] is None or eng["ws"].numel() < need:
-                eng["ws"] = None
-                eng["ws"] = torch.empty(need, dtype=torch.uint8, device=x0.device)
-            ws = eng["ws"]
+            ws = N.workspace(eng, L.rqb200_lpips_workspace_bytes(eng["handle"], B, H, W), x0.device,
+                             "rqb200_lpips_workspace_bytes: extent %d x %d refused" % (H, W))
             N.check(L.rqb200_lpips_forward(eng["handle"], N.ptr(x0), N.ptr(x1), B, H, W, N.ptr(layers), N.ptr(val), N.ptr(ws), ws.numel(),
                                            N.stream_ptr(x0.device)), "lpips_forward")
         self.last_launches = L.rqb200_lpips_last_launches(eng["handle"])
@@ -250,19 +198,10 @@ class LpipsConfig(C.Structure):
 def _lib():
     L = N.lib()
     if not getattr(L, "_lpips_bound", False):
-        L.rqb200_lpips_create.restype = C.c_void_p
-        L.rqb200_lpips_create.argtypes = [C.POINTER(LpipsConfig)]
-        L.rqb200_lpips_destroy.argtypes = [C.c_void_p]
-        L.rqb200_lpips_destroy.restype = None
-        L.rqb200_lpips_set_tensor.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int64]
-        L.rqb200_lpips_params_bytes.restype = C.c_size_t
-        L.rqb200_lpips_params_bytes.argtypes = [C.c_void_p]
-        L.rqb200_lpips_finalize.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        N.bind_plan_engine(L, "lpips", LpipsConfig)
         L.rqb200_lpips_workspace_bytes.restype = C.c_size_t
         L.rqb200_lpips_workspace_bytes.argtypes = [C.c_void_p] + [C.c_int] * 3
         L.rqb200_lpips_forward.argtypes = [C.c_void_p] * 3 + [C.c_int] * 3 + [C.c_void_p] * 3 + [C.c_size_t, C.c_void_p]
-        L.rqb200_lpips_last_launches.restype = C.c_int64
-        L.rqb200_lpips_last_launches.argtypes = [C.c_void_p]
         L.rqb200_dbg_lpips_input.argtypes = [C.c_void_p] * 5 + [C.c_int] * 3 + [C.c_void_p]
         L.rqb200_dbg_lpips_pool.argtypes = [C.c_void_p] * 4 + [C.c_int] * 4 + [C.c_void_p]
         L.rqb200_dbg_lpips_head.argtypes = [C.c_void_p] * 3 + [C.c_int] * 3 + [C.c_void_p]

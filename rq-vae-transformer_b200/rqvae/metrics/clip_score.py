@@ -250,7 +250,7 @@ def clip_config_of(state_dict):
     return cfg
 
 
-class CLIP(nn.Module):
+class CLIP(N.EngineCache, nn.Module):
     """OpenAI's CLIP (ViT image tower) with its state_dict layout; encode_image / encode_text run in the native engine.
 
     ``precision``: None (the default: RQB200_PRECISION, 'auto' = exact) or 'exact' runs fp32 FFMA; 'fast' runs the transformer GEMMs
@@ -274,34 +274,9 @@ class CLIP(nn.Module):
         self.text_projection = nn.Parameter(torch.empty(transformer_width, embed_dim))
         self.logit_scale = nn.Parameter(torch.ones([]) * np.log(1 / 0.07))
         self.embed_dim = embed_dim
-        self.precision = None
-        self._eng = {}
-        self._eng_fp = None
-        self.last_launches = 0
 
     # ------------------------------------------------------------------ native engine plumbing
-    def _invalidate_native(self):
-        for e in self._eng.values():
-            N.lib().rqb200_clip_destroy(e["handle"])
-        self._eng = {}
-
-    def _apply(self, fn, *a, **k):
-        self._invalidate_native()
-        return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, *a, **k):
-        self._invalidate_native()
-        return super().load_state_dict(*a, **k)
-
-    def __del__(self):
-        try:
-            self._invalidate_native()
-        except Exception:
-            pass
-
-    def _mode(self):
-        p = self.precision or N.default_precision()
-        return N.MODE_FAST if p == "fast" else N.MODE_EXACT
+    _DESTROY = "rqb200_clip_destroy"
 
     def _config(self, mode):
         v = self.visual
@@ -311,40 +286,12 @@ class CLIP(nn.Module):
 
     def _engine(self, device):
         mode = self._mode()
-        fp = N.param_fingerprint(self)
-        if fp != self._eng_fp:
-            self._invalidate_native()
-            self._eng_fp = fp
-        key = (str(device), mode)
-        if key in self._eng:
-            return self._eng[key]
-        L = _lib()
-        cfg = self._config(mode)
-        handle = L.rqb200_clip_create(C.byref(cfg))
-        if not handle:
-            raise N.NativeError("rqb200_clip_create: " + L.rqb200_last_error().decode())
-        eng = {"handle": handle, "keep": {}, "ws": None}
-        self._eng[key] = eng
-        for k, v in self.state_dict().items():
-            if k == "logit_scale":
-                continue
-            N.require_cuda(v)
-            t = v.detach().float().contiguous()
-            eng["keep"][k] = t
-            N.check(L.rqb200_clip_set_tensor(handle, k.encode(), N.ptr(t), N.dtype_code(t), t.numel()), "clip_set_tensor")
-        params = torch.empty(L.rqb200_clip_params_bytes(handle), dtype=torch.uint8, device=device)
-        eng["params"] = params
-        with torch.cuda.device(device):
-            N.check(L.rqb200_clip_finalize(handle, N.ptr(params), params.numel(), N.stream_ptr(device)), "clip_finalize")
-        return eng
+        return self._cached_engine((str(device), mode), N.param_fingerprint(self), lambda: N.plan_engine(
+            _lib(), "clip", self._config(mode), {k: v for k, v in self.state_dict().items() if k != "logit_scale"}, device))
 
-    def _workspace(self, eng, need, device):
-        if need == 0:
-            raise N.NativeError("rqb200_clip: the engine refused the input's extent")
-        if eng["ws"] is None or eng["ws"].numel() < need:
-            eng["ws"] = None
-            eng["ws"] = torch.empty(need, dtype=torch.uint8, device=device)
-        return eng["ws"]
+    @staticmethod
+    def _workspace(eng, need, device):
+        return N.workspace(eng, need, device, "rqb200_clip: the engine refused the input's extent")
 
     @torch.no_grad()
     def _encode_images(self, x, flags):
@@ -504,14 +451,7 @@ class ClipConfig(C.Structure):
 def _lib():
     L = N.lib()
     if not getattr(L, "_clip_bound", False):
-        L.rqb200_clip_create.restype = C.c_void_p
-        L.rqb200_clip_create.argtypes = [C.POINTER(ClipConfig)]
-        L.rqb200_clip_destroy.argtypes = [C.c_void_p]
-        L.rqb200_clip_destroy.restype = None
-        L.rqb200_clip_set_tensor.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int64]
-        L.rqb200_clip_params_bytes.restype = C.c_size_t
-        L.rqb200_clip_params_bytes.argtypes = [C.c_void_p]
-        L.rqb200_clip_finalize.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        N.bind_plan_engine(L, "clip", ClipConfig)
         L.rqb200_clip_workspace_bytes.restype = C.c_size_t
         L.rqb200_clip_workspace_bytes.argtypes = [C.c_void_p] + [C.c_int] * 4
         L.rqb200_clip_text_workspace_bytes.restype = C.c_size_t
@@ -519,8 +459,6 @@ def _lib():
         L.rqb200_clip_encode_image.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         L.rqb200_clip_encode_text.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         L.rqb200_clip_cosine.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-        L.rqb200_clip_last_launches.restype = C.c_int64
-        L.rqb200_clip_last_launches.argtypes = [C.c_void_p]
         L.rqb200_clip_resize_plan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p]
         L.rqb200_dbg_clip_preprocess.argtypes = [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_void_p, C.c_void_p]
         L.rqb200_dbg_clip_attn.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_void_p]

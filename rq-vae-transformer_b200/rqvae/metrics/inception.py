@@ -157,7 +157,7 @@ def block_extents(H, W, resize_input):
     return out
 
 
-class InceptionV3(nn.Module):
+class InceptionV3(N.EngineCache, nn.Module):
     """Pretrained InceptionV3 network returning feature maps (the reference's class; compute in the native engine).
 
     ``precision``: None (the default: RQB200_PRECISION, 'auto' = exact) or 'exact' run every conv on fp32 FFMA; 'fast' runs them (but
@@ -204,63 +204,15 @@ class InceptionV3(nn.Module):
             self.fc.bias.copy_(inception.fc.bias)
         for param in self.parameters():
             param.requires_grad = requires_grad
-        self.precision = None
-        self._eng = {}
-        self._eng_fp = None
-        self.last_launches = 0
 
     # ------------------------------------------------------------------ native engine plumbing
-    def _invalidate_native(self):
-        for e in self._eng.values():
-            N.lib().rqb200_inception_destroy(e["handle"])
-        self._eng = {}
-
-    def _apply(self, fn, *a, **k):
-        self._invalidate_native()
-        return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, *a, **k):
-        self._invalidate_native()
-        return super().load_state_dict(*a, **k)
-
-    def __del__(self):
-        try:
-            self._invalidate_native()
-        except Exception:
-            pass
-
-    def _mode(self):
-        p = self.precision or N.default_precision()
-        return N.MODE_FAST if p == "fast" else N.MODE_EXACT
+    _DESTROY = "rqb200_inception_destroy"
 
     def _engine(self, device):
         mode = self._mode()
-        fp = N.param_fingerprint(self)
-        if fp != self._eng_fp:
-            self._invalidate_native()
-            self._eng_fp = fp
-        key = (str(device), mode)
-        if key in self._eng:
-            return self._eng[key]
-        L = _lib()
-        cfg = IncConfig(self.last_needed_block, mode)
-        handle = L.rqb200_inception_create(C.byref(cfg))
-        if not handle:
-            raise N.NativeError("rqb200_inception_create: " + L.rqb200_last_error().decode())
-        eng = {"handle": handle, "keep": {}, "ws": None}
-        self._eng[key] = eng
-        for k, v in self.state_dict().items():
-            if k.endswith("num_batches_tracked"):
-                continue
-            N.require_cuda(v)
-            t = v.detach().float().contiguous()
-            eng["keep"][k] = t
-            N.check(L.rqb200_inception_set_tensor(handle, k.encode(), N.ptr(t), N.dtype_code(t), t.numel()), "inception_set_tensor")
-        params = torch.empty(L.rqb200_inception_params_bytes(handle), dtype=torch.uint8, device=device)
-        eng["params"] = params
-        with torch.cuda.device(device):
-            N.check(L.rqb200_inception_finalize(handle, N.ptr(params), params.numel(), N.stream_ptr(device)), "inception_finalize")
-        return eng
+        return self._cached_engine((str(device), mode), N.param_fingerprint(self), lambda: N.plan_engine(
+            _lib(), "inception", IncConfig(self.last_needed_block, mode),
+            {k: v for k, v in self.state_dict().items() if not k.endswith("num_batches_tracked")}, device))
 
     def _check_input(self, inp):
         if not isinstance(inp, torch.Tensor) or inp.dim() != 4:
@@ -294,13 +246,8 @@ class InceptionV3(nn.Module):
             outs[k] = torch.empty(shape, dtype=torch.float32, device=x.device)
         lg = torch.empty(B, 1008, dtype=torch.float32, device=x.device) if logits else None
         with torch.cuda.device(x.device):
-            need = L.rqb200_inception_workspace_bytes(eng["handle"], B, H, W, flags)
-            if need == 0:
-                raise N.NativeError("rqb200_inception_workspace_bytes: extent %d x %d refused" % (H, W))
-            if eng["ws"] is None or eng["ws"].numel() < need:
-                eng["ws"] = None
-                eng["ws"] = torch.empty(need, dtype=torch.uint8, device=x.device)
-            ws = eng["ws"]
+            ws = N.workspace(eng, L.rqb200_inception_workspace_bytes(eng["handle"], B, H, W, flags), x.device,
+                             "rqb200_inception_workspace_bytes: extent %d x %d refused" % (H, W))
             N.check(L.rqb200_inception_forward(eng["handle"], N.ptr(x), B, H, W, flags, *[N.ptr(o) for o in outs], N.ptr(lg), N.ptr(ws),
                                                ws.numel(), N.stream_ptr(x.device)), "inception_forward")
         self.last_launches = L.rqb200_inception_last_launches(eng["handle"])
@@ -324,19 +271,10 @@ class IncConfig(C.Structure):
 def _lib():
     L = N.lib()
     if not getattr(L, "_inception_bound", False):
-        L.rqb200_inception_create.restype = C.c_void_p
-        L.rqb200_inception_create.argtypes = [C.POINTER(IncConfig)]
-        L.rqb200_inception_destroy.argtypes = [C.c_void_p]
-        L.rqb200_inception_destroy.restype = None
-        L.rqb200_inception_set_tensor.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_int64]
-        L.rqb200_inception_params_bytes.restype = C.c_size_t
-        L.rqb200_inception_params_bytes.argtypes = [C.c_void_p]
-        L.rqb200_inception_finalize.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        N.bind_plan_engine(L, "inception", IncConfig)
         L.rqb200_inception_workspace_bytes.restype = C.c_size_t
         L.rqb200_inception_workspace_bytes.argtypes = [C.c_void_p] + [C.c_int] * 4
         L.rqb200_inception_forward.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_void_p] * 6 + [C.c_size_t, C.c_void_p]
-        L.rqb200_inception_last_launches.restype = C.c_int64
-        L.rqb200_inception_last_launches.argtypes = [C.c_void_p]
         L.rqb200_dbg_inception_conv.argtypes = [C.c_void_p] * 4 + [C.c_int] * 12 + [C.c_void_p]
         L.rqb200_dbg_inception_conv_tc.argtypes = [C.c_void_p] * 8 + [C.c_int] * 12 + [C.c_void_p]
         L.rqb200_dbg_inception_input.argtypes = [C.c_void_p] * 2 + [C.c_int] * 5 + [C.c_void_p]

@@ -58,7 +58,7 @@ class _Stack(_Holder):
         self.blocks = nn.ModuleList([_Block(cfg.block) for _ in range(cfg.n_layer)])
 
 
-class RQTransformer(Stage2Model):
+class RQTransformer(N.EngineCache, Stage2Model):
     def __init__(self, config):
         super().__init__()
         self.config = config = config.copy()
@@ -97,34 +97,16 @@ class RQTransformer(Stage2Model):
         if config.block_size_cond > 1:
             self.cond_classifier = nn.Sequential(OrderedDict([("layer_norm", nn.LayerNorm(E)),
                                                               ("linear", nn.Linear(E, config.vocab_size_cond))]))
-        self.precision = None
         self.noise_budget_bytes = 256 << 20      # bound on the Exp(1) noise buffer sample() draws per span of positions
-        self._eng = {}
-        self._eng_fp = None
         self._cache = None
         self._step = None                        # the stepped cached_forward sequence (init_cache / _step_route)
-        self.last_launches = 0
 
     # ------------------------------------------------------------------ native engine plumbing
+    _DESTROY = "rqb200_ar_destroy"
+
     def _invalidate_native(self):
-        for e in self._eng.values():
-            N.lib().rqb200_ar_destroy(e["handle"])
-        self._eng = {}
+        super()._invalidate_native()
         self._step = None                        # its KV caches lived in the engines' workspaces
-
-    def _apply(self, fn, *a, **k):
-        self._invalidate_native()
-        return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, *a, **k):
-        self._invalidate_native()
-        return super().load_state_dict(*a, **k)
-
-    def __del__(self):
-        try:
-            self._invalidate_native()
-        except Exception:
-            pass
 
     def _mode(self, amp):
         p = self.precision or N.default_precision()
@@ -186,19 +168,14 @@ class RQTransformer(Stage2Model):
         else:
             fp = (N.param_fingerprint(self), codebook._version)
             cb_id = codebook.data_ptr()
-        if fp != self._eng_fp:               # weights changed behind the module's own hooks (wrapper load, in-place write)
-            self._invalidate_native()
-            self._eng_fp = fp
-        key = (str(dev), mode, cb_id, slot)
-        if key not in self._eng and slot != 0:
+        return self._cached_engine((str(dev), mode, cb_id, slot), fp, lambda: self._build_engine(codebook, mode, slot))
+
+    def _build_engine(self, codebook, mode, slot):
+        if slot != 0:
             # engines of one model share the packed weights of slot 0; each slot owns its workspace, KV cache and graphs
             base = self._engine(codebook, mode, 0)
-            eng = dict(base, handle=base["make"](), ws=None)
-            self._eng[key] = eng
-            return eng
-        if key in self._eng:
-            return self._eng[key]
-        N.require_cuda(self.pos_emb_hw, *(codebook if per_depth else [codebook]))
+            return dict(base, handle=base["make"](), ws=None)
+        N.require_cuda(self.pos_emb_hw, *(codebook if isinstance(codebook, list) else [codebook]))
         self._check_computable()
         L = N.lib()
         cfg, w, keep, streamed = self._engine_structs(codebook, mode)
@@ -209,10 +186,7 @@ class RQTransformer(Stage2Model):
                 raise N.NativeError("rqb200_ar_create: " + L.rqb200_last_error().decode())
             return hnd
 
-        handle = make()
-        eng = {"handle": handle, "keep": keep, "ws": None, "make": make, "weight_dtype": cfg.weight_dtype, "streamed": streamed}
-        self._eng[key] = eng
-        return eng
+        return {"handle": make(), "keep": keep, "ws": None, "make": make, "weight_dtype": cfg.weight_dtype, "streamed": streamed}
 
     def _engine_structs(self, codebook, mode):
         """the rqb200_ar_config / rqb200_ar_weights of one engine build and the tensors they point into: (cfg, w, keep, streamed),

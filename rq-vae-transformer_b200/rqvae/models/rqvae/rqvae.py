@@ -17,7 +17,7 @@ from .modules import Decoder, Encoder, ResnetBlock
 from .quantizations import RQBottleneck
 
 
-class RQVAE(Stage1Model):
+class RQVAE(N.EngineCache, Stage1Model):
     def __init__(self, *, embed_dim=64, n_embed=512, decay=0.99, loss_type="mse", latent_loss_weight=0.25,
                  bottleneck_type="rq", ddconfig=None, checkpointing=False, **kwargs):
         super().__init__()
@@ -36,44 +36,15 @@ class RQVAE(Stage1Model):
         self.quant_conv = nn.Conv2d(ddconfig["z_channels"], embed_dim, 1)
         self.post_quant_conv = nn.Conv2d(embed_dim, ddconfig["z_channels"], 1)
         self.loss_type, self.latent_loss_weight = loss_type, latent_loss_weight
-        self.precision = None            # None -> _native.default_precision() ('auto' == exact until told otherwise)
-        self._eng = {}                   # (device, mode) -> dict(handle, tensors, ws)
-        self._eng_fp = None              # parameter fingerprint the cached engines were built from
-        self.last_launches = 0
 
     # ------------------------------------------------------------------ native engine plumbing
-    def _invalidate_native(self):
-        for e in self._eng.values():
-            N.lib().rqb200_vae_destroy(e["handle"])
-        self._eng = {}
-
-    def _apply(self, fn, *a, **k):
-        self._invalidate_native()
-        return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, *a, **k):
-        self._invalidate_native()
-        return super().load_state_dict(*a, **k)
-
-    def __del__(self):
-        try:
-            self._invalidate_native()
-        except Exception:
-            pass
-
-    def _mode(self):
-        p = self.precision or N.default_precision()
-        return N.MODE_FAST if p == "fast" else N.MODE_EXACT
+    _DESTROY = "rqb200_vae_destroy"
 
     def _engine(self, device):
         mode = self._mode()
-        fp = N.param_fingerprint(self)
-        if fp != self._eng_fp:               # weights changed behind the module's own hooks (wrapper load, in-place write)
-            self._invalidate_native()
-            self._eng_fp = fp
-        key = (str(device), mode)
-        if key in self._eng:
-            return self._eng[key]
+        return self._cached_engine((str(device), mode), N.param_fingerprint(self), lambda: self._build_engine(mode))
+
+    def _build_engine(self, mode):
         L = N.lib()
         dd = self.ddconfig
         cfg = N.VaeConfig()
@@ -137,17 +108,7 @@ class RQVAE(Stage1Model):
         else:
             reg("codebook", tabs.float())
         N.check(L.rqb200_vae_finalize(handle), "vae_finalize")
-        eng = {"handle": handle, "keep": keep, "ws": {}}
-        self._eng[key] = eng
-        return eng
-
-    def _ws(self, eng, B, device, hw):
-        """the workspace for B images of hw = (H, W) pixels; the largest buffer so far is kept"""
-        need = N.lib().rqb200_vae_workspace_bytes_hw(eng["handle"], B, *hw)
-        ws = eng["ws"].get("buf")
-        if ws is None or ws.numel() < need:
-            eng["ws"]["buf"] = ws = torch.empty(need, dtype=torch.uint8, device=device)
-        return ws, need
+        return {"handle": handle, "keep": keep, "ws": None}
 
     def _run(self, fn_name, x, out_shape, hw, ext=()):
         """one native call on x -> out_shape.  hw: the call's pixel extent (H, W); ext: the extent arguments the *_hw entry points
@@ -157,7 +118,8 @@ class RQVAE(Stage1Model):
         B = x.shape[0]
         out = torch.empty(out_shape, dtype=torch.float32, device=x.device)
         with torch.cuda.device(x.device):
-            ws, need = self._ws(eng, B, x.device, hw)
+            # no refusal message: only decode_code of an empty batch gets a zero size, and the engine's own call reports it
+            ws = N.workspace(eng, N.lib().rqb200_vae_workspace_bytes_hw(eng["handle"], B, *hw), x.device)
             fn = getattr(N.lib(), fn_name)
             N.check(fn(eng["handle"], N.ptr(x), B, *ext, N.ptr(out), N.ptr(ws), ws.numel(), N.stream_ptr(x.device)), fn_name)
         self.last_launches = N.lib().rqb200_vae_last_launches(eng["handle"])
