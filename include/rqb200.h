@@ -408,6 +408,41 @@ int rqb200_lpips_forward(rqb200_lpips* h, const float* x0, const float* x1, int 
                          void* workspace, size_t workspace_bytes, void* stream);
 int64_t rqb200_lpips_last_launches(const rqb200_lpips* h);
 
+/* ------------------------------------------------------------------------------------------------ ResNet-101
+ * torchvision's resnet101 (rqvae/metrics/resnet.py: ResNet101, the v1.5 Bottleneck with the stride on its 3x3), the ImageNet classifier
+ * of rejection sampling, forward only as a static layer plan (csrc/resnet_engine.cu).  Tensors are registered under torchvision's
+ * state_dict keys as they are (fp32, device): "conv1.weight", "bn1.*", "layer{1..4}.{i}.conv{1,2,3}.weight", "...bn{1,2,3}.*",
+ * "layer{1..4}.0.downsample.{0,1}.*" and "fc.weight" [1000, 2048] / "fc.bias", with * = weight, bias, running_mean, running_var.
+ * rqb200_resnet_finalize names the first missing or mis-sized key, then folds each BatchNorm (eps 1e-5) into its conv in fp64 on
+ * `stream`, into the caller's parameter buffer of rqb200_resnet_params_bytes(h) bytes, which must stay alive and unchanged while the
+ * engine is used; fc is read from the registered tensors at each forward.  Two tiers: RQB200_MODE_EXACT runs every conv on fp32 FFMA;
+ * RQB200_MODE_FAST runs every conv but the stem conv1 (Cin = 3, fp32 FFMA on both tiers) on the wgmma implicit GEMM with split-fp16
+ * operands.  The residual stream and fc are fp32 on both tiers.  The section is additive (rqb200_version() is unchanged): a caller
+ * finds it by looking up the rqb200_resnet_create symbol. */
+typedef struct rqb200_resnet rqb200_resnet;
+typedef struct {
+    int32_t mode;       /* RQB200_MODE_EXACT or RQB200_MODE_FAST */
+} rqb200_resnet_config;
+
+/* rqb200_resnet_forward flags */
+#define RQB200_RESNET_FEATURES 1            /* write the pooled features [B, 2048] to `features` */
+#define RQB200_RESNET_CROP(c) ((c) << 8)    /* take the centre c x c window first (torchvision CenterCrop's offsets); 0: the whole image */
+
+rqb200_resnet* rqb200_resnet_create(const rqb200_resnet_config* cfg);
+void rqb200_resnet_destroy(rqb200_resnet* h);
+int rqb200_resnet_set_tensor(rqb200_resnet* h, const char* key, const void* ptr, int dtype, int64_t numel);
+size_t rqb200_resnet_params_bytes(const rqb200_resnet* h);
+int rqb200_resnet_finalize(rqb200_resnet* h, void* params, size_t params_bytes, void* stream);
+/* the workspace of rqb200_resnet_forward on B images of H x W with these flags; 0 unless B >= 1, the crop fits in H x W and the extent
+ * the network sees is at least 32 x 32.  A batch whose activations exceed 2 GiB runs in chunks inside one call. */
+size_t rqb200_resnet_workspace_bytes(rqb200_resnet* h, int B, int H, int W, int flags);
+/* x NCHW [B, 3, H, W] f32 pixels in [0, 1] -> logits [B, 1000] f32 (and features [B, 2048] with RQB200_RESNET_FEATURES), after the
+ * optional centre crop and transforms.Normalize(mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225)).  Nothing is allocated and
+ * nothing synchronises.  An image's outputs do not depend on the other images of the batch. */
+int rqb200_resnet_forward(rqb200_resnet* h, const float* x, int B, int H, int W, int flags, float* logits, float* features, void* workspace,
+                          size_t workspace_bytes, void* stream);
+int64_t rqb200_resnet_last_launches(const rqb200_resnet* h);
+
 /* ------------------------------------------------------------------------------------------------ diagnostics
  * Single-kernel entry points used by tests/ and bench.py's roofline leg; not part of the reference-facing surface.
  * rqb200_dbg_gemm_tc: one launch of the wgmma weight-streaming GEMM (csrc/gemm_tc.cu):
@@ -580,6 +615,21 @@ int rqb200_dbg_lpips_head(const float* F, const float* w, float* d, int n, int h
 /* rqb200_dbg_lpips_mean: tap k's spatial average of d [n, hw] in fp64: tapmean [n, 5] (f64) entry k, layer_out [n, 5] (nullable) its
  *   f32 value, and at k == 4 val [n] = the sum of tapmean's five entries. */
 int rqb200_dbg_lpips_mean(const float* d, int n, int hw, int k, double* tapmean, float* layer_out, float* val, void* stream);
+
+/* The ResNet engine's kernels (csrc/resnet_engine.cu), one launch each.  Maps are NHWC f32.
+ * rqb200_dbg_resnet_input: x NCHW [B, 3, H, W] -> y NHWC [B, c, c, 3] (the centre crop, crop = c > 0) or [B, H, W, 3] (crop = 0), each
+ *   (v - mean[ch]) / std[ch] with ImageNet's mean and std in fp32. */
+int rqb200_dbg_resnet_input(const float* x, float* y, int B, int H, int W, int crop, void* stream);
+/* rqb200_dbg_resnet_conv: the residual forms of the fp32 FFMA conv: act(conv(X, Wt) + bias + residual) of X [B, H, W, Cin] with Wt
+ *   OHWI [Cout, k, k, Cin], zero padding pad on every side and stride `stride`; output pixel m's channel n goes to out[m * ldy + yoff + n]
+ *   and reads residual (nullable) at the same index; act = ReLU when relu != 0, else the identity. */
+int rqb200_dbg_resnet_conv(const float* X, const float* Wt, const float* bias, const float* residual, float* out, int B, int H, int W, int Cin,
+                           int Cout, int k, int pad, int stride, int ldy, int yoff, int relu, void* stream);
+/* rqb200_dbg_resnet_conv_tc: the same on the fast tier's wgmma conv (split-fp16 operands as rqb200_dbg_inception_conv_tc; Cin % 8 == 0,
+ *   Cout, ldy and yoff multiples of 16, stride 1 or 2), out (nullable) fp32 and out_hi / out_lo (both or neither) its fp16 halves. */
+int rqb200_dbg_resnet_conv_tc(const void* X16, const void* X16lo, const void* W16, const void* W16lo, const float* bias, const float* residual,
+                              float* out, void* out_hi, void* out_lo, int B, int H, int W, int Cin, int Cout, int k, int pad, int stride,
+                              int ldy, int yoff, int relu, void* stream);
 
 #ifdef __cplusplus
 }

@@ -18,13 +18,16 @@ constexpr int CB_M = 64, CB_N = 64, CB_K = 16, C_THREADS = 256;
 template <typename WT>
 __device__ __forceinline__ float w_at(const WT* p, int64_t i) { return to_f32<WT>(p[i]); }
 
-// INC = false: the VAE's form (one symmetric pad, output rows of Cout).  INC = true: the Inception engine's form -- separate
-// pad_h / pad_w (1x7, 7x1, 1x3, 3x1 and 5x5 kernels), bias + ReLU, and the output written into channels [yoff, yoff + Cout) of
-// rows of ldy floats (a branch's slice of its block's concat buffer).  A separate instantiation, so the VAE's launches keep their code.
-template <typename WT, bool INC = false>
-__global__ void __launch_bounds__(C_THREADS)
-conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const float* __restrict__ bias, const float* R,
-                  float* Y, ConvGeom g) {
+// Epilogue forms of the conv body.  EPI_VAE: the VAE's form (one symmetric pad, output rows of Cout, optional residual R [M, Cout]).
+// The plan forms (Inception, LPIPS, ResNet) take separate pad_h / pad_w (1x7, 7x1, 1x3, 3x1, 5x5 and 7x7 kernels) and write channels
+// [yoff, yoff + Cout) of rows of ldy floats (a branch's slice of its block's concat buffer): EPI_RELU = ReLU(acc + bias); EPI_RES_RELU /
+// EPI_RES_ID = act(acc + bias + R) with R (nullable) fp32 read at the output's own index (a ResNet block's identity), act ReLU or none.
+enum ConvEpi { EPI_VAE = 0, EPI_RELU = 1, EPI_RES_RELU = 2, EPI_RES_ID = 3 };
+
+template <typename WT, int EPI>
+__device__ __forceinline__ void conv_igemm_body(const float* __restrict__ X, const WT* __restrict__ W, const float* __restrict__ bias,
+                                                const float* R, float* Y, const ConvGeom& g) {
+    constexpr bool INC = EPI != EPI_VAE;
     __shared__ float As[CB_K][CB_M + 4];
     __shared__ float Ws[CB_K][CB_N + 4];
     const int t = threadIdx.x, tx = t & 15, ty = t >> 4;
@@ -107,8 +110,14 @@ conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const f
             int n = n0 + tx * 4 + j;
             if (n >= N) continue;
             float v = acc[i][j] + (bias ? bias[n] : 0.f);
-            if (INC) {
+            if (EPI == EPI_RELU) {
                 Y[mm * g.ldy + g.yoff + n] = fmaxf(v, 0.f);
+                continue;
+            }
+            if (INC) {
+                const int64_t o = mm * g.ldy + g.yoff + n;
+                if (R) v = v + R[o];
+                Y[o] = EPI == EPI_RES_RELU ? fmaxf(v, 0.f) : v;
                 continue;
             }
             if (R) v = R[mm * N + n] + v;                                  // x + h  (layers.py:120,182)
@@ -116,6 +125,22 @@ conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const f
             else Y[mm * N + n] = v;
         }
     }
+}
+
+// INC = false: the VAE's form; INC = true: the Inception and LPIPS plans' conv + bias + ReLU.  Separate instantiations, so each keeps its code.
+template <typename WT, bool INC = false>
+__global__ void __launch_bounds__(C_THREADS)
+conv_igemm_kernel(const float* __restrict__ X, const WT* __restrict__ W, const float* __restrict__ bias, const float* R,
+                  float* Y, ConvGeom g) {
+    conv_igemm_body<WT, INC ? EPI_RELU : EPI_VAE>(X, W, bias, R, Y, g);
+}
+
+// the ResNet plan's residual forms: act(conv + bias [+ R]), fp32 weights
+template <bool RELU>
+__global__ void __launch_bounds__(C_THREADS)
+conv_igemm_res_kernel(const float* __restrict__ X, const float* __restrict__ W, const float* __restrict__ bias, const float* R, float* Y,
+                      ConvGeom g) {
+    conv_igemm_body<float, RELU ? EPI_RES_RELU : EPI_RES_ID>(X, W, bias, R, Y, g);
 }
 
 ConvGeom vae_conv_geom(int B, int H, int W, int Cin, int Cout, int ks, int stride, int upsample, int in_nchw, int out_nchw) {
@@ -152,6 +177,18 @@ int launch_conv_relu(const float* X, const float* W, const float* bias, float* Y
     dim3 grid((unsigned)ceil_div(M, CB_M), (unsigned)ceil_div(g.Cout, CB_N));
     conv_igemm_kernel<float, true><<<grid, C_THREADS, 0, st>>>(X, W, bias, nullptr, Y, g);
     return check_launch("conv_igemm_relu");
+}
+
+// the residual forms of the same conv (the ResNet engine): Y = act(conv + bias + R), R (nullable) fp32 rows of g.ldy floats read at the
+// output's own index; act = ReLU when relu, else the identity
+int launch_conv_res(const float* X, const float* W, const float* bias, const float* R, float* Y, const ConvGeom& g, bool relu,
+                    cudaStream_t st) {
+    const int64_t M = (int64_t)g.B * g.Ho * g.Wo;
+    if (M <= 0) return 0;
+    dim3 grid((unsigned)ceil_div(M, CB_M), (unsigned)ceil_div(g.Cout, CB_N));
+    if (relu) conv_igemm_res_kernel<true><<<grid, C_THREADS, 0, st>>>(X, W, bias, R, Y, g);
+    else conv_igemm_res_kernel<false><<<grid, C_THREADS, 0, st>>>(X, W, bias, R, Y, g);
+    return check_launch("conv_igemm_res");
 }
 
 // ------------------------------------------------------------------------------------------------ GroupNorm(32) (+SiLU)

@@ -845,7 +845,8 @@ int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, con
 // ------------------------------------------------------------------------------------------------ Inception convs (fast tier)
 // The Inception engine's convs on conv_tc_kernel's layout, generalised: any KH x KW with separate top/bottom and left/right zero
 // padding (the tap's box starts at x * stride + kx - pad_w, y * stride + ky - pad_h; TMA zero-fills every box element at a negative
-// or past-the-end coordinate, which IS the padding), stride-2 "valid" convs, and Cin % 8 == 0 rather than % 64: the activation's
+// or past-the-end coordinate, which IS the padding, also with the element stride 2 of a padded stride-2 conv, whose box can start at
+// -1), stride-2 convs, and Cin % 8 == 0 rather than % 64: the activation's
 // tensor map has the true channel extent Cin, so the last 64-channel slab's channels past Cin are zero-filled in A and multiply the
 // next tap's weights (or the weight map's own zero fill) to zero.  That keeps the activations unpadded, so the engine's concat
 // buffers stay exactly the reference's channel layout.  Epilogue: bias + ReLU, stored at channel yoff of rows of ldy as fp32 and
@@ -860,12 +861,14 @@ struct IncTcParams {
     __half* out_hi;                // fp16 hi / lo of the same values, [B, H, W, ldy], or null
     __half* out_lo;
     int ldy, yoff;
+    const float* residual;         // residual forms only: fp32 [B, H, W, ldy] read at the output's own index, or null
 };
 
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(CT_THREADS, 1)
-inc_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, IncTcParams p) {
+// EPI: 0 = ReLU(acc + bias) (the Inception and LPIPS plans); 1 / 2 = act(acc + bias [+ residual]) with act ReLU / the identity (the
+// ResNet plan's bottleneck conv3 and downsample convs)
+template <int BN, int STAGES, int EPI>
+__device__ __forceinline__ void inc_conv_tc_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo,
+                                                 const CUtensorMap& tmBlo, const IncTcParams& p) {
     constexpr int B_BYTES = BN * 64 * 2;
     constexpr int STAGE_BYTES = 2 * (CT_A_BYTES + B_BYTES);
     constexpr int OFF_B = 2 * CT_A_BYTES;                    // [A_hi | A_lo | B_hi | B_lo]
@@ -947,13 +950,28 @@ inc_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             const int n0 = nt * BN + c;
             if (n0 >= p.Cout || !valid) return;                     // Cout % 16 == 0: a 16-channel chunk is all in or all out
             float w[16];
-#pragma unroll
-            for (int i = 0; i < 16; i += 4) {
-                const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
-                w[i] = fmaxf(v[i] + bb.x, 0.f); w[i + 1] = fmaxf(v[i + 1] + bb.y, 0.f);
-                w[i + 2] = fmaxf(v[i + 2] + bb.z, 0.f); w[i + 3] = fmaxf(v[i + 3] + bb.w, 0.f);
-            }
             const int64_t o = pix * p.ldy + p.yoff + n0;
+            if (EPI == 0) {
+#pragma unroll
+                for (int i = 0; i < 16; i += 4) {
+                    const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
+                    w[i] = fmaxf(v[i] + bb.x, 0.f); w[i + 1] = fmaxf(v[i + 1] + bb.y, 0.f);
+                    w[i + 2] = fmaxf(v[i + 2] + bb.z, 0.f); w[i + 3] = fmaxf(v[i + 3] + bb.w, 0.f);
+                }
+            } else {
+#pragma unroll
+                for (int i = 0; i < 16; i += 4) {
+                    const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + i);
+                    w[i] = v[i] + bb.x; w[i + 1] = v[i + 1] + bb.y; w[i + 2] = v[i + 2] + bb.z; w[i + 3] = v[i + 3] + bb.w;
+                    if (p.residual) {
+                        const float4 rr = *reinterpret_cast<const float4*>(p.residual + o + i);
+                        w[i] += rr.x; w[i + 1] += rr.y; w[i + 2] += rr.z; w[i + 3] += rr.w;
+                    }
+                    if (EPI == 1) {
+                        w[i] = fmaxf(w[i], 0.f); w[i + 1] = fmaxf(w[i + 1], 0.f); w[i + 2] = fmaxf(w[i + 2], 0.f); w[i + 3] = fmaxf(w[i + 3], 0.f);
+                    }
+                }
+            }
             if (p.out) {
 #pragma unroll
                 for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(p.out + o + i) = make_float4(w[i], w[i + 1], w[i + 2], w[i + 3]);
@@ -979,6 +997,21 @@ inc_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 }
 
 template <int BN, int STAGES>
+__global__ void __launch_bounds__(CT_THREADS, 1)
+inc_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, IncTcParams p) {
+    inc_conv_tc_body<BN, STAGES, 0>(tmA, tmB, tmAlo, tmBlo, p);
+}
+
+// the residual forms (the ResNet plan): act(conv + bias [+ p.residual]), act ReLU when RELU, else the identity
+template <int BN, int STAGES, bool RELU>
+__global__ void __launch_bounds__(CT_THREADS, 1)
+inc_conv_tc_res_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, IncTcParams p) {
+    inc_conv_tc_body<BN, STAGES, RELU ? 1 : 2>(tmA, tmB, tmAlo, tmBlo, p);
+}
+
+template <int BN, int STAGES>
 static int launch_inc_conv_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
                                 const IncTcParams& p, int n_sm, cudaStream_t st) {
     constexpr size_t smem = (size_t)STAGES * 2 * (CT_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 256;
@@ -989,9 +1022,22 @@ static int launch_inc_conv_tc_t(const CUtensorMap& tmA, const CUtensorMap& tmB, 
     return check_launch("inc_conv_tc");
 }
 
+template <int BN, int STAGES, bool RELU>
+static int launch_inc_conv_tc_res_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmAlo, const CUtensorMap& tmBlo,
+                                    const IncTcParams& p, int n_sm, cudaStream_t st) {
+    constexpr size_t smem = (size_t)STAGES * 2 * (CT_A_BYTES + BN * 128) + 128 * ((BN < 32 ? BN : 32) + 4) * 4 + 1024 + 256;
+    static_assert(smem <= 227 * 1024, "inc_conv_tc: shared memory budget");
+    RQB_ENSURE_SMEM(smem, (inc_conv_tc_res_kernel<BN, STAGES, RELU>));
+    const int total = p.tiles_x * p.tiles_y * p.tiles_b * p.n_tiles_n;
+    inc_conv_tc_res_kernel<BN, STAGES, RELU><<<total < n_sm ? total : n_sm, CT_THREADS, smem, st>>>(tmA, tmB, tmAlo, tmBlo, p);
+    return check_launch("inc_conv_tc_res");
+}
+
 int launch_inc_conv_tc(const void* X16, const void* X16lo, const void* W16, const void* W16lo, const float* bias, float* out,
                        void* out_hi, void* out_lo, int B, int Hi, int Wi, int Cin, int Cout, int KH, int KW, int pad_h, int pad_w,
-                       int stride, int ldy, int yoff, cudaStream_t st) {
+                       int stride, int ldy, int yoff, cudaStream_t st, int epi, const float* residual) {
+    if (epi < 0 || epi > 2 || (residual && epi == 0))
+        return fail(RQB200_EINVAL, "inc_conv_tc: epilogue must be 0 (ReLU), 1 (residual + ReLU) or 2 (residual, no ReLU)");
     if (!X16 || !X16lo || !W16 || !W16lo || !bias || (!out && !out_hi) || (out_hi && !out_lo))
         return fail(RQB200_EINVAL, "inc_conv_tc: need both operand halves, a bias and an fp32 or an fp16 hi + lo output");
     if (Cin % 8 || Cout % 16 || ldy % 16 || yoff % 16 || yoff + Cout > ldy || (stride != 1 && stride != 2) || KH < 1 || KW < 1 ||
@@ -1009,7 +1055,7 @@ int launch_inc_conv_tc(const void* X16, const void* X16lo, const void* W16, cons
     p.tiles_x = (int)ceil_div(p.W, p.TW); p.tiles_y = (int)ceil_div(p.H, p.TH); p.tiles_b = (int)ceil_div(B, p.NB);
     const int BN = Cout >= 128 ? 128 : 64;
     p.n_tiles_n = (int)ceil_div(Cout, BN);
-    p.bias = bias; p.out = out; p.out_hi = (__half*)out_hi; p.out_lo = (__half*)out_lo; p.ldy = ldy; p.yoff = yoff;
+    p.bias = bias; p.out = out; p.out_hi = (__half*)out_hi; p.out_lo = (__half*)out_lo; p.ldy = ldy; p.yoff = yoff; p.residual = residual;
     const uint64_t K = (uint64_t)KH * KW * Cin;
     CUtensorMap tmA, tmB, tmAlo, tmBlo;
     RQB_TRY(make_tmap_2d(&tmB, W16, 1, K, (uint64_t)Cout, K * 2, 64, (uint32_t)BN));
@@ -1019,6 +1065,12 @@ int launch_inc_conv_tc(const void* X16, const void* X16lo, const void* W16, cons
     RQB_TRY(make_tmap_4d_nhwc(&tmAlo, X16lo, (uint64_t)Cin, (uint64_t)Wi, (uint64_t)Hi, (uint64_t)B, 64, (uint32_t)p.TW, (uint32_t)p.TH,
                               (uint32_t)p.NB, (uint32_t)stride));
     const int n_sm = sm_count();
+    if (epi == 1)
+        return BN == 128 ? launch_inc_conv_tc_res_t<128, 3, true>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
+                         : launch_inc_conv_tc_res_t<64, 4, true>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
+    if (epi == 2)
+        return BN == 128 ? launch_inc_conv_tc_res_t<128, 3, false>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
+                         : launch_inc_conv_tc_res_t<64, 4, false>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
     return BN == 128 ? launch_inc_conv_tc_t<128, 3>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st)
                      : launch_inc_conv_tc_t<64, 4>(tmA, tmB, tmAlo, tmBlo, p, n_sm, st);
 }

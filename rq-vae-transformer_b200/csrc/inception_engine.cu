@@ -106,7 +106,7 @@ int launch_inc_input(const float* x, float* y, int B, int H, int W, int resize, 
     return check_launch("inc_input");
 }
 int launch_inc_pool(const float* X, float* Y, int B, int H, int W, int C, int stride, int pad, int mode, int ldy, int yoff,
-                    cudaStream_t st, __half* Yhi = nullptr, __half* Ylo = nullptr) {
+                    cudaStream_t st, __half* Yhi, __half* Ylo) {
     const int Ho = (H + 2 * pad - 3) / stride + 1, Wo = (W + 2 * pad - 3) / stride + 1;
     inc_pool_kernel<<<grid_1d((int64_t)B * Ho * Wo * C), 256, 0, st>>>(X, Y, B, H, W, C, Ho, Wo, stride, pad, mode, ldy, yoff, Yhi, Ylo);
     return check_launch(mode == 0 ? "inc_maxpool" : "inc_avgpool");

@@ -113,6 +113,10 @@ ConvGeom vae_conv_geom(int B, int H, int W, int Cin, int Cout, int ks, int strid
 int launch_conv(const float* X, const void* W, int wdtype, const float* bias, const float* R, float* Y, const ConvGeom& g,
                 cudaStream_t st);
 int launch_conv_relu(const float* X, const float* W, const float* bias, float* Y, const ConvGeom& g, cudaStream_t st);
+// the ResNet plan's residual forms of launch_conv_relu: Y = act(conv + bias + R), R (nullable) fp32 rows of g.ldy floats read at the
+// output's own index, act ReLU when relu, else the identity
+int launch_conv_res(const float* X, const float* W, const float* bias, const float* R, float* Y, const ConvGeom& g, bool relu,
+                    cudaStream_t st);
 int launch_groupnorm_silu(const float* X, const float* gamma, const float* beta, float* Y, double* stats_ws, int B, int HW,
                           int C, int silu, cudaStream_t st);
 int launch_vae_attn(const float* qkv, float* out, int B, int HW, int C, cudaStream_t st);
@@ -127,10 +131,12 @@ int launch_conv_tc(const void* X16, const void* W16, const void* X16lo, const vo
                    cudaStream_t st, int stride = 1, double* gn_part = nullptr);
 bool conv_tc_gn_fusable(int H, int W, int Cout, int ks, int stride);
 // the Inception engine's fast-tier conv (conv_tc.cu, inc_conv_tc_kernel): X NHWC [B, Hi, Wi, Cin] fp16 hi + lo, W OHWI [Cout, KH, KW, Cin]
-// fp16 hi + lo, out[pix * ldy + yoff + n] = ReLU(conv + bias) as fp32 (out) and / or fp16 hi + lo (out_hi, out_lo)
+// fp16 hi + lo, out[pix * ldy + yoff + n] = ReLU(conv + bias) as fp32 (out) and / or fp16 hi + lo (out_hi, out_lo).  epi 1 / 2 (the
+// ResNet plan, inc_conv_tc_res_kernel): act(conv + bias + residual) with act ReLU / the identity; residual (nullable) fp32 rows of ldy
+// floats read at the output's own index.
 int launch_inc_conv_tc(const void* X16, const void* X16lo, const void* W16, const void* W16lo, const float* bias, float* out,
                        void* out_hi, void* out_lo, int B, int Hi, int Wi, int Cin, int Cout, int KH, int KW, int pad_h, int pad_w,
-                       int stride, int ldy, int yoff, cudaStream_t st);
+                       int stride, int ldy, int yoff, cudaStream_t st, int epi = 0, const float* residual = nullptr);
 int launch_rows_gemm_tc(const void* X16, const void* W16, const float* bias, const float* residual, float* out_f32, void* out_16,
                         int gelu, int fmt, int64_t M, int N_out, int K, cudaStream_t st);
 int launch_groupnorm_f16(const float* X, const float* gamma, const float* beta, void* Y16, void* Y16lo, double* stats_ws, int B,
@@ -180,9 +186,20 @@ int launch_conv_prep(const float* w, const float* bias, const float* const* bn, 
                      int64_t b_off, int Cout, int Cin, int KH, int KW, cudaStream_t st);
 // One plan conv + bias + ReLU, weights at w_off / bias at b_off of P.  The fast tier with the input's fp16 hi / lo operands (x_hi set)
 // runs inc_conv_tc_kernel, writing y (fp32) and / or y_hi / y_lo (either nullable); otherwise the fp32 FFMA kernel reads x and
-// writes y, and on the fast tier y's rows are then cast into y_hi / y_lo for the next conv.
+// writes y, and on the fast tier y's rows are then cast into y_hi / y_lo (when y_hi is set) for the next conv.
+// The residual forms (the ResNet plan): relu = false or a residual (fp32 rows of g.ldy floats at the output's index) compute
+// act(conv + bias [+ residual]) on the same two kernels' residual instantiations.
 int launch_plan_conv(bool fast, const SplitParams& P, int64_t w_off, int64_t b_off, const float* x, const __half* x_hi,
-                     const __half* x_lo, float* y, __half* y_hi, __half* y_lo, const ConvGeom& g, cudaStream_t st);
+                     const __half* x_lo, float* y, __half* y_hi, __half* y_lo, const ConvGeom& g, cudaStream_t st,
+                     const float* residual = nullptr, bool relu = true);
+
+// inception_engine.cu, shared with the ResNet plan.  3x3 pool of X NHWC [B, H, W, C] with stride and pad into channels [yoff, yoff + C)
+// of rows of ldy floats: mode 0 max (padding acts as -inf), mode 1 average over the pixels inside the map; Yhi / Ylo (nullable): the
+// values' fp16 hi / lo halves at the same index too
+int launch_inc_pool(const float* X, float* Y, int B, int H, int W, int C, int stride, int pad, int mode, int ldy, int yoff,
+                    cudaStream_t st, __half* Yhi = nullptr, __half* Ylo = nullptr);
+// global average pool: X NHWC [B, HW, C] -> Y [B, C]
+int launch_inc_gap(const float* X, float* Y, int B, int HW, int C, cudaStream_t st);
 
 // gemm_tc.cu -- wgmma weight-streaming GEMM (fast tier)
 // GT_H16_QGELU: QuickGELU x * sigmoid(1.702 x) (CLIP's MLP) instead of the exact GELU; 16-bit weights, splits == 1

@@ -50,12 +50,15 @@ int launch_conv_prep(const float* w, const float* bias, const float* const* bn, 
 }
 
 int launch_plan_conv(bool fast, const SplitParams& P, int64_t w_off, int64_t b_off, const float* x, const __half* x_hi,
-                     const __half* x_lo, float* y, __half* y_hi, __half* y_lo, const ConvGeom& g, cudaStream_t st) {
+                     const __half* x_lo, float* y, __half* y_hi, __half* y_lo, const ConvGeom& g, cudaStream_t st, const float* residual,
+                     bool relu) {
+    const bool res = residual || !relu;           // a residual form (the ResNet plan)
     if (fast && x_hi)
         return launch_inc_conv_tc(x_hi, x_lo, P.hi + w_off, P.lo + w_off, P.f32 + b_off, y, y_hi, y_lo, g.B, g.Hi, g.Wi, g.Cin, g.Cout, g.KH,
-                                  g.KW, g.pad, g.pad_w, g.stride, g.ldy, g.yoff, st);
-    RQB_TRY(launch_conv_relu(x, P.f32 + w_off, P.f32 + b_off, y, g, st));
-    return fast ? launch_cast_f16(y, y_hi, y_lo, g.B, g.Ho, g.Wo, g.ldy, 0, st) : 0;
+                                  g.KW, g.pad, g.pad_w, g.stride, g.ldy, g.yoff, st, res ? (relu ? 1 : 2) : 0, residual);
+    if (res) RQB_TRY(launch_conv_res(x, P.f32 + w_off, P.f32 + b_off, residual, y, g, relu, st));
+    else RQB_TRY(launch_conv_relu(x, P.f32 + w_off, P.f32 + b_off, y, g, st));
+    return fast && y_hi ? launch_cast_f16(y, y_hi, y_lo, g.B, g.Ho, g.Wo, g.ldy, 0, st) : 0;
 }
 
 }  // namespace rqb

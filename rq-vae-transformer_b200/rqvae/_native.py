@@ -168,7 +168,10 @@ EXPORTS = ["rqb200_last_error", "rqb200_version", "rqb200_device_count", "rqb200
            "rqb200_dbg_clip_preprocess", "rqb200_dbg_clip_attn", "rqb200_dbg_clip_attn_flash", "rqb200_lpips_create",
            "rqb200_lpips_destroy", "rqb200_lpips_set_tensor", "rqb200_lpips_params_bytes", "rqb200_lpips_finalize",
            "rqb200_lpips_workspace_bytes", "rqb200_lpips_forward", "rqb200_lpips_last_launches", "rqb200_dbg_lpips_input",
-           "rqb200_dbg_lpips_pool", "rqb200_dbg_lpips_head", "rqb200_dbg_lpips_mean"]
+           "rqb200_dbg_lpips_pool", "rqb200_dbg_lpips_head", "rqb200_dbg_lpips_mean", "rqb200_resnet_create", "rqb200_resnet_destroy",
+           "rqb200_resnet_set_tensor", "rqb200_resnet_params_bytes", "rqb200_resnet_finalize", "rqb200_resnet_workspace_bytes",
+           "rqb200_resnet_forward", "rqb200_resnet_last_launches", "rqb200_dbg_resnet_input", "rqb200_dbg_resnet_conv",
+           "rqb200_dbg_resnet_conv_tc"]
 
 
 def check(rc, what=""):

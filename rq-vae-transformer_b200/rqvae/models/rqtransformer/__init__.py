@@ -1,6 +1,7 @@
 """Stage-2 prior: parameter tree + native AR engine binding (see transformers.py)."""
 from .configs import RQTransformerConfig  # noqa: F401  (re-exported for callers that build structured configs)
 from .transformers import RQTransformer  # noqa: F401
+from .rejection import rejection_sample  # noqa: F401
 
 
 def get_rqtransformer(config):
